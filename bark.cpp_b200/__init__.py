@@ -1,10 +1,10 @@
-"""ctypes binding of libbark_b200.so — the B200-native drop-in for bark.cpp's hot path.
+"""ctypes binding of libbark_b200.so — the H100-native drop-in for bark.cpp's hot path.
 
 The product is the C-ABI shared library (include/bark.h, include/bark_b200.h); this module only
 loads it and mirrors the reference's call sequence (bark_context_default_params -> bark_load_model
 -> bark_generate_audio -> bark_get_audio_data -> bark_free, examples/main/main.cpp:49-91) for the
 Python-side tests and the benchmark.  There is no CPU path: loading fails loudly when the CUDA
-extension has not been built, and bark_load_model fails when no sm_100 device is present.
+extension has not been built, and bark_load_model fails when no sm_90 (H100) device is present.
 
 The directory name contains a dot, so import it through `__graft_entry__.load_package()`.
 """
@@ -289,7 +289,7 @@ class Bark:
 
 
 def fast_gemm(A: np.ndarray, W: np.ndarray) -> np.ndarray:
-    """C = A W^T on the tcgen05 path; A [M][K], W [N][K] float16."""
+    """C = A W^T on the wgmma path; A [M][K], W [N][K] float16."""
     A = np.ascontiguousarray(A, np.float16); W = np.ascontiguousarray(W, np.float16)
     M, K = A.shape; N = W.shape[0]
     out = np.zeros((M, N), np.float32)
@@ -299,7 +299,7 @@ def fast_gemm(A: np.ndarray, W: np.ndarray) -> np.ndarray:
 
 
 def fast_attention(q: np.ndarray, k: np.ndarray, v: np.ndarray, n_head: int) -> np.ndarray:
-    """Non-causal attention on the tcgen05 path; q, k, v [n][E] float16 -> [n][E] float16."""
+    """Non-causal attention on the wgmma path; q, k, v [n][E] float16 -> [n][E] float16."""
     q, k, v = (np.ascontiguousarray(a, np.float16) for a in (q, k, v))
     n, E = q.shape
     out = np.zeros((n, E), np.float16)

@@ -506,14 +506,14 @@ extern "C" struct bark_context * bark_load_model(const char * model_path, struct
     if (dev < 0 || dev >= n_dev) { fprintf(stderr, "%s: CUDA device %d out of range (%d present)\n", __func__, dev, n_dev); return nullptr; }
     cudaDeviceProp prop;
     if (cudaSetDevice(dev) != cudaSuccess || cudaGetDeviceProperties(&prop, dev) != cudaSuccess) { fprintf(stderr, "%s: cannot use CUDA device %d: %s\n", __func__, dev, cudaGetErrorString(cudaGetLastError())); return nullptr; }
-    if (prop.major != 10) {
-        fprintf(stderr, "%s: device %d is sm_%d%d; this library is built for sm_100a (B200) only\n", __func__, dev, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        fprintf(stderr, "%s: device %d is sm_%d%d; this library is built for sm_90a (H100) only\n", __func__, dev, prop.major, prop.minor);
         return nullptr;
     }
     bark_context * ctx = new bark_context();
     ctx->device = dev;
     ctx->n_sm = ctx->n_sm_total = prop.multiProcessorCount;
-    if (ctx->n_sm >= 132) ctx->n_sm = 128;                    // CTAs of the persistent decode step: 128 measured 1-2 % faster than 148 (fewer pollers per exchange; profiles/r02_decode_headstart_cta_sweep.txt)
+    if (ctx->n_sm >= 132) ctx->n_sm = 128;                    // CTAs of the persistent decode step: a power of two below the SM count (fewer pollers per exchange)
     { const char * e = getenv("BARK_B200_MODE"); ctx->fast_mode = e && !strcmp(e, "fast"); }             // "fast": tensor-core fine passes (fast_kernels.cu), not bit-identical
     { const char * e = getenv("BARK_B200_DECODE_CTAS"); if (e && atoi(e) >= 64 && atoi(e) <= ctx->n_sm) ctx->n_sm = atoi(e); }   // experiment knob: CTAs of the persistent decode kernel
     { const char * e = getenv("BARK_B200_SAMPLE_FLAG_EVERY"); ctx->debug_flag_every = e ? atoi(e) : 0; }
@@ -527,9 +527,9 @@ extern "C" struct bark_context * bark_load_model(const char * model_path, struct
     ctx->headstart[1] = ctx->att_ns; ctx->headstart[2] = ctx->headstart[4] = ctx->first_ns;
     { const char * e = getenv("BARK_B200_HEADSTART"); if (e) { unsigned v[6]; if (sscanf(e, "%u:%u:%u:%u:%u:%u", &v[0], &v[1], &v[2], &v[3], &v[4], &v[5]) == 6) for (int i = 0; i < 6; i++) ctx->headstart[i] = std::min(v[i], 100000u); } }
     { const char * e = getenv("BARK_B200_KV_PREFETCH"); ctx->kv_prefetch = e && !strcmp(e, "1"); }
-    { const char * e = getenv("BARK_B200_FUSE_SAMPLER"); ctx->fuse_sampler = e && !strcmp(e, "1"); }        // "1": the decode kernel's last CTA samples the token (one launch per token); measured neutral end to end
+    { const char * e = getenv("BARK_B200_FUSE_SAMPLER"); ctx->fuse_sampler = e && !strcmp(e, "1"); }        // "1": the decode kernel's last CTA samples the token (one launch per token); off by default
     { const char * e = getenv("BARK_B200_GEMM_F32C"); ctx->gemm_f32c = e && !strcmp(e, "1"); }
-    { const char * e = getenv("BARK_B200_ADAPT"); ctx->adapt_on = e && !strcmp(e, "1"); }                     // "1": self-tuning head starts (experiment; measured WORSE: the feedback is collective and runs away)
+    { const char * e = getenv("BARK_B200_ADAPT"); ctx->adapt_on = e && !strcmp(e, "1"); }                     // "1": self-tuning head starts (experiment: the feedback is collective and can run away)
     ctx->params = params;
     const bool loaded = guarded(false, [&] {                  // a CUDA failure while loading (out of memory, ...) is a failed load, not an abort
     BARK_CUDA_CHECK(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
@@ -726,7 +726,7 @@ static int bark_b200_fast_gemm_impl(const uint16_t * A, const uint16_t * W, floa
 }
 extern "C" int bark_b200_fast_gemm(const uint16_t * A, const uint16_t * W, float * C, int M, int N, int K) { return guarded((int) 0, [&] { return bark_b200_fast_gemm_impl(A, W, C, M, N, K); }); }
 static int bark_b200_fast_attention_impl(const uint16_t * q, const uint16_t * k, const uint16_t * v, uint16_t * out, int n, int E, int H) {
-    if (!q || !k || !v || !out || n < 256 || n % 256 || E != H * 64) return 0;
+    if (!q || !k || !v || !out || n < 128 || n % 128 || E != H * 64) return 0;
     std::vector<uint16_t> qk((size_t) n * 2 * E), vt((size_t) E * n);
     for (int r = 0; r < n; r++) {
         memcpy(&qk[(size_t) r * 2 * E], q + (size_t) r * E, (size_t) E * 2); memcpy(&qk[(size_t) r * 2 * E + E], k + (size_t) r * E, (size_t) E * 2);
@@ -758,4 +758,4 @@ extern "C" int bark_b200_decode_adapt(struct bark_context * ctx, int which, unsi
 }
 extern "C" int bark_b200_fast_mode(struct bark_context * ctx) { return ctx && ctx->fast_mode ? 1 : 0; }
 
-extern "C" const char * bark_b200_version(void) { return "bark_b200 r2 (sm_100a; parity path + opt-in tcgen05 fast mode)"; }
+extern "C" const char * bark_b200_version(void) { return "bark_b200 r3 (sm_90a; parity path + opt-in wgmma fast mode)"; }

@@ -103,6 +103,14 @@ __global__ void __launch_bounds__(256) conv1d_lane_kernel(const float * __restri
     }
 }
 
+// SMs of the current device: the grid-shaping target of the convolutions below (results do not depend on it)
+static int device_sms() {
+    int dev = 0, n = 0;
+    BARK_CUDA_CHECK(cudaGetDevice(&dev));
+    BARK_CUDA_CHECK(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
+    return n;
+}
+
 void conv1d(const float * x, int Cin, int T, const ConvW & cv, bool elu_in, const float * resid, float * y, cudaStream_t s) {
     const int K = Cin * cv.k, nsteps = K / 32, ngroups = (nsteps + 7) / 8;
     if (ngroups > 4) { fprintf(stderr, "bark_b200: unsupported conv shape Cin=%d k=%d\n", Cin, cv.k); throw std::runtime_error("unsupported configuration (see the message above)"); }
@@ -112,7 +120,8 @@ void conv1d(const float * x, int Cin, int T, const ConvW & cv, bool elu_in, cons
     const int tiles = (T + TT - 1) / TT;
     // enough blocks to fill the machine: split the output channels when there are few time tiles
     int o_per_block = cv.cout;
-    while (o_per_block > 8 && tiles * ((cv.cout + o_per_block - 1) / o_per_block) < 4 * 148) o_per_block = (o_per_block + 1) / 2;
+    const int n_sm = device_sms();
+    while (o_per_block > 8 && tiles * ((cv.cout + o_per_block - 1) / o_per_block) < 4 * n_sm) o_per_block = (o_per_block + 1) / 2;
     const dim3 grid(tiles, (cv.cout + o_per_block - 1) / o_per_block);
     g_next_flops = 2.0 * (double) T * cv.cout * K;
 #define CONV_CASE(KW, NG)                                                                                                   \
@@ -183,7 +192,8 @@ void convtr1d(const float * x, int Cin, int T, const ConvW & cv, int stride, flo
     const size_t smem = (size_t) Cin * S * sizeof(float);
     const int tiles = (T + TF - 1) / TF;
     int gy = (cv.cout * stride + 7) / 8;
-    while (gy > 1 && tiles * gy > 8 * 148) gy = (gy + 1) / 2;
+    const int n_sm = device_sms();
+    while (gy > 1 && tiles * gy > 8 * n_sm) gy = (gy + 1) / 2;
     g_next_flops = 2.0 * 2.0 * (double) T * stride * cv.cout * Cin;
     if (ngroups <= 1) BARK_LAUNCH(convtr1d_lane_kernel<1>, dim3(tiles, gy), 256, smem, s, x, Cin, T, cv.w, cv.Kp, cv.b, cv.cout, stride, y);
     else              BARK_LAUNCH(convtr1d_lane_kernel<2>, dim3(tiles, gy), 256, smem, s, x, Cin, T, cv.w, cv.Kp, cv.b, cv.cout, stride, y);
@@ -283,7 +293,7 @@ void lstm_layer(const float * x, int C, int T, const __half * wih_li, const __ha
     BARK_LAUNCH(lstm_inproj_lane_kernel, dim3((T + 7) / 8, 32), 256, (size_t) 8 * C * sizeof(float), s, x, C, T, wih_li, Kp, bih, G4, gi_scratch);
     BARK_CUDA_CHECK(cudaMemsetAsync(counter, 0, sizeof(unsigned), s));
     constexpr int UPB = 4;
-    const int blocks = Hn / UPB;                         // 128 CTAs for H = 512: co-resident on 148 SMs (cooperative launch checks it)
+    const int blocks = Hn / UPB;                         // 128 CTAs for H = 512: co-resident on the 132 SMs of an H100 (cooperative launch checks it)
     const size_t smem = (size_t)(Hn + 4 * UPB) * sizeof(float);
     void * args[] = {(void *) &gi_scratch, (void *) &T, (void *) &Hn, (void *) &whh_li, (void *) &Kp, (void *) &bhh, (void *) &skip, (void *) &hbuf, (void *) &counter, (void *) &out};
     if (g_prof_on) prof_begin("lstm_recur_kernel", s, 0.0, 2.0 * (double) T * G4 * Hn);

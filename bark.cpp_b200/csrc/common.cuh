@@ -1,4 +1,4 @@
-// Shared device/host helpers for the B200-native bark hot path (sm_100a only).
+// Shared device/host helpers for the H100-native bark hot path (sm_90a only).
 //
 // "Lane order": the reference's CPU dot products (ggml.c:2144 ggml_vec_dot_f32, ggml.c:2251
 // ggml_vec_dot_f16, pinned AVX2/FMA build) keep 32 independent float accumulators — element k goes

@@ -30,13 +30,13 @@ struct bark_context {
     unsigned tag_base = 0;                           // epoch counter of the decode kernel's tagged exchanges (advances 6*L per token)
     int n_sm = 0, n_sm_total = 0; bool use_decode_kernel = true;   // n_sm: CTAs of the persistent decode kernel (knob); n_sm_total: SMs of the device
     bool kv_reuse = true; unsigned long long n_kv_reused = 0;   // coarse windows start from the cached prefix (bark_api.cu run_coarse)
-    // decode-kernel knobs (BARK_B200_DECODE_TIMING_TID / BARK_B200_POLL_NS / BARK_B200_POLL_FIRST_NS); defaults from the measured sweep
-    // in profiles/r01_decode_knob_sweep.md: 40 ns back-off between polls, 500 ns head start for the two residual exchanges
+    // decode-kernel knobs (BARK_B200_DECODE_TIMING_TID / BARK_B200_POLL_NS / BARK_B200_POLL_FIRST_NS); defaults:
+    // 40 ns back-off between polls, 500 ns head start for the two residual exchanges
     bool kv_prefetch = false;          // BARK_B200_KV_PREFETCH=1: bulk L2 prefetch of the next layer's K / V rows inside the decode step
     bool fuse_sampler = false; unsigned * d_done_counter = nullptr;  // BARK_B200_FUSE_SAMPLER=1: the decode kernel samples its own token (6411 instead of 8037 launches per clip; 233.3 vs 233.7 ms: neutral, so off)
     bool decode_cluster = false;                     // BARK_B200_DECODE=cluster: the decode step inside one 16-CTA cluster (decode_kernels.cu) where the model fits
     bool gemm_f32c = false;                          // BARK_B200_GEMM_F32C=1: multi-row passes of f16 models keep operands as f16 values in f32 containers
-    bool adapt_on = false;                           // BARK_B200_ADAPT=1: self-tuning head starts instead of the fixed knobs below (measured worse, see decode_kernels.cu)
+    bool adapt_on = false;                           // BARK_B200_ADAPT=1: self-tuning head starts instead of the fixed knobs below (experiment, see decode_kernels.cu)
     unsigned headstart[6] = {0, 2000, 500, 400, 500, 0};   // BARK_B200_HEADSTART=q:att:x1:ff:x2:scores (ns): sleep before the first poll of each exchange
     int timing_tid = 0; unsigned poll_ns = 40, first_ns = 500, att_ns = 2000;   // att_ns (BARK_B200_POLL_ATT_NS): head start before CTAs without a soft_max tile poll for the attention output
     unsigned long long * d_timing = nullptr;         // optional phase timestamps of the decode kernel (BARK_B200_DECODE_TIMING=1)

@@ -7,20 +7,18 @@
 //  * Weights are a pure stream: each CTA owns a contiguous row range of every matrix (lane-interleaved rows), each warp a
 //    contiguous slice of that range.  As soon as a warp finishes a phase, its lane 0 issues ONE TMA bulk copy
 //    (cp.async.bulk + a per-warp mbarrier) of its rows of the phase after next into a private shared-memory staging area, so
-//    HBM latency hides behind two phases and no block-wide barrier surrounds the weight stream.  (Measured before: a
-//    CTA-wide TMA ring fed by one elected thread cost 1.3 us per phase on the critical path; per-lane 16-byte cp.async cost
-//    0.5-0.9 us of issue time per phase with 2 us tails.)  The copies carry an L2 evict-first policy: 188 MB of weights per
-//    token would otherwise flush the KV cache, the exchange words, local memory and the kernel's own code out of the 126 MB
-//    L2 on every token — the source of sporadic 2-4 us stragglers that every other CTA then waits for.
+//    HBM latency hides behind two phases and no block-wide barrier surrounds the weight stream (a CTA-wide TMA ring fed by one
+//    elected thread puts that thread on the critical path of every phase).  The copies carry an L2 evict-first policy: the
+//    weights streamed per token (188 MB for bark-small, ≈ 625 MB for bark-large) would otherwise flush the KV cache, the exchange words, local memory and
+//    the kernel's own code out of the 50 MB L2 on every token, and every other CTA waits for the one that missed.
 //  * Activations cross CTAs as TAGGED words: every exchanged float travels in one 8-byte {value, epoch} store; consumers
 //    spin on the words they need until the epoch matches.  Data and "ready" flag arrive in the same L2 transaction, so a
 //    grid-wide dependency costs one store->load latency instead of store + fence + atomic + poll + load (a classic
-//    barrier measured 1.5-2 us here; 6 per layer).  Epochs are unique per use and never reset.
+//    barrier would be needed 6 times per layer).  Epochs are unique per use and never reset.
 //    The vectors EVERY CTA gathers (q, attention output, residual stream, MLP activations) are published into kReplicas copies
 //    (lanes 0..7 of the producing warp store the same word into 8 buffers) and CTA c polls copy c % 8 with 16-byte loads: an L2
-//    line then has 18 readers instead of 148 and half as many requests.  tools/microbench/exchange_rounds.cu: one grid-wide
-//    dependency of 768 words costs 2.2x less this way (profiles/r02_exchange_rounds.md) — the hot lines, not the latency of one
-//    L2 round trip, were what made an exchange cost 1.5-2 us.
+//    line then has 1/8 of the CTAs as readers and half as many requests (tools/microbench/exchange_rounds.cu times one grid-wide
+//    dependency both ways) — hot lines, not the latency of one L2 round trip, are what makes an exchange expensive.
 //  * KV rows of older positions are prefetched into registers BEFORE waiting for q / the probabilities.
 //  * Nothing the phases need lives in local memory: block-wide state is in static shared memory (BlockCtx).
 //
@@ -106,14 +104,13 @@ __device__ __forceinline__ void publish_all(tagged_t * base, int n, int i, float
     if (lane < kReplicas) publish(base + (size_t) lane * n + i, v, tag);
 }
 __shared__ unsigned s_poll_ns, s_first_ns, s_att_ns;                           // back-off between polls (DecodeArgs::poll_ns, default 40); head start given to the two residual exchanges
-// Adaptive head start.  Polling is not free: 148 x 512 threads re-reading tagged words every ~100 ns approach the L2's request rate and
-// slow the very producers they wait for (polling from the start of each exchange costs +21 us per token, profiles/r02_decode.md), while
-// sleeping past the arrival sits on the critical path.  So every CTA keeps, per exchange type, how long it sleeps before its FIRST
+// Adaptive head start.  Polling is not free: one CTA per SM x 512 threads re-reading tagged words every ~100 ns approach the L2's request
+// rate and slow the very producers they wait for, while sleeping past the arrival sits on the critical path.  So every CTA keeps, per exchange type, how long it sleeps before its FIRST
 // poll and steers it toward "one or two polls were needed": no poll needed -> it slept too long, shorten; more than two -> lengthen.
 // The values survive from token to token in global memory (DecodeArgs::adapt); they change timing only, never results.
-// MEASURED (round 2, profiles/r02_decode.md): OFF by default.  The feedback is collective — a CTA that sleeps too long delays its own
-// next phase, every other CTA then sees "many polls" and lengthens ITS sleep — and the values run away (359-431 us per token against
-// 273 us with the fixed 500 ns / 2000 ns head starts).  Kept behind BARK_B200_ADAPT=1 as a documented negative result.
+// OFF by default: the feedback is collective — a CTA that sleeps too long delays its own next phase, every other CTA then sees "many
+// polls" and lengthens ITS sleep — and the values can run away from the fixed 500 ns / 2000 ns head starts.  Kept behind
+// BARK_B200_ADAPT=1 as an experiment.
 enum { XT_Q = 0, XT_ATT = 1, XT_X1 = 2, XT_FF = 3, XT_X2 = 4, XT_SC = 5, XT_COUNT = 8 };
 __shared__ unsigned s_adapt[XT_COUNT], s_obs[XT_COUNT], s_adapt_on;
 __device__ __forceinline__ void adapt_observe(int xt, unsigned rounds) {
@@ -220,8 +217,7 @@ __device__ __noinline__ void consume_to_smem(const tagged_t * g, int n, uint32_t
     consume_to_smem_inl<MAXJ>(g, n, tag, dst, mode, xt);
 }
 
-// FP64 is scarce on this part (a double division is ~2400 cycles of dependent latency — measured: it dominated the whole
-// LayerNorm), so the kernel never divides in double on the common path.  It only has to decide which FLOAT the
+// A double division is a long dependent-latency sequence (on the LayerNorm critical path it would dominate), so the kernel never divides in double on the common path.  It only has to decide which FLOAT the
 // reference's (float)(sum / n) is: with c = sum * (1/n) and a rigorous half-width w covering both the summation-order
 // uncertainty and the error of the multiply-by-reciprocal, both ends of [c - w, c + w] rounding to the same float
 // settles it; the exact (slow) path runs otherwise.
@@ -269,8 +265,8 @@ __device__ __noinline__ void block_layernorm(const float * xs, int E, double inv
     {
         // the 16 warp partials are combined by a 4-level xor butterfly inside every warp (lane l starts from partial l & 15): every lane of
         // every warp ends with the same bits (each level adds the same two values on both sides, addition is commutative), any order is
-        // covered by the bracket below.  The earlier form — every thread loads all 16 partials and adds them itself — cost 0.35 us per
-        // statistic (32 LDS + 30 adds per thread, FP64 issue-bound; profiles/r02_decode_fine_stamps.txt).
+        // covered by the bracket below.  The alternative — every thread loads all 16 partials and adds them itself — is 32 LDS + 30 FP64
+        // adds per thread and issue-bound.
         double qd[1]; float qf[1];
         qd[0] = sA[lane & (kWarps - 1)]; qf[0] = fA[lane & (kWarps - 1)];
 #pragma unroll
@@ -666,8 +662,8 @@ __device__ __noinline__ void run_phase(int phase, int ep, int layer, uint32_t ot
 
 // P2 of a layer (scores) for the CTAs that take score tasks, and P3 (soft_max + P.V) for the CTAs that own a soft_max tile, are real
 // calls with their own register allocation.  Inlined into the 128-register kernel body the "prefetched" V values were spilled right after
-// each load (LDG -> STL in the SASS: every load waited for its data, 0.3 us each, 2.2-4.6 us per layer on the soft_max CTAs —
-// profiles/r02_decode_fine_stamps.txt); here they stay in registers.
+// each load (LDG -> STL in the SASS: every load waited for its data, on the soft_max CTAs that are the critical path); here they stay
+// in registers.
 // Where this warp keeps the K rows of its score tasks: the tail of half 0 of its staging slot, behind the rows of the two phases that
 // use that half (c_attn and c_fc of every layer: the split of rows over CTAs and warps is the same in every layer).  cap = tasks that fit.
 template <int DSTEPS>
@@ -703,10 +699,10 @@ __device__ __noinline__ void p2_stage_keys(int layer, int H, int n_kv, unsigned 
 
 // P2 of a layer (scores) for the CTAs that take score tasks, and P3 (soft_max + P.V) for the CTAs that own a soft_max tile, are real
 // calls with their own register allocation.  Inlined into the 128-register kernel body the "prefetched" K / V values were spilled right
-// after each load (LDG -> STL in the SASS: every load waited for its data, 0.3 us each, 2.2-4.6 us per layer on the soft_max CTAs —
-// profiles/r02_decode_fine_stamps.txt); now neither lives in registers at all.
+// after each load (LDG -> STL in the SASS: every load waited for its data, on the soft_max CTAs that are the critical path); now neither
+// lives in registers at all.
 // Task i of this warp is t = gw + i * nw = (h, k); (h, k) advance incrementally (one division for the stride instead of two per task; a
-// float-reciprocal divmod per task was measured at +216 bytes of spills and +19 % per token).  Eight dot products at a time are reduced
+// float-reciprocal divmod per task spills in this kernel).  Eight dot products at a time are reduced
 // TOGETHER by a transposed butterfly: stage xor 16 swaps half of the eight partials, xor 8 a quarter, xor 4 one, then xor 1 / xor 2 on
 // the single survivor — per task exactly the additions of lane_tree_reduce (each add sees the same two values, addition is commutative),
 // 11 shuffles instead of 40, and eight lanes publish the eight scores at once.
@@ -719,7 +715,7 @@ __device__ __noinline__ void p2_scores(int il, int H, int n_kv, float scale, uin
     const float * Kc = s_bc.mem_k + (size_t) il * ctx * E;
     // tasks t = gw + i * nw over (head, OLDER position) = (t / n_past, t % n_past); the H scores of the NEW position (its key arrives through
     // the exchange) are one extra task each for the first H warps — kept out of the loop below: with the poll of the exchange word inlined
-    // sixteen times the loop was ~400 instructions per batch and sixteen warps per SM issue every one of them (1.3-2.3 us per layer)
+    // sixteen times the loop was ~400 instructions per batch and sixteen warps per SM issue every one of them
     const int total = H * n_past, gw = (int)(blockIdx.x - score_cta0) * kWarps + warp, nw = (int)(gridDim.x - score_cta0) * kWarps;
     const int sq = nw / n_past, sr = nw - sq * n_past;
     uint32_t off; int cap; key_tail<DSTEPS>(warp, off, cap);
@@ -796,7 +792,7 @@ __device__ __noinline__ void p3_attention(int il, int n_kv, int np, int pv_h, in
     // lane: one instruction moves four chain steps of the warp), into the unused tail of its own staging half: half 1 holds the warp's
     // c_proj rows right now, at most a third of it.  The copies drain while the scores are computed elsewhere and cost neither registers
     // nor waiting.  (Held in registers, the 33 values were spilled right after each load — LDG -> STL in the SASS, every load waiting for
-    // its data: 2.2-4.6 us per layer on exactly the CTAs that are the critical path; profiles/r02_decode_fine_stamps.txt.)
+    // its data, on exactly the CTAs that are the critical path.)
     // When the tail is too small (f32 weights and a long context) the P.V loop loads from global memory itself.
     const int v = tid >> 4, dd = tid & 15, h = pv_h;
     const int col0 = pv_h * D + pv_c * 16;
@@ -1089,11 +1085,10 @@ __global__ void __launch_bounds__(kThreads, 1) gpt_decode_step_kernel(DecodeArgs
 // Decode step, CLUSTER version (BARK_B200_DECODE=cluster, bark-small-sized f16 models): the whole token inside ONE thread-block
 // cluster of 16 CTAs.
 //
-// Why: in the 148-CTA kernel above every grid-wide dependency costs 1.3-2 us through L2 (store -> visible -> polled; 7 per layer,
-// ~45 % of the token) and polling itself slows the producers.  Inside a cluster a dependency is "store into the 16 CTAs' shared
-// memory (DSMEM) + barrier.cluster" = 0.3-0.5 us, with no polling at all.  The price is bandwidth: 16 SMs pull 94 GB/s each
-// (profiles/r02_stream_bw_per_sm.txt) = 1.5 TB/s, so the 188 MB of weights bound a token at ~125 us instead of 31 us.  At today's
-// 270 us per token that trade is a clear win; the kernel is bandwidth-bound on purpose.
+// Why: in the grid-wide kernel above every dependency goes through L2 (store -> visible -> polled; 7 per layer) and polling itself
+// slows the producers.  Inside a cluster a dependency is "store into the 16 CTAs' shared memory (DSMEM) + barrier.cluster", with
+// no polling at all.  The price is bandwidth: only 16 SMs pull the weight stream.  Opt-in; 16 CTAs is a non-portable cluster size
+// that the H100 allows (cudaFuncAttributeNonPortableClusterSizeAllowed).
 //
 //   * CTA h owns head h: its warps compute exactly the q / k / v rows of that head (4 + 4 + 4 rows per warp for 64-wide heads), so
 //     LN1 -> QKV -> scores -> soft_max -> P.V runs inside one CTA with block barriers only.  The 64 attention outputs are stored into
@@ -1301,7 +1296,7 @@ __global__ void __launch_bounds__(kThreads, 1) gpt_decode_cluster_kernel(DecodeA
                 }
             }
             __syncthreads();
-            // ---- soft_max (ggml.c:13953-14042), same decisions as the 148-CTA kernel ----
+            // ---- soft_max (ggml.c:13953-14042), same decisions as the grid-wide kernel ----
             float * p = probs;
             float mx = __int_as_float(0xff800000);
             for (int i = tid; i < n_kv; i += kThreads) mx = fmaxf(mx, p[i]);

@@ -1,19 +1,18 @@
-// FAST MODE (BARK_B200_MODE=fast, opt-in): the dense contractions of the hot path on the 5th-generation tensor cores.
+// FAST MODE (BARK_B200_MODE=fast, opt-in): the dense contractions of the hot path on the Hopper tensor cores (wgmma).
 //
 // The fine model's 1024-row passes (bark.cpp:1416-1584; mul_mat sites bark.cpp:1278,1344,1371,1380,1403 and the non-causal
 // attention bark.cpp:1495-1530) are genuine GEMMs.  The parity path (gemm_kernels.cu) must replay the reference's 32 IEEE FMA chains
-// per output and therefore runs on the fp32 pipe; tcgen05 accumulates in a different order, so this path cannot be bit-identical
+// per output and therefore runs on the fp32 pipe; wgmma accumulates in a different order, so this path cannot be bit-identical
 // and is validated by teacher forcing instead (tests/test_fast_mode.py: max |dlogit|, top-1 agreement, CDF-flip rate).
 //
-//   umma_gemm_kernel   C[M][N] = A[M][K] * W[N][K]^T, f16 operands, f32 accumulate in TMEM.
-//                      warp 0: TMA producer (cp.async.bulk.tensor 2-D tiles, 128-byte swizzle, mbarrier complete_tx ring)
-//                      warp 1: TMEM allocator + single-thread tcgen05.mma issuer (kind::f16, M = 128, N = BN, K = 16 per instruction,
-//                              smem descriptors, tcgen05.commit frees the ring slot / publishes the accumulator)
-//                      warps 2-5: epilogue, tcgen05.ld 32x32b (one accumulator row per thread), fused: f16 store (+ V^T for the
-//                              attention kernel), residual add, GELU table -> f16, plain f32 store
-//   flash_attn_kernel  non-causal attention of one (head, 128-query tile) over all keys in blocks of 256: S = Q K^T into TMEM,
-//                      online soft_max by 128 threads (one query row each), P (f16) written to shared memory in the swizzled
-//                      K-major operand layout, O += P V through a second tcgen05.mma; no score matrix ever reaches HBM.
+//   wgmma_gemm_kernel  C[M][N] = A[M][K] * W[N][K]^T, f16 operands, f32 accumulate in registers.  Block tile 128 x BN.
+//                      warp 8: TMA producer (cp.async.bulk.tensor 2-D tiles, 128-byte swizzle, mbarrier complete_tx ring)
+//                      warpgroups 0-1: 64 rows each, wgmma.mma_async m64nBNk16 from shared-memory descriptors, one stage kept in
+//                              flight; fused epilogue from the accumulator registers: f16 store (+ V^T for the attention kernel),
+//                              residual add, GELU -> f16, plain f32 store
+//   flash_attn_kernel  non-causal attention of one (head, 128-query tile) over all keys in blocks of 128: each warpgroup owns 64
+//                      queries, S = Q K^T into registers (wgmma), online soft_max in registers, P (f16) stays in registers as the
+//                      A operand of O += P V (wgmma with A from registers); no score matrix ever reaches shared memory or HBM.
 //   ln_rows_f16_kernel LayerNorm -> f16 row-major operand (float statistics; the parity path's double sums are not needed here)
 #include "gpt_kernels.h"
 #include "epilogue.cuh"
@@ -29,14 +28,15 @@ __device__ __forceinline__ uint32_t smem_u32(const void * p) { return (uint32_t)
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count)); }
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory"); }
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
-// bounded wait: a protocol bug traps (the launch fails with an error) instead of hanging the GPU
+// bounded wait: a protocol bug traps (the launch fails with an error) instead of hanging the GPU.  No printf here: a function call
+// inside the MMA warpgroups' loop makes ptxas serialize every wgmma of the kernel.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     uint32_t done = 0;
     const long long t0 = clock64();
     while (true) {
         asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(done) : "r"(bar), "r"(parity) : "memory");
         if (done) break;
-        if (clock64() - t0 > 4000000000ll) { printf("bark_b200 fast mode: mbarrier wait timed out (block %d,%d thread %d)\n", blockIdx.x, blockIdx.y, threadIdx.x); __trap(); }
+        if (clock64() - t0 > 4000000000ll) __trap();
     }
 }
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap * map, int c0, int c1, uint32_t bar) {
@@ -47,43 +47,66 @@ __device__ __forceinline__ void prefetch_tmap(const CUtensorMap * map) { asm vol
 // programmatic dependent launch: wait for the preceding kernel's results / let the following kernel start its prologue
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t cols) {      // whole warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) { asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory"); }
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// completion of all MMAs issued so far by this thread -> one arrival on `bar` (implies tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint32_t bar) { asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory"); }
-// 32 consecutive accumulator columns of this thread's TMEM lane (lane = 32 * (warp % 4) + laneid)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                   "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                 : "r"(taddr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+
+// ---- wgmma (sm_90a) ---------------------------------------------------------------------------------------------------
+// Accumulator fragment of an m64nN tile, thread t of the warpgroup (w = t / 32, g = (t % 32) / 4, c = t % 4):
+//   d[4j + 0], d[4j + 1] = row 16w + g,     columns 8j + 2c, 8j + 2c + 1
+//   d[4j + 2], d[4j + 3] = row 16w + g + 8, same columns
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator accesses across the asynchronous MMAs that read / write them
+template <int R> __device__ __forceinline__ void fence_regs(float (&d)[R]) {
 #pragma unroll
-    for (int i = 0; i < 32; i++) v[i] = __uint_as_float(r[i]);
+    for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i]) :: "memory");
+}
+// D[64][64] (+)= A[64][16] * B[64][16]^T, both operands K-major in shared memory (descriptors); scale_d = 0 overwrites D
+__device__ __forceinline__ void wgmma_ss_n64(float (&d)[32], uint64_t da, uint64_t db, int scale_d) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "l"(da), "l"(db), "r"(scale_d));
+}
+// D[64][128] (+)= A[64][16] * B[128][16]^T, both operands K-major in shared memory (descriptors); scale_d = 0 overwrites D
+__device__ __forceinline__ void wgmma_ss_n128(float (&d)[64], uint64_t da, uint64_t db, int scale_d) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(da), "l"(db), "r"(scale_d));
+}
+// D[64][256] (+)= A[64][16] * B[256][16]^T, both operands K-major in shared memory (descriptors); scale_d = 0 overwrites D
+__device__ __forceinline__ void wgmma_ss_n256(float (&d)[128], uint64_t da, uint64_t db, int scale_d) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+                 : "l"(da), "l"(db), "r"(scale_d));
+}
+// D[64][64] += A[64][16] * B[64][16]^T with A in registers (four f16x2 per thread, the accumulator fragment layout), B K-major in shared memory
+__device__ __forceinline__ void wgmma_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t db) {
+    asm volatile("wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, 1, 1, 1, 0;"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
 }
 
-// Shared-memory matrix descriptor of a K-major operand tile written by TMA with the 128-byte swizzle: rows of 64 f16 (128 B),
-// 8-row groups 1024 B apart (SBO), one swizzle atom along K (LBO unused), descriptor version 1 (sm_100), layout SWIZZLE_128B = 2.
-// Advancing by one MMA (K = 16 elements = 32 B) adds 2 to the encoded start address.  (cute/arch/mma_sm100_desc.hpp: SmemDescriptor.)
+// Shared-memory matrix descriptor (sm_90 wgmma) of a K-major operand tile written by TMA with the 128-byte swizzle: rows of 64 f16
+// (128 B), 8-row groups 1024 B apart (stride byte offset), one swizzle atom along K (leading byte offset unused), layout type 1 =
+// SWIZZLE_128B.  Advancing by one MMA (K = 16 elements = 32 B) adds 2 to the encoded start address.  Tiles are 1024-byte aligned.
 __device__ __forceinline__ uint64_t kmajor_sw128_desc(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr & 0x3ffffu) >> 4) | ((uint64_t)(1024u >> 4) << 32) | (1ull << 46) | (2ull << 61);
+    return (uint64_t)((smem_addr & 0x3ffffu) >> 4) | (1ull << 16) | ((uint64_t)(1024u >> 4) << 32) | (1ull << 62);
 }
-// kind::f16 instruction descriptor (cute/arch/mma_sm100_desc.hpp: InstrDescriptor): D = f32, A = B = f16, both K-major, M x N
-__host__ __device__ constexpr uint32_t f16_idesc(int M, int N) { return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24); }
+
+template <int BN> struct WgmmaN;
+template <> struct WgmmaN<64>  { __device__ __forceinline__ static void mma(float (&d)[32], uint64_t a, uint64_t b, int sc)  { wgmma_ss_n64(d, a, b, sc); } };
+template <> struct WgmmaN<128> { __device__ __forceinline__ static void mma(float (&d)[64], uint64_t a, uint64_t b, int sc)  { wgmma_ss_n128(d, a, b, sc); } };
+template <> struct WgmmaN<256> { __device__ __forceinline__ static void mma(float (&d)[128], uint64_t a, uint64_t b, int sc) { wgmma_ss_n256(d, a, b, sc); } };
+
+__device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
+    const __half2 h = __floats2half2_rn(lo, hi);
+    return *reinterpret_cast<const uint32_t *>(&h);
+}
 
 constexpr int kBM = 128, kBK = 64;                 // CTA tile rows; K elements per pipeline stage (= one 128-byte swizzle atom)
-constexpr int kGemmThreads = 192;
+constexpr int kGemmThreads = 288;                  // warpgroups 0-1: MMA + epilogue; warp 8: TMA producer
 
 }  // namespace
 
@@ -91,9 +114,9 @@ constexpr int kGemmThreads = 192;
 // GEMM
 // ------------------------------------------------------------------------------------------------
 // GELU as the reference's table defines it (ggml.c:2546-2571: f16(x) -> 0.5 x (1 + tanh(sqrt(2/pi) x (1 + 0.044715 x^2))) -> f16), evaluated
-// with the hardware tanh instead of a 64 K-entry table: 128 dependent table look-ups per thread made the GELU epilogue 3/4 of the
-// fc GEMM's time (profiles/r02_fast_mode.md).  tanh.approx is accurate to ~2^-11 relative: the result can differ from the table by
-// one f16 ulp, which is inside fast mode's tolerance (it is not the bit-exact path).
+// with the hardware tanh instead of a 64 K-entry table: dependent table look-ups per output would dominate the fc GEMM's epilogue.
+// tanh.approx is accurate to ~2^-11 relative: the result can differ from the table by one f16 ulp, which is inside fast mode's
+// tolerance (it is not the bit-exact path).
 __device__ __forceinline__ float gelu_fast(float v) {
     const float x = __half2float(__float2half_rn(v));
     float t;
@@ -101,36 +124,56 @@ __device__ __forceinline__ float gelu_fast(float v) {
     return 0.5f * x * (1.0f + t);
 }
 
+// two horizontally adjacent outputs (m, n), (m, n + 1) of the fused epilogue
+__device__ __forceinline__ void fast_epilogue_pair(const FastEpi & ep, int m, int n, int N, float v0, float v1) {
+    const bool two = n + 1 < N, vec = two && (ep.ldo & 1) == 0;
+    if (ep.mode == FEPI_F32 || ep.mode == FEPI_RESID) {
+        float * dst = ep.out32 + (size_t) m * ep.ldo + n;
+        if (vec) {
+            float2 o = make_float2(v0, v1);
+            if (ep.mode == FEPI_RESID) { const float2 x = *reinterpret_cast<const float2 *>(dst); o.x += x.x; o.y += x.y; }
+            *reinterpret_cast<float2 *>(dst) = o;
+        } else {
+            dst[0] = ep.mode == FEPI_RESID ? v0 + dst[0] : v0;
+            if (two) dst[1] = ep.mode == FEPI_RESID ? v1 + dst[1] : v1;
+        }
+    } else if (ep.mode == FEPI_QKV16 && n >= ep.v_col0) {      // V^T for the attention kernel (v_col0 is even: a pair never straddles it)
+        ep.vt[(size_t)(n - ep.v_col0) * ep.vt_ld + m] = __float2half_rn(v0);
+        if (two) ep.vt[(size_t)(n + 1 - ep.v_col0) * ep.vt_ld + m] = __float2half_rn(v1);
+    } else {
+        if (ep.mode == FEPI_GELU16) { v0 = gelu_fast(v0); v1 = gelu_fast(v1); }
+        __half * dst = ep.out16 + (size_t) m * ep.ldo + n;
+        if (vec) *reinterpret_cast<uint32_t *>(dst) = pack_half2(v0, v1);
+        else {
+            dst[0] = __float2half_rn(v0);
+            if (two) dst[1] = __float2half_rn(v1);
+        }
+    }
+}
+
 template <int BN>
-__global__ void __launch_bounds__(kGemmThreads, 1) umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                                                                     int M, int N, int K, FastEpi ep) {
+__global__ void __launch_bounds__(kGemmThreads, 1) wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                                                                      int M, int N, int K, FastEpi ep) {
     constexpr int kStages = BN >= 256 ? 4 : BN >= 128 ? 6 : 8;
     constexpr int kABytes = kBM * kBK * 2, kBBytes = BN * kBK * 2, kStageBytes = kABytes + kBBytes;
-    constexpr uint32_t kTmemCols = BN < 32 ? 32 : BN;
     extern __shared__ unsigned char smem_raw[];
     unsigned char * smem = (unsigned char *)(((uintptr_t) smem_raw + 1023) & ~(uintptr_t) 1023);      // swizzle-128B tiles need 1024-byte alignment
-    uint64_t * bars = reinterpret_cast<uint64_t *>(smem + kStages * kStageBytes);                      // full[kStages], empty[kStages], tmem_full
-    uint32_t * tmem_slot = reinterpret_cast<uint32_t *>(bars + 2 * kStages + 1);
-    const uint32_t full0 = smem_u32(bars), empty0 = full0 + kStages * 8, tfull = empty0 + kStages * 8;
+    uint64_t * bars = reinterpret_cast<uint64_t *>(smem + kStages * kStageBytes);                      // full[kStages], empty[kStages]
+    const uint32_t full0 = smem_u32(bars), empty0 = full0 + kStages * 8;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m0 = blockIdx.y * kBM, n0 = blockIdx.x * BN;
     const int nk = K / kBK;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         prefetch_tmap(&tmA); prefetch_tmap(&tmB);
-        for (int s = 0; s < kStages; s++) { mbar_init(full0 + s * 8, 1); mbar_init(empty0 + s * 8, 1); }
-        mbar_init(tfull, 1);
+        for (int s = 0; s < kStages; s++) { mbar_init(full0 + s * 8, 1); mbar_init(empty0 + s * 8, 8); }   // empty: lane 0 of each MMA warp
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) tmem_alloc(smem_u32(tmem_slot), kTmemCols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
     pdl_launch_dependents();                                  // the next kernel of the chain may begin its prologue on SMs as they free up
     pdl_wait();                                               // everything above overlapped the previous kernel's tail; its outputs are needed from here on
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {                                      // ===== TMA producer =====
             for (int kb = 0; kb < nk; kb++) {
                 const int s = kb % kStages;
@@ -141,84 +184,50 @@ __global__ void __launch_bounds__(kGemmThreads, 1) umma_gemm_kernel(const __grid
                 tma_load_2d(dst + kABytes, &tmB, kb * kBK, n0, full0 + s * 8);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {                                      // ===== MMA issuer =====
-            constexpr uint32_t idesc = f16_idesc(kBM, BN);
-            for (int kb = 0; kb < nk; kb++) {
-                const int s = kb % kStages;
-                mbar_wait(full0 + s * 8, (kb / kStages) & 1);
-                tc_fence_after();
-                const uint32_t a = smem_u32(smem + (size_t) s * kStageBytes);
-                const uint64_t da = kmajor_sw128_desc(a), db = kmajor_sw128_desc(a + kABytes);
-#pragma unroll
-                for (int k = 0; k < kBK / 16; k++) umma_f16(tmem, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0);
-                umma_commit(empty0 + s * 8);                  // the slot is free once these MMAs have read it
-            }
-            umma_commit(tfull);                               // accumulator complete
-        }
-    } else {                                                  // ===== epilogue: warps 2..5 own TMEM lane quarters 2, 3, 0, 1 =====
-        const int q = warp & 3;
-        mbar_wait(tfull, 0);
-        tc_fence_after();
-        const int m = m0 + q * 32 + lane;
-#pragma unroll 1
-        for (int c = 0; c < BN / 32; c++) {
-            float v[32];
-            tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), v);
-            const int n = n0 + c * 32;
-            if (m >= M || n >= N) continue;
-            const bool full = n + 32 <= N;
-            if (ep.mode == FEPI_F32 || ep.mode == FEPI_RESID) {
-                float * dst = ep.out32 + (size_t) m * ep.ldo + n;
-                if (full && (ep.ldo & 3) == 0) {
-#pragma unroll
-                    for (int i = 0; i < 32; i += 4) {
-                        float4 o = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-                        if (ep.mode == FEPI_RESID) { const float4 x = *reinterpret_cast<const float4 *>(dst + i); o.x += x.x; o.y += x.y; o.z += x.z; o.w += x.w; }
-                        *reinterpret_cast<float4 *>(dst + i) = o;
-                    }
-                } else {
-                    for (int i = 0; i < 32 && n + i < N; i++) dst[i] = ep.mode == FEPI_RESID ? v[i] + dst[i] : v[i];
-                }
-            } else if (ep.mode == FEPI_QKV16 && n >= ep.v_col0) {
-                // V^T for the attention kernel: for a fixed column the 32 lanes of the warp write 32 consecutive halves (64 bytes)
-                for (int i = 0; i < 32 && n + i < N; i++) ep.vt[(size_t)(n + i - ep.v_col0) * ep.vt_ld + m] = __float2half_rn(v[i]);
-            } else {
-                __half * dst = ep.out16 + (size_t) m * ep.ldo + n;
-                if (ep.mode == FEPI_GELU16) {
-#pragma unroll
-                    for (int i = 0; i < 32; i++) v[i] = gelu_fast(v[i]);
-                }
-                if (full && (ep.ldo & 7) == 0) {
-#pragma unroll
-                    for (int i = 0; i < 32; i += 8) {
-                        uint4 pk;
-                        __half2 h0 = __floats2half2_rn(v[i], v[i + 1]), h1 = __floats2half2_rn(v[i + 2], v[i + 3]), h2 = __floats2half2_rn(v[i + 4], v[i + 5]), h3 = __floats2half2_rn(v[i + 6], v[i + 7]);
-                        pk.x = *reinterpret_cast<uint32_t *>(&h0); pk.y = *reinterpret_cast<uint32_t *>(&h1); pk.z = *reinterpret_cast<uint32_t *>(&h2); pk.w = *reinterpret_cast<uint32_t *>(&h3);
-                        *reinterpret_cast<uint4 *>(dst + i) = pk;
-                    }
-                } else {
-                    for (int i = 0; i < 32 && n + i < N; i++) dst[i] = __float2half_rn(v[i]);
-                }
-            }
-        }
+        return;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem, kTmemCols);
+    // ===== warpgroup wg: rows m0 + 64 wg .. + 63 of the tile =====
+    const int wg = warp >> 2;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; i++) acc[i] = 0.0f;
+    for (int kb = 0; kb < nk; kb++) {
+        const int s = kb % kStages;
+        mbar_wait(full0 + s * 8, (kb / kStages) & 1);
+        const uint32_t a = smem_u32(smem + (size_t) s * kStageBytes);
+        const uint64_t da = kmajor_sw128_desc(a + wg * 64 * 128), db = kmajor_sw128_desc(a + kABytes);
+        fence_regs(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBK / 16; k++) WgmmaN<BN>::mma(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
+        wgmma_commit();
+        wgmma_wait<1>();                                      // stage kb stays in flight; stage kb - 1 is complete
+        fence_regs(acc);
+        if (kb > 0 && lane == 0) mbar_arrive(empty0 + ((kb - 1) % kStages) * 8);
+    }
+    wgmma_wait<0>();
+    fence_regs(acc);
+    const int w = warp & 3, g = lane >> 2, c = lane & 3;
+    const int r0 = m0 + wg * 64 + w * 16 + g;
+#pragma unroll
+    for (int j = 0; j < BN / 8; j++) {
+        const int n = n0 + 8 * j + 2 * c;
+        if (n >= N) continue;
+        if (r0 < M)     fast_epilogue_pair(ep, r0, n, N, acc[4 * j], acc[4 * j + 1]);
+        if (r0 + 8 < M) fast_epilogue_pair(ep, r0 + 8, n, N, acc[4 * j + 2], acc[4 * j + 3]);
+    }
 }
 
 // ------------------------------------------------------------------------------------------------
-// attention (non-causal, head size 64, keys in blocks of 256)
+// attention (non-causal, head size 64, keys in blocks of 128)
 // ------------------------------------------------------------------------------------------------
-constexpr int kKeyBlk = 256, kHeadD = 64;
+constexpr int kKeyBlk = 128, kHeadD = 64, kKvStages = 4;
 struct FlashSmem {
-    static constexpr int q = 0;                                    // [128 queries][64] f16, swizzled K-major        16 KB
-    static constexpr int k = q + 128 * 128;                        // 2 stages x [256 keys][64] f16                  64 KB
-    static constexpr int v = k + 2 * kKeyBlk * 128;                // 2 stages x 4 atoms x [64 d][64 keys] f16       64 KB
-    static constexpr int p = v + 2 * kKeyBlk * 128;                // 4 atoms x [128 queries][64 keys] f16           64 KB
-    static constexpr int bars = p + 4 * 128 * 128;                 // q_full, kv_full[2], kv_empty[2], s_full, p_ready, pv_full
-    static constexpr int total = bars + 16 * 8;
+    static constexpr int q = 0;                                    // [128 queries][64] f16, swizzled K-major                16 KB
+    static constexpr int k = q + 128 * 128;                        // kKvStages x [128 keys][64] f16                         64 KB
+    static constexpr int v = k + kKvStages * kKeyBlk * 128;        // kKvStages x 2 atoms x [64 d][64 keys] f16              64 KB
+    static constexpr int bars = v + kKvStages * kKeyBlk * 128;     // q_full, kv_full[kKvStages], kv_empty[kKvStages]
+    static constexpr int total = bars + (1 + 2 * kKvStages) * 8;
 };
 
 // tmQK: the [N][ldq] f16 buffer holding Q (columns h*64) and K (columns k_col0 + h*64), box 64 x 128;  tmVT: V^T [E][N] f16, box 64 keys x 64 rows
@@ -226,179 +235,25 @@ __global__ void __launch_bounds__(kGemmThreads, 1) flash_attn_kernel(const __gri
                                                                       int n_keys, int k_col0, float scale_log2e, __half * __restrict__ out, int ldo) {
     extern __shared__ unsigned char smem_raw[];
     unsigned char * smem = (unsigned char *)(((uintptr_t) smem_raw + 1023) & ~(uintptr_t) 1023);
-    uint64_t * bars = reinterpret_cast<uint64_t *>(smem + FlashSmem::bars);
-    uint32_t * tmem_slot = reinterpret_cast<uint32_t *>(bars + 12);
-    const uint32_t b0 = smem_u32(bars);
-    const uint32_t q_full = b0, kv_full0 = b0 + 8, kv_empty0 = b0 + 24, s_full = b0 + 40, p_ready = b0 + 48, pv_full = b0 + 56;
+    const uint32_t b0 = smem_u32(smem + FlashSmem::bars);
+    const uint32_t q_full = b0, kv_full0 = b0 + 8, kv_empty0 = b0 + 8 + kKvStages * 8;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int h = blockIdx.y, q0 = blockIdx.x * 128;
     const int nblk = n_keys / kKeyBlk;
+    constexpr uint32_t kStage = kKeyBlk * 128;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         prefetch_tmap(&tmQK); prefetch_tmap(&tmVT);
         mbar_init(q_full, 1);
-        for (int s = 0; s < 2; s++) { mbar_init(kv_full0 + s * 8, 1); mbar_init(kv_empty0 + s * 8, 1); }
-        mbar_init(s_full, 1); mbar_init(p_ready, 128); mbar_init(pv_full, 1);
+        for (int s = 0; s < kKvStages; s++) { mbar_init(kv_full0 + s * 8, 1); mbar_init(kv_empty0 + s * 8, 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) tmem_alloc(smem_u32(tmem_slot), 512);       // S: columns [0, 256), P.V of one block: [256, 320)
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
     pdl_launch_dependents();
     pdl_wait();
-    const uint32_t sQ = smem_u32(smem + FlashSmem::q), sK = smem_u32(smem + FlashSmem::k), sV = smem_u32(smem + FlashSmem::v), sP = smem_u32(smem + FlashSmem::p);
+    const uint32_t sQ = smem_u32(smem + FlashSmem::q), sK = smem_u32(smem + FlashSmem::k), sV = smem_u32(smem + FlashSmem::v);
 
-    if (warp == 0) {
-        if (lane == 0) {                                      // ===== TMA producer =====
-            mbar_expect_tx(q_full, 128 * 128);
-            tma_load_2d(sQ, &tmQK, h * kHeadD, q0, q_full);
-            for (int j = 0; j < nblk; j++) {
-                const int s = j & 1;
-                mbar_wait(kv_empty0 + s * 8, ((j >> 1) & 1) ^ 1);
-                mbar_expect_tx(kv_full0 + s * 8, 2 * kKeyBlk * 128);
-                for (int r = 0; r < 2; r++) tma_load_2d(sK + s * kKeyBlk * 128 + r * 128 * 128, &tmQK, k_col0 + h * kHeadD, j * kKeyBlk + r * 128, kv_full0 + s * 8);
-                for (int a = 0; a < 4; a++) tma_load_2d(sV + s * kKeyBlk * 128 + a * 64 * 128, &tmVT, j * kKeyBlk + a * 64, h * kHeadD, kv_full0 + s * 8);
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {                                      // ===== MMA issuer =====
-            constexpr uint32_t idesc_s = f16_idesc(128, kKeyBlk), idesc_o = f16_idesc(128, kHeadD);
-            mbar_wait(q_full, 0);
-            for (int j = 0; j < nblk; j++) {
-                const int s = j & 1;
-                mbar_wait(kv_full0 + s * 8, (j >> 1) & 1);
-                tc_fence_after();
-                const uint64_t dq = kmajor_sw128_desc(sQ), dk = kmajor_sw128_desc(sK + s * kKeyBlk * 128);
-#pragma unroll
-                for (int k = 0; k < kHeadD / 16; k++) umma_f16(tmem, dq + 2 * k, dk + 2 * k, idesc_s, k != 0);      // S = Q K^T  (128 x 256, K = 64)
-                umma_commit(s_full);
-                mbar_wait(p_ready, j & 1);                    // the soft_max threads have read S and written P
-                tc_fence_after();
-#pragma unroll
-                for (int kk = 0; kk < kKeyBlk / 16; kk++) {   // O_blk = P V  (128 x 64, K = 256 keys): atom kk / 4, 32-byte step kk % 4
-                    const uint64_t dp = kmajor_sw128_desc(sP + (kk >> 2) * 128 * 128) + 2 * (kk & 3);
-                    const uint64_t dv = kmajor_sw128_desc(sV + s * kKeyBlk * 128 + (kk >> 2) * 64 * 128) + 2 * (kk & 3);
-                    umma_f16(tmem + 256, dp, dv, idesc_o, kk != 0);
-                }
-                umma_commit(kv_empty0 + s * 8);
-                umma_commit(pv_full);
-            }
-        }
-    } else {                                                  // ===== soft_max + output: one query row per thread =====
-        const int q = warp & 3, row = q * 32 + lane;
-        const uint32_t tlane = (uint32_t)(q * 32) << 16;
-        float o[kHeadD];
-#pragma unroll
-        for (int i = 0; i < kHeadD; i++) o[i] = 0.0f;
-        float m_run = -INFINITY, l_run = 0.0f;
-        for (int j = 0; j < nblk; j++) {
-            mbar_wait(s_full, j & 1);
-            tc_fence_after();
-            float mx = m_run;
-#pragma unroll 1
-            for (int c = 0; c < kKeyBlk / 32; c++) {
-                float v[32]; tmem_ld32(tmem + tlane + c * 32, v);
-#pragma unroll
-                for (int i = 0; i < 32; i++) mx = fmaxf(mx, v[i]);
-            }
-            const float alpha = exp2f((m_run - mx) * scale_log2e);
-            float sum = 0.0f;
-#pragma unroll 1
-            for (int c = 0; c < kKeyBlk / 32; c++) {
-                float v[32]; tmem_ld32(tmem + tlane + c * 32, v);
-                uint32_t pk[16];
-#pragma unroll
-                for (int i = 0; i < 32; i += 2) {
-                    const float p0 = exp2f((v[i] - mx) * scale_log2e), p1 = exp2f((v[i + 1] - mx) * scale_log2e);
-                    const __half2 hp = __floats2half2_rn(p0, p1);
-                    sum += __low2float(hp) + __high2float(hp);         // the sum of what the tensor core will actually multiply
-                    pk[i >> 1] = *reinterpret_cast<const uint32_t *>(&hp);
-                }
-                // keys 32c .. 32c+31 of this row: atom c / 2, 16-byte chunks (c % 2) * 4 + 0..3, XOR-swizzled with row % 8
-                const uint32_t base = sP + (c >> 1) * 128 * 128 + row * 128;
-#pragma unroll
-                for (int w = 0; w < 4; w++) {
-                    const uint32_t chunk = (uint32_t)((c & 1) * 4 + w) ^ (uint32_t)(row & 7);
-                    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(base + chunk * 16), "r"(pk[4 * w]), "r"(pk[4 * w + 1]), "r"(pk[4 * w + 2]), "r"(pk[4 * w + 3]) : "memory");
-                }
-            }
-            l_run = l_run * alpha + sum;
-            m_run = mx;
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // P was written through the generic proxy, the tensor core reads it through the async proxy
-            tc_fence_before();
-            mbar_arrive(p_ready);
-            mbar_wait(pv_full, j & 1);
-            tc_fence_after();
-#pragma unroll
-            for (int c = 0; c < kHeadD / 32; c++) {
-                float v[32]; tmem_ld32(tmem + tlane + 256 + c * 32, v);
-#pragma unroll
-                for (int i = 0; i < 32; i++) o[c * 32 + i] = o[c * 32 + i] * alpha + v[i];
-            }
-        }
-        const float inv = 1.0f / l_run;
-        __half * dst = out + (size_t)(q0 + row) * ldo + h * kHeadD;
-#pragma unroll
-        for (int i = 0; i < kHeadD; i += 8) {
-            __half hh[8];
-#pragma unroll
-            for (int e = 0; e < 8; e++) hh[e] = __float2half_rn(o[i + e] * inv);
-            *reinterpret_cast<uint4 *>(dst + i) = *reinterpret_cast<const uint4 *>(hh);
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem, 512);
-}
-
-// ------------------------------------------------------------------------------------------------
-// attention, pipelined (the default): key blocks of 128 with S, P and the block's P.V double-buffered, so the tensor pipe computes
-// S of block j+1 while the 128 soft_max threads work on block j, and the O update of block j-1 is deferred until P of block j is
-// on its way (its P.V result sits in the other TMEM buffer meanwhile).  flash_attn_kernel above is the serial first version
-// (BARK_B200_FLASH=v1), kept for A-B runs: every soft_max step there waits for the MMA before and after it.
-// ------------------------------------------------------------------------------------------------
-constexpr int kKeyBlk2 = 128, kKvStages = 3;
-struct Flash2Smem {
-    static constexpr int q = 0;                                    // [128 queries][64] f16                            16 KB
-    static constexpr int k = q + 128 * 128;                        // 3 stages x [128 keys][64] f16                    48 KB
-    static constexpr int v = k + kKvStages * kKeyBlk2 * 128;       // 3 stages x 2 atoms x [64 d][64 keys] f16         48 KB
-    static constexpr int p = v + kKvStages * kKeyBlk2 * 128;       // 2 buffers x 2 atoms x [128 queries][64 keys]     64 KB
-    static constexpr int bars = p + 2 * 2 * 128 * 128;             // q_full, kv_full[3], kv_empty[3], s_full[2], p_ready[2], pv_full[2]
-    static constexpr int total = bars + 16 * 8 + 4 * 128 * 4;          // + [2][2][128] floats: row maxima exchanged by the two threads of a row (flash_attn3_kernel)
-};
-
-__global__ void __launch_bounds__(kGemmThreads, 1) flash_attn2_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CUtensorMap tmVT,
-                                                                       int n_keys, int k_col0, float scale_log2e, __half * __restrict__ out, int ldo) {
-    extern __shared__ unsigned char smem_raw[];
-    unsigned char * smem = (unsigned char *)(((uintptr_t) smem_raw + 1023) & ~(uintptr_t) 1023);
-    uint64_t * bars = reinterpret_cast<uint64_t *>(smem + Flash2Smem::bars);
-    uint32_t * tmem_slot = reinterpret_cast<uint32_t *>(bars + 14);
-    const uint32_t b0 = smem_u32(bars);
-    const uint32_t q_full = b0, kv_full0 = b0 + 8, kv_empty0 = b0 + 32, s_full0 = b0 + 56, p_ready0 = b0 + 72, pv_full0 = b0 + 88;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int h = blockIdx.y, q0 = blockIdx.x * 128;
-    const int nblk = n_keys / kKeyBlk2;
-
-    if (warp == 0 && lane == 0) {
-        prefetch_tmap(&tmQK); prefetch_tmap(&tmVT);
-        mbar_init(q_full, 1);
-        for (int s = 0; s < kKvStages; s++) { mbar_init(kv_full0 + s * 8, 1); mbar_init(kv_empty0 + s * 8, 1); }
-        for (int s = 0; s < 2; s++) { mbar_init(s_full0 + s * 8, 1); mbar_init(p_ready0 + s * 8, 128); mbar_init(pv_full0 + s * 8, 1); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) tmem_alloc(smem_u32(tmem_slot), 512);       // S[2]: columns [0,128) [128,256);  P.V[2]: [256,320) [320,384)
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    pdl_launch_dependents();
-    pdl_wait();
-    const uint32_t sQ = smem_u32(smem + Flash2Smem::q), sK = smem_u32(smem + Flash2Smem::k), sV = smem_u32(smem + Flash2Smem::v), sP = smem_u32(smem + Flash2Smem::p);
-    constexpr uint32_t kStage = kKeyBlk2 * 128, kPBuf = 2 * 128 * 128;
-
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {                                      // ===== TMA producer =====
             mbar_expect_tx(q_full, 128 * 128);
             tma_load_2d(sQ, &tmQK, h * kHeadD, q0, q_full);
@@ -406,259 +261,85 @@ __global__ void __launch_bounds__(kGemmThreads, 1) flash_attn2_kernel(const __gr
                 const int s = j % kKvStages;
                 mbar_wait(kv_empty0 + s * 8, ((j / kKvStages) & 1) ^ 1);
                 mbar_expect_tx(kv_full0 + s * 8, 2 * kStage);
-                tma_load_2d(sK + s * kStage, &tmQK, k_col0 + h * kHeadD, j * kKeyBlk2, kv_full0 + s * 8);
-                for (int a = 0; a < 2; a++) tma_load_2d(sV + s * kStage + a * 64 * 128, &tmVT, j * kKeyBlk2 + a * 64, h * kHeadD, kv_full0 + s * 8);
+                tma_load_2d(sK + s * kStage, &tmQK, k_col0 + h * kHeadD, j * kKeyBlk, kv_full0 + s * 8);
+                for (int a = 0; a < 2; a++) tma_load_2d(sV + s * kStage + a * 64 * 128, &tmVT, j * kKeyBlk + a * 64, h * kHeadD, kv_full0 + s * 8);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {                                      // ===== MMA issuer =====
-            constexpr uint32_t idesc_s = f16_idesc(128, kKeyBlk2), idesc_o = f16_idesc(128, kHeadD);
-            auto issue_s = [&](int j) {                       // S_j = Q K_j^T  (128 x 128, K = 64) into S[j & 1]
-                const int s = j % kKvStages;
-                mbar_wait(kv_full0 + s * 8, (j / kKvStages) & 1);
-                tc_fence_after();
-                const uint64_t dq = kmajor_sw128_desc(sQ), dk = kmajor_sw128_desc(sK + s * kStage);
-#pragma unroll
-                for (int k = 0; k < kHeadD / 16; k++) umma_f16(tmem + (uint32_t)(j & 1) * 128, dq + 2 * k, dk + 2 * k, idesc_s, k != 0);
-                umma_commit(s_full0 + (j & 1) * 8);
-            };
-            mbar_wait(q_full, 0);
-            issue_s(0);
-            for (int j = 0; j < nblk; j++) {
-                if (j + 1 < nblk) issue_s(j + 1);             // runs on the tensor pipe while the soft_max threads work on block j
-                mbar_wait(p_ready0 + (j & 1) * 8, (j >> 1) & 1);
-                tc_fence_after();
-                const int s = j % kKvStages;
-#pragma unroll
-                for (int kk = 0; kk < kKeyBlk2 / 16; kk++) {  // P.V of block j (128 x 64, K = 128 keys) into PV[j & 1]
-                    const uint64_t dp = kmajor_sw128_desc(sP + (uint32_t)(j & 1) * kPBuf + (kk >> 2) * 128 * 128) + 2 * (kk & 3);
-                    const uint64_t dv = kmajor_sw128_desc(sV + s * kStage + (kk >> 2) * 64 * 128) + 2 * (kk & 3);
-                    umma_f16(tmem + 256 + (uint32_t)(j & 1) * 64, dp, dv, idesc_o, kk != 0);
-                }
-                umma_commit(kv_empty0 + s * 8);
-                umma_commit(pv_full0 + (j & 1) * 8);
-            }
-        }
-    } else {                                                  // ===== soft_max + output: one query row per thread =====
-        const int q = warp & 3, row = q * 32 + lane;
-        const uint32_t tlane = (uint32_t)(q * 32) << 16;
-        float o[kHeadD];
-#pragma unroll
-        for (int i = 0; i < kHeadD; i++) o[i] = 0.0f;
-        float m_run = -INFINITY, l_run = 0.0f, alpha_prev = 0.0f;
-        auto accumulate = [&](int j, float alpha) {           // O = O * alpha + (P.V of block j)
-            mbar_wait(pv_full0 + (j & 1) * 8, (j >> 1) & 1);
-            tc_fence_after();
-#pragma unroll
-            for (int c = 0; c < kHeadD / 32; c++) {
-                float v[32]; tmem_ld32(tmem + tlane + 256 + (uint32_t)(j & 1) * 64 + c * 32, v);
-#pragma unroll
-                for (int i = 0; i < 32; i++) o[c * 32 + i] = o[c * 32 + i] * alpha + v[i];
-            }
-        };
-        for (int j = 0; j < nblk; j++) {
-            mbar_wait(s_full0 + (j & 1) * 8, (j >> 1) & 1);
-            tc_fence_after();
-            const uint32_t ts = tmem + tlane + (uint32_t)(j & 1) * 128;
-            float mx = m_run;
-#pragma unroll 1
-            for (int c = 0; c < kKeyBlk2 / 32; c++) {
-                float v[32]; tmem_ld32(ts + c * 32, v);
-#pragma unroll
-                for (int i = 0; i < 32; i++) mx = fmaxf(mx, v[i]);
-            }
-            const float alpha = exp2f((m_run - mx) * scale_log2e);
-            float sum = 0.0f;
-#pragma unroll 1
-            for (int c = 0; c < kKeyBlk2 / 32; c++) {
-                float v[32]; tmem_ld32(ts + c * 32, v);
-                uint32_t pk[16];
-#pragma unroll
-                for (int i = 0; i < 32; i += 2) {
-                    const float p0 = exp2f((v[i] - mx) * scale_log2e), p1 = exp2f((v[i + 1] - mx) * scale_log2e);
-                    const __half2 hp = __floats2half2_rn(p0, p1);
-                    sum += __low2float(hp) + __high2float(hp);
-                    pk[i >> 1] = *reinterpret_cast<const uint32_t *>(&hp);
-                }
-                const uint32_t base = sP + (uint32_t)(j & 1) * kPBuf + (c >> 1) * 128 * 128 + row * 128;
-#pragma unroll
-                for (int w = 0; w < 4; w++) {
-                    const uint32_t chunk = (uint32_t)((c & 1) * 4 + w) ^ (uint32_t)(row & 7);
-                    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(base + chunk * 16), "r"(pk[4 * w]), "r"(pk[4 * w + 1]), "r"(pk[4 * w + 2]), "r"(pk[4 * w + 3]) : "memory");
-                }
-            }
-            l_run = l_run * alpha + sum;
-            m_run = mx;
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            tc_fence_before();
-            mbar_arrive(p_ready0 + (j & 1) * 8);
-            if (j > 0) accumulate(j - 1, alpha_prev);         // block j-1's P.V has been in TMEM for a while by now
-            alpha_prev = alpha;
-        }
-        accumulate(nblk - 1, alpha_prev);
-        const float inv = 1.0f / l_run;
-        __half * dst = out + (size_t)(q0 + row) * ldo + h * kHeadD;
-#pragma unroll
-        for (int i = 0; i < kHeadD; i += 8) {
-            __half hh[8];
-#pragma unroll
-            for (int e = 0; e < 8; e++) hh[e] = __float2half_rn(o[i + e] * inv);
-            *reinterpret_cast<uint4 *>(dst + i) = *reinterpret_cast<const uint4 *>(hh);
-        }
+        return;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem, 512);
-}
-
-// Same pipeline with EIGHT soft_max warps (two per scheduler): warps sw and sw + 4 share a TMEM lane quarter (32 query rows) and split the
-// 128 key columns of a block (and the 64 output columns) in halves; only the row maximum crosses between the two threads of a row
-// (shared memory + a 64-thread named barrier).  With four warps the soft_max was issue-bound: one warp per scheduler, ~10 instructions
-// per key per thread.
-__global__ void __launch_bounds__(320, 1) flash_attn3_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CUtensorMap tmVT,
-                                                                       int n_keys, int k_col0, float scale_log2e, __half * __restrict__ out, int ldo) {
-    extern __shared__ unsigned char smem_raw[];
-    unsigned char * smem = (unsigned char *)(((uintptr_t) smem_raw + 1023) & ~(uintptr_t) 1023);
-    uint64_t * bars = reinterpret_cast<uint64_t *>(smem + Flash2Smem::bars);
-    uint32_t * tmem_slot = reinterpret_cast<uint32_t *>(bars + 14);
-    const uint32_t b0 = smem_u32(bars);
-    const uint32_t q_full = b0, kv_full0 = b0 + 8, kv_empty0 = b0 + 32, s_full0 = b0 + 56, p_ready0 = b0 + 72, pv_full0 = b0 + 88;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int h = blockIdx.y, q0 = blockIdx.x * 128;
-    const int nblk = n_keys / kKeyBlk2;
-
-    if (warp == 0 && lane == 0) {
-        prefetch_tmap(&tmQK); prefetch_tmap(&tmVT);
-        mbar_init(q_full, 1);
-        for (int s = 0; s < kKvStages; s++) { mbar_init(kv_full0 + s * 8, 1); mbar_init(kv_empty0 + s * 8, 1); }
-        for (int s = 0; s < 2; s++) { mbar_init(s_full0 + s * 8, 1); mbar_init(p_ready0 + s * 8, 256); mbar_init(pv_full0 + s * 8, 1); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    // ===== warpgroup wg: queries q0 + 64 wg .. + 63; this thread holds rows g and g + 8 of its warp's 16 =====
+    const int wg = warp >> 2, w = warp & 3, g = lane >> 2, c = lane & 3;
+    float o[kHeadD / 2], sc[kKeyBlk / 2];
+#pragma unroll
+    for (int i = 0; i < kHeadD / 2; i++) o[i] = 0.0f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.0f, 0.0f};        // l_run: this thread's share of the row sums
+    const uint64_t dq = kmajor_sw128_desc(sQ + wg * 64 * 128);
+    mbar_wait(q_full, 0);
+    for (int j = 0; j < nblk; j++) {
+        const int s = j % kKvStages;
+        mbar_wait(kv_full0 + s * 8, (j / kKvStages) & 1);
+        // S = Q K^T  (64 x 128, K = 64)
+        const uint64_t dk = kmajor_sw128_desc(sK + s * kStage);
+        fence_regs(sc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kHeadD / 16; k++) wgmma_ss_n128(sc, dq + 2 * k, dk + 2 * k, k != 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(sc);
+        // online soft_max of rows g (r = 0) and g + 8 (r = 1): a row lives in the four threads of a quad
+        float alpha[2];
+#pragma unroll
+        for (int r = 0; r < 2; r++) {
+            float mx = m_run[r];
+#pragma unroll
+            for (int i = 0; i < kKeyBlk / 8; i++) mx = fmaxf(mx, fmaxf(sc[4 * i + 2 * r], sc[4 * i + 2 * r + 1]));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            alpha[r] = exp2f((m_run[r] - mx) * scale_log2e);
+            m_run[r] = mx;
+        }
+        // P (f16) as the A operand of P V: k-step kk covers keys 16 kk .. 16 kk + 15 = accumulator column groups 2 kk, 2 kk + 1
+        uint32_t pa[kKeyBlk / 16][4];
+        float sum[2] = {0.0f, 0.0f};
+#pragma unroll
+        for (int i = 0; i < kKeyBlk / 8; i++) {
+#pragma unroll
+            for (int r = 0; r < 2; r++) {
+                const __half2 hp = __floats2half2_rn(exp2f((sc[4 * i + 2 * r] - m_run[r]) * scale_log2e), exp2f((sc[4 * i + 2 * r + 1] - m_run[r]) * scale_log2e));
+                sum[r] += __low2float(hp) + __high2float(hp);         // the sum of what the tensor core will actually multiply
+                pa[i >> 1][(i & 1) * 2 + r] = *reinterpret_cast<const uint32_t *>(&hp);
+            }
+        }
+#pragma unroll
+        for (int r = 0; r < 2; r++) l_run[r] = l_run[r] * alpha[r] + sum[r];
+#pragma unroll
+        for (int i = 0; i < kHeadD / 8; i++) { o[4 * i] *= alpha[0]; o[4 * i + 1] *= alpha[0]; o[4 * i + 2] *= alpha[1]; o[4 * i + 3] *= alpha[1]; }
+        // O += P V  (64 x 64, K = 128 keys): V^T atom kk / 4, 32-byte step kk % 4
+        fence_regs(o);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < kKeyBlk / 16; kk++) wgmma_rs_n64(o, pa[kk], kmajor_sw128_desc(sV + s * kStage + (kk >> 2) * 64 * 128) + 2 * (kk & 3));
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(o);
+        if (lane == 0) mbar_arrive(kv_empty0 + s * 8);        // this warp's reads of stage s are complete
     }
-    if (warp == 1) tmem_alloc(smem_u32(tmem_slot), 512);       // S[2]: columns [0,128) [128,256);  P.V[2]: [256,320) [320,384)
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    pdl_launch_dependents();
-    pdl_wait();
-    const uint32_t sQ = smem_u32(smem + Flash2Smem::q), sK = smem_u32(smem + Flash2Smem::k), sV = smem_u32(smem + Flash2Smem::v), sP = smem_u32(smem + Flash2Smem::p);
-    constexpr uint32_t kStage = kKeyBlk2 * 128, kPBuf = 2 * 128 * 128;
-
-    if (warp == 0) {
-        if (lane == 0) {                                      // ===== TMA producer =====
-            mbar_expect_tx(q_full, 128 * 128);
-            tma_load_2d(sQ, &tmQK, h * kHeadD, q0, q_full);
-            for (int j = 0; j < nblk; j++) {
-                const int s = j % kKvStages;
-                mbar_wait(kv_empty0 + s * 8, ((j / kKvStages) & 1) ^ 1);
-                mbar_expect_tx(kv_full0 + s * 8, 2 * kStage);
-                tma_load_2d(sK + s * kStage, &tmQK, k_col0 + h * kHeadD, j * kKeyBlk2, kv_full0 + s * 8);
-                for (int a = 0; a < 2; a++) tma_load_2d(sV + s * kStage + a * 64 * 128, &tmVT, j * kKeyBlk2 + a * 64, h * kHeadD, kv_full0 + s * 8);
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {                                      // ===== MMA issuer =====
-            constexpr uint32_t idesc_s = f16_idesc(128, kKeyBlk2), idesc_o = f16_idesc(128, kHeadD);
-            auto issue_s = [&](int j) {                       // S_j = Q K_j^T  (128 x 128, K = 64) into S[j & 1]
-                const int s = j % kKvStages;
-                mbar_wait(kv_full0 + s * 8, (j / kKvStages) & 1);
-                tc_fence_after();
-                const uint64_t dq = kmajor_sw128_desc(sQ), dk = kmajor_sw128_desc(sK + s * kStage);
+    float inv[2];
 #pragma unroll
-                for (int k = 0; k < kHeadD / 16; k++) umma_f16(tmem + (uint32_t)(j & 1) * 128, dq + 2 * k, dk + 2 * k, idesc_s, k != 0);
-                umma_commit(s_full0 + (j & 1) * 8);
-            };
-            mbar_wait(q_full, 0);
-            issue_s(0);
-            for (int j = 0; j < nblk; j++) {
-                if (j + 1 < nblk) issue_s(j + 1);             // runs on the tensor pipe while the soft_max threads work on block j
-                mbar_wait(p_ready0 + (j & 1) * 8, (j >> 1) & 1);
-                tc_fence_after();
-                const int s = j % kKvStages;
-#pragma unroll
-                for (int kk = 0; kk < kKeyBlk2 / 16; kk++) {  // P.V of block j (128 x 64, K = 128 keys) into PV[j & 1]
-                    const uint64_t dp = kmajor_sw128_desc(sP + (uint32_t)(j & 1) * kPBuf + (kk >> 2) * 128 * 128) + 2 * (kk & 3);
-                    const uint64_t dv = kmajor_sw128_desc(sV + s * kStage + (kk >> 2) * 64 * 128) + 2 * (kk & 3);
-                    umma_f16(tmem + 256 + (uint32_t)(j & 1) * 64, dp, dv, idesc_o, kk != 0);
-                }
-                umma_commit(kv_empty0 + s * 8);
-                umma_commit(pv_full0 + (j & 1) * 8);
-            }
-        }
-    } else {                                                  // ===== soft_max + output: two threads per query row (column halves) =====
-        const int sw = warp - 2, q = warp & 3, half = sw >> 2, row = q * 32 + lane;
-        const uint32_t tlane = (uint32_t)(q * 32) << 16;
-        float * xmax = reinterpret_cast<float *>(smem + Flash2Smem::bars + 15 * 8 + 8);      // [2][128] row maxima of the two halves (behind the barriers)
-        auto pair_sync = [&]() { asm volatile("bar.sync %0, 64;" ::"r"(1 + q) : "memory"); };   // the two warps of this lane quarter
-        float o[32];
-#pragma unroll
-        for (int i = 0; i < 32; i++) o[i] = 0.0f;
-        float m_run = -INFINITY, l_run = 0.0f, alpha_prev = 0.0f;
-        auto accumulate = [&](int j, float alpha) {           // O[:, half] = O * alpha + (P.V of block j)[:, half]
-            mbar_wait(pv_full0 + (j & 1) * 8, (j >> 1) & 1);
-            tc_fence_after();
-            float v[32]; tmem_ld32(tmem + tlane + 256 + (uint32_t)(j & 1) * 64 + half * 32, v);
-#pragma unroll
-            for (int i = 0; i < 32; i++) o[i] = o[i] * alpha + v[i];
-        };
-        for (int j = 0; j < nblk; j++) {
-            mbar_wait(s_full0 + (j & 1) * 8, (j >> 1) & 1);
-            tc_fence_after();
-            const uint32_t ts = tmem + tlane + (uint32_t)(j & 1) * 128 + half * 64;
-            float mx = m_run;
-#pragma unroll 1
-            for (int c = 0; c < 2; c++) {
-                float v[32]; tmem_ld32(ts + c * 32, v);
-#pragma unroll
-                for (int i = 0; i < 32; i++) mx = fmaxf(mx, v[i]);
-            }
-            xmax[((j & 1) * 2 + half) * 128 + row] = mx;
-            pair_sync();
-            mx = fmaxf(mx, xmax[((j & 1) * 2 + (half ^ 1)) * 128 + row]);
-            const float alpha = exp2f((m_run - mx) * scale_log2e);
-            float sum = 0.0f;
-#pragma unroll 1
-            for (int c = 0; c < 2; c++) {
-                float v[32]; tmem_ld32(ts + c * 32, v);
-                uint32_t pk[16];
-#pragma unroll
-                for (int i = 0; i < 32; i += 2) {
-                    const float p0 = exp2f((v[i] - mx) * scale_log2e), p1 = exp2f((v[i + 1] - mx) * scale_log2e);
-                    const __half2 hp = __floats2half2_rn(p0, p1);
-                    sum += __low2float(hp) + __high2float(hp);
-                    pk[i >> 1] = *reinterpret_cast<const uint32_t *>(&hp);
-                }
-                const uint32_t base = sP + (uint32_t)(j & 1) * kPBuf + half * 128 * 128 + row * 128;      // this half's 64 keys = atom `half`
-#pragma unroll
-                for (int w = 0; w < 4; w++) {
-                    const uint32_t chunk = (uint32_t)(c * 4 + w) ^ (uint32_t)(row & 7);
-                    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(base + chunk * 16), "r"(pk[4 * w]), "r"(pk[4 * w + 1]), "r"(pk[4 * w + 2]), "r"(pk[4 * w + 3]) : "memory");
-                }
-            }
-            l_run = l_run * alpha + sum;
-            m_run = mx;
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            tc_fence_before();
-            mbar_arrive(p_ready0 + (j & 1) * 8);
-            if (j > 0) accumulate(j - 1, alpha_prev);
-            alpha_prev = alpha;
-        }
-        accumulate(nblk - 1, alpha_prev);
-        xmax[half * 128 + row] = l_run;                       // the row sum is the sum of the two halves' sums (same maxima, same rescaling)
-        pair_sync();
-        const float inv = 1.0f / (l_run + xmax[(half ^ 1) * 128 + row]);
-        __half * dst = out + (size_t)(q0 + row) * ldo + h * kHeadD + half * 32;
-#pragma unroll
-        for (int i = 0; i < 32; i += 8) {
-            __half hh[8];
-#pragma unroll
-            for (int e = 0; e < 8; e++) hh[e] = __float2half_rn(o[i + e] * inv);
-            *reinterpret_cast<uint4 *>(dst + i) = *reinterpret_cast<const uint4 *>(hh);
-        }
+    for (int r = 0; r < 2; r++) {
+        float l = l_run[r];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        inv[r] = 1.0f / l;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem, 512);
+    const int row = q0 + wg * 64 + w * 16 + g;
+#pragma unroll
+    for (int i = 0; i < kHeadD / 8; i++) {
+        const int col = h * kHeadD + 8 * i + 2 * c;
+        *reinterpret_cast<uint32_t *>(out + (size_t) row * ldo + col) = pack_half2(o[4 * i] * inv[0], o[4 * i + 1] * inv[0]);
+        *reinterpret_cast<uint32_t *>(out + (size_t)(row + 8) * ldo + col) = pack_half2(o[4 * i + 2] * inv[1], o[4 * i + 3] * inv[1]);
+    }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -717,61 +398,50 @@ static bool make_map(CUtensorMap * m, const void * base, int rows, int cols, int
 template <int BN>
 static bool launch_gemm(const __half * A, int lda, const __half * W, int ldw, int M, int N, int K, const FastEpi & ep, cudaStream_t s) {
     constexpr int kStages = BN >= 256 ? 4 : BN >= 128 ? 6 : 8;
-    const size_t smem = (size_t) kStages * (kBM * kBK * 2 + BN * kBK * 2) + (2 * kStages + 1) * 8 + 16 + 1024;
+    const size_t smem = (size_t) kStages * (kBM * kBK * 2 + BN * kBK * 2) + 2 * kStages * 8 + 1024;
     static std::atomic<unsigned long long> configured{0};     // kernel attributes are per device (one host thread per GPU may share this process)
-    if (first_use_on_this_device(configured)) BARK_CUDA_CHECK(cudaFuncSetAttribute(umma_gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
+    if (first_use_on_this_device(configured)) BARK_CUDA_CHECK(cudaFuncSetAttribute(wgmma_gemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
     CUtensorMap ta, tb;
     if (!make_map(&ta, A, M, K, lda, kBM) || !make_map(&tb, W, N, K, ldw, BN)) return false;
     const dim3 grid((N + BN - 1) / BN, (M + kBM - 1) / kBM);
     g_next_flops = 2.0 * M * N * (double) K;
     g_next_bytes = 2.0 * ((double) M * K + (double) N * K) + (double) M * N * (ep.mode == FEPI_F32 ? 4 : ep.mode == FEPI_RESID ? 8 : 2);
-    BARK_LAUNCH_PDL((umma_gemm_kernel<BN>), grid, dim3(kGemmThreads), smem, s, ta, tb, M, N, K, ep);
+    BARK_LAUNCH_PDL((wgmma_gemm_kernel<BN>), grid, dim3(kGemmThreads), smem, s, ta, tb, M, N, K, ep);
     return true;
 }
 
 // C = A W^T on the tensor cores.  A [M][lda] f16, W [N][ldw] f16 (both K-contiguous), K % 64 == 0.
 bool fast_gemm(const __half * A, int lda, const __half * W, int ldw, int M, int N, int K, const FastEpi & ep, int n_sm, cudaStream_t s) {
     if (K % kBK != 0 || K < kBK || M < 1 || N < 1) { fprintf(stderr, "bark_b200 fast mode: unsupported GEMM shape %d x %d x %d\n", M, N, K); return false; }
-    // Tile width.  These GEMMs are a few microseconds each, so the choice is about filling 148 SMs, one CTA per SM at a time:
+    // Tile width.  These GEMMs are a few microseconds each, so the choice is about filling the SMs, one CTA per SM at a time:
     //   time(BN) ~ waves x (fixed per-CTA cost + operand bytes of one CTA / per-SM fill rate)
-    // with the measured ~3 us of prologue + epilogue drain per CTA and ~120 GB/s (64 B/clk) from L2 into one SM's shared memory
-    // (profiles/r02_fast_mode.md).  Narrow tiles re-read the 128 activation rows for every column tile, wide tiles leave SMs idle.
+    // with an assumed ~3 us of prologue + epilogue drain per CTA and ~64 B/clk (~120 GB/s) from L2 into one SM's shared memory.
+    // Narrow tiles re-read the 128 activation rows for every column tile, wide tiles leave SMs idle.
     const int tiles_m = (M + kBM - 1) / kBM;
     auto cost = [&](int bn) {
         const int tiles = tiles_m * ((N + bn - 1) / bn);
         return (double)((tiles + n_sm - 1) / n_sm) * (3.0 + (double)(kBM + bn) * K * 2.0 / 120e3);
     };
     int best = 256;
-    for (int bn : {128, 64, 32}) {
-        if (bn == 32 && (N % 32 != 0 || ep.mode == FEPI_QKV16)) continue;
+    for (int bn : {128, 64})
         if (cost(bn) < cost(best) - 1e-9) best = bn;
-    }
     if (best == 256) return launch_gemm<256>(A, lda, W, ldw, M, N, K, ep, s);
     if (best == 128) return launch_gemm<128>(A, lda, W, ldw, M, N, K, ep, s);
-    if (best == 64) return launch_gemm<64>(A, lda, W, ldw, M, N, K, ep, s);
-    return launch_gemm<32>(A, lda, W, ldw, M, N, K, ep, s);
+    return launch_gemm<64>(A, lda, W, ldw, M, N, K, ep, s);
 }
 
 // att[N][E] (f16) = soft_max(Q K^T / sqrt(64)) V per head; qk: [N][ldq] f16 with Q at column h*64 and K at k_col0 + h*64; vt: V^T [E][N] f16
 bool fast_attention(const __half * qk, int ldq, int k_col0, const __half * vt, int n, int E, int H, __half * out, cudaStream_t s) {
-    if (E / H != kHeadD || n % kKeyBlk != 0 || n < kKeyBlk) { fprintf(stderr, "bark_b200 fast mode: attention needs head size 64 and a multiple of 256 positions (got %d heads of %d, %d positions)\n", H, E / H, n); return false; }
-    static const bool v1 = [] { const char * e = getenv("BARK_B200_FLASH"); return e && !strcmp(e, "v1"); }();       // the serial first version, for A-B runs
-    static const bool v2 = [] { const char * e = getenv("BARK_B200_FLASH"); return e && !strcmp(e, "v2"); }();       // pipelined, four soft_max warps
-    const size_t smem = (v1 ? (size_t) FlashSmem::total : (size_t) Flash2Smem::total) + 1024;
+    if (E / H != kHeadD || n % kKeyBlk != 0 || n < kKeyBlk) { fprintf(stderr, "bark_b200 fast mode: attention needs head size 64 and a multiple of %d positions (got %d heads of %d, %d positions)\n", kKeyBlk, H, E / H, n); return false; }
+    const size_t smem = (size_t) FlashSmem::total + 1024;
     static std::atomic<unsigned long long> configured{0};
-    if (first_use_on_this_device(configured)) {
-        BARK_CUDA_CHECK(cudaFuncSetAttribute(flash_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) FlashSmem::total + 1024));
-        BARK_CUDA_CHECK(cudaFuncSetAttribute(flash_attn2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) Flash2Smem::total + 1024));
-        BARK_CUDA_CHECK(cudaFuncSetAttribute(flash_attn3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) Flash2Smem::total + 1024));
-    }
+    if (first_use_on_this_device(configured)) BARK_CUDA_CHECK(cudaFuncSetAttribute(flash_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
     CUtensorMap tqk, tvt;
     if (!make_map(&tqk, qk, n, k_col0 + E, ldq, 128) || !make_map(&tvt, vt, E, n, n, 64)) return false;
     const float scale_log2e = (1.0f / sqrtf((float) kHeadD)) * 1.4426950408889634f;
     g_next_flops = 4.0 * (double) n * n * E;
     g_next_bytes = 2.0 * 4.0 * (double) n * E;
-    if (v1) BARK_LAUNCH_PDL(flash_attn_kernel, dim3(n / 128, H), dim3(kGemmThreads), smem, s, tqk, tvt, n, k_col0, scale_log2e, out, E);
-    else if (v2) BARK_LAUNCH_PDL(flash_attn2_kernel, dim3(n / 128, H), dim3(kGemmThreads), smem, s, tqk, tvt, n, k_col0, scale_log2e, out, E);
-    else    BARK_LAUNCH_PDL(flash_attn3_kernel, dim3(n / 128, H), dim3(320), smem, s, tqk, tvt, n, k_col0, scale_log2e, out, E);
+    BARK_LAUNCH_PDL(flash_attn_kernel, dim3(n / 128, H), dim3(kGemmThreads), smem, s, tqk, tvt, n, k_col0, scale_log2e, out, E);
     return true;
 }
 

@@ -10,12 +10,6 @@
 //
 // Both operands are in the group-major layout (common.cuh), so a pipeline stage of the block tile is a handful of
 // contiguous spans: 2-4 TMA bulk copies into a 4-stage shared-memory ring (mbarrier complete_tx).
-//
-// F2 variants (the default since they were validated bit-exact on a B200, round 2; BARK_B200_FFMA2=0 selects the scalar-FMA
-// kernels for A-B runs): the 64 independent FMAs of a chain step
-// are issued as 32 packed FFMA2 (sm_100 `fma.rn.f32x2`, __ffma2_rn: "numeric behavior per component is the same as
-// __fmaf_rn"), with the scalar operand broadcast by the instruction itself.  Same arithmetic, same order, half the issue
-// slots — the tiled kernels are issue-bound (43 % of issue slots busy, 59-76 % of the instructions are FMAs).
 #include "epilogue.cuh"
 #include "gpt_kernels.h"
 
@@ -89,14 +83,13 @@ template <> struct QuadOp<float> {
 // same time share activation rows in L2); 8 warps as 4 (m) x 2 (o), 8 x 8 outputs per warp.
 //
 // Both operands are group-major: for one 128-column group the 32 activation rows of a tile are one contiguous span, the
-// 16 weight rows another, so a pipeline stage is 2 (f32) or 4 (f16) bulk copies issued by ONE thread.  (A first version
-// with row-major operands needed 48 row copies per stage; the copy instruction takes uniform operands, the compiler
-// serialised the 48 lanes, and the issuing warp - also a consumer - fell ~1.5k cycles behind per stage: ncu showed 30% of
-// all stall samples on the `full`-barrier wait of the other seven warps.)
+// 16 weight rows another, so a pipeline stage is 2 (f32) or 4 (f16) bulk copies issued by ONE thread.  (Row-major
+// operands would need 48 row copies per stage; the copy instruction takes uniform operands, so the compiler serialises the
+// 48 lanes and the issuing warp - also a consumer - falls behind, with the other seven warps waiting on the `full` barrier.)
 //
 // The k-steps of ALL of a CTA's tiles form one stream through the 4-stage ring.  Nobody waits to refill a slot: every warp
 // bumps the slot's counter when it is done reading, and the warp that arrives last issues the copies for stage s + 4.
-template <typename T, bool F2 = false>
+template <typename T>
 __global__ void __launch_bounds__(256, 2) lane_gemm_tiled_kernel(const T * __restrict__ Wg, int K, int w_gs, int O, const T * __restrict__ act, int act_gs, int M, MatmulEpilogue ep) {
     typedef typename QuadOp<T>::V QV;
     constexpr int GPS = QuadOp<T>::kGroupsPerStage;
@@ -164,20 +157,10 @@ __global__ void __launch_bounds__(256, 2) lane_gemm_tiled_kernel(const T * __res
                             for (int mi = 0; mi < 8; mi++) af[mi] = QuadOp<T>::elem(pa[mi], c);
 #pragma unroll
                             for (int oi = 0; oi < 8; oi++) wf[oi] = QuadOp<T>::elem(pw[oi], c);
-                            if constexpr (F2) {
-#pragma unroll
-                                for (int mi = 0; mi < 8; mi++)
-#pragma unroll
-                                    for (int op = 0; op < 8; op += 2) {
-                                        const float2 r = __ffma2_rn(make_float2(wf[op], wf[op + 1]), make_float2(af[mi], af[mi]), make_float2(acc[mi * 8 + op], acc[mi * 8 + op + 1]));
-                                        acc[mi * 8 + op] = r.x; acc[mi * 8 + op + 1] = r.y;
-                                    }
-                            } else {
 #pragma unroll
                             for (int mi = 0; mi < 8; mi++)
 #pragma unroll
                                 for (int oi = 0; oi < 8; oi++) acc[mi * 8 + oi] = __fmaf_rn(wf[oi], af[mi], acc[mi * 8 + oi]);
-                            }
                         }
                     }
                 }
@@ -202,9 +185,6 @@ __global__ void __launch_bounds__(256, 2) lane_gemm_tiled_kernel(const T * __res
     }
 }
 
-// packed-FMA variants of the three tiled kernels (see the header comment) unless BARK_B200_FFMA2=0
-static bool use_ffma2() { const char * e = getenv("BARK_B200_FFMA2"); return !(e && e[0] == '0' && e[1] == 0); }   // read per launch so one process can A-B the two
-
 void lane_gemm_tiled(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, cudaStream_t s, bool f32_containers) {
     const size_t smem = (size_t) kStages * kStageBytes + kStages * 8 + kStages * 4 + 64;
     int dev = 0, n_sm = 0;
@@ -214,26 +194,18 @@ void lane_gemm_tiled(const DMat & W, const void * act, int act_gs, int rows, con
     if (first_use_on_this_device(configured)) {
         BARK_CUDA_CHECK(cudaFuncSetAttribute(lane_gemm_tiled_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
         BARK_CUDA_CHECK(cudaFuncSetAttribute(lane_gemm_tiled_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
-        BARK_CUDA_CHECK(cudaFuncSetAttribute((lane_gemm_tiled_kernel<__half, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
-        BARK_CUDA_CHECK(cudaFuncSetAttribute((lane_gemm_tiled_kernel<float, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
     }
     if (f32_containers && W.type == W_F16) {                 // f16 values in f32 containers on both sides: the float kernel, bit-identical results
         if (!W.p_gm32) { fprintf(stderr, "bark_b200: matrix has no f32-expanded copy\n"); throw std::runtime_error("unsupported configuration (see the message above)"); }
         const int n_tiles32 = ((W.n_out + kBO - 1) / kBO) * ((rows + kBM - 1) / kBM);
         const int grid32 = min(n_tiles32, 2 * n_sm);
-        if (use_ffma2()) BARK_LAUNCH((lane_gemm_tiled_kernel<float, true>), grid32, 256, smem, s, (const float *) W.p_gm32, W.K, W.o_pad * kGmGroup, W.n_out, (const float *) act, act_gs, rows, ep);
-        else             BARK_LAUNCH((lane_gemm_tiled_kernel<float>), grid32, 256, smem, s, (const float *) W.p_gm32, W.K, W.o_pad * kGmGroup, W.n_out, (const float *) act, act_gs, rows, ep);
+        BARK_LAUNCH((lane_gemm_tiled_kernel<float>), grid32, 256, smem, s, (const float *) W.p_gm32, W.K, W.o_pad * kGmGroup, W.n_out, (const float *) act, act_gs, rows, ep);
         return;
     }
     if (!W.p_gm) { fprintf(stderr, "bark_b200: matrix has no group-major copy for the tiled mat-mul\n"); throw std::runtime_error("unsupported configuration (see the message above)"); }
     const int n_tiles = ((W.n_out + kBO - 1) / kBO) * ((rows + kBM - 1) / kBM);
     const int grid = min(n_tiles, 2 * n_sm);                   // persistent: two CTAs per SM (registers and shared memory allow exactly that)
     const int w_gs = W.o_pad * kGmGroup;
-    if (use_ffma2()) {
-        if (W.type == W_F16) BARK_LAUNCH((lane_gemm_tiled_kernel<__half, true>), grid, 256, smem, s, (const __half *) W.p_gm, W.K, w_gs, W.n_out, (const __half *) act, act_gs, rows, ep);
-        else                 BARK_LAUNCH((lane_gemm_tiled_kernel<float, true>), grid, 256, smem, s, (const float *) W.p_gm, W.K, w_gs, W.n_out, (const float *) act, act_gs, rows, ep);
-        return;
-    }
     if (W.type == W_F16) BARK_LAUNCH((lane_gemm_tiled_kernel<__half>), grid, 256, smem, s, (const __half *) W.p_gm, W.K, w_gs, W.n_out, (const __half *) act, act_gs, rows, ep);
     else                 BARK_LAUNCH((lane_gemm_tiled_kernel<float>), grid, 256, smem, s, (const float *) W.p_gm, W.K, w_gs, W.n_out, (const float *) act, act_gs, rows, ep);
 }
@@ -242,7 +214,7 @@ void lane_gemm_tiled(const DMat & W, const void * act, int act_gs, int rows, con
 // attention, multi-row (bark.cpp:1302-1339 / 1495-1530): 8 x 8 tiles per warp, same lane mapping
 // ------------------------------------------------------------------------------------------------
 // scores[h][q][k] = vec_dot_f32(D, K[k][h], Q[q][h]) * scale, -inf where k > n_past + q (causal)
-template <int DSTEPS, bool F2 = false>
+template <int DSTEPS>
 __global__ void __launch_bounds__(256) attn_scores_tiled_kernel(const float * __restrict__ Q, const float * __restrict__ Kc, int N, int n_kv, int n_past, int E,
                                                                 float scale, int causal, float * __restrict__ S) {
     constexpr int D = DSTEPS * 32;
@@ -260,17 +232,6 @@ __global__ void __launch_bounds__(256) attn_scores_tiled_kernel(const float * __
         }
     }
     float acc[64];
-    if constexpr (F2) {
-#pragma unroll
-        for (int qi = 0; qi < 8; qi++)
-#pragma unroll
-            for (int kp = 0; kp < 8; kp += 2) {
-                float2 a = make_float2(0.0f, 0.0f);
-#pragma unroll
-                for (int c = 0; c < DSTEPS; c++) a = __ffma2_rn(make_float2(kf[kp][c], kf[kp + 1][c]), make_float2(qf[qi][c], qf[qi][c]), a);
-                acc[qi * 8 + kp] = a.x; acc[qi * 8 + kp + 1] = a.y;
-            }
-    } else {
 #pragma unroll
     for (int qi = 0; qi < 8; qi++)
 #pragma unroll
@@ -280,7 +241,6 @@ __global__ void __launch_bounds__(256) attn_scores_tiled_kernel(const float * __
             for (int c = 0; c < DSTEPS; c++) a = __fmaf_rn(kf[ki][c], qf[qi][c], a);
             acc[qi * 8 + ki] = a;
         }
-    }
     const int base = butterfly_reduce64(acc, lane);
     const int q = q0 + (base >> 3), k = k0 + (base & 7);
     if (q < N) {
@@ -296,7 +256,6 @@ __global__ void __launch_bounds__(256) attn_scores_tiled_kernel(const float * __
 
 // KQV[q][h*D+d] = vec_dot_f32(n_kv, V^T[d], P[q]) -> activation operand for c_proj.  Warp = 8 queries x 8 head columns;
 // lane v walks k = v, v+32, ...
-template <bool F2 = false>
 __global__ void __launch_bounds__(256) attn_pv_tiled_kernel(const float * __restrict__ S, const float * __restrict__ Vc, int N, int n_kv, int E, int D,
                                                             void * __restrict__ act, int wt, int Kp) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -317,16 +276,8 @@ __global__ void __launch_bounds__(256) attn_pv_tiled_kernel(const float * __rest
 #pragma unroll
         for (int qi = 0; qi < 8; qi++) {
             const float p = __ldg(prow[qi] + k);
-            if constexpr (F2) {
-#pragma unroll
-                for (int dp = 0; dp < 8; dp += 2) {
-                    const float2 r = __ffma2_rn(make_float2(vf[dp], vf[dp + 1]), make_float2(p, p), make_float2(acc[qi * 8 + dp], acc[qi * 8 + dp + 1]));
-                    acc[qi * 8 + dp] = r.x; acc[qi * 8 + dp + 1] = r.y;
-                }
-            } else {
 #pragma unroll
             for (int di = 0; di < 8; di++) acc[qi * 8 + di] = __fmaf_rn(vf[di], p, acc[qi * 8 + di]);
-            }
         }
     }
     const int base = butterfly_reduce64(acc, lane);
@@ -348,13 +299,6 @@ __global__ void __launch_bounds__(256) attn_pv_tiled_kernel(const float * __rest
 void attention_tiled_scores(const float * Q, const float * Kc, int N, int n_kv, int n_past, int E, int H, float scale, bool causal, float * scores, cudaStream_t s) {
     const int D = E / H;
     const dim3 grid((n_kv + 63) / 64, (N + 7) / 8, H);
-    if (use_ffma2()) {
-        if (D == 64)       BARK_LAUNCH((attn_scores_tiled_kernel<2, true>), grid, 256, 0, s, Q, Kc, N, n_kv, n_past, E, scale, causal ? 1 : 0, scores);
-        else if (D == 32)  BARK_LAUNCH((attn_scores_tiled_kernel<1, true>), grid, 256, 0, s, Q, Kc, N, n_kv, n_past, E, scale, causal ? 1 : 0, scores);
-        else if (D == 96)  BARK_LAUNCH((attn_scores_tiled_kernel<3, true>), grid, 256, 0, s, Q, Kc, N, n_kv, n_past, E, scale, causal ? 1 : 0, scores);
-        else               BARK_LAUNCH((attn_scores_tiled_kernel<4, true>), grid, 256, 0, s, Q, Kc, N, n_kv, n_past, E, scale, causal ? 1 : 0, scores);
-        return;
-    }
     if (D == 64)       BARK_LAUNCH(attn_scores_tiled_kernel<2>, grid, 256, 0, s, Q, Kc, N, n_kv, n_past, E, scale, causal ? 1 : 0, scores);
     else if (D == 32)  BARK_LAUNCH(attn_scores_tiled_kernel<1>, grid, 256, 0, s, Q, Kc, N, n_kv, n_past, E, scale, causal ? 1 : 0, scores);
     else if (D == 96)  BARK_LAUNCH(attn_scores_tiled_kernel<3>, grid, 256, 0, s, Q, Kc, N, n_kv, n_past, E, scale, causal ? 1 : 0, scores);
@@ -363,8 +307,7 @@ void attention_tiled_scores(const float * Q, const float * Kc, int N, int n_kv, 
 
 void attention_tiled_pv(const float * scores, const float * Vc, int N, int n_kv, int E, int H, void * act, WType wt, int Kp, cudaStream_t s) {
     const int D = E / H;
-    if (use_ffma2()) { BARK_LAUNCH((attn_pv_tiled_kernel<true>), dim3((N + 7) / 8, H), 32 * ((D + 7) / 8), 0, s, scores, Vc, N, n_kv, E, D, act, (int) wt, Kp); return; }
-    BARK_LAUNCH((attn_pv_tiled_kernel<false>), dim3((N + 7) / 8, H), 32 * ((D + 7) / 8), 0, s, scores, Vc, N, n_kv, E, D, act, (int) wt, Kp);
+    BARK_LAUNCH(attn_pv_tiled_kernel, dim3((N + 7) / 8, H), 32 * ((D + 7) / 8), 0, s, scores, Vc, N, n_kv, E, D, act, (int) wt, Kp);
 }
 
 }  // namespace bark

@@ -86,7 +86,7 @@ void build_decode_tables(bark_context * ctx, GPTModel & m) {
     m.gx = tagged(R * E); m.gq = tagged(R * E); m.gk = tagged((size_t) E); m.gv = tagged((size_t) E); m.gatt = tagged(R * E);
     m.gff = tagged(R * 4 * E); m.gscores = tagged((size_t) m.n_head * m.block_size);
     m.glogits = (float *) ctx_alloc(ctx, (size_t) m.n_out_vocab * 4);
-    {   // adaptive head starts, [n_cta][8] (XT_* order: q, att, x1, ff, x2, scores): start from the measured fixed knobs
+    {   // adaptive head starts, [n_cta][8] (XT_* order: q, att, x1, ff, x2, scores): start from the fixed knobs
         std::vector<unsigned> init((size_t) ctx->n_sm_total * 8, 0u);
         for (int c = 0; c < ctx->n_sm_total; c++) { init[(size_t) c * 8 + 1] = ctx->att_ns; init[(size_t) c * 8 + 2] = ctx->first_ns; init[(size_t) c * 8 + 4] = ctx->first_ns; }
         m.d_adapt = (unsigned *) ctx_alloc(ctx, init.size() * 4);
@@ -238,7 +238,7 @@ bool fine_eval(bark_context * ctx, const int32_t * in_buffer, int nn, float * lo
     return true;
 }
 
-// FAST MODE: the same pass on the tensor cores (fast_kernels.cu): LayerNorm -> f16, tcgen05 GEMMs with fused epilogues, flash-style
+// FAST MODE: the same pass on the tensor cores (fast_kernels.cu): LayerNorm -> f16, wgmma GEMMs with fused epilogues, flash-style
 // attention.  Same inputs / outputs as fine_eval; logits agree with the reference to f16-operand accuracy, not bit for bit.
 bool fine_eval_fast(bark_context * ctx, const int32_t * in_buffer, int nn, float * logits_host) {
     GPTModel & m = ctx->fine;

@@ -52,7 +52,7 @@ void expand_f16_to_f32(const void * src_f16, void * dst_f32, size_t n, cudaStrea
 void attention_tiled_scores(const float * Q, const float * Kc, int N, int n_kv, int n_past, int E, int H, float scale, bool causal, float * scores, cudaStream_t s);
 void attention_tiled_pv(const float * scores, const float * Vc, int N, int n_kv, int E, int H, void * act, WType wt, int Kp, cudaStream_t s);
 
-// ---- fast mode (fast_kernels.cu, BARK_B200_MODE=fast): tcgen05 GEMM + flash-style attention for the dense passes -------------------
+// ---- fast mode (fast_kernels.cu, BARK_B200_MODE=fast): wgmma GEMM + flash-style attention for the dense passes -------------------
 enum { FEPI_F32 = 0, FEPI_RESID = 1, FEPI_GELU16 = 2, FEPI_F16 = 3, FEPI_QKV16 = 4 };
 struct FastEpi {
     int mode = FEPI_F32;

@@ -17,7 +17,7 @@ struct DMat {                 // 2-D weight [n_out][K] in LI layout (f32 / f16) 
     void * mins = nullptr, * qh = nullptr;   // experimental types: f16 block minima (q4_1, q5_1), fifth bits (q5_0, q5_1)
     void * p_gm = nullptr; int o_pad = 0;   // second copy in the group-major layout (common.cuh) for the tiled GEMM; rows padded to o_pad
     void * p_gm32 = nullptr;                // f16 matrices, BARK_B200_GEMM_F32C=1: the group-major copy expanded to f32 (gemm_kernels.cu)
-    void * p_rm = nullptr;                  // fast mode only: the file's row-major [n_out][K] f16 matrix = K-major tcgen05 operand (fast_kernels.cu)
+    void * p_rm = nullptr;                  // fast mode only: the file's row-major [n_out][K] f16 matrix = K-major wgmma operand (fast_kernels.cu)
     WType type = W_F16;
 };
 

@@ -1,4 +1,4 @@
-// q4_1, q5_0, q5_1 and q8_0 GPT weights (validated bit-exact against the oracle on a B200 in round 2) — the other
+// q4_1, q5_0, q5_1 and q8_0 GPT weights (bit-exact against the oracle: tests/test_parity_gpu.py) — the other
 // types the reference's `quantize` tool writes.  Same scheme as q4_kernels.cu (eight lanes own the eight float accumulators of one
 // output, one dp4a + one fma per 32-element block, hsum_float_8 as three xor-shuffles), with the per-type details of the pinned AVX2
 // build (ggml-quants.c): q5 codes take their fifth bit from qh, q4_1 / q5_1 add `m_w * s_a` per block in ONE scalar fused chain

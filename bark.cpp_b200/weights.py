@@ -11,7 +11,7 @@ LayerNorm biases N(0, 0.02^2), lm_head N(0, 0.2^2), codec conv / LSTM weights N(
 stored F16, codec biases N(0, 0.02^2), codebooks N(0, 1).
 
 The numpy PCG64 stream is platform independent, so the same (config, seed) gives the same bytes in
-the build container and on the GPU box.
+every machine.
 """
 from __future__ import annotations
 

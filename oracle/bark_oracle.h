@@ -9,9 +9,9 @@
  * with ggml's CPU kernels restated in the AVX2/FMA lane order of the pinned reference build
  * (oracle/Makefile: -mavx2 -mfma -mf16c; SURVEY.md App. C).
  *
- * Pinning: every function here is checked bit-for-bit against oracle/_ref/libbark_ref.so (the
- * unmodified reference compiled from /root/reference) by tests/test_oracle_vs_ref.py in the build
- * container, and against the committed fixtures in tests/golden/ everywhere else.
+ * Pinning: every function here is checked bit-for-bit against the outputs of the unmodified reference
+ * (oracle/_ref/libbark_ref.so, compiled by oracle/Makefile) stored in tests/golden/ (tests/test_oracle_vs_ref.py,
+ * tests/test_oracle_golden.py).
  *
  * Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline leg may load this library.
  */

@@ -2,7 +2,7 @@
 
   Oracle : oracle/libbark_oracle.so  — our plain-C restatement (oracle/bark_oracle.c)
   Ref    : oracle/_ref/libbark_ref.so — the unmodified reference compiled by oracle/Makefile
-           (only exists where it was built from /root/reference; it travels to the GPU box)
+           (exists where build() found the reference's source tree: REFERENCE_DIR below)
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs import this.
 """
@@ -14,7 +14,7 @@ import subprocess
 
 import numpy as np
 
-# The C oracle uses OpenMP.  On big shared hosts (the GPU box reports 128 logical CPUs but the container gets far fewer
+# The C oracle uses OpenMP.  On big shared hosts (a host may report 128 logical CPUs while a container gets far fewer
 # cycles) a 128-thread team that spin-waits between the hundreds of tiny parallel regions of the LSTM loop can stall
 # for minutes, so cap the team and make idle threads sleep.  Must be set before libgomp initialises.
 os.environ.setdefault("OMP_NUM_THREADS", str(min(16, os.cpu_count() or 1)))
@@ -34,10 +34,16 @@ def build_oracle():
     subprocess.check_call(["make", "-C", HERE, "oracle"], stdout=subprocess.DEVNULL)
 
 
-def build_ref():
-    """Only possible where /root/reference exists (the build container)."""
-    if os.path.isdir("/root/reference"):
-        subprocess.check_call(["make", "-C", HERE, "ref", "-j8"], stdout=subprocess.DEVNULL)
+# The reference's source tree (a PABannier/bark.cpp checkout with its submodules): BARK_REFERENCE_DIR overrides the default location.
+REFERENCE_DIR = os.environ.get("BARK_REFERENCE_DIR") or "/root/reference"
+
+
+def build_ref() -> bool:
+    """Compile oracle/_ref/libbark_ref.so from REFERENCE_DIR (oracle/Makefile); False when that tree does not exist."""
+    if not os.path.isdir(REFERENCE_DIR):
+        return False
+    subprocess.check_call(["make", "-C", HERE, "ref", "-j8", f"REF={REFERENCE_DIR}"], stdout=subprocess.DEVNULL)
+    return True
 
 
 def have_ref() -> bool:
@@ -117,7 +123,7 @@ class Ref:
 
     def __init__(self, path: str, seed: int = 0, n_steps: int = 768, temp=0.7, fine_temp=0.5, min_eos_p=0.2):
         if not have_ref():
-            raise RuntimeError("oracle/_ref/libbark_ref.so not built (needs /root/reference)")
+            raise RuntimeError(f"oracle/_ref/libbark_ref.so not built (no reference tree at {REFERENCE_DIR}; set BARK_REFERENCE_DIR)")
         L = self.L = C.CDLL(REF_SO)
         L.ref_load.restype = vp
         L.ref_load.argtypes = [C.c_char_p, C.c_uint32, C.c_int, C.c_int]

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE — not product code.
 //
 // Thin C-ABI shim around the UNMODIFIED reference (PABannier/bark.cpp).  It is compiled by
-// oracle/Makefile from the sources where they lie under $(REF) (= /root/reference); nothing from
+// oracle/Makefile from the sources where they lie under $(REF) (make ref REF=...); nothing from
 // the reference is copied into this repository.  The single-TU include below is only there to
 // reach the reference's file-static stage functions and bark_context fields so that tests can
 //   (a) read the token streams the reference produced (bark.cpp:147-151),

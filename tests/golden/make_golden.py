@@ -1,5 +1,5 @@
 """Regenerates tests/golden/*.npz by running the UNMODIFIED reference (oracle/_ref/libbark_ref.so, built from
-/root/reference by oracle/Makefile) on seeded synthetic weight files.  Run in the build container:
+the reference tree by oracle/Makefile) on seeded synthetic weight files.  Run where the reference build exists:
 
     python tests/golden/make_golden.py
 
@@ -10,6 +10,7 @@ structure (AVX2, 4x8) produced the tokens (SURVEY.md App. C/E: the reference's t
 import hashlib
 import importlib
 import os
+import tempfile
 import sys
 
 import numpy as np
@@ -37,7 +38,7 @@ def main():
     orc = graft.load_oracle_bindings()
     os.environ["BARK_B200_QUIET"] = "1"
     out_dir = os.path.dirname(os.path.abspath(__file__))
-    tmp = "/tmp/bark_b200_fixtures"
+    tmp = os.path.join(tempfile.gettempdir(), f"bark_b200_fixtures_{os.getuid()}")
     os.makedirs(tmp, exist_ok=True)
     import ctypes as C
     for config, ftype, wseed, seed, n_steps, prompt, quant in CASES:

@@ -1,7 +1,7 @@
 """Regenerates tests/golden/small_f32_n12.npz — BASELINE.json configs[0] at its true size: bark-small dimensions, f32 GPT + f16 codec,
 one prompt, seed 0, the UNMODIFIED reference (oracle/_ref/libbark_ref.so) at -t 4, n_steps_text_encoder = 12 (a 15 s CPU run).
 
-    python tests/golden/make_golden_small.py          (build container only: needs /root/reference for oracle/_ref)
+    python tests/golden/make_golden_small.py          (needs the reference build oracle/_ref)
 
 The 1.6 GB weight file is not committed: bark.cpp_b200/weights.py regenerates it bit-identically from (config, ftype, seed); its sha1
 is stored in the fixture.
@@ -9,6 +9,7 @@ is stored in the fixture.
 import hashlib
 import importlib
 import os
+import tempfile
 import sys
 
 import numpy as np
@@ -23,7 +24,7 @@ def main():
     graft.load_package()
     weights = importlib.import_module("bark_cpp_b200.weights")
     orc = graft.load_oracle_bindings()
-    tmp = os.environ.get("BARK_B200_FIXTURES", "/tmp/bark_b200_fixtures")
+    tmp = os.environ.get("BARK_B200_FIXTURES", os.path.join(tempfile.gettempdir(), f"bark_b200_fixtures_{os.getuid()}"))
     os.makedirs(tmp, exist_ok=True)
     path = os.path.join(tmp, "small_f32_1234.bin")
     if not os.path.exists(path):

@@ -1,5 +1,5 @@
 """Regenerates the true-size fixtures of BASELINE.json configs[1..3] by running the UNMODIFIED reference
-(oracle/_ref/libbark_ref.so, built from /root/reference by oracle/Makefile):
+(oracle/_ref/libbark_ref.so, built by oracle/Makefile from the reference tree named by BARK_REFERENCE_DIR):
 
   small_f16_n138.npz       configs[1]: bark-small f16, THE BENCH CLIP (prompt "hello world", seed 0, n_steps_text_encoder = 138 ->
                            414 coarse steps = 7 sliding windows with prefix reuse, 207 frames, 66 240 samples)
@@ -12,7 +12,7 @@
                            E = 1024 / 24 layers / 16 heads against the unmodified reference itself
   small_f16_q4_0_n12.npz   configs[3]: bark-small, GPT weights quantised to q4_0 by the REFERENCE's bark_model_quantize, 12 steps
 
-    python tests/golden/make_golden_true_size.py [small|large|q4]        (build container only: needs oracle/_ref)
+    python tests/golden/make_golden_true_size.py [small|large|q4]        (needs the reference build oracle/_ref)
 
 Weight files are not committed: bark.cpp_b200/weights.py regenerates them bit-identically from (config, ftype, seed), the library's
 own bark_model_quantize reproduces the reference's q4_0 file byte for byte (tests/test_quantize.py); sha1 sums are in the fixtures.
@@ -21,6 +21,7 @@ import ctypes as C
 import hashlib
 import importlib
 import os
+import tempfile
 import sys
 import time
 
@@ -51,7 +52,7 @@ def main():
     graft.load_package()
     weights = importlib.import_module("bark_cpp_b200.weights")
     orc = graft.load_oracle_bindings()
-    tmp = os.environ.get("BARK_B200_FIXTURES", "/tmp/bark_b200_fixtures")
+    tmp = os.environ.get("BARK_B200_FIXTURES", os.path.join(tempfile.gettempdir(), f"bark_b200_fixtures_{os.getuid()}"))
     os.makedirs(tmp, exist_ok=True)
     out_dir = os.path.dirname(os.path.abspath(__file__))
     for name in (sys.argv[1:] or list(CASES)):

@@ -1,7 +1,7 @@
 """Static guard on the persistent decode step (no GPU needed): the production instantiations must not spill.
 
 Round 2's largest single gain came from finding that the "prefetched" K / V registers of this 128-register kernel were stack slots —
-every LDG followed by an STL of its own result, i.e. every load waited for its data (DESIGN.md §4.1, profiles/r02_decode_fine_stamps.txt).
+every LDG followed by an STL of its own result, i.e. every load waited for its data (DESIGN.md §4.1).
 `cuobjdump -res-usage` of the built library is cheap to check, so a change that brings spills back fails here instead of on the GPU clock.
 """
 import os

@@ -1,6 +1,6 @@
 """CPU: the C oracle (oracle/bark_oracle.c) against the committed golden vectors, which were produced by the
 unmodified reference (tests/golden/make_golden.py).  This is what pins the oracle on machines where
-/root/reference does not exist (the GPU box)."""
+the reference build does not exist."""
 import glob
 import hashlib
 import os

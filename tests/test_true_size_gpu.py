@@ -1,5 +1,5 @@
-"""BASELINE.json configs[1..3] at their TRUE size on the CUDA path, against fixtures the unmodified reference produced in the build
-container (tests/golden/make_golden_true_size.py; /root/reference does not exist on the GPU box):
+"""BASELINE.json configs[1..3] at their TRUE size on the CUDA path, against fixtures the unmodified reference produced where it was
+built (tests/golden/make_golden_true_size.py; no test needs the reference build):
 
   configs[1]  bark-small f16, THE BENCH CLIP: 138 semantic steps -> 414 coarse steps (7 sliding windows, exact prefix reuse, n_kv up to
               ~690, 64-step device batches) -> 207 frames x 8 codebooks -> 66 240 samples.  Token ids bit-exact, waveform <= 1e-3 relative.

@@ -1,5 +1,5 @@
 // Dependent-chain latencies on one warp (cycles per operation): DADD, DFMA, FADD, 32-bit SHFL, 64-bit SHFL (two 32-bit), SHFL + DADD level
-// (one level of the LayerNorm warp tree), bar.sync with 16 warps.  Build on the GPU box: nvcc -O3 -arch=sm_100a -o lat lat.cu
+// (one level of the LayerNorm warp tree), bar.sync with 16 warps.  Build: nvcc -O3 -arch=sm_90a -o lat lat.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 template <int MODE>

@@ -1,7 +1,7 @@
 // How fast can G SMs stream weights?  Decides whether the decode step can run inside ONE 16-CTA cluster (DSMEM exchanges, ~0.3 us per
-// dependency) instead of across 148 CTAs through L2 (1.3-2 us per dependency): the weight stream of a token (188 MB) must then come
+// dependency) instead of across all CTAs through L2: the weight stream of a token (188 MB) must then come
 // through 16 SMs' L2->shared-memory paths.
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a tools/microbench/stream_bw.cu -o /tmp/stream_bw
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a tools/microbench/stream_bw.cu -o /tmp/stream_bw
 // Each CTA: lane 0 of warp 0 issues cp.async.bulk copies of `chunk` bytes into a ring of shared-memory stages (mbarrier complete_tx);
 // the other warps wait for each stage, touch it (one LDS per thread) and release it.  Every CTA streams its own region (cold: HBM).
 #include <cuda_runtime.h>
@@ -58,7 +58,7 @@ int main() {
     const int STAGES = 12;
     CK(cudaFuncSetAttribute(stream_kernel<STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, STAGES * 16384));
     printf("# G CTAs (one per SM) streaming disjoint cold regions through a %d-stage shared-memory ring (cp.async.bulk)\n", STAGES);
-    for (int chunk : {16384, 4096}) for (int G : {1, 4, 8, 16, 32, 64, 148}) {
+    for (int chunk : {16384, 4096}) for (int G : {1, 4, 8, 16, 32, 64, 132}) {
         const size_t per = ((size_t) 16 << 20);
         CK(cudaMemset(d, 2, total));                     // evict the L2 (3 GB written)
         stream_kernel<STAGES><<<G, 512, STAGES * 16384>>>(d, per, chunk, d_out, d_sink);
