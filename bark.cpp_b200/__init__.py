@@ -125,7 +125,7 @@ def lib() -> C.CDLL:
     L.bark_b200_fast_mode.restype = C.c_int
     L.bark_b200_fast_mode.argtypes = [vp]
     L.bark_b200_fast_gemm.restype = C.c_int
-    L.bark_b200_fast_gemm.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int]
+    L.bark_b200_fast_gemm.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
     L.bark_b200_fast_attention.restype = C.c_int
     L.bark_b200_fast_attention.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int]
     L.ggml_time_us.restype = C.c_int64
@@ -288,14 +288,38 @@ class Bark:
         return int(lib().bark_b200_layernorm_fallbacks(self.ctx))
 
 
-def fast_gemm(A: np.ndarray, W: np.ndarray) -> np.ndarray:
-    """C = A W^T on the wgmma path; A [M][K], W [N][K] float16."""
+FAST_EPILOGUES = {"f32": 0, "resid": 1, "gelu16": 2, "qkv16": 4}      # FEPI_* (csrc/gpt_kernels.h)
+
+
+class GuardBandError(RuntimeError):
+    """The GEMM stored outside its output."""
+
+
+def fast_gemm(A: np.ndarray, W: np.ndarray, epilogue: str = "f32", bn: int = 0, resid: np.ndarray | None = None, return_bn: bool = False):
+    """A W^T on the wgmma path through one of the fine pass's epilogues; A [M][K], W [N][K] float16, K % 64 == 0.
+
+    Returns float32 [M][N] for "f32" and for "resid" (resid [M][N] float32 + A W^T), float16 [M][N] for "gelu16", and for "qkv16"
+    (N % 6 == 0) the pair (float16 [M][2N/3], the V columns transposed: float16 [N/3][M]).  bn = 0 lets the cost model pick the tile
+    width, 64 / 128 / 256 force it; with return_bn the result is (outputs, the tile width that ran)."""
     A = np.ascontiguousarray(A, np.float16); W = np.ascontiguousarray(W, np.float16)
     M, K = A.shape; N = W.shape[0]
-    out = np.zeros((M, N), np.float32)
-    if not lib().bark_b200_fast_gemm(_p(A), _p(W), _p(out), M, N, K):
-        raise RuntimeError("bark_b200_fast_gemm failed")
-    return out
+    assert W.shape[1] == K, (A.shape, W.shape)
+    if epilogue == "resid":
+        out = np.array(resid, np.float32, order="C", copy=True)
+        assert out.shape == (M, N), out.shape
+    elif epilogue == "qkv16":
+        assert N % 6 == 0, N
+        out = np.zeros(M * N, np.float16)
+    else:
+        out = np.zeros((M, N), np.float16 if epilogue == "gelu16" else np.float32)
+    r = lib().bark_b200_fast_gemm(_p(A), _p(W), _p(out), M, N, K, FAST_EPILOGUES[epilogue], bn)
+    if r == -1:
+        raise GuardBandError(f"bark_b200_fast_gemm ({epilogue}, {M}x{N}x{K}, bn {bn}) wrote outside its output")
+    if r <= 0:
+        raise RuntimeError(f"bark_b200_fast_gemm ({epilogue}, {M}x{N}x{K}, bn {bn}) failed")
+    if epilogue == "qkv16":
+        out = (out[:M * 2 * N // 3].reshape(M, 2 * N // 3), out[M * 2 * N // 3:].reshape(N // 3, M))
+    return (out, r) if return_bn else out
 
 
 def fast_attention(q: np.ndarray, k: np.ndarray, v: np.ndarray, n_head: int) -> np.ndarray:

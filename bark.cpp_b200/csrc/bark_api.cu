@@ -708,23 +708,56 @@ static int bark_b200_decode_timing_impl(struct bark_context * ctx, unsigned long
     return std::min(n, 256 * 32);
 }
 extern "C" int bark_b200_decode_timing(struct bark_context * ctx, unsigned long long * out, int n) { return guarded((int) 0, [&] { return bark_b200_decode_timing_impl(ctx, out, n); }); }
-// fast-mode kernels on host buffers (tests): C[M][N] = A[M][K] W[N][K]^T (f16 in, f32 out), and attention over [n][E] f16 q / k / v
-static int bark_b200_fast_gemm_impl(const uint16_t * A, const uint16_t * W, float * C, int M, int N, int K) {
+// fast-mode kernels on host buffers (tests): C = A[M][K] W[N][K]^T through one of the fine pass's GEMM epilogues (bark_b200.h), and
+// attention over [n][E] f16 q / k / v.  Every device output region of the GEMM sits between guard bands of a fixed byte pattern that
+// are checked after the kernel, and starts as NaN (RESID: as the residual from C), so a stray or a missing store shows up.
+static int bark_b200_fast_gemm_impl(const uint16_t * A, const uint16_t * W, void * C, int M, int N, int K, int epilogue, int bn) {
     if (!A || !W || !C || M < 1 || N < 1 || K < 64 || K % 64) return 0;
-    __half * dA, * dW; float * dC; int dev = 0, n_sm = 0;
+    if (epilogue != FEPI_F32 && epilogue != FEPI_RESID && epilogue != FEPI_GELU16 && epilogue != FEPI_QKV16) return 0;
+    if (epilogue == FEPI_QKV16 && N % 6) return 0;
+    constexpr size_t kGuard = 4096;
+    constexpr unsigned char kPattern = 0x5a;
+    // output regions in the order they are laid out in C: [M][N] f32 or f16; QKV16: Q|K [M][2N/3] f16, then V^T [N/3][M] f16
+    size_t bytes[2] = {(size_t) M * N * (epilogue == FEPI_GELU16 ? 2 : 4), 0};
+    if (epilogue == FEPI_QKV16) { bytes[0] = (size_t) M * (2 * N / 3) * 2; bytes[1] = (size_t) M * (N / 3) * 2; }
+    __half * dA, * dW; unsigned char * reg[2] = {nullptr, nullptr}; int dev = 0, n_sm = 0;
     BARK_CUDA_CHECK(cudaGetDevice(&dev)); BARK_CUDA_CHECK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
-    BARK_CUDA_CHECK(cudaMalloc(&dA, (size_t) M * K * 2)); BARK_CUDA_CHECK(cudaMalloc(&dW, (size_t) N * K * 2)); BARK_CUDA_CHECK(cudaMalloc(&dC, (size_t) M * N * 4));
+    BARK_CUDA_CHECK(cudaMalloc(&dA, (size_t) M * K * 2)); BARK_CUDA_CHECK(cudaMalloc(&dW, (size_t) N * K * 2));
     BARK_CUDA_CHECK(cudaMemcpy(dA, A, (size_t) M * K * 2, cudaMemcpyHostToDevice)); BARK_CUDA_CHECK(cudaMemcpy(dW, W, (size_t) N * K * 2, cudaMemcpyHostToDevice));
-    BARK_CUDA_CHECK(cudaMemset(dC, 0xff, (size_t) M * N * 4));
-    FastEpi ep; ep.mode = FEPI_F32; ep.out32 = dC; ep.ldo = N;
-    const bool ok = fast_gemm(dA, K, dW, K, M, N, K, ep, n_sm, 0);
+    for (int r = 0; r < 2 && bytes[r]; r++) {
+        BARK_CUDA_CHECK(cudaMalloc(&reg[r], bytes[r] + 2 * kGuard));
+        BARK_CUDA_CHECK(cudaMemset(reg[r], kPattern, bytes[r] + 2 * kGuard));
+        if (epilogue == FEPI_RESID) BARK_CUDA_CHECK(cudaMemcpy(reg[r] + kGuard, C, bytes[r], cudaMemcpyHostToDevice));
+        else                        BARK_CUDA_CHECK(cudaMemset(reg[r] + kGuard, 0xff, bytes[r]));
+    }
+    FastEpi ep; ep.mode = epilogue; ep.ldo = N;
+    if (epilogue == FEPI_F32 || epilogue == FEPI_RESID) ep.out32 = (float *)(reg[0] + kGuard);
+    else                                                ep.out16 = (__half *)(reg[0] + kGuard);
+    if (epilogue == FEPI_QKV16) { ep.ldo = 2 * N / 3; ep.vt = (__half *)(reg[1] + kGuard); ep.vt_ld = M; ep.v_col0 = 2 * N / 3; }     // the fine pass's arguments
+    const int ran = fast_gemm(dA, K, dW, K, M, N, K, ep, n_sm, bn, 0);
     const cudaError_t e = cudaDeviceSynchronize();
+    bool guards_intact = true;
     if (e != cudaSuccess) fprintf(stderr, "bark_b200_fast_gemm: %s\n", cudaGetErrorString(e));
-    else BARK_CUDA_CHECK(cudaMemcpy(C, dC, (size_t) M * N * 4, cudaMemcpyDeviceToHost));
-    cudaFree(dA); cudaFree(dW); cudaFree(dC);
-    return ok && e == cudaSuccess;
+    else {
+        std::vector<unsigned char> g(kGuard);
+        size_t off = 0;
+        for (int r = 0; r < 2 && bytes[r]; r++) {
+            for (const unsigned char * band : {reg[r], reg[r] + kGuard + bytes[r]}) {
+                BARK_CUDA_CHECK(cudaMemcpy(g.data(), band, kGuard, cudaMemcpyDeviceToHost));
+                for (unsigned char b : g) guards_intact &= b == kPattern;
+            }
+            BARK_CUDA_CHECK(cudaMemcpy((unsigned char *) C + off, reg[r] + kGuard, bytes[r], cudaMemcpyDeviceToHost));
+            off += bytes[r];
+        }
+    }
+    cudaFree(dA); cudaFree(dW); cudaFree(reg[0]); cudaFree(reg[1]);
+    if (!ran || e != cudaSuccess) return 0;
+    if (!guards_intact) { fprintf(stderr, "bark_b200_fast_gemm: a store landed outside the output (guard band overwritten)\n"); return -1; }
+    return ran;
 }
-extern "C" int bark_b200_fast_gemm(const uint16_t * A, const uint16_t * W, float * C, int M, int N, int K) { return guarded((int) 0, [&] { return bark_b200_fast_gemm_impl(A, W, C, M, N, K); }); }
+extern "C" int bark_b200_fast_gemm(const uint16_t * A, const uint16_t * W, void * C, int M, int N, int K, int epilogue, int bn) {
+    return guarded((int) 0, [&] { return bark_b200_fast_gemm_impl(A, W, C, M, N, K, epilogue, bn); });
+}
 static int bark_b200_fast_attention_impl(const uint16_t * q, const uint16_t * k, const uint16_t * v, uint16_t * out, int n, int E, int H) {
     if (!q || !k || !v || !out || n < 128 || n % 128 || E != H * 64) return 0;
     std::vector<uint16_t> qk((size_t) n * 2 * E), vt((size_t) E * n);

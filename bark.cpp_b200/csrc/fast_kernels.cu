@@ -3,7 +3,7 @@
 // The fine model's 1024-row passes (bark.cpp:1416-1584; mul_mat sites bark.cpp:1278,1344,1371,1380,1403 and the non-causal
 // attention bark.cpp:1495-1530) are genuine GEMMs.  The parity path (gemm_kernels.cu) must replay the reference's 32 IEEE FMA chains
 // per output and therefore runs on the fp32 pipe; wgmma accumulates in a different order, so this path cannot be bit-identical
-// and is validated by teacher forcing instead (tests/test_fast_mode.py: max |dlogit|, top-1 agreement, CDF-flip rate).
+// and is validated by kernel tests with exact answers and by teacher forcing instead (tests/test_fast_mode.py).
 //
 //   wgmma_gemm_kernel  C[M][N] = A[M][K] * W[N][K]^T, f16 operands, f32 accumulate in registers.  Block tile 128 x BN.
 //                      warp 8: TMA producer (cp.async.bulk.tensor 2-D tiles, 128-byte swizzle, mbarrier complete_tx ring)
@@ -114,14 +114,18 @@ constexpr int kGemmThreads = 288;                  // warpgroups 0-1: MMA + epil
 // GEMM
 // ------------------------------------------------------------------------------------------------
 // GELU as the reference's table defines it (ggml.c:2546-2571: f16(x) -> 0.5 x (1 + tanh(sqrt(2/pi) x (1 + 0.044715 x^2))) -> f16), evaluated
-// with the hardware tanh instead of a 64 K-entry table: dependent table look-ups per output would dominate the fc GEMM's epilogue.
-// tanh.approx is accurate to ~2^-11 relative: the result can differ from the table by one f16 ulp, which is inside fast mode's
-// tolerance (it is not the bit-exact path).
+// in closed form instead of a 64 K-entry table: dependent table look-ups per output would dominate the fc GEMM's epilogue.
+// It uses 0.5 x (1 + tanh y) = x / (1 + 2^(-2 y log2(e))), which does not cancel for negative x: 1 + tanh y does, and there the
+// ~2^-11 relative error of tanh.approx becomes thousands of f16 ulps of the small result.  ex2.approx and the fast reciprocal are
+// accurate to ~2^-22 relative, so for every f16 input the result is within one f16 ulp of the table, or within 2^-22 where the
+// table's own float tanh is quantised near -1 (tests/test_fast_mode.py).
+// For x <= -10 the denominator exceeds 2^126 or is infinite and the result is -0, as the table's 0.
 __device__ __forceinline__ float gelu_fast(float v) {
     const float x = __half2float(__float2half_rn(v));
-    float t;
-    asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.79788456080286535588f * x * (1.0f + 0.044715f * x * x)));
-    return 0.5f * x * (1.0f + t);
+    const float y = 0.79788456080286535588f * x * (1.0f + 0.044715f * x * x);
+    float e;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(-2.88539008177792681f * y));       // 2^(-2 y log2(e)) = e^(-2y)
+    return __fdividef(x, 1.0f + e);
 }
 
 // two horizontally adjacent outputs (m, n), (m, n + 1) of the fused epilogue
@@ -410,9 +414,11 @@ static bool launch_gemm(const __half * A, int lda, const __half * W, int ldw, in
     return true;
 }
 
-// C = A W^T on the tensor cores.  A [M][lda] f16, W [N][ldw] f16 (both K-contiguous), K % 64 == 0.
-bool fast_gemm(const __half * A, int lda, const __half * W, int ldw, int M, int N, int K, const FastEpi & ep, int n_sm, cudaStream_t s) {
-    if (K % kBK != 0 || K < kBK || M < 1 || N < 1) { fprintf(stderr, "bark_b200 fast mode: unsupported GEMM shape %d x %d x %d\n", M, N, K); return false; }
+// C = A W^T on the tensor cores.  A [M][lda] f16, W [N][ldw] f16 (both K-contiguous), K % 64 == 0.  bn = 0 lets the cost model below
+// pick the tile width; 64 / 128 / 256 force it (tests).  Returns the tile width launched, 0 on failure.
+int fast_gemm(const __half * A, int lda, const __half * W, int ldw, int M, int N, int K, const FastEpi & ep, int n_sm, int bn, cudaStream_t s) {
+    if (K % kBK != 0 || K < kBK || M < 1 || N < 1) { fprintf(stderr, "bark_b200 fast mode: unsupported GEMM shape %d x %d x %d\n", M, N, K); return 0; }
+    if (bn != 0 && bn != 64 && bn != 128 && bn != 256) { fprintf(stderr, "bark_b200 fast mode: tile width %d is not 64, 128 or 256\n", bn); return 0; }
     // Tile width.  These GEMMs are a few microseconds each, so the choice is about filling the SMs, one CTA per SM at a time:
     //   time(BN) ~ waves x (fixed per-CTA cost + operand bytes of one CTA / per-SM fill rate)
     // with an assumed ~3 us of prologue + epilogue drain per CTA and ~64 B/clk (~120 GB/s) from L2 into one SM's shared memory.
@@ -422,12 +428,16 @@ bool fast_gemm(const __half * A, int lda, const __half * W, int ldw, int M, int 
         const int tiles = tiles_m * ((N + bn - 1) / bn);
         return (double)((tiles + n_sm - 1) / n_sm) * (3.0 + (double)(kBM + bn) * K * 2.0 / 120e3);
     };
-    int best = 256;
-    for (int bn : {128, 64})
-        if (cost(bn) < cost(best) - 1e-9) best = bn;
-    if (best == 256) return launch_gemm<256>(A, lda, W, ldw, M, N, K, ep, s);
-    if (best == 128) return launch_gemm<128>(A, lda, W, ldw, M, N, K, ep, s);
-    return launch_gemm<64>(A, lda, W, ldw, M, N, K, ep, s);
+    int best = bn;
+    if (best == 0) {
+        best = 256;
+        for (int b : {128, 64})
+            if (cost(b) < cost(best) - 1e-9) best = b;
+    }
+    const bool ok = best == 256 ? launch_gemm<256>(A, lda, W, ldw, M, N, K, ep, s)
+                  : best == 128 ? launch_gemm<128>(A, lda, W, ldw, M, N, K, ep, s)
+                                : launch_gemm<64>(A, lda, W, ldw, M, N, K, ep, s);
+    return ok ? best : 0;
 }
 
 // att[N][E] (f16) = soft_max(Q K^T / sqrt(64)) V per head; qk: [N][ldq] f16 with Q at column h*64 and K at k_col0 + h*64; vt: V^T [E][N] f16

@@ -257,18 +257,18 @@ bool fine_eval_fast(bark_context * ctx, const int32_t * in_buffer, int nn, float
         const GPTLayer & L = m.layers[(size_t) il];
         fast_layernorm(ws.x, N, E, L.ln_1_g, L.ln_1_b, ctx->f_a16, s);
         FastEpi qkv; qkv.mode = FEPI_QKV16; qkv.out16 = ctx->f_qk16; qkv.ldo = 2 * E; qkv.vt = ctx->f_vt16; qkv.vt_ld = N; qkv.v_col0 = 2 * E;
-        if (!fast_gemm(ctx->f_a16, E, (const __half *) L.c_attn.p_rm, E, N, 3 * E, E, qkv, n_sm, s)) return false;
+        if (!fast_gemm(ctx->f_a16, E, (const __half *) L.c_attn.p_rm, E, N, 3 * E, E, qkv, n_sm, 0, s)) return false;
         if (!fast_attention(ctx->f_qk16, 2 * E, E, ctx->f_vt16, N, E, H, ctx->f_att16, s)) return false;
         FastEpi res; res.mode = FEPI_RESID; res.out32 = ws.x; res.ldo = E;
-        if (!fast_gemm(ctx->f_att16, E, (const __half *) L.c_proj.p_rm, E, N, E, E, res, n_sm, s)) return false;
+        if (!fast_gemm(ctx->f_att16, E, (const __half *) L.c_proj.p_rm, E, N, E, E, res, n_sm, 0, s)) return false;
         fast_layernorm(ws.x, N, E, L.ln_2_g, L.ln_2_b, ctx->f_a16, s);
-        FastEpi ge; ge.mode = FEPI_GELU16; ge.out16 = ctx->f_h16; ge.ldo = 4 * E; ge.gelu_tab = ctx->d_gelu_tab;
-        if (!fast_gemm(ctx->f_a16, E, (const __half *) L.fc.p_rm, E, N, 4 * E, E, ge, n_sm, s)) return false;
-        if (!fast_gemm(ctx->f_h16, 4 * E, (const __half *) L.proj.p_rm, 4 * E, N, E, 4 * E, res, n_sm, s)) return false;
+        FastEpi ge; ge.mode = FEPI_GELU16; ge.out16 = ctx->f_h16; ge.ldo = 4 * E;
+        if (!fast_gemm(ctx->f_a16, E, (const __half *) L.fc.p_rm, E, N, 4 * E, E, ge, n_sm, 0, s)) return false;
+        if (!fast_gemm(ctx->f_h16, 4 * E, (const __half *) L.proj.p_rm, 4 * E, N, E, 4 * E, res, n_sm, 0, s)) return false;
     }
     fast_layernorm(ws.x, N, E, m.ln_f_g, m.ln_f_b, ctx->f_a16, s);
     FastEpi st; st.mode = FEPI_F32; st.out32 = ws.logits; st.ldo = m.n_out_vocab;
-    if (!fast_gemm(ctx->f_a16, E, (const __half *) m.lm_head[nn - 1].p_rm, E, N, m.n_out_vocab, E, st, n_sm, s)) return false;
+    if (!fast_gemm(ctx->f_a16, E, (const __half *) m.lm_head[nn - 1].p_rm, E, N, m.n_out_vocab, E, st, n_sm, 0, s)) return false;
     ctx->last_logits = ws.logits;
     if (logits_host) {
         const size_t nb = (size_t) N * m.n_out_vocab * sizeof(float);

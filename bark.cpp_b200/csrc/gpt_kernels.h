@@ -53,14 +53,14 @@ void attention_tiled_scores(const float * Q, const float * Kc, int N, int n_kv, 
 void attention_tiled_pv(const float * scores, const float * Vc, int N, int n_kv, int E, int H, void * act, WType wt, int Kp, cudaStream_t s);
 
 // ---- fast mode (fast_kernels.cu, BARK_B200_MODE=fast): wgmma GEMM + flash-style attention for the dense passes -------------------
-enum { FEPI_F32 = 0, FEPI_RESID = 1, FEPI_GELU16 = 2, FEPI_F16 = 3, FEPI_QKV16 = 4 };
+enum { FEPI_F32 = 0, FEPI_RESID = 1, FEPI_GELU16 = 2, FEPI_QKV16 = 4 };
 struct FastEpi {
     int mode = FEPI_F32;
     float * out32 = nullptr; __half * out16 = nullptr; int ldo = 0;      // row-major targets
     __half * vt = nullptr; int vt_ld = 0, v_col0 = 0;                    // QKV16: columns >= v_col0 are written transposed, vt[(n - v_col0) * vt_ld + m]
-    const __half * gelu_tab = nullptr;
 };
-bool fast_gemm(const __half * A, int lda, const __half * W, int ldw, int M, int N, int K, const FastEpi & ep, int n_sm, cudaStream_t s);
+// bn: 0 = the cost model's tile width, else 64 / 128 / 256 forced.  Returns the tile width launched, 0 on failure.
+int  fast_gemm(const __half * A, int lda, const __half * W, int ldw, int M, int N, int K, const FastEpi & ep, int n_sm, int bn, cudaStream_t s);
 bool fast_attention(const __half * qk, int ldq, int k_col0, const __half * vt, int n, int E, int H, __half * out, cudaStream_t s);
 void fast_layernorm(const float * x, int rows, int E, const float * g, const float * b, __half * out, cudaStream_t s);
 

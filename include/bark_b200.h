@@ -74,10 +74,16 @@ BARK_API unsigned long long bark_b200_shard_nvlink_bytes(struct bark_context * c
 /* FAST MODE (BARK_B200_MODE=fast in the environment at load; opt-in, NOT bit-identical to the reference): the fine model's
  * 1024-row passes (bark.cpp:1416-1584) run as wgmma tensor-core GEMMs + flash-style attention (csrc/fast_kernels.cu).
  * The two kernel hooks below run on host buffers without a context, for the numerics tests:
- *   bark_b200_fast_gemm ....... C[M][N] (f32) = A[M][K] (f16 bits) * W[N][K]^T (f16 bits), K % 64 == 0
+ *   bark_b200_fast_gemm ....... A[M][K] (f16 bits) * W[N][K]^T (f16 bits), K % 64 == 0, through the fine pass's epilogue `epilogue`:
+ *                                 0 F32     C = f32 [M][N]
+ *                                 1 RESID   C = f32 [M][N], holds the residual on entry and residual + A W^T on return
+ *                                 2 GELU16  C = f16 [M][N] (bits), GELU of the product
+ *                                 4 QKV16   N % 6 == 0; C = f16 [M][2N/3] (columns < 2N/3), then f16 [N/3][M] (columns >= 2N/3, transposed)
+ *                               bn: 0 = the tile width the cost model picks, 64 / 128 / 256 = that width forced.
+ *                               Returns the tile width that ran, 0 on failure, -1 if a store landed in the guard bands around the output.
  *   bark_b200_fast_attention .. out[n][E] (f16 bits) = soft_max(Q K^T / 8) V per 64-wide head, non-causal, n % 128 == 0 */
 BARK_API int  bark_b200_fast_mode(struct bark_context * ctx);              /* 1 if this context runs the fast fine passes */
-BARK_API int  bark_b200_fast_gemm(const uint16_t * A, const uint16_t * W, float * C, int M, int N, int K);
+BARK_API int  bark_b200_fast_gemm(const uint16_t * A, const uint16_t * W, void * C, int M, int N, int K, int epilogue, int bn);
 BARK_API int  bark_b200_fast_attention(const uint16_t * q, const uint16_t * k, const uint16_t * v, uint16_t * out, int n, int E, int H);
 
 #ifdef __cplusplus
