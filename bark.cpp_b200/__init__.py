@@ -48,7 +48,7 @@ EXPORTS = [
     "bark_b200_sample", "bark_b200_sample_rows", "bark_b200_reseed", "bark_b200_tokenize", "bark_b200_forward_text_encoder",
     "bark_b200_forward_coarse_encoder", "bark_b200_forward_fine_encoder", "bark_b200_get_tokens", "bark_b200_set_tokens",
     "bark_b200_get_stats", "bark_b200_get_hparams", "bark_b200_kernel_launches", "bark_b200_layernorm_fallbacks",
-    "bark_b200_profile_enable", "bark_b200_profile_report", "bark_b200_io_counters", "bark_b200_decode_timing", "bark_b200_decode_adapt",
+    "bark_b200_profile_enable", "bark_b200_profile_report", "bark_b200_io_counters", "bark_b200_decode_timing",
     "bark_b200_shard_init", "bark_b200_shard_connect", "bark_b200_shard_nvlink_bytes",
     "bark_b200_fast_mode", "bark_b200_fast_gemm", "bark_b200_fast_attention",
     "ggml_time_init", "ggml_time_us", "ggml_time_ms", "ggml_init", "ggml_free",
@@ -114,8 +114,6 @@ def lib() -> C.CDLL:
     L.bark_b200_io_counters.argtypes = [C.POINTER(C.c_ulonglong), C.POINTER(C.c_ulonglong), C.c_int]
     L.bark_b200_decode_timing.restype = C.c_int
     L.bark_b200_decode_timing.argtypes = [vp, C.c_void_p, C.c_int]
-    L.bark_b200_decode_adapt.restype = C.c_int
-    L.bark_b200_decode_adapt.argtypes = [vp, C.c_int, C.c_void_p, C.c_int]
     L.bark_b200_shard_init.restype = C.c_int
     L.bark_b200_shard_init.argtypes = [vp, C.c_int, C.c_int, vp]
     L.bark_b200_shard_connect.restype = C.c_int

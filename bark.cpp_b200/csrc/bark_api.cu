@@ -200,7 +200,6 @@ bool run_chain(bark_context * ctx, GPTModel & m, const std::vector<int32_t> & fi
         BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->d_u, ctx->h_u, (size_t) n * sizeof(double), cudaMemcpyHostToDevice, s)); bark::g_h2d_bytes += (size_t) n * sizeof(double);
     }
     const bool chain = ctx->use_decode_kernel && m.decode_ok;
-    const bool fused = chain && fused_sampler_available(ctx, m, samp_n);
     std::vector<int> past_before((size_t) n);
     std::vector<int32_t> cur_in = first_in;
     std::vector<float> host_logits;
@@ -212,11 +211,6 @@ bool run_chain(bark_context * ctx, GPTModel & m, const std::vector<int32_t> & fi
             past_before[(size_t) j] = *n_past;
             if (j == start) { if (!gpt_eval(ctx, m, cur_in.data(), (int) cur_in.size(), n_past, merge_ctx && *n_past == 0, nullptr, lo, lo + samp_n)) return false; }
             const int force = ctx->debug_flag_every > 0 && (ctx->n_sample_calls++ % ctx->debug_flag_every) == 0;
-            if (j > start && fused) {                         // decode + sample in ONE launch (the kernel's last CTA draws the token)
-                const FusedSample fs{samp_n, temp, ctx->d_u + j, ctx->d_stok + j, lo, ctx->d_feed, ctx->d_seos + j, ctx->d_sflags + j, force};
-                if (!gpt_decode_chained(ctx, m, ctx->d_feed, n_past, lo, lo + samp_n, &fs)) return false;
-                continue;
-            }
             if (j > start && !gpt_decode_chained(ctx, m, ctx->d_feed, n_past, lo, lo + samp_n)) return false;
             sample_rows(ctx->last_logits + lo, m.n_out_vocab, samp_n, 1, temp, ctx->d_u + j, ctx->d_stok + j, lo, ctx->d_feed, ctx->d_seos + j, ctx->d_sflags + j, force, s);
         }
@@ -418,7 +412,7 @@ void alloc_workspace(bark_context * ctx) {
     int E = 0, H = 0; size_t kp_bytes = 0, n_logits = 0;
     for (GPTModel * m : {&ctx->semantic, &ctx->coarse, &ctx->fine}) {
         E = std::max(E, (int) m->n_embd); H = std::max(H, (int) m->n_head);
-        const size_t es = (m->wtype == W_F16 && !ctx->gemm_f32c) ? 2 : 4;
+        const size_t es = m->wtype == W_F16 ? 2 : 4;
         kp_bytes = std::max(kp_bytes, (size_t) li_padded_k(4 * m->n_embd, (int) es) * es);
     }
     n_logits = std::max<size_t>({(size_t) ctx->semantic.n_out_vocab, (size_t) ctx->coarse.n_out_vocab, (size_t) 1024 * ctx->fine.n_out_vocab});
@@ -454,7 +448,6 @@ void alloc_workspace(bark_context * ctx) {
     ctx->d_u = (double *) ctx_alloc(ctx, 1024 * 8); ctx->d_stok = (int32_t *) ctx_alloc(ctx, 1024 * 4);
     ctx->d_sflags = (int32_t *) ctx_alloc(ctx, 1024 * 4); ctx->d_seos = (float *) ctx_alloc(ctx, 1024 * 4);
     ctx->d_feed = (int32_t *) ctx_alloc(ctx, 64); BARK_CUDA_CHECK(cudaMemset(ctx->d_feed, 0, 64));
-    ctx->d_done_counter = (unsigned *) ctx_alloc(ctx, 64); BARK_CUDA_CHECK(cudaMemset(ctx->d_done_counter, 0, 64));
     BARK_CUDA_CHECK(cudaMemset(ctx->d_u, 0, 1024 * 8));
     BARK_CUDA_CHECK(cudaMallocHost(&ctx->h_u, 1024 * 8)); BARK_CUDA_CHECK(cudaMallocHost(&ctx->h_stok, 1024 * 4));
     BARK_CUDA_CHECK(cudaMallocHost(&ctx->h_sflags, 1024 * 4)); BARK_CUDA_CHECK(cudaMallocHost(&ctx->h_seos, 1024 * 4));
@@ -522,14 +515,7 @@ extern "C" struct bark_context * bark_load_model(const char * model_path, struct
     { const char * e = getenv("BARK_B200_DECODE"); ctx->use_decode_kernel = !(e && !strcmp(e, "multi")); ctx->decode_cluster = e && !strcmp(e, "cluster"); }   // "multi": one kernel per op (debug / A-B)
     { const char * e = getenv("BARK_B200_DECODE_TIMING_TID"); if (e && atoi(e) >= 0 && atoi(e) < 512) ctx->timing_tid = atoi(e) & ~31; }
     { const char * e = getenv("BARK_B200_POLL_NS"); if (e && atoi(e) >= 0 && atoi(e) <= 100000) ctx->poll_ns = (unsigned) atoi(e); }
-    { const char * e = getenv("BARK_B200_POLL_ATT_NS"); if (e && atoi(e) >= 0 && atoi(e) <= 100000) ctx->att_ns = (unsigned) atoi(e); }
-    { const char * e = getenv("BARK_B200_POLL_FIRST_NS"); if (e && atoi(e) >= 0 && atoi(e) <= 100000) ctx->first_ns = (unsigned) atoi(e); }
-    ctx->headstart[1] = ctx->att_ns; ctx->headstart[2] = ctx->headstart[4] = ctx->first_ns;
     { const char * e = getenv("BARK_B200_HEADSTART"); if (e) { unsigned v[6]; if (sscanf(e, "%u:%u:%u:%u:%u:%u", &v[0], &v[1], &v[2], &v[3], &v[4], &v[5]) == 6) for (int i = 0; i < 6; i++) ctx->headstart[i] = std::min(v[i], 100000u); } }
-    { const char * e = getenv("BARK_B200_KV_PREFETCH"); ctx->kv_prefetch = e && !strcmp(e, "1"); }
-    { const char * e = getenv("BARK_B200_FUSE_SAMPLER"); ctx->fuse_sampler = e && !strcmp(e, "1"); }        // "1": the decode kernel's last CTA samples the token (one launch per token); off by default
-    { const char * e = getenv("BARK_B200_GEMM_F32C"); ctx->gemm_f32c = e && !strcmp(e, "1"); }
-    { const char * e = getenv("BARK_B200_ADAPT"); ctx->adapt_on = e && !strcmp(e, "1"); }                     // "1": self-tuning head starts (experiment: the feedback is collective and can run away)
     ctx->params = params;
     const bool loaded = guarded(false, [&] {                  // a CUDA failure while loading (out of memory, ...) is a failed load, not an abort
     BARK_CUDA_CHECK(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
@@ -776,19 +762,6 @@ static int bark_b200_fast_attention_impl(const uint16_t * q, const uint16_t * k,
     return ok && e == cudaSuccess;
 }
 extern "C" int bark_b200_fast_attention(const uint16_t * q, const uint16_t * k, const uint16_t * v, uint16_t * out, int n, int E, int H) { return guarded((int) 0, [&] { return bark_b200_fast_attention_impl(q, k, v, out, n, E, H); }); }
-// the decode kernel's self-tuned head starts, [n_cta][8] nanoseconds (decode_kernels.cu XT_* order); which: 0 semantic, 1 coarse
-extern "C" int bark_b200_decode_adapt(struct bark_context * ctx, int which, unsigned * out, int n) {
-    if (!ctx || !out || which < 0 || which > 1) return 0;
-    return guarded(0, [&] {
-        const GPTModel * m = pick(ctx, which);
-        if (!m->d_adapt) return 0;
-        const int cnt = std::min(n, ctx->n_sm_total * 8);
-        BARK_CUDA_CHECK(cudaSetDevice(ctx->device));
-        BARK_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-        BARK_CUDA_CHECK(cudaMemcpy(out, m->d_adapt, (size_t) cnt * 4, cudaMemcpyDeviceToHost));
-        return cnt;
-    });
-}
 extern "C" int bark_b200_fast_mode(struct bark_context * ctx) { return ctx && ctx->fast_mode ? 1 : 0; }
 
 extern "C" const char * bark_b200_version(void) { return "bark_b200 r3 (sm_90a; parity path + opt-in wgmma fast mode)"; }

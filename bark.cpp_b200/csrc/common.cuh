@@ -86,9 +86,6 @@ extern thread_local double g_next_bytes, g_next_flops;
 
 // weight element types as stored in ggml_weights.bin (ggml_type values, SURVEY App. A)
 enum WType : int { W_F32 = 0, W_F16 = 1, W_Q4_0 = 2, W_Q4_1 = 3, W_Q5_0 = 6, W_Q5_1 = 7, W_Q8_0 = 8 };   // 3..8: qx_kernels.cu
-// activation-operand format only (never a file type): f16-rounded values kept in f32 containers, for f16 weight matrices whose tiled-GEMM
-// copy was expanded to f32 at load — the same numbers and the same arithmetic, without f16->f32 conversions in the mat-mul's inner loop
-constexpr int W_F16R32 = 101;
 inline bool is_quant(WType t) { return t != W_F32 && t != W_F16; }
 
 // ---------------------------------------------------------------------------------------------

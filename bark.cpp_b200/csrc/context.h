@@ -30,15 +30,11 @@ struct bark_context {
     unsigned tag_base = 0;                           // epoch counter of the decode kernel's tagged exchanges (advances 6*L per token)
     int n_sm = 0, n_sm_total = 0; bool use_decode_kernel = true;   // n_sm: CTAs of the persistent decode kernel (knob); n_sm_total: SMs of the device
     bool kv_reuse = true; unsigned long long n_kv_reused = 0;   // coarse windows start from the cached prefix (bark_api.cu run_coarse)
-    // decode-kernel knobs (BARK_B200_DECODE_TIMING_TID / BARK_B200_POLL_NS / BARK_B200_POLL_FIRST_NS); defaults:
+    // decode-kernel knobs (BARK_B200_DECODE_TIMING_TID / BARK_B200_POLL_NS / BARK_B200_HEADSTART); defaults:
     // 40 ns back-off between polls, 500 ns head start for the two residual exchanges
-    bool kv_prefetch = false;          // BARK_B200_KV_PREFETCH=1: bulk L2 prefetch of the next layer's K / V rows inside the decode step
-    bool fuse_sampler = false; unsigned * d_done_counter = nullptr;  // BARK_B200_FUSE_SAMPLER=1: the decode kernel samples its own token (6411 instead of 8037 launches per clip; 233.3 vs 233.7 ms: neutral, so off)
     bool decode_cluster = false;                     // BARK_B200_DECODE=cluster: the decode step inside one 16-CTA cluster (decode_kernels.cu) where the model fits
-    bool gemm_f32c = false;                          // BARK_B200_GEMM_F32C=1: multi-row passes of f16 models keep operands as f16 values in f32 containers
-    bool adapt_on = false;                           // BARK_B200_ADAPT=1: self-tuning head starts instead of the fixed knobs below (experiment, see decode_kernels.cu)
     unsigned headstart[6] = {0, 2000, 500, 400, 500, 0};   // BARK_B200_HEADSTART=q:att:x1:ff:x2:scores (ns): sleep before the first poll of each exchange
-    int timing_tid = 0; unsigned poll_ns = 40, first_ns = 500, att_ns = 2000;   // att_ns (BARK_B200_POLL_ATT_NS): head start before CTAs without a soft_max tile poll for the attention output
+    int timing_tid = 0; unsigned poll_ns = 40;
     unsigned long long * d_timing = nullptr;         // optional phase timestamps of the decode kernel (BARK_B200_DECODE_TIMING=1)
 
     // BARK_B200_MODE=fast: the fine model's passes run on the tensor cores (fast_kernels.cu); not bit-identical to the reference
@@ -101,10 +97,7 @@ bool codec_decode(bark_context * ctx, const int32_t * codes, int T);
 // sampling.cu / gpt_forward.cu / bark_api.cu
 void sample_rows(const float * logits, int ld, int n, int rows, float temp, const double * d_u, int32_t * d_out_tok, int tok_add, int32_t * d_feed,
                  float * d_eos_p, int32_t * d_flags, int force_flag, cudaStream_t s);
-// fs != null: the decode kernel also samples the token (fused sampler), leaving it in fs->d_tok / fs->d_feed
-struct FusedSample { int n; float temp; const double * d_u; int32_t * d_tok; int tok_add; int32_t * d_feed; float * d_eos; int32_t * d_flags; int force; };
-bool fused_sampler_available(const bark_context * ctx, const GPTModel & m, int samp_n);
-bool gpt_decode_chained(bark_context * ctx, GPTModel & m, const int32_t * d_token, int * n_past, int lm_lo, int lm_hi, const FusedSample * fs = nullptr);
+bool gpt_decode_chained(bark_context * ctx, GPTModel & m, const int32_t * d_token, int * n_past, int lm_lo, int lm_hi);
 bool sample_device(bark_context * ctx, GPTModel & m, const float * d_logits, int ld, int n, int rows, float temp, int32_t * out_tok, float * out_eos);
 int32_t sample_token_given_u(const float * logits, int n, float temp, double u, float * eos_p);
 

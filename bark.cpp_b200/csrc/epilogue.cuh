@@ -14,7 +14,6 @@ namespace bark {
 __device__ __forceinline__ void store_act(void * act, int wt, int gs, int m, int k, float v) {
     if (wt == W_Q4_0) { ((float *) act)[(size_t) m * gs + k] = v; return; }
     const size_t off = gm_offset(m, k, (size_t) gs);
-    if (wt == W_F16R32) { ((float *) act)[off] = round_f16(v); return; }
     if (wt == W_F16) ((__half *) act)[off] = __float2half_rn(v);
     else             ((float *) act)[off] = v;
 }

@@ -185,7 +185,7 @@ __global__ void __launch_bounds__(256, 2) lane_gemm_tiled_kernel(const T * __res
     }
 }
 
-void lane_gemm_tiled(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, cudaStream_t s, bool f32_containers) {
+void lane_gemm_tiled(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, cudaStream_t s) {
     const size_t smem = (size_t) kStages * kStageBytes + kStages * 8 + kStages * 4 + 64;
     int dev = 0, n_sm = 0;
     BARK_CUDA_CHECK(cudaGetDevice(&dev));
@@ -194,13 +194,6 @@ void lane_gemm_tiled(const DMat & W, const void * act, int act_gs, int rows, con
     if (first_use_on_this_device(configured)) {
         BARK_CUDA_CHECK(cudaFuncSetAttribute(lane_gemm_tiled_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
         BARK_CUDA_CHECK(cudaFuncSetAttribute(lane_gemm_tiled_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
-    }
-    if (f32_containers && W.type == W_F16) {                 // f16 values in f32 containers on both sides: the float kernel, bit-identical results
-        if (!W.p_gm32) { fprintf(stderr, "bark_b200: matrix has no f32-expanded copy\n"); throw std::runtime_error("unsupported configuration (see the message above)"); }
-        const int n_tiles32 = ((W.n_out + kBO - 1) / kBO) * ((rows + kBM - 1) / kBM);
-        const int grid32 = min(n_tiles32, 2 * n_sm);
-        BARK_LAUNCH((lane_gemm_tiled_kernel<float>), grid32, 256, smem, s, (const float *) W.p_gm32, W.K, W.o_pad * kGmGroup, W.n_out, (const float *) act, act_gs, rows, ep);
-        return;
     }
     if (!W.p_gm) { fprintf(stderr, "bark_b200: matrix has no group-major copy for the tiled mat-mul\n"); throw std::runtime_error("unsupported configuration (see the message above)"); }
     const int n_tiles = ((W.n_out + kBO - 1) / kBO) * ((rows + kBM - 1) / kBM);

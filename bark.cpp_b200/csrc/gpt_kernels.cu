@@ -225,14 +225,7 @@ __global__ void __launch_bounds__(256) lane_matmul_kernel(const T * __restrict__
 
 static bool use_tiled() { static const bool t = [] { const char * e = getenv("BARK_B200_GEMM"); return !(e && !strcmp(e, "simple")); }(); return t; }
 
-__global__ void expand_f16_kernel(const __half * __restrict__ src, float * __restrict__ dst, size_t n) {
-    for (size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t) gridDim.x * blockDim.x) dst[i] = __half2float(src[i]);
-}
-void expand_f16_to_f32(const void * src_f16, void * dst_f32, size_t n, cudaStream_t s) {
-    BARK_LAUNCH(expand_f16_kernel, 1184, 256, 0, s, (const __half *) src_f16, (float *) dst_f32, n);
-}
-
-void lane_matmul(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, cudaStream_t s, bool f32_containers) {
+void lane_matmul(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, cudaStream_t s) {
     if (W.type == W_Q4_0) { q4_matmul(W, act, act_gs, rows, ep, s); return; }      // act_gs = f32 row stride for this type
     if (qx_supported(W.type)) { qx_matmul(W, act, act_gs, rows, ep, s); return; }
     const int gx = (W.n_out + 7) / 8;
@@ -241,8 +234,7 @@ void lane_matmul(const DMat & W, const void * act, int act_gs, int rows, const M
         g_next_bytes = (double) W.n_out * W.K * es + (double) rows * (W.K * es + W.n_out * 4.0);
         g_next_flops = 2.0 * rows * (double) W.n_out * W.K;
     }
-    if (rows >= 16 && use_tiled() && (W.type == W_F16 || W.type == W_F32)) { lane_gemm_tiled(W, act, act_gs, rows, ep, s, f32_containers); return; }
-    if (f32_containers) { fprintf(stderr, "bark_b200: f32-container operands need the tiled mat-mul (rows >= 16)\n"); throw std::runtime_error("unsupported configuration (see the message above)"); }
+    if (rows >= 16 && use_tiled() && (W.type == W_F16 || W.type == W_F32)) { lane_gemm_tiled(W, act, act_gs, rows, ep, s); return; }
     if (W.type == W_F16) {
         if (rows == 1) BARK_LAUNCH((lane_matmul_kernel<__half, 1>), dim3(gx, 1), 256, 0, s, (const __half *) W.p, W.K, W.Kp, W.n_out, (const __half *) act, act_gs, rows, ep);
         else           BARK_LAUNCH((lane_matmul_kernel<__half, 8>), dim3(gx, (rows + 7) / 8), 256, 0, s, (const __half *) W.p, W.K, W.Kp, W.n_out, (const __half *) act, act_gs, rows, ep);

@@ -27,7 +27,7 @@ void gpt_embed_fine(const GPTModel & m, const int32_t * d_ids, int nn, float * x
 void layernorm_act(const float * x, int rows, int E, const float * g, const float * b, void * act, WType wt, int Kp,
                    unsigned * fallback_counter, cudaStream_t s);
 
-void lane_matmul(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, cudaStream_t s, bool f32_containers = false);
+void lane_matmul(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, cudaStream_t s);
 
 void attention(const float * Q, const float * Kc, const float * Vc, int N, int n_kv, int n_past, int E, int H, bool causal,
                float * scores, void * act, WType wt, int Kp, cudaStream_t s);
@@ -47,8 +47,7 @@ void   qx_embed_fine(const GPTModel & m, const int32_t * d_ids, int nn, float * 
 void   qx_matmul(const DMat & W, const void * act_f32, int ld_act, int rows, const MatmulEpilogue & ep, cudaStream_t s);
 
 // ---- register-tiled multi-row kernels (gemm_kernels.cu) ------------------------------------------------------------
-void lane_gemm_tiled(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, cudaStream_t s, bool f32_containers = false);
-void expand_f16_to_f32(const void * src_f16, void * dst_f32, size_t n, cudaStream_t s);
+void lane_gemm_tiled(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, cudaStream_t s);
 void attention_tiled_scores(const float * Q, const float * Kc, int N, int n_kv, int n_past, int E, int H, float scale, bool causal, float * scores, cudaStream_t s);
 void attention_tiled_pv(const float * scores, const float * Vc, int N, int n_kv, int E, int H, void * act, WType wt, int Kp, cudaStream_t s);
 
@@ -81,14 +80,8 @@ struct DecodeArgs {
     int E, H, L, block_size, n_past, token, lm_lo, lm_hi;
     const int32_t * token_ptr; int n_vocab_in;   // token_ptr != null: read the input token from device memory (written by sample_rows_kernel), clamped to the vocabulary
     double inv_E;                        // 1.0 / E (double), for the division-free LayerNorm decision
-    // fused sampler (samp_n > 0): the CTA that finishes its lm_head rows last samples the token from logits [lm_lo, lm_lo + samp_n)
-    // (sampling.cuh) — one launch per token instead of two
-    int samp_n; float samp_temp; const double * samp_u; int32_t * samp_tok; int samp_tok_add; int32_t * samp_feed; float * samp_eos; int32_t * samp_flags; int samp_force;
-    unsigned * done_counter;
-    unsigned headstart[6];               // fixed head start (ns) before the first poll of each exchange: q, att (CTAs without a soft_max tile), x1, ff, x2, scores
-    int kv_prefetch;                     // 1: every CTA asks the TMA engine to pull its slice of the NEXT layer's K / V rows into L2 (cp.async.bulk.prefetch.L2) one layer ahead
-    unsigned * adapt;                    // [n_cta][8] adaptive head starts of the exchanges, carried from token to token (null: fixed knobs)
-    int timing_tid; unsigned poll_ns, first_ns, att_ns;   // debug: stamping thread; back-off between polls of the tagged words; delay before the first poll of the residual exchanges (ns)
+    unsigned headstart[6];               // head start (ns) before the first poll of each exchange: q, att (CTAs without a soft_max tile), x1, ff, x2, scores
+    int timing_tid; unsigned poll_ns;    // debug: stamping thread; back-off between polls of the tagged words (ns)
 };
 int  decode_tags_per_step(int n_layer);
 void launch_decode_step(const DecodeArgs & args, WType wt, int n_sm, cudaStream_t s);

@@ -169,11 +169,6 @@ bool load_gpt(bark_context * ctx, std::ifstream & f, GPTModel & m, const char * 
                 const size_t gm_bytes = (size_t) gm_groups(d.K) * d.o_pad * kGmGroup * (m.wtype == W_F16 ? 2 : 4);
                 d.p_gm = ctx_alloc(ctx, gm_bytes);
                 permute_to_gm(raw, d.p_gm, d.n_out, d.o_pad, d.K, m.wtype, ctx->stream);
-                if (ctx->gemm_f32c && m.wtype == W_F16) {    // f16 values in f32 containers for the tiled mat-mul (no conversions in its inner loop)
-                    const size_t n_el = gm_bytes / 2;
-                    d.p_gm32 = ctx_alloc(ctx, n_el * 4);
-                    expand_f16_to_f32(d.p_gm, d.p_gm32, n_el, ctx->stream);
-                }
             }
             BARK_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
             if (ctx->fast_mode && !causal && m.wtype == W_F16) { d.p_rm = raw; ctx->device_allocs.push_back(raw); }   // fast mode: the tensor cores read the file's own row-major layout

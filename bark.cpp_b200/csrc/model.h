@@ -16,7 +16,6 @@ struct DMat {                 // 2-D weight [n_out][K] in LI layout (f32 / f16) 
     void * scales = nullptr;        // quantised: f16 block scales [n_out][K/32]; p then holds the 16-byte nibble words (32 B for q8_0) [n_out][K/32]
     void * mins = nullptr, * qh = nullptr;   // experimental types: f16 block minima (q4_1, q5_1), fifth bits (q5_0, q5_1)
     void * p_gm = nullptr; int o_pad = 0;   // second copy in the group-major layout (common.cuh) for the tiled GEMM; rows padded to o_pad
-    void * p_gm32 = nullptr;                // f16 matrices, BARK_B200_GEMM_F32C=1: the group-major copy expanded to f32 (gemm_kernels.cu)
     void * p_rm = nullptr;                  // fast mode only: the file's row-major [n_out][K] f16 matrix = K-major wgmma operand (fast_kernels.cu)
     WType type = W_F16;
 };
@@ -42,7 +41,6 @@ struct GPTModel {
     void * d_phases = nullptr, * d_layer_vecs = nullptr;
     unsigned long long * gx = nullptr, * gq = nullptr, * gk = nullptr, * gv = nullptr, * gatt = nullptr, * gff = nullptr, * gscores = nullptr;
     float * glogits = nullptr;
-    unsigned * d_adapt = nullptr;     // per-CTA adaptive head starts of the exchanges (decode_kernels.cu)
     // per-model statistics, same meaning as gpt_model::t_* (bark.cpp:114-118)
     int64_t t_sample_us = 0, t_predict_us = 0, t_main_us = 0, n_sample = 0;
 };

@@ -17,9 +17,109 @@
 // Flagged rows (probability ~1e-7 per row) are re-sampled on the host with the reference's exact sequence, using the same
 // u, so the token stream is identical to the host path in all cases.
 #include "gpt_kernels.h"
-#include "sampling.cuh"
 
 namespace bark {
+
+// gpt_sample for ONE logit row by one thread block of kSampleThreads threads.  sh: [n] floats of shared memory; lg: the n logits of the row
+template <int kSampleThreads>
+__device__ __forceinline__ void sample_row_body(float * sh, const float * lg, int n, float temp, double u, int32_t * out_tok, int tok_add, int32_t * feed,
+                                                float * eos_p, int32_t * flags, int force_flag) {
+    __shared__ float s_f[kSampleThreads / 32]; __shared__ int s_i[kSampleThreads / 32]; __shared__ double s_d[kSampleThreads / 32];
+    __shared__ float s_sum; __shared__ int s_amb;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    constexpr int NW = kSampleThreads / 32;
+    const float div = temp == 0.0f ? 0.7f : temp;        // the argmax path still divides by 0.7 (bark.cpp:226-228)
+    bool ambiguous = force_flag != 0;
+    if (tid == 0) s_amb = 0;
+
+    float mx = __int_as_float(0xff800000);
+    for (int i = tid; i < n; i += kSampleThreads) { const float l = __fdiv_rn(__ldcg(lg + i), div); sh[i] = l; mx = fmaxf(mx, l); }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if (lane == 0) s_f[warp] = mx;
+    __syncthreads();
+    mx = s_f[0];
+#pragma unroll
+    for (int w = 1; w < NW; w++) mx = fmaxf(mx, s_f[w]);
+    for (int i = tid; i < n; i += kSampleThreads) {
+        const double y = exp((double) __fsub_rn(sh[i], mx));
+        if (__double2float_rn(y * (1.0 - 0x1p-50)) != __double2float_rn(y * (1.0 + 0x1p-50))) ambiguous = true;
+        sh[i] = __double2float_rn(y);
+    }
+    __syncthreads();
+    if (tid == 0) {                                      // sequential float sum (bark.cpp:191-195): the order IS the result
+        float sum = 0.0f;
+        int i = 0;
+        for (; i + 8 <= n; i += 8) {
+            const float4 a = *reinterpret_cast<const float4 *>(sh + i), b = *reinterpret_cast<const float4 *>(sh + i + 4);
+            sum = __fadd_rn(sum, a.x); sum = __fadd_rn(sum, a.y); sum = __fadd_rn(sum, a.z); sum = __fadd_rn(sum, a.w);
+            sum = __fadd_rn(sum, b.x); sum = __fadd_rn(sum, b.y); sum = __fadd_rn(sum, b.z); sum = __fadd_rn(sum, b.w);
+        }
+        for (; i < n; i++) sum = __fadd_rn(sum, sh[i]);
+        s_sum = sum;
+    }
+    __syncthreads();
+    const float sum = s_sum;
+    for (int i = tid; i < n; i += kSampleThreads) sh[i] = __fdiv_rn(sh[i], sum);
+    __syncthreads();
+
+    int token = 0;
+    if (temp == 0.0f) {                                  // gpt_argmax_sample: first strict maximum
+        float best = __int_as_float(0xff800000); int bi = 0x7fffffff;
+        for (int i = tid; i < n; i += kSampleThreads) { const float p = sh[i]; if (p > best) { best = p; bi = i; } }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float ob = __shfl_xor_sync(0xffffffffu, best, o); const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+            if (ob > best || (ob == best && oi < bi)) { best = ob; bi = oi; }
+        }
+        if (lane == 0) { s_f[warp] = best; s_i[warp] = bi; }
+        __syncthreads();
+        best = s_f[0]; bi = s_i[0];
+#pragma unroll
+        for (int w = 1; w < NW; w++) if (s_f[w] > best || (s_f[w] == best && s_i[w] < bi)) { best = s_f[w]; bi = s_i[w]; }
+        token = bi;
+    } else {
+        // thread t owns the contiguous chunk [t*c, (t+1)*c): local sums, block scan of the chunk sums, then the crossing search
+        const int c = (n + kSampleThreads - 1) / kSampleThreads, lo = min(n, tid * c), hi = min(n, lo + c);
+        double part = 0.0;
+        for (int i = lo; i < hi; i++) part += (double) sh[i];
+        double incl = part;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const double t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
+        if (lane == 31) s_d[warp] = incl;
+        __syncthreads();
+        double before = 0.0, total = 0.0;
+#pragma unroll
+        for (int w = 0; w < NW; w++) { if (w < warp) before += s_d[w]; total += s_d[w]; }
+        const double thr = u * total;               // cp[i] >= u  <=>  (sum_{j<=i} p_j) / total >= u, up to rounding
+        const double eps = 8.0 * (double) n * 0x1p-53 * total;
+        double run = before + incl - part;
+        int first = 0x7fffffff;
+        for (int i = lo; i < hi; i++) {
+            run += (double) sh[i];
+            if (i < n - 1) {                             // the last partial sum is forced to 1.0 >= u
+                if (fabs(run - thr) <= eps) ambiguous = true;
+                if (run >= thr && first == 0x7fffffff) first = i;
+            }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) first = min(first, __shfl_xor_sync(0xffffffffu, first, o));
+        if (lane == 0) s_i[warp] = first;
+        __syncthreads();
+        first = s_i[0];
+#pragma unroll
+        for (int w = 1; w < NW; w++) first = min(first, s_i[w]);
+        token = first == 0x7fffffff ? n - 1 : first;
+    }
+    if (ambiguous) s_amb = 1;
+    __syncthreads();
+    if (tid == 0) {
+        *out_tok = token + tok_add;
+        if (feed) *feed = token + tok_add;
+        if (eos_p) *eos_p = sh[n - 1];                   // probability of the LAST logit (bark.cpp:216-218)
+        *flags = s_amb;
+    }
+}
 
 // 256 threads per row when many rows are sampled at once (fine passes: 1024 rows), 1024 threads for the single row of a decode
 // step (the exp / division / scan passes of a 10 048-wide semantic row are 4x shorter; the sequential sum is unchanged)

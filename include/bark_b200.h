@@ -57,8 +57,6 @@ BARK_API void bark_b200_io_counters(unsigned long long * h2d_bytes, unsigned lon
 /* with BARK_B200_DECODE_TIMING=1 in the environment at load: %globaltimer stamps [256][32] of the last decode step (rows 0..L: the
  * stamping thread of CTA 0 per layer; rows 64 + cta: every CTA at layer 5; slot meaning in tools/decode_timing.py) */
 BARK_API int  bark_b200_decode_timing(struct bark_context * ctx, unsigned long long * out, int n);
-/* the decode kernel's self-tuned head starts before the first poll of each exchange, [n_cta][8] nanoseconds; which: 0 semantic, 1 coarse */
-BARK_API int  bark_b200_decode_adapt(struct bark_context * ctx, int which, unsigned * out, int n);
 
 
 /* ROW-SHARDED FINE STAGE (BASELINE configs[4]; csrc/shard.cu): one process per GPU; every rank loads the same file and the same coarse

@@ -1,9 +1,10 @@
 #!/usr/bin/env python
 """Average device time of the production decode-step kernel (no stamps) under different exchange knobs, on an H100.
 
-usage: python tools/decode_bench.py [--n-past 300,900] poll_ns:first_ns:att_ns [poll_ns:first_ns:att_ns ...]
-One context per setting; 60 single-token steps of the coarse model of the bark-small f16 bench file, timed with the library's
-CUDA-event profiler (bark_b200_profile_report).  Writes $BARK_TOOLS_OUT/decode_bench.json.
+usage: python tools/decode_bench.py [--n-past 300,900] poll_ns[/q:att:x1:ff:x2:scores] [...]
+One context per setting: BARK_B200_POLL_NS = poll_ns and, where given, BARK_B200_HEADSTART = the head starts (ns) after the slash.
+60 single-token steps of the coarse model of the bark-small f16 bench file per context length, timed with the library's CUDA-event profiler
+(bark_b200_profile_report).  Writes $BARK_TOOLS_OUT/decode_bench.json.
 """
 import json
 import os
@@ -30,9 +31,11 @@ def main():
         pasts = [int(v) for v in args[1].split(",")]; args = args[2:]
     out = []
     rng = np.random.default_rng(0)
-    for item in args or ["40:500:0"]:
-        poll, first, att = (int(v) for v in item.split(":"))
-        os.environ["BARK_B200_POLL_NS"], os.environ["BARK_B200_POLL_FIRST_NS"], os.environ["BARK_B200_POLL_ATT_NS"] = str(poll), str(first), str(att)
+    for item in args or ["40"]:
+        poll, _, headstart = item.partition("/")
+        os.environ["BARK_B200_POLL_NS"] = poll
+        if headstart: os.environ["BARK_B200_HEADSTART"] = headstart
+        else: os.environ.pop("BARK_B200_HEADSTART", None)
         with pkg.Bark(path) as b:
             for n_past in pasts:
                 toks = rng.integers(10000, 12048, n_past).astype(np.int32)
@@ -46,8 +49,8 @@ def main():
                 pkg.profile_enable(False)
                 v = rep.get("gpt_decode_step_kernel") or rep["gpt_decode_cluster_kernel"]
                 us = v["ms"] * 1e3 / v["launches"]
-                out.append(dict(poll_ns=poll, first_ns=first, att_ns=att, n_kv_start=n_past + 6, us_per_token=round(us, 2), launches=v["launches"]))
-                print(f"poll {poll:5d} first {first:5d} att {att:5d}  n_kv {n_past + 6:4d}..{p:4d}: {us:7.2f} us per decode step", flush=True)
+                out.append(dict(poll_ns=int(poll), headstart=headstart or "default", n_kv_start=n_past + 6, us_per_token=round(us, 2), launches=v["launches"]))
+                print(f"poll {poll:>5s} headstart {headstart or 'default'}  n_kv {n_past + 6:4d}..{p:4d}: {us:7.2f} us per decode step", flush=True)
     os.makedirs(OUT, exist_ok=True)
     json.dump(out, open(os.path.join(OUT, "decode_bench.json"), "w"), indent=1)
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-phase globaltimer stamps of the persistent decode kernel (BARK_B200_DECODE_TIMING=1), on an H100.
 
-usage: python tools/decode_timing.py [--sweep tid:poll_ns[:first_ns],...] [n_past ...]   (coarse model, bark-small f16 bench file;
+usage: python tools/decode_timing.py [--sweep tid:poll_ns,...] [n_past ...]   (coarse model, bark-small f16 bench file;
        tid = stamping thread (lane 0 of a warp), poll_ns = back-off between polls of the tagged exchange words)
 Prints, per n_past: the time between consecutive stamps on CTA 0 (median over layers) and, at layer 5, the spread over CTAs
 of each stamp.  The raw [256][32] dump is saved to $BARK_TOOLS_OUT/decode_timing_<n_kv>.npy.  Stamp ids: decode_kernels.cu tstamp().
@@ -31,30 +31,24 @@ NAMES = {0: "layer start", 1: "LN1 mean", 2: "LN1 done", 3: "QKV rows ready (mba
 SUMMARY = []
 
 
-def measure(pkg, path, pasts, tid, poll, first=0):
+def measure(pkg, path, pasts, tid, poll):
     os.environ["BARK_B200_DECODE_TIMING_TID"] = str(tid)
     os.environ["BARK_B200_POLL_NS"] = str(poll)
-    os.environ["BARK_B200_POLL_FIRST_NS"] = str(first)
     rng = np.random.default_rng(0)
     with pkg.Bark(path) as b:
         L = int(b.hparams(1)[0])
         for n_past in pasts:
             toks = rng.integers(10000, 12048, n_past).astype(np.int32)
             _, p = b.gpt_eval(1, toks, 0, False)
-            for _ in range(int(os.environ.get("WARM_STEPS", "48"))):   # warm (the adaptive head starts settle within ~20 tokens), then keep the last step's stamps
+            for _ in range(int(os.environ.get("WARM_STEPS", "48"))):   # warm, then keep the last step's stamps
                 _, p = b.gpt_eval(1, np.array([10001], np.int32), p, False)
             t = np.zeros(256 * 32, np.uint64)
             pkg.lib().bark_b200_decode_timing(b.ctx, t.ctypes.data_as(C.c_void_p), t.size)
             t = t.reshape(256, 32).astype(np.int64)
-            ad = np.zeros(132 * 8, np.uint32)
-            if pkg.lib().bark_b200_decode_adapt(b.ctx, 1, ad.ctypes.data_as(C.c_void_p), ad.size) > 0:
-                ad = ad.reshape(132, 8)
-                print("   adaptive head starts (ns), median over CTAs [q, att, x1, ff, x2, scores]:", np.median(ad[:, :6], axis=0).astype(int).tolist(),
-                      " soft_max CTAs (0..47):", np.median(ad[:48, :6], axis=0).astype(int).tolist())
-            tag = f"tid{tid}_poll{poll}_first{first}"
+            tag = f"tid{tid}_poll{poll}"
             np.save(os.path.join(OUT, f"decode_timing_{p}_{tag}.npy"), t)
             lay = t[:L + 1]
-            SUMMARY.append(dict(tid=tid, poll_ns=poll, first_ns=first, n_kv=int(p), us_per_layer=float((lay[L, 0] - lay[0, 0]) / 1e3 / L)))
+            SUMMARY.append(dict(tid=tid, poll_ns=poll, n_kv=int(p), us_per_layer=float((lay[L, 0] - lay[0, 0]) / 1e3 / L)))
             print(f"== [{tag}] n_kv {p}: {(lay[L, 0] - lay[0, 0]) / 1e3:.1f} us for {L} layers on CTA 0 ({(lay[L, 0] - lay[0, 0]) / 1e3 / L:.2f} us per layer)")
             used = [i for i in range(32) if lay[1, i] != 0]
             for a, c in zip(used[:-1], used[1:]):
