@@ -51,6 +51,7 @@ EXPORTS = [
     "bark_b200_profile_enable", "bark_b200_profile_report", "bark_b200_io_counters", "bark_b200_decode_timing",
     "bark_b200_shard_init", "bark_b200_shard_connect", "bark_b200_shard_nvlink_bytes",
     "bark_b200_fast_mode", "bark_b200_fast_gemm", "bark_b200_fast_attention",
+    "bark_b200_generate_batch", "bark_b200_batch_audio", "bark_b200_batch_tokens", "bark_b200_gpt_eval_slot", "bark_b200_gpt_step_batch",
     "ggml_time_init", "ggml_time_us", "ggml_time_ms", "ggml_init", "ggml_free",
 ]
 
@@ -126,6 +127,16 @@ def lib() -> C.CDLL:
     L.bark_b200_fast_gemm.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
     L.bark_b200_fast_attention.restype = C.c_int
     L.bark_b200_fast_attention.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int]
+    L.bark_b200_generate_batch.restype = C.c_bool
+    L.bark_b200_generate_batch.argtypes = [vp, C.POINTER(C.c_char_p), C.POINTER(C.c_uint32), C.c_int, C.c_int]
+    L.bark_b200_batch_audio.restype = C.c_int
+    L.bark_b200_batch_audio.argtypes = [vp, C.c_int, f32p, C.c_int]
+    L.bark_b200_batch_tokens.restype = C.c_int
+    L.bark_b200_batch_tokens.argtypes = [vp, C.c_int, C.c_int, i32p, C.c_int]
+    L.bark_b200_gpt_eval_slot.restype = C.c_int
+    L.bark_b200_gpt_eval_slot.argtypes = [vp, C.c_int, C.c_int, i32p, C.c_int, C.POINTER(C.c_int), C.c_int, f32p]
+    L.bark_b200_gpt_step_batch.restype = C.c_int
+    L.bark_b200_gpt_step_batch.argtypes = [vp, C.c_int, C.c_int, i32p, i32p, i32p, f32p]
     L.ggml_time_us.restype = C.c_int64
     _lib = L
     return L
@@ -215,6 +226,54 @@ class Bark:
         if not lib().bark_b200_gpt_eval(self.ctx, which, _p(t), t.size, C.byref(np_), int(merge_ctx), _p(out)):
             raise RuntimeError("bark_b200_gpt_eval failed")
         return out, np_.value
+
+    def gpt_eval_slot(self, which: int, slot: int, tokens, n_past: int, merge_ctx: bool):
+        """gpt_eval on batch slot `slot`'s KV cache (0..7) instead of the model's own; returns (logits, n_past)."""
+        t = np.ascontiguousarray(tokens, np.int32)
+        out = np.zeros(int(self.hparams(which)[6]), np.float32)
+        np_ = C.c_int(n_past)
+        if not lib().bark_b200_gpt_eval_slot(self.ctx, which, slot, _p(t), t.size, C.byref(np_), int(merge_ctx), _p(out)):
+            raise RuntimeError("bark_b200_gpt_eval_slot failed")
+        return out, np_.value
+
+    def gpt_step_batch(self, which: int, slots, tokens, n_past):
+        """One batched decode step: row r feeds tokens[r] at position n_past[r] through slot slots[r]'s cache.
+        Returns (logits [B][n_out], the advanced n_past)."""
+        sl = np.ascontiguousarray(slots, np.int32); t = np.ascontiguousarray(tokens, np.int32)
+        npa = np.array(n_past, np.int32, copy=True)
+        assert sl.size == t.size == npa.size
+        out = np.zeros((sl.size, int(self.hparams(which)[6])), np.float32)
+        if not lib().bark_b200_gpt_step_batch(self.ctx, which, sl.size, _p(sl), _p(t), _p(npa), _p(out)):
+            raise RuntimeError("bark_b200_gpt_step_batch failed")
+        return out, npa
+
+    def generate_batch(self, texts, seeds, n_threads: int = 1) -> list:
+        """Up to 8 prompts decoded together; item i equals a fresh context's generate(texts[i]) with seed seeds[i].
+        Returns the waveforms; batch_tokens(i, stage) gives the ids."""
+        n = len(texts)
+        if len(seeds) != n:
+            raise RuntimeError(f"generate_batch: {n} prompts but {len(seeds)} seeds")
+        arr = (C.c_char_p * max(n, 1))(*[t.encode() for t in texts])
+        sd = (C.c_uint32 * max(n, 1))(*[int(s) for s in seeds])
+        if not lib().bark_b200_generate_batch(self.ctx, arr, sd, n, n_threads):
+            raise RuntimeError("bark_b200_generate_batch failed")
+        out = []
+        for i in range(n):
+            m = lib().bark_b200_batch_audio(self.ctx, i, None, 0)
+            a = np.zeros(max(m, 1), np.float32)
+            lib().bark_b200_batch_audio(self.ctx, i, _p(a), m)
+            out.append(a[:m])
+        return out
+
+    def batch_tokens(self, i: int, stage: int) -> np.ndarray:
+        """Ids of item i of the last batch, shaped like tokens(stage)."""
+        n = lib().bark_b200_batch_tokens(self.ctx, i, stage, None, 0)
+        if n < 0:
+            raise IndexError(f"no batch item {i}")
+        a = np.zeros(max(n, 1), np.int32)
+        lib().bark_b200_batch_tokens(self.ctx, i, stage, _p(a), n)
+        a = a[:n]
+        return a.reshape(-1, 2) if stage == 1 else a.reshape(-1, 8) if stage == 2 else a
 
     def fine_eval(self, in_buffer, nn: int) -> np.ndarray:
         t = np.ascontiguousarray(in_buffer, np.int32)

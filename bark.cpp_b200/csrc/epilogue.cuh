@@ -34,6 +34,17 @@ __device__ __forceinline__ float gelu_lookup(const __half * __restrict__ tab, fl
     return __half2float(tab[__half_as_ushort(__float2half_rn(x))]);
 }
 
+// P.V: the columns past the last full round of 32 lane chains (n_kv & ~31 .. n_kv), folded into the chains' reduced sum in the order
+// the pinned build compiles vec_dot_f32's leftovers (oracle/bark_oracle.c orc_vec_dot_f32): runs of 8 and 4 multiply-then-add, then
+// fused multiply-adds.  v: the V column (stride E), p: the probability row.
+__device__ __forceinline__ float pv_leftovers(float sum, const float * __restrict__ v, const float * __restrict__ p, int np, int n_kv, int E) {
+    int i = np, r = n_kv - np;
+    while (r >= 8) { for (int l = 0; l < 8; l++) sum = __fadd_rn(sum, __fmul_rn(__ldg(v + (size_t)(i + l) * E), __ldg(p + i + l))); i += 8; r -= 8; }
+    if (r >= 4)    { for (int l = 0; l < 4; l++) sum = __fadd_rn(sum, __fmul_rn(__ldg(v + (size_t)(i + l) * E), __ldg(p + i + l))); i += 4; r -= 4; }
+    for (; r > 0; r--, i++) sum = __fmaf_rn(__ldg(v + (size_t) i * E), __ldg(p + i), sum);
+    return sum;
+}
+
 __device__ __forceinline__ void matmul_epilogue(const MatmulEpilogue & ep, int m, int o, float r) {
     switch (ep.mode) {
         case EPI_STORE: ep.out[(size_t) m * ep.ldo + o] = r; break;

@@ -279,13 +279,7 @@ __global__ void __launch_bounds__(256) attn_pv_tiled_kernel(const float * __rest
     const float * p = S + ((size_t) h * N + q) * n_kv;
 #pragma unroll
     for (int j = 0; j < 2; j++) {
-        float sum = acc[j];
-        const float * v = Vc + h * D + d + j;
-        int i = np, r = n_kv - np;                                                    // leftovers as compiled in the pinned build (orc_vec_dot_f32)
-        while (r >= 8) { for (int l = 0; l < 8; l++) sum = __fadd_rn(sum, __fmul_rn(__ldg(v + (size_t)(i + l) * E), __ldg(p + i + l))); i += 8; r -= 8; }
-        if (r >= 4)    { for (int l = 0; l < 4; l++) sum = __fadd_rn(sum, __fmul_rn(__ldg(v + (size_t)(i + l) * E), __ldg(p + i + l))); i += 4; r -= 4; }
-        for (; r > 0; r--, i++) sum = __fmaf_rn(__ldg(v + (size_t) i * E), __ldg(p + i), sum);
-        store_act(act, wt, Kp, q, h * D + d + j, sum);
+        store_act(act, wt, Kp, q, h * D + d + j, pv_leftovers(acc[j], Vc + h * D + d + j, p, np, n_kv, E));
     }
 }
 

@@ -18,10 +18,15 @@ int64_t now_us() {
 }
 
 
+// The rows of a batched decode step (gpt_step_batch): row b belongs to its own sequence, with its own KV cache and position.
+struct BatchRows { float * const * slot_k, * const * slot_v; const int32_t * d_pos; int max_kv; };
+
 // transformer body shared by the causal and the fine model; x [N][E] is updated in place.
-// K/V rows of this call go to k_dst/v_dst (KV-cache slot of position n_past, or the fine model's scratch),
-// attention then reads n_kv rows starting at k_all/v_all.
-static void run_layers(bark_context * ctx, GPTModel & m, int N, int n_past, bool causal) {
+// K/V rows of this call go to k_dst/v_dst (KV-cache slot of position n_past in mem_k / mem_v, or the fine model's scratch),
+// attention then reads n_kv rows starting at k_all/v_all.  batch: N rows of N sequences; their K/V rows are staged in
+// ws.kbuf / ws.vbuf and the batched attention appends each to its own cache.
+static void run_layers(bark_context * ctx, GPTModel & m, int N, int n_past, bool causal, float * mem_k = nullptr, float * mem_v = nullptr,
+                       const BatchRows * batch = nullptr) {
     Workspace & ws = ctx->ws;
     cudaStream_t s = ctx->stream;
     const int E = m.n_embd, H = m.n_head;
@@ -33,15 +38,23 @@ static void run_layers(bark_context * ctx, GPTModel & m, int N, int n_past, bool
         const GPTLayer & L = m.layers[(size_t) il];
         layernorm_act(ws.x, N, E, L.ln_1_g, L.ln_1_b, ws.act, awt, kpE, ctx->d_ln_fallbacks, s);
         float * k_all, * v_all, * k_dst, * v_dst; int n_kv;
-        if (causal) {
-            k_all = m.mem_k + (size_t) il * m.block_size * E; v_all = m.mem_v + (size_t) il * m.block_size * E;
+        if (batch) {
+            k_all = k_dst = ws.kbuf; v_all = v_dst = ws.vbuf; n_kv = 0;
+        } else if (causal) {
+            k_all = mem_k + (size_t) il * m.block_size * E; v_all = mem_v + (size_t) il * m.block_size * E;
             k_dst = k_all + (size_t) n_past * E; v_dst = v_all + (size_t) n_past * E; n_kv = n_past + N;      // bark.cpp:1294-1300
         } else {
             k_all = k_dst = ws.kbuf; v_all = v_dst = ws.vbuf; n_kv = N;
         }
         MatmulEpilogue qkv; qkv.mode = EPI_QKV; qkv.out = ws.q; qkv.ldo = E; qkv.k_out = k_dst; qkv.v_out = v_dst;
         lane_matmul(L.c_attn, ws.act, kpE, N, qkv, s);
-        attention(ws.q, k_all, v_all, N, n_kv, n_past, E, H, causal, ws.scores, ws.act, awt, kpE, s);
+        if (batch) {
+            BatchKV kv;
+            for (int b = 0; b < N; b++) { kv.k[b] = batch->slot_k[b] + (size_t) il * m.block_size * E; kv.v[b] = batch->slot_v[b] + (size_t) il * m.block_size * E; }
+            attention_batch(ws.q, ws.kbuf, ws.vbuf, kv, batch->d_pos, N, batch->max_kv, E, H, ws.scores, ws.act, awt, kpE, s);
+        } else {
+            attention(ws.q, k_all, v_all, N, n_kv, n_past, E, H, causal, ws.scores, ws.act, awt, kpE, s);
+        }
         MatmulEpilogue res; res.mode = EPI_RESID; res.out = ws.x; res.ldo = E;
         lane_matmul(L.c_proj, ws.act, kpE, N, res, s);                                                                  // + inpL
         layernorm_act(ws.x, N, E, L.ln_2_g, L.ln_2_b, ws.act, awt, kpE, ctx->d_ln_fallbacks, s);
@@ -88,7 +101,7 @@ void build_decode_tables(bark_context * ctx, GPTModel & m) {
 }
 
 // one decode token through the persistent kernel
-static void decode_step(bark_context * ctx, GPTModel & m, int token, const int32_t * d_token, int n_past, int lm_lo, int lm_hi) {
+static void decode_step(bark_context * ctx, GPTModel & m, int token, const int32_t * d_token, int n_past, int lm_lo, int lm_hi, float * mem_k, float * mem_v) {
     // Epochs are 32-bit and must never repeat while a stale word could still carry the old value (~30 M tokens for 24 layers):
     // before the counter wraps, drain the stream, clear every exchange word (epoch 0 = never published) and start over.
     const unsigned step_tags = (unsigned) decode_tags_per_step(m.n_layer);
@@ -107,7 +120,7 @@ static void decode_step(bark_context * ctx, GPTModel & m, int token, const int32
     DecodeArgs a{};
     a.phases = (const DecodePhase *) m.d_phases; a.layer_vecs = (const DecodeLayerVec *) m.d_layer_vecs;
     a.wte = m.wte[0]; a.wpe = m.wpe; a.ln_f_g = m.ln_f_g; a.ln_f_b = m.ln_f_b; a.gelu_tab = ctx->d_gelu_tab;
-    a.mem_k = m.mem_k; a.mem_v = m.mem_v;
+    a.mem_k = mem_k; a.mem_v = mem_v;
     a.gx = m.gx; a.gq = m.gq; a.gk = m.gk; a.gv = m.gv; a.gatt = m.gatt; a.gff = m.gff; a.gscores = m.gscores; a.logits = m.glogits;
     a.tag_base = ctx->tag_base; a.ln_fallbacks = ctx->d_ln_fallbacks; a.timing = ctx->d_timing;
     a.E = m.n_embd; a.H = m.n_head; a.L = m.n_layer; a.block_size = m.block_size; a.n_past = n_past; a.token = token; a.lm_lo = lm_lo; a.lm_hi = lm_hi;
@@ -126,8 +139,10 @@ static void decode_step(bark_context * ctx, GPTModel & m, int token, const int32
     ctx->tag_base += (unsigned) decode_tags_per_step(m.n_layer);
 }
 
-bool gpt_eval(bark_context * ctx, GPTModel & m, const int32_t * tokens, int n, int * n_past, bool merge_ctx, float * logits_host, int lm_lo, int lm_hi) {
+bool gpt_eval(bark_context * ctx, GPTModel & m, const int32_t * tokens, int n, int * n_past, bool merge_ctx, float * logits_host, int lm_lo, int lm_hi,
+              float * mem_k, float * mem_v) {
     if (!n_past) { fprintf(stderr, "%s: n_past is null\n", __func__); return false; }
+    if (!mem_k || !mem_v) { mem_k = m.mem_k; mem_v = m.mem_v; }
     const int64_t t0 = now_us();
     Workspace & ws = ctx->ws;
     cudaStream_t s = ctx->stream;
@@ -141,7 +156,7 @@ bool gpt_eval(bark_context * ctx, GPTModel & m, const int32_t * tokens, int n, i
     }
     if (*n_past > 0 && N == 1) {
         if (ctx->use_decode_kernel && m.decode_ok && *n_past + 1 <= m.block_size) {
-            decode_step(ctx, m, tokens[0], nullptr, *n_past, lm_lo, lm_hi);
+            decode_step(ctx, m, tokens[0], nullptr, *n_past, lm_lo, lm_hi, mem_k, mem_v);
             ctx->last_logits = m.glogits;
             if (logits_host) {
                 const size_t nb = (size_t)(lm_hi - lm_lo) * sizeof(float);
@@ -161,7 +176,7 @@ bool gpt_eval(bark_context * ctx, GPTModel & m, const int32_t * tokens, int n, i
     memcpy(ctx->h_tok, tokens, (size_t) n * sizeof(int32_t));
     BARK_CUDA_CHECK(cudaMemcpyAsync(ws.tok, ctx->h_tok, (size_t) n * sizeof(int32_t), cudaMemcpyHostToDevice, s)); g_h2d_bytes += (size_t) n * sizeof(int32_t);
     gpt_embed_causal(m, ws.tok, N, *n_past, merge, ws.x, s);
-    run_layers(ctx, m, N, *n_past, true);
+    run_layers(ctx, m, N, *n_past, true, mem_k, mem_v);
     // final norm + lm_head on the last position only (bark.cpp:1391-1405)
     const int kpE = is_quant(m.wtype) ? E : ws.max_rows * kGmGroup;
     layernorm_act(ws.x + (size_t)(N - 1) * E, 1, E, m.ln_f_g, m.ln_f_b, ws.act, is_quant(m.wtype) ? W_Q4_0 : m.wtype, kpE, ctx->d_ln_fallbacks, s);
@@ -178,13 +193,56 @@ bool gpt_eval(bark_context * ctx, GPTModel & m, const int32_t * tokens, int n, i
     return true;
 }
 
+// Output rows [lo, hi) of W as a matrix of their own.  Every output of a mat-mul is its own dot product, so the slice computes
+// the same values as the full matrix.  (Few-row kernels only: the group-major copy is not sliced.)
+static DMat output_rows(const DMat & W, int lo, int hi) {
+    DMat d = W;
+    d.n_out = hi - lo; d.p_gm = nullptr; d.p_rm = nullptr;
+    const size_t nb = (size_t) W.K / 32, r = (size_t) lo;
+    auto at = [](void * p, size_t bytes) { return p ? (void *)((unsigned char *) p + bytes) : nullptr; };
+    if (W.type == W_F16 || W.type == W_F32) { d.p = at(W.p, r * W.Kp * (W.type == W_F16 ? 2 : 4)); return d; }
+    d.p = at(W.p, r * nb * (W.type == W_Q8_0 ? 32 : 16));             // q4_0 nibble words / qx codes
+    d.scales = at(W.scales, r * nb * 2); d.mins = at(W.mins, r * nb * 2); d.qh = at(W.qh, r * nb * 4);
+    return d;
+}
+
+bool gpt_step_batch(bark_context * ctx, GPTModel & m, int B, float * const * slot_k, float * const * slot_v, const int32_t * tokens, const int * n_past,
+                    int lm_lo, int lm_hi, float * d_logits) {
+    const int64_t t0 = now_us();
+    Workspace & ws = ctx->ws;
+    cudaStream_t s = ctx->stream;
+    const int E = m.n_embd, D = E / m.n_head;
+    if (B < 1 || B > 8) { fprintf(stderr, "%s: %d rows (1 to 8)\n", __func__, B); return false; }
+    if (D % 32 || D > 128) { fprintf(stderr, "%s: unsupported head size %d (need a multiple of 32, <= 128)\n", __func__, D); return false; }
+    if (lm_hi <= 0 || lm_hi > m.n_out_vocab || lm_lo < 0 || lm_lo >= lm_hi) { lm_lo = 0; lm_hi = m.n_out_vocab; }
+    int max_kv = 0;
+    for (int b = 0; b < B; b++) {
+        if (tokens[b] < 0 || tokens[b] >= m.n_in_vocab) { fprintf(stderr, "%s: token id %d of row %d is outside the model's input vocabulary (%d)\n", __func__, tokens[b], b, m.n_in_vocab); return false; }
+        if (n_past[b] < 0 || n_past[b] + 1 > m.block_size) { fprintf(stderr, "%s: context overflow in row %d (n_past %d + 1 > %d)\n", __func__, b, n_past[b], m.block_size); return false; }
+        max_kv = std::max(max_kv, n_past[b] + 1);
+    }
+    int32_t * h = ctx->batch.h_step, * d = ctx->batch.d_step;
+    for (int b = 0; b < B; b++) { h[b] = tokens[b]; h[8 + b] = n_past[b]; }
+    BARK_CUDA_CHECK(cudaMemcpyAsync(d, h, 16 * sizeof(int32_t), cudaMemcpyHostToDevice, s)); g_h2d_bytes += 16 * sizeof(int32_t);
+    gpt_embed_causal(m, d, B, 0, false, ws.x, s, d + 8);
+    const BatchRows rows{slot_k, slot_v, d + 8, max_kv};
+    run_layers(ctx, m, B, 0, true, nullptr, nullptr, &rows);
+    const int kpE = is_quant(m.wtype) ? E : ws.max_rows * kGmGroup;
+    layernorm_act(ws.x, B, E, m.ln_f_g, m.ln_f_b, ws.act, is_quant(m.wtype) ? W_Q4_0 : m.wtype, kpE, ctx->d_ln_fallbacks, s);
+    MatmulEpilogue st; st.mode = EPI_STORE; st.out = d_logits + lm_lo; st.ldo = m.n_out_vocab;
+    lane_matmul(output_rows(m.lm_head[0], lm_lo, lm_hi), ws.act, kpE, B, st, s);          // only the sampled window, as the decode kernel does
+    ctx->last_logits = d_logits;
+    m.t_predict_us += now_us() - t0;
+    return true;
+}
+
 // One decode step whose input token is read from device memory (the previous step's sample): nothing to wait for on the
 // host, so a whole window of steps is enqueued back to back.
 bool gpt_decode_chained(bark_context * ctx, GPTModel & m, const int32_t * d_token, int * n_past, int lm_lo, int lm_hi) {
     if (!ctx->use_decode_kernel || !m.decode_ok || *n_past < 1) { fprintf(stderr, "%s: needs the persistent decode kernel and a filled KV cache\n", __func__); return false; }
     if (*n_past + 1 > m.block_size) { fprintf(stderr, "%s: context overflow (n_past %d + 1 > %d)\n", __func__, *n_past, m.block_size); return false; }
     if (lm_hi <= 0 || lm_hi > m.n_out_vocab || lm_lo < 0 || lm_lo >= lm_hi) { lm_lo = 0; lm_hi = m.n_out_vocab; }
-    decode_step(ctx, m, 0, d_token, *n_past, lm_lo, lm_hi);
+    decode_step(ctx, m, 0, d_token, *n_past, lm_lo, lm_hi, m.mem_k, m.mem_v);
     ctx->last_logits = m.glogits;
     *n_past += 1;
     return true;
@@ -265,12 +323,12 @@ bool fine_eval_fast(bark_context * ctx, const int32_t * in_buffer, int nn, float
 // Sample `rows` tokens from device-resident logits (sampling.cu); rows the kernel could not decide bit-safely are replayed
 // on the host with the reference's exact arithmetic and the same uniform draw.  Leaves tokens (and optionally the
 // probability of the last logit) in out_tok / out_eos.  The RNG stream advances exactly as gpt_sample would advance it.
-bool sample_device(bark_context * ctx, GPTModel & m, const float * d_logits, int ld, int n, int rows, float temp, int32_t * out_tok, float * out_eos) {
+bool sample_device(bark_context * ctx, GPTModel & m, std::mt19937 & rng, const float * d_logits, int ld, int n, int rows, float temp, int32_t * out_tok, float * out_eos) {
     const int64_t t0 = now_us();
     cudaStream_t s = ctx->stream;
     if (rows < 1 || rows > 1024 || n < 2 || (size_t) n * 4 > 64 * 1024) { fprintf(stderr, "%s: unsupported shape (%d rows of %d)\n", __func__, rows, n); return false; }
     if (temp != 0.0f) {
-        for (int r = 0; r < rows; r++) ctx->h_u[r] = std::generate_canonical<double, 53>(ctx->rng);   // what discrete_distribution::operator() draws
+        for (int r = 0; r < rows; r++) ctx->h_u[r] = std::generate_canonical<double, 53>(rng);   // what discrete_distribution::operator() draws
         BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->d_u, ctx->h_u, (size_t) rows * sizeof(double), cudaMemcpyHostToDevice, s)); g_h2d_bytes += (size_t) rows * sizeof(double);
     }
     const int force = ctx->debug_flag_every > 0 && (ctx->n_sample_calls++ % ctx->debug_flag_every) == 0;
@@ -295,7 +353,7 @@ bool sample_device(bark_context * ctx, GPTModel & m, const float * d_logits, int
     return true;
 }
 
-bool codec_decode(bark_context * ctx, const int32_t * codes, int T) {
+bool codec_decode(bark_context * ctx, const int32_t * codes, int T, std::vector<float> & audio) {
     if (T < 7) { fprintf(stderr, "%s: need at least 7 frames (reflect padding of the k=7 convolutions), got %d\n", __func__, T); return false; }
     CodecModel & cm = ctx->codec;
     cudaStream_t s = ctx->stream;
@@ -333,8 +391,8 @@ bool codec_decode(bark_context * ctx, const int32_t * codes, int T) {
         std::swap(cur, t1);
     }
     conv1d(cur, C, L, cm.final_conv, true, nullptr, t1, s);           // ELU -> k7 -> [1][320 T]
-    ctx->audio.resize((size_t) L);
-    BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->audio.data(), t1, (size_t) L * sizeof(float), cudaMemcpyDeviceToHost, s)); g_d2h_bytes += (size_t) L * sizeof(float);
+    audio.resize((size_t) L);
+    BARK_CUDA_CHECK(cudaMemcpyAsync(audio.data(), t1, (size_t) L * sizeof(float), cudaMemcpyDeviceToHost, s)); g_d2h_bytes += (size_t) L * sizeof(float);
     BARK_CUDA_CHECK(cudaStreamSynchronize(s));
     return true;
 }

@@ -67,8 +67,9 @@ __device__ __forceinline__ float wte_value(const void * wte, int wt, int E, int 
 }
 
 // causal models (bark.cpp:1224-1259): one block per position
+// (pos: per-row positions of a batched decode step, else row r sits at n_past + r)
 __global__ void embed_causal_kernel(const void * __restrict__ wte, int wt, const float * __restrict__ wpe, const int32_t * __restrict__ tok,
-                                    int N, int n_past, int merge, int E, float * __restrict__ x) {
+                                    int N, int n_past, int merge, int E, float * __restrict__ x, const int32_t * __restrict__ pos) {
     const int r = blockIdx.x;
     for (int i = threadIdx.x; i < E; i += blockDim.x) {
         float v;
@@ -78,7 +79,7 @@ __global__ void embed_causal_kernel(const void * __restrict__ wte, int wt, const
         } else {
             v = wte_value(wte, wt, E, tok[r], i);
         }
-        x[(size_t) r * E + i] = __fadd_rn(v, wpe[(size_t)(r + n_past) * E + i]);
+        x[(size_t) r * E + i] = __fadd_rn(v, wpe[(size_t)(pos ? pos[r] : r + n_past) * E + i]);
     }
 }
 
@@ -94,9 +95,9 @@ __global__ void embed_fine_kernel(FineTables tabs, int wt, const float * __restr
     }
 }
 
-void gpt_embed_causal(const GPTModel & m, const int32_t * d_tok, int N, int n_past, bool merge, float * x, cudaStream_t s) {
-    if (qx_supported(m.wtype)) { qx_embed_causal(m, d_tok, N, n_past, merge, x, s); return; }
-    BARK_LAUNCH(embed_causal_kernel, N, 256, 0, s, m.wte[0], (int) m.wtype, m.wpe, d_tok, N, n_past, merge ? 1 : 0, m.n_embd, x);
+void gpt_embed_causal(const GPTModel & m, const int32_t * d_tok, int N, int n_past, bool merge, float * x, cudaStream_t s, const int32_t * d_pos) {
+    if (qx_supported(m.wtype)) { qx_embed_causal(m, d_tok, N, n_past, merge, x, s, d_pos); return; }
+    BARK_LAUNCH(embed_causal_kernel, N, 256, 0, s, m.wte[0], (int) m.wtype, m.wpe, d_tok, N, n_past, merge ? 1 : 0, m.n_embd, x, d_pos);
 }
 void gpt_embed_fine(const GPTModel & m, const int32_t * d_ids, int nn, float * x, cudaStream_t s, int row0, int rows) {
     if (qx_supported(m.wtype)) { qx_embed_fine(m, d_ids, nn, x, s); return; }
@@ -274,12 +275,9 @@ __global__ void attn_scores_kernel(const float * __restrict__ Q, const float * _
     }
 }
 
-// soft_max over one row (ggml.c:13953-14042 + ggml_vec_soft_max_f32 AVX2 branch ggml.c:2845-2888): in place
-__global__ void attn_softmax_kernel(float * __restrict__ S, int rows, int n_kv) {
+// soft_max over one row of n_kv <= 1024 by one warp (ggml.c:13953-14042 + ggml_vec_soft_max_f32 AVX2 branch ggml.c:2845-2888): in place
+__device__ __forceinline__ void softmax_row(float * __restrict__ p, int n_kv) {
     const int lane = threadIdx.x & 31;
-    const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    if (row >= rows) return;
-    float * p = S + (size_t) row * n_kv;
     float mx = __int_as_float(0xff800000);
     for (int i = lane; i < n_kv; i += 32) mx = fmaxf(mx, p[i]);
 #pragma unroll
@@ -342,6 +340,12 @@ __global__ void attn_softmax_kernel(float * __restrict__ S, int rows, int n_kv) 
     for (int i = lane; i < n_kv; i += 32) p[i] = __fmul_rn(p[i], sc);
 }
 
+__global__ void attn_softmax_kernel(float * __restrict__ S, int rows, int n_kv) {
+    const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (row >= rows) return;
+    softmax_row(S + (size_t) row * n_kv, n_kv);
+}
+
 // KQV[q][h*D+d] = vec_dot_f32(n_kv, V^T[d][:], P[q][:]) (ggml.c:2144 incl. the compiled leftover handling,
 // see oracle/bark_oracle.c orc_vec_dot_f32) -> activation operand for c_proj
 __global__ void attn_pv_kernel(const float * __restrict__ S, const float * __restrict__ Vc, int N, int n_kv, int E, int H, int D,
@@ -358,12 +362,111 @@ __global__ void attn_pv_kernel(const float * __restrict__ S, const float * __res
 #pragma unroll
         for (int l = 0; l < 32; l++) acc[l] = __fmaf_rn(v[(size_t)(k0 + l) * E], p[k0 + l], acc[l]);
     }
-    float sum = lane_tree_reduce_local(acc);
-    int i = np, r = n_kv - np;
-    while (r >= 8) { for (int l = 0; l < 8; l++) sum = __fadd_rn(sum, __fmul_rn(v[(size_t)(i + l) * E], p[i + l])); i += 8; r -= 8; }
-    if (r >= 4)    { for (int l = 0; l < 4; l++) sum = __fadd_rn(sum, __fmul_rn(v[(size_t)(i + l) * E], p[i + l])); i += 4; r -= 4; }
-    for (; r > 0; r--, i++) sum = __fmaf_rn(v[(size_t) i * E], p[i], sum);
-    store_act(act, wt, Kp, q, h * D + d, sum);
+    store_act(act, wt, Kp, q, h * D + d, pv_leftovers(lane_tree_reduce_local(acc), v, p, np, n_kv, E));
+}
+
+// ------------------------------------------------------------------------------------------------
+// batched decode attention (gpt_step_batch): row b of the step is the one new query of its own sequence, with its own KV cache
+// and n_kv = pos[b] + 1.  No two rows share keys, so the tiled kernels' query tile does not apply; the arithmetic per row is
+// theirs: the lane-chain dot + lane_tree_reduce, softmax_row, the lane-chain P.V + pv_leftovers.
+// ------------------------------------------------------------------------------------------------
+// scores[b][h][k] = vec_dot_f32(D, K_b[k][h], Q[b][h]) * scale for k <= pos[b] (nothing is masked: the query is the last position).
+// A warp takes 8 keys, a CTA 64, the grid spreads each row's keys over (n_kv + 63) / 64 CTAs.  The row's new key is read from the
+// staging buffer; the CTA with blockIdx.x == 0 also appends the head's slice of the new K and V rows to the row's cache (P.V reads
+// V from there after this launch).
+// kv.k[b] / kv.v[b] by selects: a dynamic index into a by-value kernel argument would copy the argument to the stack
+__device__ __forceinline__ float * row_cache(float * const (&p)[8], int b) {
+    float * r = p[0];
+#pragma unroll
+    for (int i = 1; i < 8; i++) if (b == i) r = p[i];
+    return r;
+}
+
+template <int DSTEPS>
+__global__ void __launch_bounds__(256) attn_scores_batch_kernel(const float * __restrict__ Q, const float * __restrict__ Kst, const float * __restrict__ Vst,
+                                                                BatchKV kv, const int32_t * __restrict__ pos, int E, int ld_s, float scale, float * __restrict__ S) {
+    constexpr int D = DSTEPS * 32;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int h = blockIdx.y, b = blockIdx.z, last = pos[b];
+    float * const Kc = row_cache(kv.k, b);
+    if (blockIdx.x == 0) {
+        float * const Vc = row_cache(kv.v, b);
+        for (int i = threadIdx.x; i < D; i += blockDim.x) {
+            Kc[(size_t) last * E + h * D + i] = Kst[(size_t) b * E + h * D + i];
+            Vc[(size_t) last * E + h * D + i] = Vst[(size_t) b * E + h * D + i];
+        }
+    }
+    const int k0 = (blockIdx.x * 8 + warp) * 8;
+    if (k0 > last) return;
+    float qv[DSTEPS], kf[8][DSTEPS];
+#pragma unroll
+    for (int c = 0; c < DSTEPS; c++) qv[c] = __ldg(Q + (size_t) b * E + h * D + c * 32 + lane);
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+        const int k = min(k0 + i, last);
+        const float * kr = (k == last ? Kst + (size_t) b * E : Kc + (size_t) k * E) + h * D;
+#pragma unroll
+        for (int c = 0; c < DSTEPS; c++) kf[i][c] = kr[c * 32 + lane];
+    }
+    float * srow = S + ((size_t) b * gridDim.y + h) * ld_s;
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+        float acc = 0.0f;
+#pragma unroll
+        for (int c = 0; c < DSTEPS; c++) acc = __fmaf_rn(kf[i][c], qv[c], acc);
+        const float r = lane_tree_reduce(acc);
+        if (lane == 0 && k0 + i <= last) srow[k0 + i] = __fmul_rn(r, scale);       // ggml_scale_inplace
+    }
+}
+
+__global__ void attn_softmax_batch_kernel(float * __restrict__ S, int rows, int H, int ld_s, const int32_t * __restrict__ pos) {
+    const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);          // row = b * H + h
+    if (row >= rows) return;
+    softmax_row(S + (size_t) row * ld_s, pos[row / H] + 1);
+}
+
+// KQV[b][h*D+d] = vec_dot_f32(n_kv, V_b^T[h*D+d], P[b][h]) -> activation operand.  One warp per CTA, grid (D / 8, head, row): each
+// warp owns 8 head columns, so the (row, head) pairs' V reads are spread over D / 8 CTAs each; lane v walks the chain k = v, v+32, ...
+// of its 8 columns (one 32-byte load of V per step).  A chain is never split, so the arithmetic is the one-CTA-per-head layout's.
+__global__ void __launch_bounds__(32) attn_pv_batch_kernel(const float * __restrict__ S, BatchKV kv, const int32_t * __restrict__ pos, int E, int D, int ld_s,
+                                                           void * __restrict__ act, int wt, int Kp) {
+    const int lane = threadIdx.x & 31;
+    const int h = blockIdx.y, b = blockIdx.z, d0 = blockIdx.x * 8;
+    const int n_kv = pos[b] + 1, np = n_kv & ~31;
+    const float * p = S + ((size_t) b * gridDim.y + h) * ld_s;
+    const float * vbase = row_cache(kv.v, b) + h * D + d0;
+    float acc[8];
+#pragma unroll
+    for (int j = 0; j < 8; j++) acc[j] = 0.0f;
+#pragma unroll 4
+    for (int k = lane; k < np; k += 32) {
+        const float4 v0 = __ldg(reinterpret_cast<const float4 *>(vbase + (size_t) k * E));
+        const float4 v1 = __ldg(reinterpret_cast<const float4 *>(vbase + (size_t) k * E) + 1);
+        const float pk = __ldg(p + k);
+        acc[0] = __fmaf_rn(v0.x, pk, acc[0]); acc[1] = __fmaf_rn(v0.y, pk, acc[1]); acc[2] = __fmaf_rn(v0.z, pk, acc[2]); acc[3] = __fmaf_rn(v0.w, pk, acc[3]);
+        acc[4] = __fmaf_rn(v1.x, pk, acc[4]); acc[5] = __fmaf_rn(v1.y, pk, acc[5]); acc[6] = __fmaf_rn(v1.z, pk, acc[6]); acc[7] = __fmaf_rn(v1.w, pk, acc[7]);
+    }
+    float mine = 0.0f;                                                              // lane j < 8 finishes column d0 + j
+#pragma unroll
+    for (int j = 0; j < 8; j++) { const float r = lane_tree_reduce(acc[j]); if (lane == j) mine = r; }
+    if (lane < 8) store_act(act, wt, Kp, b, h * D + d0 + lane, pv_leftovers(mine, vbase + lane, p, np, n_kv, E));
+}
+
+void attention_batch(const float * Q, const float * Kst, const float * Vst, const BatchKV & kv, const int32_t * d_pos, int B, int max_kv, int E, int H,
+                     float * scores, void * act, WType wt, int Kp, cudaStream_t s) {
+    const int D = E / H;
+    const float scale = 1.0f / sqrtf((float) E / (float) H);                 // bark.cpp:1318
+    const dim3 grid((max_kv + 63) / 64, H, B);
+    g_next_bytes = 4.0 * B * ((double) max_kv * E + 3.0 * E + (double) H * max_kv); g_next_flops = 2.0 * B * (double) max_kv * E;
+    if (D == 64)       BARK_LAUNCH(attn_scores_batch_kernel<2>, grid, 256, 0, s, Q, Kst, Vst, kv, d_pos, E, max_kv, scale, scores);
+    else if (D == 32)  BARK_LAUNCH(attn_scores_batch_kernel<1>, grid, 256, 0, s, Q, Kst, Vst, kv, d_pos, E, max_kv, scale, scores);
+    else if (D == 96)  BARK_LAUNCH(attn_scores_batch_kernel<3>, grid, 256, 0, s, Q, Kst, Vst, kv, d_pos, E, max_kv, scale, scores);
+    else if (D == 128) BARK_LAUNCH(attn_scores_batch_kernel<4>, grid, 256, 0, s, Q, Kst, Vst, kv, d_pos, E, max_kv, scale, scores);
+    else { fprintf(stderr, "bark_b200: unsupported head size %d (need a multiple of 32, <= 128)\n", D); throw std::runtime_error("unsupported configuration (see the message above)"); }
+    g_next_bytes = 8.0 * B * H * (double) max_kv;
+    BARK_LAUNCH(attn_softmax_batch_kernel, (B * H + 7) / 8, 256, 0, s, scores, B * H, H, max_kv, d_pos);
+    g_next_bytes = 4.0 * B * ((double) max_kv * E + (double) H * max_kv + E); g_next_flops = 2.0 * B * (double) max_kv * E;
+    BARK_LAUNCH(attn_pv_batch_kernel, dim3(D / 8, H, B), 32, 0, s, scores, kv, d_pos, E, D, max_kv, act, (int) wt, Kp);
 }
 
 void attention(const float * Q, const float * Kc, const float * Vc, int N, int n_kv, int n_past, int E, int H, bool causal,

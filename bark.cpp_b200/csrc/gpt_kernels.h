@@ -20,7 +20,8 @@ struct MatmulEpilogue {
 void permute_to_li(const void * src_rowmajor, void * dst_li, int n_out, int K, WType t, cudaStream_t s);
 void permute_to_gm(const void * src_rowmajor, void * dst_gm, int n_out, int o_pad, int K, WType t, cudaStream_t s);
 
-void gpt_embed_causal(const GPTModel & m, const int32_t * d_tok, int N, int n_past, bool merge, float * x, cudaStream_t s);
+// d_pos (device, optional): row r sits at position d_pos[r] instead of n_past + r (the rows of a batched decode step)
+void gpt_embed_causal(const GPTModel & m, const int32_t * d_tok, int N, int n_past, bool merge, float * x, cudaStream_t s, const int32_t * d_pos = nullptr);
 void gpt_embed_fine(const GPTModel & m, const int32_t * d_ids, int nn, float * x, cudaStream_t s, int row0 = 0, int rows = 1024);   // rows [row0, row0 + rows) of the window
 
 // `Kp` of the activation operands below is the GROUP STRIDE of the group-major layout (elements), not a row length
@@ -32,6 +33,13 @@ void lane_matmul(const DMat & W, const void * act, int act_gs, int rows, const M
 void attention(const float * Q, const float * Kc, const float * Vc, int N, int n_kv, int n_past, int E, int H, bool causal,
                float * scores, void * act, WType wt, int Kp, cudaStream_t s);
 
+// Decode attention for B <= 8 rows of different sequences (batched step): row b's query is Q[b], its new K / V rows are staged in
+// Kst[b] / Vst[b] and are appended to its cache (kv.k[b], kv.v[b]: the layer's [block_size][E] slab) at position d_pos[b]; it attends
+// over d_pos[b] + 1 keys.  max_kv = the largest of those.  Result -> activation operand, as attention() leaves it.
+struct BatchKV { float * k[8], * v[8]; };
+void attention_batch(const float * Q, const float * Kst, const float * Vst, const BatchKV & kv, const int32_t * d_pos, int B, int max_kv, int E, int H,
+                     float * scores, void * act, WType wt, int Kp, cudaStream_t s);
+
 // ---- q4_0 weights (q4_kernels.cu) ---------------------------------------------------------------------------------
 void q4_split(const void * raw_blocks, size_t n_blocks, void * qs, void * scales, cudaStream_t s);
 void q4_set_scratch(void * q8, void * q8_scales);      // int8 [rows][K] + f32 [rows][K/32] for the activation operand, owned by the context
@@ -42,7 +50,7 @@ bool   qx_supported(WType t);
 size_t qx_block_bytes(WType t);
 void   qx_split(const void * raw_blocks, size_t n_blocks, WType t, void * qs, void * qh, void * d, void * m, cudaStream_t s);
 void   qx_set_scratch(void * q8, void * q8_scales, void * q8_sums);
-void   qx_embed_causal(const GPTModel & m, const int32_t * d_tok, int N, int n_past, bool merge, float * x, cudaStream_t s);
+void   qx_embed_causal(const GPTModel & m, const int32_t * d_tok, int N, int n_past, bool merge, float * x, cudaStream_t s, const int32_t * d_pos);
 void   qx_embed_fine(const GPTModel & m, const int32_t * d_ids, int nn, float * x, cudaStream_t s);
 void   qx_matmul(const DMat & W, const void * act_f32, int ld_act, int rows, const MatmulEpilogue & ep, cudaStream_t s);
 

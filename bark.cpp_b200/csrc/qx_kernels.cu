@@ -31,7 +31,7 @@ __device__ __forceinline__ float wte_value_q(const void * wte, int t, int E, int
 }
 
 __global__ void embed_causal_q_kernel(const void * __restrict__ wte, int wt, const float * __restrict__ wpe, const int32_t * __restrict__ tok,
-                                      int N, int n_past, int merge, int E, float * __restrict__ x) {
+                                      int N, int n_past, int merge, int E, float * __restrict__ x, const int32_t * __restrict__ pos) {
     const int r = blockIdx.x;
     for (int i = threadIdx.x; i < E; i += blockDim.x) {
         float v;
@@ -41,7 +41,7 @@ __global__ void embed_causal_q_kernel(const void * __restrict__ wte, int wt, con
         } else {
             v = wte_value_q(wte, wt, E, tok[r], i);
         }
-        x[(size_t) r * E + i] = __fadd_rn(v, wpe[(size_t)(r + n_past) * E + i]);
+        x[(size_t) r * E + i] = __fadd_rn(v, wpe[(size_t)(pos ? pos[r] : r + n_past) * E + i]);
     }
 }
 struct FineTablesQ { const void * wte[8]; };
@@ -159,8 +159,8 @@ void qx_split(const void * raw_blocks, size_t n_blocks, WType t, void * qs, void
 
 void qx_set_scratch(void * q8, void * q8_scales, void * q8_sums) { g_qx_q8 = (int8_t *) q8; g_qx_d = (float *) q8_scales; g_qx_s = (float *) q8_sums; }
 
-void qx_embed_causal(const GPTModel & m, const int32_t * d_tok, int N, int n_past, bool merge, float * x, cudaStream_t s) {
-    BARK_LAUNCH(embed_causal_q_kernel, N, 256, 0, s, m.wte[0], (int) m.wtype, m.wpe, d_tok, N, n_past, merge ? 1 : 0, m.n_embd, x);
+void qx_embed_causal(const GPTModel & m, const int32_t * d_tok, int N, int n_past, bool merge, float * x, cudaStream_t s, const int32_t * d_pos) {
+    BARK_LAUNCH(embed_causal_q_kernel, N, 256, 0, s, m.wte[0], (int) m.wtype, m.wpe, d_tok, N, n_past, merge ? 1 : 0, m.n_embd, x, d_pos);
 }
 void qx_embed_fine(const GPTModel & m, const int32_t * d_ids, int nn, float * x, cudaStream_t s) {
     FineTablesQ t; for (int i = 0; i < 8; i++) t.wte[i] = m.wte[i];

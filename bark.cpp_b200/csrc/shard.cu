@@ -111,14 +111,14 @@ bool fine_eval_shard(bark_context * ctx, const int32_t * in_buffer, int nn) {
 
 // Samples this rank's rows with ITS slice of the window's uniforms (the host RNG advances by all 1024 draws, as the reference's
 // loop over the rows does), then gathers the 1024 ids of the pass on every rank.
-bool sample_shard(bark_context * ctx, int n, float temp, int32_t * out_all /*[1024]*/) {
+bool sample_shard(bark_context * ctx, std::mt19937 & rng, int n, float temp, int32_t * out_all /*[1024]*/) {
     GPTModel & m = ctx->fine;
     ShardState & S = ctx->shard;
     cudaStream_t s = ctx->stream;
     const int rows = 1024 / S.world, row0 = S.rank * rows;
     const int64_t t0 = now_us();
     double u_all[1024];
-    if (temp != 0.0f) for (int r = 0; r < 1024; r++) u_all[r] = std::generate_canonical<double, 53>(ctx->rng);
+    if (temp != 0.0f) for (int r = 0; r < 1024; r++) u_all[r] = std::generate_canonical<double, 53>(rng);
     memcpy(ctx->h_u, u_all + row0, (size_t) rows * sizeof(double));
     BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->d_u, ctx->h_u, (size_t) rows * sizeof(double), cudaMemcpyHostToDevice, s)); g_h2d_bytes += (size_t) rows * sizeof(double);
     sample_rows(ctx->last_logits, m.n_out_vocab, n, rows, temp, ctx->d_u, ctx->d_stok, 0, nullptr, ctx->d_seos, ctx->d_sflags, 0, s);

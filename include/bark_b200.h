@@ -69,6 +69,29 @@ BARK_API int  bark_b200_shard_init(struct bark_context * ctx, int rank, int worl
 BARK_API int  bark_b200_shard_connect(struct bark_context * ctx, const void * all_handles);
 BARK_API unsigned long long bark_b200_shard_nvlink_bytes(struct bark_context * ctx, int reset);
 
+/* BATCHED GENERATION: up to 8 prompts per context, their semantic and coarse decode steps evaluated together (one pass over the
+ * weights per step for all of them).  Item i's prompt, semantic, coarse and fine ids and waveform are bit-identical to a fresh
+ * bark_load_model(path, params, seeds[i]) followed by bark_generate_audio(ctx, texts[i]): they do not depend on n, on i's place in the
+ * batch or on the other items.  The context's own generation state is not touched: its RNG, the ids bark_b200_get_tokens returns
+ * and what bark_get_audio_data returns.  ctx->params applies to every item; the progress callback is not called during a batch.
+ * Statistics: t_eval_us and the stage times are the batch's wall time, the n_sample_* counts are summed over the items.
+ * Per-item KV caches (f32, 151 MB per item for bark-small, 402 MB for bark-large) are allocated on the first batch of n items, grown
+ * by a larger one and freed by bark_free.
+ *   bark_b200_generate_batch ... 1 <= n <= 8 prompts with their seeds; false (message on stderr) for anything else, a null text, or a
+ *                                context whose fine stage is sharded (bark_b200_shard_connect)
+ *   bark_b200_batch_audio ...... samples of item i of the last successful batch; copies min(n, cap) to out (may be NULL); -1 if no such item.
+ *                                A failed batch leaves those results and the context's statistics as they were.
+ *   bark_b200_batch_tokens ..... ids of item i; stage as bark_b200_get_tokens (0 semantic, 1 coarse [T][2], 2 fine [T][8], 3 prompt)
+ * Test hooks: the batched step on the slots' KV caches (slot 0..7, which: 0 semantic, 1 coarse, host buffers):
+ *   bark_b200_gpt_eval_slot .... bark_b200_gpt_eval on slot's cache instead of the model's own
+ *   bark_b200_gpt_step_batch ... one decode step of B distinct slots: row r feeds tokens[r] at position n_past[r] through slots[r]'s
+ *                                cache; logits_out [B][n_out_vocab]; n_past[r] advances by one */
+BARK_API bool bark_b200_generate_batch(struct bark_context * ctx, const char * const * texts, const uint32_t * seeds, int n, int n_threads);
+BARK_API int  bark_b200_batch_audio(struct bark_context * ctx, int i, float * out, int cap);
+BARK_API int  bark_b200_batch_tokens(struct bark_context * ctx, int i, int stage, int32_t * out, int cap);
+BARK_API int  bark_b200_gpt_eval_slot(struct bark_context * ctx, int which, int slot, const int32_t * tokens, int n, int * n_past, int merge_ctx, float * logits_out);
+BARK_API int  bark_b200_gpt_step_batch(struct bark_context * ctx, int which, int B, const int32_t * slots, const int32_t * tokens, int * n_past, float * logits_out);
+
 /* FAST MODE (BARK_B200_MODE=fast in the environment at load; opt-in, NOT bit-identical to the reference): the fine model's
  * 1024-row passes (bark.cpp:1416-1584) run as wgmma tensor-core GEMMs + flash-style attention (csrc/fast_kernels.cu).
  * The two kernel hooks below run on host buffers without a context, for the numerics tests:
