@@ -50,7 +50,7 @@ EXPORTS = [
     "bark_b200_get_stats", "bark_b200_get_hparams", "bark_b200_kernel_launches", "bark_b200_layernorm_fallbacks",
     "bark_b200_profile_enable", "bark_b200_profile_report", "bark_b200_io_counters", "bark_b200_decode_timing",
     "bark_b200_shard_init", "bark_b200_shard_connect", "bark_b200_shard_nvlink_bytes",
-    "bark_b200_fast_mode", "bark_b200_fast_gemm", "bark_b200_fast_attention",
+    "bark_b200_fast_mode", "bark_b200_fast_gemm", "bark_b200_fast_attention", "bark_b200_parity_attention",
     "bark_b200_generate_batch", "bark_b200_batch_audio", "bark_b200_batch_tokens", "bark_b200_gpt_eval_slot", "bark_b200_gpt_step_batch",
     "ggml_time_init", "ggml_time_us", "ggml_time_ms", "ggml_init", "ggml_free",
 ]
@@ -127,6 +127,8 @@ def lib() -> C.CDLL:
     L.bark_b200_fast_gemm.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
     L.bark_b200_fast_attention.restype = C.c_int
     L.bark_b200_fast_attention.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int]
+    L.bark_b200_parity_attention.restype = C.c_int
+    L.bark_b200_parity_attention.argtypes = [vp, vp, vp, vp] + [C.c_int] * 7
     L.bark_b200_generate_batch.restype = C.c_bool
     L.bark_b200_generate_batch.argtypes = [vp, C.POINTER(C.c_char_p), C.POINTER(C.c_uint32), C.c_int, C.c_int]
     L.bark_b200_batch_audio.restype = C.c_int
@@ -386,6 +388,22 @@ def fast_attention(q: np.ndarray, k: np.ndarray, v: np.ndarray, n_head: int) -> 
     out = np.zeros((n, E), np.float16)
     if not lib().bark_b200_fast_attention(_p(q), _p(k), _p(v), _p(out), n, E, n_head):
         raise RuntimeError("bark_b200_fast_attention failed")
+    return out
+
+
+ATTN_PATHS = {"auto": 0, "fused": 1, "tiled": 2}
+
+
+def parity_attention(q: np.ndarray, k: np.ndarray, v: np.ndarray, n_head: int, n_past: int = 0, causal: bool = False, path: str = "auto") -> np.ndarray:
+    """Bit-exact multi-row attention; q [N][E], k, v [n_kv][E] float32 -> [N][E] float32.  causal masks key j for query i when
+    j > n_past + i.  path: "auto" (what the library picks for the shape), "fused" or "tiled" (three kernels, few rows only)."""
+    q, k, v = (np.ascontiguousarray(a, np.float32) for a in (q, k, v))
+    N, E = q.shape
+    n_kv = k.shape[0]
+    assert k.shape == v.shape == (n_kv, E), (q.shape, k.shape, v.shape)
+    out = np.zeros((N, E), np.float32)
+    if not lib().bark_b200_parity_attention(_p(q), _p(k), _p(v), _p(out), N, n_kv, n_past, E, n_head, int(causal), ATTN_PATHS[path]):
+        raise RuntimeError("bark_b200_parity_attention failed")
     return out
 
 

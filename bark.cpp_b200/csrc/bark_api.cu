@@ -666,9 +666,9 @@ bool generate_batch(bark_context * ctx, const char * const * texts, const uint32
 }
 
 void alloc_workspace(bark_context * ctx) {
-    int E = 0, H = 0; size_t kp_bytes = 0, n_logits = 0;
+    int E = 0, H = 0, max_block = 0; size_t kp_bytes = 0, n_logits = 0;
     for (GPTModel * m : {&ctx->semantic, &ctx->coarse, &ctx->fine}) {
-        E = std::max(E, (int) m->n_embd); H = std::max(H, (int) m->n_head);
+        E = std::max(E, (int) m->n_embd); H = std::max(H, (int) m->n_head); max_block = std::max(max_block, (int) m->block_size);
         const size_t es = m->wtype == W_F16 ? 2 : 4;
         kp_bytes = std::max(kp_bytes, (size_t) li_padded_k(4 * m->n_embd, (int) es) * es);
     }
@@ -682,7 +682,8 @@ void alloc_workspace(bark_context * ctx) {
     ws.q    = (float *) ctx_alloc(ctx, R * E * 4);
     ws.kbuf = (float *) ctx_alloc(ctx, R * E * 4);
     ws.vbuf = (float *) ctx_alloc(ctx, R * E * 4);
-    ws.scores = (float *) ctx_alloc(ctx, (size_t) H * R * R * 4);
+    // scores of the batched decode step (<= 8 rows x H heads x max_kv) and of the three-kernel attention for few rows (gpt_kernels.h)
+    ws.scores = (float *) ctx_alloc(ctx, std::max((size_t) 8 * max_block, (size_t) attn_tiled_max_rows(H, ctx->n_sm_total) * 1024) * H * 4);
     ws.logits = (float *) ctx_alloc(ctx, n_logits * 4);
     ws.tok  = (int32_t *) ctx_alloc(ctx, 8 * 1024 * 4);
     if (is_quant(ctx->semantic.wtype) || is_quant(ctx->coarse.wtype) || is_quant(ctx->fine.wtype)) {
@@ -1019,6 +1020,40 @@ static int bark_b200_fast_attention_impl(const uint16_t * q, const uint16_t * k,
 }
 extern "C" int bark_b200_fast_attention(const uint16_t * q, const uint16_t * k, const uint16_t * v, uint16_t * out, int n, int E, int H) { return guarded((int) 0, [&] { return bark_b200_fast_attention_impl(q, k, v, out, n, E, H); }); }
 extern "C" int bark_b200_fast_mode(struct bark_context * ctx) { return ctx && ctx->fast_mode ? 1 : 0; }
+// parity-path attention on host f32 buffers (tests, tools/attn_bench.py): the result is written as f32 rows [N][E], the operand form
+// store_act produces for quantised weights.  path: 0 = as attention() chooses for this shape, 1 = attn_fused_kernel, 2 = three kernels.
+static int bark_b200_parity_attention_impl(const float * q, const float * k, const float * v, float * out, int N, int n_kv, int n_past, int E, int H,
+                                           int causal, int path) {
+    if (!q || !k || !v || !out || N < 1 || n_kv < 1 || n_kv > 1024 || n_past < 0 || H < 1 || E % H || path < 0 || path > 2) return 0;
+    const int D = E / H;
+    if (D % 32 || D > 128) return 0;
+    struct Buffers {                                          // freed on every exit, including a CUDA failure thrown mid-way
+        float * p[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+        ~Buffers() { for (float * b : p) cudaFree(b); }
+    } d;
+    float *& dq = d.p[0], *& dk = d.p[1], *& dv = d.p[2], *& dout = d.p[3], *& dsc = d.p[4];
+    BARK_CUDA_CHECK(cudaMalloc(&dq, (size_t) N * E * 4)); BARK_CUDA_CHECK(cudaMalloc(&dk, (size_t) n_kv * E * 4));
+    BARK_CUDA_CHECK(cudaMalloc(&dv, (size_t) n_kv * E * 4)); BARK_CUDA_CHECK(cudaMalloc(&dout, (size_t) N * E * 4));
+    BARK_CUDA_CHECK(cudaMalloc(&dsc, (size_t) H * N * n_kv * 4));
+    BARK_CUDA_CHECK(cudaMemcpy(dq, q, (size_t) N * E * 4, cudaMemcpyHostToDevice)); BARK_CUDA_CHECK(cudaMemcpy(dk, k, (size_t) n_kv * E * 4, cudaMemcpyHostToDevice));
+    BARK_CUDA_CHECK(cudaMemcpy(dv, v, (size_t) n_kv * E * 4, cudaMemcpyHostToDevice));
+    BARK_CUDA_CHECK(cudaMemset(dout, 0xff, (size_t) N * E * 4));          // NaN: a missing store shows up
+    if (path == ATTN_TILED) {                                 // the three kernels' row limit is the score buffer's, which this call sizes itself
+        int dev = 0, n_sm = 0;
+        BARK_CUDA_CHECK(cudaGetDevice(&dev)); BARK_CUDA_CHECK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
+        if (N > attn_tiled_max_rows(H, n_sm)) return 0;
+    }
+    attention(dq, dk, dv, N, n_kv, n_past, E, H, causal != 0, dsc, dout, W_Q4_0, E, 0, (AttnPath) path);
+    BARK_CUDA_CHECK(cudaGetLastError());                      // a launch the configuration rejects
+    const cudaError_t e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) { fprintf(stderr, "bark_b200_parity_attention: %s\n", cudaGetErrorString(e)); return 0; }
+    BARK_CUDA_CHECK(cudaMemcpy(out, dout, (size_t) N * E * 4, cudaMemcpyDeviceToHost));
+    return 1;
+}
+extern "C" int bark_b200_parity_attention(const float * q, const float * k, const float * v, float * out, int N, int n_kv, int n_past, int E, int H, int causal,
+                                          int path) {
+    return guarded((int) 0, [&] { return bark_b200_parity_attention_impl(q, k, v, out, N, n_kv, n_past, E, H, causal, path); });
+}
 
 // batched generation (include/bark_b200.h)
 extern "C" bool bark_b200_generate_batch(struct bark_context * ctx, const char * const * texts, const uint32_t * seeds, int n, int n_threads) {

@@ -1,5 +1,5 @@
-// Device-side pieces shared by the mat-mul kernels: activation-operand writers, operand unpacking, GELU table lookup
-// and the mat-mul epilogues.
+// Device-side pieces shared by the mat-mul and attention kernels: activation-operand writers, operand unpacking, GELU table lookup,
+// the attention soft_max and P.V leftovers, and the mat-mul epilogues.
 #pragma once
 #include "gpt_kernels.h"
 
@@ -34,14 +34,79 @@ __device__ __forceinline__ float gelu_lookup(const __half * __restrict__ tab, fl
     return __half2float(tab[__half_as_ushort(__float2half_rn(x))]);
 }
 
+// soft_max over one row of n_kv <= 1024 by one warp (ggml.c:13953-14042 + ggml_vec_soft_max_f32 AVX2 branch ggml.c:2845-2888): in place
+__device__ __forceinline__ void softmax_row(float * __restrict__ p, int n_kv) {
+    const int lane = threadIdx.x & 31;
+    float mx = __int_as_float(0xff800000);
+    for (int i = lane; i < n_kv; i += 32) mx = fmaxf(mx, p[i]);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    const int nchunks = n_kv >> 3;
+    float csum[4] = {0.f, 0.f, 0.f, 0.f};                                    // chunk c is owned by lane c%32, slot c/32 (n_kv <= 1024)
+#pragma unroll
+    for (int slot = 0; slot < 4; slot++) {
+        const int c = slot * 32 + lane;
+        if (c < nchunks) {
+            float v[8];
+#pragma unroll
+            for (int l = 0; l < 8; l++) { v[l] = ggml_v_expf_dev(__fsub_rn(p[c * 8 + l], mx)); }
+#pragma unroll
+            for (int l = 0; l < 8; l++) p[c * 8 + l] = v[l];
+            const float t0 = __fadd_rn(v[4], v[0]), t1 = __fadd_rn(v[5], v[1]), t2 = __fadd_rn(v[6], v[2]), t3 = __fadd_rn(v[7], v[3]);
+            csum[slot] = __fadd_rn(__fadd_rn(t0, t2), __fadd_rn(t1, t3));
+        }
+    }
+    // The reference accumulates the chunk sums sequentially in double, then the tail (ggml.c:2845-2888).  All terms are positive, so a
+    // tree sum S brackets the sequential one within +-2n*2^-53*S: if 1/sum rounds to the same float at both ends of the bracket the
+    // order cannot matter (the persistent decode step decides the same way); otherwise replay the sequential chain (128 dependent
+    // shuffle + add steps per row: it used to run for every row).
+    for (int i = nchunks * 8; i < n_kv; i++) {                                // scalar tail through libm expf
+        const float val = glibc_expf_dev(__fsub_rn(p[i], mx));
+        if (lane == 0) p[i] = val;
+    }
+    __syncwarp();
+    double tsum = 0.0;
+#pragma unroll
+    for (int slot = 0; slot < 4; slot++) tsum += (double) csum[slot];         // (zero where this lane owns no chunk)
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) tsum += __shfl_xor_sync(0xffffffffu, tsum, o);
+    float sc;
+    {
+        const double dl = 2.0 * (double)(nchunks + 8) * 0x1p-53 * tsum * (1.0 + 1e-6);
+        double lo = tsum - dl, hi = tsum + dl;
+        for (int i = nchunks * 8; i < n_kv; i++) { const double tl = (double) p[i]; lo = __dadd_rn(lo, tl); hi = __dadd_rn(hi, tl); }
+        const double mid = 0.5 * (lo + hi);
+        double y = (double) __frcp_rn((float) mid);                          // 1/mid to ~2^-50: float seed + 2 Newton steps
+        double e = __fma_rn(-mid, y, 1.0); y = __fma_rn(y, e, y);
+        e = __fma_rn(-mid, y, 1.0);        y = __fma_rn(y, e, y);
+        const double rw = (hi - lo) * y * 0.5 + 0x1p-48;
+        sc = __double2float_rn(y * (1.0 - rw));
+        if (sc != __double2float_rn(y * (1.0 + rw))) {                        // rare: the reference's own order
+            double sum = 0.0;
+#pragma unroll
+            for (int slot = 0; slot < 4; slot++) {
+                const int base = slot * 32;
+                if (base < nchunks) {
+                    const int cnt = min(32, nchunks - base);
+                    for (int l = 0; l < cnt; l++) sum = __dadd_rn(sum, (double) __shfl_sync(0xffffffffu, csum[slot], l));
+                }
+            }
+            for (int i = nchunks * 8; i < n_kv; i++) sum = __dadd_rn(sum, (double) p[i]);
+            sc = __double2float_rn(__ddiv_rn(1.0, sum));
+        }
+    }
+    __syncwarp();
+    for (int i = lane; i < n_kv; i += 32) p[i] = __fmul_rn(p[i], sc);
+}
+
 // P.V: the columns past the last full round of 32 lane chains (n_kv & ~31 .. n_kv), folded into the chains' reduced sum in the order
 // the pinned build compiles vec_dot_f32's leftovers (oracle/bark_oracle.c orc_vec_dot_f32): runs of 8 and 4 multiply-then-add, then
-// fused multiply-adds.  v: the V column (stride E), p: the probability row.
+// fused multiply-adds.  v: the V column (stride E), p: the probability row (global or shared memory: plain loads, never __ldg).
 __device__ __forceinline__ float pv_leftovers(float sum, const float * __restrict__ v, const float * __restrict__ p, int np, int n_kv, int E) {
     int i = np, r = n_kv - np;
-    while (r >= 8) { for (int l = 0; l < 8; l++) sum = __fadd_rn(sum, __fmul_rn(__ldg(v + (size_t)(i + l) * E), __ldg(p + i + l))); i += 8; r -= 8; }
-    if (r >= 4)    { for (int l = 0; l < 4; l++) sum = __fadd_rn(sum, __fmul_rn(__ldg(v + (size_t)(i + l) * E), __ldg(p + i + l))); i += 4; r -= 4; }
-    for (; r > 0; r--, i++) sum = __fmaf_rn(__ldg(v + (size_t) i * E), __ldg(p + i), sum);
+    while (r >= 8) { for (int l = 0; l < 8; l++) sum = __fadd_rn(sum, __fmul_rn(v[(size_t)(i + l) * E], p[i + l])); i += 8; r -= 8; }
+    if (r >= 4)    { for (int l = 0; l < 4; l++) sum = __fadd_rn(sum, __fmul_rn(v[(size_t)(i + l) * E], p[i + l])); i += 4; r -= 4; }
+    for (; r > 0; r--, i++) sum = __fmaf_rn(v[(size_t) i * E], p[i], sum);
     return sum;
 }
 

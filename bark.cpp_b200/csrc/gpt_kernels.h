@@ -30,12 +30,19 @@ void layernorm_act(const float * x, int rows, int E, const float * g, const floa
 
 void lane_matmul(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, cudaStream_t s);
 
+// Multi-row attention (gemm_kernels.cu): N query rows Q[N][E] against n_kv <= 1024 key / value rows Kc, Vc [n_kv][E], H heads of 32, 64,
+// 96 or 128; causal masks key k for query q when k > n_past + q.  Result -> activation operand for c_proj.
+// Enough rows to give every SM a (head, 32-query) tile: attn_fused_kernel, scores in shared memory.  Up to attn_tiled_max_rows(H, SMs)
+// rows: three kernels that pass the scores through `scores` (H * N * n_kv floats).  Both give the same bits; path forces one (tests).
+enum AttnPath : int { ATTN_AUTO = 0, ATTN_FUSED = 1, ATTN_TILED = 2 };
+int  attn_tiled_max_rows(int H, int n_sm);
 void attention(const float * Q, const float * Kc, const float * Vc, int N, int n_kv, int n_past, int E, int H, bool causal,
-               float * scores, void * act, WType wt, int Kp, cudaStream_t s);
+               float * scores, void * act, WType wt, int Kp, cudaStream_t s, AttnPath path = ATTN_AUTO);
 
 // Decode attention for B <= 8 rows of different sequences (batched step): row b's query is Q[b], its new K / V rows are staged in
 // Kst[b] / Vst[b] and are appended to its cache (kv.k[b], kv.v[b]: the layer's [block_size][E] slab) at position d_pos[b]; it attends
-// over d_pos[b] + 1 keys.  max_kv = the largest of those.  Result -> activation operand, as attention() leaves it.
+// over d_pos[b] + 1 keys.  max_kv = the largest of those.  scores: B * H * max_kv floats.  Result -> activation operand, as attention()
+// leaves it.
 struct BatchKV { float * k[8], * v[8]; };
 void attention_batch(const float * Q, const float * Kst, const float * Vst, const BatchKV & kv, const int32_t * d_pos, int B, int max_kv, int E, int H,
                      float * scores, void * act, WType wt, int Kp, cudaStream_t s);
@@ -56,8 +63,6 @@ void   qx_matmul(const DMat & W, const void * act_f32, int ld_act, int rows, con
 
 // ---- register-tiled multi-row kernels (gemm_kernels.cu) ------------------------------------------------------------
 void lane_gemm_tiled(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, cudaStream_t s);
-void attention_tiled_scores(const float * Q, const float * Kc, int N, int n_kv, int n_past, int E, int H, float scale, bool causal, float * scores, cudaStream_t s);
-void attention_tiled_pv(const float * scores, const float * Vc, int N, int n_kv, int E, int H, void * act, WType wt, int Kp, cudaStream_t s);
 
 // ---- fast mode (fast_kernels.cu, BARK_B200_MODE=fast): wgmma GEMM + flash-style attention for the dense passes -------------------
 enum { FEPI_F32 = 0, FEPI_RESID = 1, FEPI_GELU16 = 2, FEPI_QKV16 = 4 };

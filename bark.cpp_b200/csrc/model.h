@@ -65,7 +65,7 @@ struct Workspace {
     void  * act2 = nullptr;     // second operand buffer (GELU output feeding mlp/c_proj)
     float * q = nullptr;        // [rows][E]
     float * kbuf = nullptr, * vbuf = nullptr;   // fine model K/V [rows][E]
-    float * scores = nullptr;   // [H][rows][n_kv]
+    float * scores = nullptr;   // [B <= 8][H][max_kv] (attention_batch) or [H][N][n_kv] for N <= attn_tiled_max_rows (attention)
     float * logits = nullptr;   // [rows][n_out]
     int32_t * tok = nullptr;    // device copy of the ids fed this step
 };

@@ -107,6 +107,14 @@ BARK_API int  bark_b200_fast_mode(struct bark_context * ctx);              /* 1 
 BARK_API int  bark_b200_fast_gemm(const uint16_t * A, const uint16_t * W, void * C, int M, int N, int K, int epilogue, int bn);
 BARK_API int  bark_b200_fast_attention(const uint16_t * q, const uint16_t * k, const uint16_t * v, uint16_t * out, int n, int E, int H);
 
+/* Parity-path attention on host buffers without a context (tests, tools/attn_bench.py): out[N][E] = soft_max(mask(Q K^T / sqrt(E/H))) V
+ * per head, bit-identical to the reference's ggml graph, for q [N][E], k / v [n_kv][E] f32, n_kv <= 1024, head size E/H in
+ * {32, 64, 96, 128}.  causal != 0 masks key j for query i when j > n_past + i.  path: 0 = the kernels the library picks for this
+ * shape, 1 = the fused kernel (scores in shared memory), 2 = the three-kernel path for few rows (N <= 32 * (ceil(SMs / H) - 1)).
+ * Returns 1 on success, 0 on failure. */
+BARK_API int  bark_b200_parity_attention(const float * q, const float * k, const float * v, float * out, int N, int n_kv, int n_past, int E, int H, int causal,
+                                         int path);
+
 #ifdef __cplusplus
 }
 #endif
