@@ -50,7 +50,7 @@ EXPORTS = [
     "bark_b200_get_stats", "bark_b200_get_hparams", "bark_b200_kernel_launches", "bark_b200_layernorm_fallbacks",
     "bark_b200_profile_enable", "bark_b200_profile_report", "bark_b200_io_counters", "bark_b200_decode_timing",
     "bark_b200_shard_init", "bark_b200_shard_connect", "bark_b200_shard_nvlink_bytes",
-    "bark_b200_fast_mode", "bark_b200_fast_gemm", "bark_b200_fast_attention", "bark_b200_parity_attention",
+    "bark_b200_fast_mode", "bark_b200_fast_gemm", "bark_b200_fast_attention", "bark_b200_parity_attention", "bark_b200_parity_gemm",
     "bark_b200_generate_batch", "bark_b200_batch_audio", "bark_b200_batch_tokens", "bark_b200_gpt_eval_slot", "bark_b200_gpt_step_batch",
     "ggml_time_init", "ggml_time_us", "ggml_time_ms", "ggml_init", "ggml_free",
 ]
@@ -129,6 +129,8 @@ def lib() -> C.CDLL:
     L.bark_b200_fast_attention.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int]
     L.bark_b200_parity_attention.restype = C.c_int
     L.bark_b200_parity_attention.argtypes = [vp, vp, vp, vp] + [C.c_int] * 7
+    L.bark_b200_parity_gemm.restype = C.c_int
+    L.bark_b200_parity_gemm.argtypes = [vp, vp, vp] + [C.c_int] * 6 + [vp]
     L.bark_b200_generate_batch.restype = C.c_bool
     L.bark_b200_generate_batch.argtypes = [vp, C.POINTER(C.c_char_p), C.POINTER(C.c_uint32), C.c_int, C.c_int]
     L.bark_b200_batch_audio.restype = C.c_int
@@ -405,6 +407,41 @@ def parity_attention(q: np.ndarray, k: np.ndarray, v: np.ndarray, n_head: int, n
     if not lib().bark_b200_parity_attention(_p(q), _p(k), _p(v), _p(out), N, n_kv, n_past, E, n_head, int(causal), ATTN_PATHS[path]):
         raise RuntimeError("bark_b200_parity_attention failed")
     return out
+
+
+PARITY_EPILOGUES = {"store": 0, "resid": 1, "gelu": 2, "qkv": 3}      # EPI_* (csrc/gpt_kernels.h)
+
+
+def parity_gemm(A: np.ndarray, W: np.ndarray, epilogue: str = "store", variant: int = 0, resid: np.ndarray | None = None,
+                gelu_tab: np.ndarray | None = None, return_variant: bool = False):
+    """Bit-exact A W^T on the parity path's tiled GEMM; A [M][K], W [N][K] both float16 or both float32, K % 32 == 0.
+
+    Returns float32 [M][N] for "store" and for "resid" (resid [M][N] float32 + A W^T), [M][N] in the operands' dtype for "gelu"
+    (GELU through gelu_tab, 65536 uint16 f16 bits), and for "qkv" (N % 3 == 0) the triple Q, K, V of float32 [M][N/3].
+    variant = 0 lets the library pick the block tile, 1 (32 x 16) / 2 (32 x 32) force one; with return_variant the result is (outputs, variant)."""
+    dt = np.float16 if np.asarray(A).dtype == np.float16 else np.float32
+    A = np.ascontiguousarray(A, dt); W = np.ascontiguousarray(W, dt)
+    M, K = A.shape; N = W.shape[0]
+    assert W.shape[1] == K, (A.shape, W.shape)
+    if epilogue == "resid":
+        out = np.array(resid, np.float32, order="C", copy=True)
+        assert out.shape == (M, N), out.shape
+    else:
+        out = np.zeros((M, N), dt if epilogue == "gelu" else np.float32)
+    tab = None
+    if epilogue == "gelu":
+        tab = np.ascontiguousarray(gelu_tab, np.uint16)
+        assert tab.shape == (65536,), tab.shape
+    r = lib().bark_b200_parity_gemm(_p(A), _p(W), _p(out), M, N, K, 1 if dt == np.float16 else 0, PARITY_EPILOGUES[epilogue], variant,
+                                    None if tab is None else _p(tab))
+    if r == -1:
+        raise GuardBandError(f"bark_b200_parity_gemm ({epilogue}, {M}x{N}x{K}, variant {variant}) wrote outside its output")
+    if r <= 0:
+        raise RuntimeError(f"bark_b200_parity_gemm ({epilogue}, {M}x{N}x{K}, variant {variant}) failed")
+    if epilogue == "qkv":
+        flat = out.reshape(-1)
+        out = tuple(flat[i * M * (N // 3):(i + 1) * M * (N // 3)].reshape(M, N // 3) for i in range(3))
+    return (out, r) if return_variant else out
 
 
 def kernel_launches() -> int:

@@ -1055,6 +1055,71 @@ extern "C" int bark_b200_parity_attention(const float * q, const float * k, cons
     return guarded((int) 0, [&] { return bark_b200_parity_attention_impl(q, k, v, out, N, n_kv, n_past, E, H, causal, path); });
 }
 
+// parity-path tiled GEMM on host buffers (tests, tools/gemm_bench.py): A [M][K] and W [N][K] go through permute_to_gm, as the loader
+// and the activation writers lay them out (row capacity and o_pad rounded up to the tallest / widest tile); the result comes back
+// row-major.  Every output region sits between guard bands and starts as NaN (RESID: as the residual from C).
+static int bark_b200_parity_gemm_impl(const void * A, const void * W, void * C, int M, int N, int K, int wtype, int epilogue, int variant,
+                                      const uint16_t * gelu_tab) {
+    if (!A || !W || !C || M < 1 || N < 1 || K < 32 || K % 32 || (wtype != W_F32 && wtype != W_F16) || variant < 0) return 0;
+    if (epilogue < EPI_STORE || epilogue > EPI_QKV || (epilogue == EPI_QKV && N % 3) || (epilogue == EPI_GELU_ACT && !gelu_tab)) return 0;
+    constexpr size_t kGuard = 4096;
+    constexpr unsigned char kPattern = 0x5a;
+    const size_t es = wtype == W_F16 ? 2 : 4;
+    const int rows_cap = (M + 31) / 32 * 32, o_pad = (N + kGemmOPad - 1) / kGemmOPad * kGemmOPad;
+    const size_t a_bytes = (size_t) gm_groups(K) * rows_cap * kGmGroup * es, w_bytes = (size_t) gm_groups(K) * o_pad * kGmGroup * es;
+    // output: STORE / RESID / QKV f32 [M][N] (QKV: Q, K, V blocks of [M][N/3] each); GELU_ACT: the group-major operand of the next mul_mat
+    const size_t out_bytes = epilogue == EPI_GELU_ACT ? (size_t) gm_groups(N) * rows_cap * kGmGroup * es : (size_t) M * N * 4;
+    struct Buffers {                                          // freed on every exit, including a CUDA failure thrown mid-way
+        void * p[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+        ~Buffers() { for (void * b : p) cudaFree(b); }
+    } d;
+    void *& d_rm = d.p[0], *& d_a = d.p[1], *& d_w = d.p[2], *& d_out = d.p[3], *& d_tab = d.p[4];
+    BARK_CUDA_CHECK(cudaMalloc(&d_rm, (size_t) std::max(M, N) * K * es));
+    BARK_CUDA_CHECK(cudaMalloc(&d_a, a_bytes)); BARK_CUDA_CHECK(cudaMalloc(&d_w, w_bytes));
+    BARK_CUDA_CHECK(cudaMemcpy(d_rm, A, (size_t) M * K * es, cudaMemcpyHostToDevice));
+    permute_to_gm(d_rm, d_a, M, rows_cap, K, (WType) wtype, 0);
+    BARK_CUDA_CHECK(cudaStreamSynchronize(0));
+    BARK_CUDA_CHECK(cudaMemcpy(d_rm, W, (size_t) N * K * es, cudaMemcpyHostToDevice));
+    permute_to_gm(d_rm, d_w, N, o_pad, K, (WType) wtype, 0);
+    BARK_CUDA_CHECK(cudaMalloc(&d_out, out_bytes + 2 * kGuard));
+    unsigned char * const reg = (unsigned char *) d_out;
+    BARK_CUDA_CHECK(cudaMemset(reg, kPattern, out_bytes + 2 * kGuard));
+    if (epilogue == EPI_RESID) BARK_CUDA_CHECK(cudaMemcpy(reg + kGuard, C, out_bytes, cudaMemcpyHostToDevice));
+    else                       BARK_CUDA_CHECK(cudaMemset(reg + kGuard, 0xff, out_bytes));
+    DMat dm; dm.n_out = N; dm.K = K; dm.type = (WType) wtype; dm.p_gm = d_w; dm.o_pad = o_pad;
+    MatmulEpilogue ep; ep.mode = epilogue;
+    float * const out = (float *)(reg + kGuard);
+    if (epilogue == EPI_STORE || epilogue == EPI_RESID) { ep.out = out; ep.ldo = N; }
+    else if (epilogue == EPI_QKV) { const int E = N / 3; ep.out = out; ep.k_out = out + (size_t) M * E; ep.v_out = out + 2 * (size_t) M * E; ep.ldo = E; }
+    else {
+        BARK_CUDA_CHECK(cudaMalloc(&d_tab, 65536 * 2));
+        BARK_CUDA_CHECK(cudaMemcpy(d_tab, gelu_tab, 65536 * 2, cudaMemcpyHostToDevice));
+        ep.act_out = out; ep.act_wt = wtype; ep.act_Kp = rows_cap * kGmGroup; ep.gelu_tab = (const __half *) d_tab;
+    }
+    const int ran = lane_gemm_tiled(dm, d_a, rows_cap * kGmGroup, M, ep, 0, variant);
+    BARK_CUDA_CHECK(cudaGetLastError());
+    const cudaError_t e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) { fprintf(stderr, "bark_b200_parity_gemm: %s\n", cudaGetErrorString(e)); return 0; }
+    if (!ran) return 0;
+    std::vector<unsigned char> h(out_bytes + 2 * kGuard);
+    BARK_CUDA_CHECK(cudaMemcpy(h.data(), reg, h.size(), cudaMemcpyDeviceToHost));
+    bool guards_intact = true;
+    for (size_t i = 0; i < kGuard; i++) guards_intact &= h[i] == kPattern && h[kGuard + out_bytes + i] == kPattern;
+    if (!guards_intact) { fprintf(stderr, "bark_b200_parity_gemm: a store landed outside the output (guard band overwritten)\n"); return -1; }
+    const unsigned char * o = h.data() + kGuard;
+    if (epilogue != EPI_GELU_ACT) memcpy(C, o, out_bytes);
+    else {                                                    // group-major -> row-major [M][N]
+        const size_t gs = (size_t) rows_cap * kGmGroup;
+        for (int m = 0; m < M; m++)
+            for (int k = 0; k < N; k++) memcpy((unsigned char *) C + ((size_t) m * N + k) * es, o + gm_offset(m, k, gs) * es, es);
+    }
+    return ran;
+}
+extern "C" int bark_b200_parity_gemm(const void * A, const void * W, void * C, int M, int N, int K, int wtype, int epilogue, int variant,
+                                     const uint16_t * gelu_tab) {
+    return guarded((int) 0, [&] { return bark_b200_parity_gemm_impl(A, W, C, M, N, K, wtype, epilogue, variant, gelu_tab); });
+}
+
 // batched generation (include/bark_b200.h)
 extern "C" bool bark_b200_generate_batch(struct bark_context * ctx, const char * const * texts, const uint32_t * seeds, int n, int n_threads) {
     (void) n_threads;

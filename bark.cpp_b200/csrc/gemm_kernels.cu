@@ -4,9 +4,10 @@
 // Bit-exactness fixes the shape of the tiling: every output element is 32 lane partials (common.cuh "Lane order"),
 // each a serial FMA chain over k = v, v+32, ..., so a warp's 32 lanes all work on the SAME outputs — lane v owns
 // virtual lane v of an 8 x 8 output tile (64 accumulators per lane, 2048 per warp).  Operand reuse therefore comes
-// from registers (each converted operand feeds 8 FMAs) and shared memory (a 32 x 16 block tile), not from giving
-// different lanes different outputs.  The 32 partials of all 64 outputs are then combined with a transposed
-// butterfly (62 shuffles instead of 64 x 5) that performs exactly the additions of GGML_F32x8_REDUCE.
+// from registers (each converted operand feeds 8 FMAs) and shared memory (a 32 x 32 or 32 x 16 block tile), not from giving
+// different lanes different outputs.  The 32 partials of all 64 outputs are then combined through shared memory and
+// lane_tree_reduce_local, or with a transposed butterfly (62 shuffles instead of 64 x 5); both perform exactly the additions
+// of GGML_F32x8_REDUCE.
 //
 // Both operands are in the group-major layout (common.cuh), so a pipeline stage of the block tile is a handful of
 // contiguous spans: 2-4 TMA bulk copies into a 4-stage shared-memory ring (mbarrier complete_tx).
@@ -32,7 +33,12 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         "bra WAIT_%=;\n\t"
         "DONE_%=:\n\t}" ::"r"(bar), "r"(parity) : "memory");
 }
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
+// atomicAdd with acquire-release semantics at CTA scope: one instruction instead of fence.sc + atomic + fence.sc
+__device__ __forceinline__ int atom_add_acq_rel_cta(int * p, int v) {
+    int old;
+    asm volatile("atom.acq_rel.cta.shared::cta.add.u32 %0, [%1], %2;" : "=r"(old) : "r"(smem_u32(p)), "r"(v) : "memory");
+    return old;
+}
 __device__ __forceinline__ void tma_bulk_g2s(uint32_t dst, const void * src, uint32_t bytes, uint32_t bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
@@ -58,8 +64,25 @@ __device__ __forceinline__ int butterfly_reduce64(float (&r)[64], int lane) {
     return ((lane & 16) << 1) | ((lane & 8) << 1) | ((lane & 4) << 1) | ((lane & 1) << 2) | (lane & 2);
 }
 
-constexpr int kBM = 32, kBO = 16, kStages = 4;
-constexpr int kStageBytes = (kBM + kBO) * 512;           // 24 KB: 256 columns of f16 (two groups) or 128 columns of f32 (one group)
+constexpr int kStages = 4;
+constexpr int kRedLd = 36;       // row stride (floats) of the tile-end reduction scratch: 16-byte reads of 8 consecutive rows hit 8 bank quads
+
+// Block-tile configurations (the `variant` of lane_gemm_tiled): WM x WO warps, each with an 8 x OT output tile, MINB CTAs per SM.
+// A stage holds (BM + BO) rows x 512 bytes: 256 columns of f16 (two groups) or 128 columns of f32 (one group).
+// PIPE (f16): the operand words of a stage are loaded as 32-bit halves (chain steps 0-1, 2-3), each half one group ahead of the
+// FMAs that use it, so the next half's loads are in flight under the current half's FMAs in the same registers.
+template <int WM_, int WO_, int OT_, int MINB_, bool PIPE_ = false> struct TileCfg {
+    static constexpr int WM = WM_, WO = WO_, OT = OT_, MINB = MINB_;
+    static constexpr bool PIPE = PIPE_;
+    static constexpr int kWarps = WM * WO, kThreads = 32 * kWarps, kBM = 8 * WM, kBO = OT * WO, kNAcc = 8 * OT;
+    static constexpr int kStageBytes = (kBM + kBO) * 512;
+    // one CTA per SM leaves room to combine the lane partials through shared memory; two per SM keep the transposed butterfly
+    static constexpr bool kSmemReduce = MINB == 1;
+    static constexpr size_t kRedOff = ((size_t) kStages * kStageBytes + kStages * 12 + 15) & ~(size_t) 15;
+    static constexpr size_t kSmem = kRedOff + (kSmemReduce ? (size_t) kWarps * 32 * kRedLd * 4 : 0);
+};
+typedef TileCfg<4, 2, 8, 2>  Tile32x16;      // variant 1: 32 x 16, 8 warps of 8 x 8, 2 CTAs per SM (few rows: twice the tiles)
+typedef TileCfg<4, 4, 8, 1, true> Tile32x32;  // variant 2: 32 x 32, 16 warps of 8 x 8, 1 CTA per SM, operand loads pipelined (f16)
 
 // lane v's four elements of one row of one 128-column group (group-major layout, common.cuh)
 template <typename T> struct QuadOp;
@@ -78,28 +101,84 @@ template <> struct QuadOp<float> {
     __device__ __forceinline__ static float elem(const uint4 & u, int c) { return __uint_as_float(c == 0 ? u.x : c == 1 ? u.y : c == 2 ? u.z : u.w); }
 };
 
+// One 128-column group of a warp's 8 x OT tile: acc[mi * OT + oi] += its 4 chain steps (FULL) or the first `steps` of them (the last
+// group of a K that is not a multiple of 128).  ga / gw: lane v's word of the tile's first activation / weight row.
+template <typename T, int OT, bool FULL>
+__device__ __forceinline__ void fma_group(const unsigned char * ga, const unsigned char * gw, float (&acc)[8 * OT], int steps) {
+    typedef typename QuadOp<T>::V QV;
+    constexpr int kRowB = kGmGroup * sizeof(T);
+    QV pa[8], pw[OT];
+#pragma unroll
+    for (int mi = 0; mi < 8; mi++) pa[mi] = *reinterpret_cast<const QV *>(ga + mi * kRowB);
+#pragma unroll
+    for (int oi = 0; oi < OT; oi++) pw[oi] = *reinterpret_cast<const QV *>(gw + oi * kRowB);
+#pragma unroll
+    for (int c = 0; c < 4; c++) {
+        if (FULL || c < steps) {
+            float af[8], wf[OT];
+#pragma unroll
+            for (int mi = 0; mi < 8; mi++) af[mi] = QuadOp<T>::elem(pa[mi], c);
+#pragma unroll
+            for (int oi = 0; oi < OT; oi++) wf[oi] = QuadOp<T>::elem(pw[oi], c);
+#pragma unroll
+            for (int mi = 0; mi < 8; mi++)
+#pragma unroll
+                for (int oi = 0; oi < OT; oi++) acc[mi * OT + oi] = __fmaf_rn(wf[oi], af[mi], acc[mi * OT + oi]);
+        }
+    }
+}
+
+// f16, chain steps 2h and 2h+1 of a group from the h-th 32-bit halves of the operand words (a: 8 activation rows, w: OT weight rows)
+template <int OT>
+__device__ __forceinline__ void fma_half(const uint32_t (&a)[8], const uint32_t (&w)[OT], float (&acc)[8 * OT]) {
+#pragma unroll
+    for (int c = 0; c < 2; c++) {
+        float af[8], wf[OT];
+#pragma unroll
+        for (int mi = 0; mi < 8; mi++) { const __half2 h = *reinterpret_cast<const __half2 *>(&a[mi]); af[mi] = c ? __high2float(h) : __low2float(h); }
+#pragma unroll
+        for (int oi = 0; oi < OT; oi++) { const __half2 h = *reinterpret_cast<const __half2 *>(&w[oi]); wf[oi] = c ? __high2float(h) : __low2float(h); }
+#pragma unroll
+        for (int mi = 0; mi < 8; mi++)
+#pragma unroll
+            for (int oi = 0; oi < OT; oi++) acc[mi * OT + oi] = __fmaf_rn(wf[oi], af[mi], acc[mi * OT + oi]);
+    }
+}
+template <int OT>
+__device__ __forceinline__ void load_half(const unsigned char * ga, const unsigned char * gw, int h, uint32_t (&a)[8], uint32_t (&w)[OT]) {
+#pragma unroll
+    for (int mi = 0; mi < 8; mi++) a[mi] = *reinterpret_cast<const uint32_t *>(ga + mi * 256 + h * 4);
+#pragma unroll
+    for (int oi = 0; oi < OT; oi++) w[oi] = *reinterpret_cast<const uint32_t *>(gw + oi * 256 + h * 4);
+}
+
 }  // namespace
 
-// C[m][o] = lane-order dot(act[m], W[o]).  Persistent CTAs walk 32 x 16 block tiles (o fastest, so CTAs running at the
-// same time share activation rows in L2); 8 warps as 4 (m) x 2 (o), 8 x 8 outputs per warp.
+// C[m][o] = lane-order dot(act[m], W[o]).  Persistent CTAs walk BM x BO block tiles (o fastest, so CTAs running at the same time
+// share activation rows in L2); WM x WO warps, 8 x OT outputs per warp (TileCfg).
 //
-// Both operands are group-major: for one 128-column group the 32 activation rows of a tile are one contiguous span, the
-// 16 weight rows another, so a pipeline stage is 2 (f32) or 4 (f16) bulk copies issued by ONE thread.  (Row-major
-// operands would need 48 row copies per stage; the copy instruction takes uniform operands, so the compiler serialises the
-// 48 lanes and the issuing warp - also a consumer - falls behind, with the other seven warps waiting on the `full` barrier.)
+// Both operands are group-major: for one 128-column group the BM activation rows of a tile are one contiguous span, the BO weight
+// rows another, so a pipeline stage is 2 (f32) or 4 (f16) bulk copies issued by ONE thread.  (Row-major operands would need a copy
+// per row; the copy instruction takes uniform operands, so the compiler serialises the lanes and the issuing warp - also a
+// consumer - falls behind, with the other warps waiting on the `full` barrier.)
 //
 // The k-steps of ALL of a CTA's tiles form one stream through the 4-stage ring.  Nobody waits to refill a slot: every warp
-// bumps the slot's counter when it is done reading, and the warp that arrives last issues the copies for stage s + 4.
-template <typename T>
-__global__ void __launch_bounds__(256, 2) lane_gemm_tiled_kernel(const T * __restrict__ Wg, int K, int w_gs, int O, const T * __restrict__ act, int act_gs, int M, MatmulEpilogue ep) {
-    typedef typename QuadOp<T>::V QV;
-    constexpr int GPS = QuadOp<T>::kGroupsPerStage;
+// bumps the slot's counter when it is done reading (an acquire-release atomic: its reads happen before the refill), and the warp
+// whose bump completes a multiple of the warp count issues the copies for stage s + 4.  The counters only grow, so no reset store
+// has to be ordered before the next round's bumps.
+//
+// Tile end: with one CTA per SM each warp writes its partials to its own shared-memory scratch 32 outputs at a time and lane u
+// then adds the 32 partials of output u with lane_tree_reduce_local (32 stores + 8 16-byte loads + 31 adds per lane and slice);
+// with two CTAs per SM there is no room for the scratch and the transposed butterfly does it in registers.
+template <typename T, typename Cfg>
+__global__ void __launch_bounds__(Cfg::kThreads, Cfg::MINB) lane_gemm_tiled_kernel(const T * __restrict__ Wg, int K, int w_gs, int O, const T * __restrict__ act, int act_gs, int M, MatmulEpilogue ep) {
+    constexpr int GPS = QuadOp<T>::kGroupsPerStage, OT = Cfg::OT, kBM = Cfg::kBM, kBO = Cfg::kBO, kStageBytes = Cfg::kStageBytes;
     constexpr int kRowB = kGmGroup * sizeof(T);              // bytes of one row of one group: 256 (f16) / 512 (f32)
     extern __shared__ __align__(128) unsigned char smem[];
     const uint32_t full = smem_u32(smem + kStages * kStageBytes);
     int * const cnt = reinterpret_cast<int *>(smem + kStages * kStageBytes + kStages * 8);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int wm = warp >> 1, wo = warp & 1;
+    const int wm = warp / Cfg::WO, wo = warp % Cfg::WO;
     const int nsteps = K >> 5;                                // chain steps per lane
     const int ngroups = (nsteps + 3) >> 2;                    // 128-column groups; the last may be partial
     const int nstages = (ngroups + GPS - 1) / GPS;            // pipeline stages per tile
@@ -132,76 +211,110 @@ __global__ void __launch_bounds__(256, 2) lane_gemm_tiled_kernel(const T * __res
     for (int ti = 0; ti < my_tiles; ti++) {
         const int tile = blockIdx.x + ti * gridDim.x;
         const int m0 = (tile / tiles_o) * kBM, o0 = (tile % tiles_o) * kBO;
-        float acc[64];
+        float acc[Cfg::kNAcc];
 #pragma unroll
-        for (int i = 0; i < 64; i++) acc[i] = 0.0f;
+        for (int i = 0; i < Cfg::kNAcc; i++) acc[i] = 0.0f;
         for (int sg = 0; sg < nstages; sg++, step++) {
             const int slot = step % kStages;
             mbar_wait(full + slot * 8, (uint32_t)(step / kStages) & 1);
             const unsigned char * st = smem + (size_t) slot * kStageBytes;
+            const unsigned char * const ga0 = st + lane * sizeof(typename QuadOp<T>::V) + wm * 8 * kRowB;
+            const unsigned char * const gw0 = st + kBM * kRowB + lane * sizeof(typename QuadOp<T>::V) + wo * OT * kRowB;
+            if constexpr (Cfg::PIPE) {
+                if (nsteps - sg * GPS * 4 >= GPS * 4) {       // every group of the stage full (uniform across the block)
+                    uint32_t a0[8], w0[OT], a1[8], w1[OT];
+                    load_half<OT>(ga0, gw0, 0, a0, w0);
+#pragma unroll
+                    for (int j = 0; j < GPS; j++) {
+                        const int off = j * (kBM + kBO) * kRowB;
+                        load_half<OT>(ga0 + off, gw0 + off, 1, a1, w1);
+                        fma_half<OT>(a0, w0, acc);
+                        if (j + 1 < GPS) load_half<OT>(ga0 + off + (kBM + kBO) * kRowB, gw0 + off + (kBM + kBO) * kRowB, 0, a0, w0);
+                        fma_half<OT>(a1, w1, acc);
+                    }
+                    goto released;
+                }
+            }
 #pragma unroll
             for (int j = 0; j < GPS; j++) {
                 const int g = sg * GPS + j;
                 if (g < ngroups) {                            // uniform across the block
-                    const int steps = min(4, nsteps - g * 4); // chain steps present in this group
-                    const unsigned char * ga = st + j * (kBM + kBO) * kRowB + lane * sizeof(QV), * gw = ga + kBM * kRowB;
-                    QV pa[8], pw[8];
-#pragma unroll
-                    for (int mi = 0; mi < 8; mi++) pa[mi] = *reinterpret_cast<const QV *>(ga + (wm * 8 + mi) * kRowB);
-#pragma unroll
-                    for (int oi = 0; oi < 8; oi++) pw[oi] = *reinterpret_cast<const QV *>(gw + (wo * 8 + oi) * kRowB);
-#pragma unroll
-                    for (int c = 0; c < 4; c++) {
-                        if (c < steps) {
-                            float af[8], wf[8];
-#pragma unroll
-                            for (int mi = 0; mi < 8; mi++) af[mi] = QuadOp<T>::elem(pa[mi], c);
-#pragma unroll
-                            for (int oi = 0; oi < 8; oi++) wf[oi] = QuadOp<T>::elem(pw[oi], c);
-#pragma unroll
-                            for (int mi = 0; mi < 8; mi++)
-#pragma unroll
-                                for (int oi = 0; oi < 8; oi++) acc[mi * 8 + oi] = __fmaf_rn(wf[oi], af[mi], acc[mi * 8 + oi]);
-                        }
-                    }
+                    const unsigned char * ga = ga0 + j * (kBM + kBO) * kRowB, * gw = gw0 + j * (kBM + kBO) * kRowB;
+                    const int steps = nsteps - g * 4;         // chain steps from this group on
+                    if (steps >= 4) fma_group<T, OT, true>(ga, gw, acc, 4);
+                    else            fma_group<T, OT, false>(ga, gw, acc, steps);
                 }
             }
+        released:
             __syncwarp();
-            if (lane == 0) {                                  // release the slot; the last of the 8 warps refills it
-                __threadfence_block();
-                if (atomicAdd_block(&cnt[slot], 1) == 7) {
-                    cnt[slot] = 0;
-                    __threadfence_block();
+            if (lane == 0) {                                  // release the slot; the last of the warps refills it
+                if ((atom_add_acq_rel_cta(&cnt[slot], 1) + 1) % Cfg::kWarps == 0) {
                     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
                     if (step + kStages < total_steps) issue(step + kStages);
                 }
             }
         }
-        const int base = butterfly_reduce64(acc, lane);        // outputs base, base+1 of the warp tile (index = mi*8 + oi)
-        const int m = m0 + wm * 8 + (base >> 3), o = o0 + wo * 8 + (base & 7);
-        if (m < M) {
-            if (o < O) matmul_epilogue(ep, m, o, acc[0]);
-            if (o + 1 < O) matmul_epilogue(ep, m, o + 1, acc[1]);
+        if constexpr (Cfg::kSmemReduce) {
+            float * const red = reinterpret_cast<float *>(smem + Cfg::kRedOff) + warp * 32 * kRedLd;
+#pragma unroll
+            for (int sl = 0; sl < Cfg::kNAcc / 32; sl++) {
+                __syncwarp();                                 // the previous slice's (or tile's) reads are done
+#pragma unroll
+                for (int j = 0; j < 32; j++) red[j * kRedLd + lane] = acc[sl * 32 + j];
+                __syncwarp();
+                float a[32];
+#pragma unroll
+                for (int q = 0; q < 8; q++) {
+                    const float4 t = *reinterpret_cast<const float4 *>(red + lane * kRedLd + q * 4);
+                    a[4 * q] = t.x; a[4 * q + 1] = t.y; a[4 * q + 2] = t.z; a[4 * q + 3] = t.w;
+                }
+                const int i = sl * 32 + lane;                 // = mi * OT + oi
+                const int m = m0 + wm * 8 + i / OT, o = o0 + wo * OT + i % OT;
+                const float r = lane_tree_reduce_local(a);
+                if (m < M && o < O) matmul_epilogue(ep, m, o, r);
+            }
+        } else {
+            static_assert(Cfg::kNAcc == 64, "the butterfly combines 64 outputs");
+            const int base = butterfly_reduce64(acc, lane);    // outputs base, base+1 of the warp tile (index = mi*8 + oi)
+            const int m = m0 + wm * 8 + (base >> 3), o = o0 + wo * 8 + (base & 7);
+            if (m < M) {
+                if (o < O) matmul_epilogue(ep, m, o, acc[0]);
+                if (o + 1 < O) matmul_epilogue(ep, m, o + 1, acc[1]);
+            }
         }
     }
 }
 
-void lane_gemm_tiled(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, cudaStream_t s) {
-    const size_t smem = (size_t) kStages * kStageBytes + kStages * 8 + kStages * 4 + 64;
+template <typename T, typename Cfg>
+static void launch_tiled(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, int n_sm, cudaStream_t s) {
+    static std::atomic<unsigned long long> configured{0};
+    if (first_use_on_this_device(configured))
+        BARK_CUDA_CHECK(cudaFuncSetAttribute(lane_gemm_tiled_kernel<T, Cfg>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) Cfg::kSmem));
+    const int n_tiles = ((W.n_out + Cfg::kBO - 1) / Cfg::kBO) * ((rows + Cfg::kBM - 1) / Cfg::kBM);
+    const int grid = min(n_tiles, Cfg::MINB * n_sm);            // persistent: as many CTAs as fit at once (registers, shared memory)
+    BARK_LAUNCH((lane_gemm_tiled_kernel<T, Cfg>), grid, Cfg::kThreads, Cfg::kSmem, s, (const T *) W.p_gm, W.K, W.o_pad * kGmGroup, W.n_out,
+                (const T *) act, act_gs, rows, ep);
+}
+
+int lane_gemm_tiled(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, cudaStream_t s, int variant) {
+    if (!W.p_gm) { fprintf(stderr, "bark_b200: matrix has no group-major copy for the tiled mat-mul\n"); throw std::runtime_error("unsupported configuration (see the message above)"); }
+    if (W.o_pad % kGemmOPad) { fprintf(stderr, "bark_b200: group-major rows padded to %d, need a multiple of %d\n", W.o_pad, kGemmOPad); throw std::runtime_error("unsupported configuration (see the message above)"); }
     int dev = 0, n_sm = 0;
     BARK_CUDA_CHECK(cudaGetDevice(&dev));
     BARK_CUDA_CHECK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
-    static std::atomic<unsigned long long> configured{0};
-    if (first_use_on_this_device(configured)) {
-        BARK_CUDA_CHECK(cudaFuncSetAttribute(lane_gemm_tiled_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
-        BARK_CUDA_CHECK(cudaFuncSetAttribute(lane_gemm_tiled_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
-    }
-    if (!W.p_gm) { fprintf(stderr, "bark_b200: matrix has no group-major copy for the tiled mat-mul\n"); throw std::runtime_error("unsupported configuration (see the message above)"); }
-    const int n_tiles = ((W.n_out + kBO - 1) / kBO) * ((rows + kBM - 1) / kBM);
-    const int grid = min(n_tiles, 2 * n_sm);                   // persistent: two CTAs per SM (registers and shared memory allow exactly that)
-    const int w_gs = W.o_pad * kGmGroup;
-    if (W.type == W_F16) BARK_LAUNCH((lane_gemm_tiled_kernel<__half>), grid, 256, smem, s, (const __half *) W.p_gm, W.K, w_gs, W.n_out, (const __half *) act, act_gs, rows, ep);
-    else                 BARK_LAUNCH((lane_gemm_tiled_kernel<float>), grid, 256, smem, s, (const float *) W.p_gm, W.K, w_gs, W.n_out, (const float *) act, act_gs, rows, ep);
+    // f16: the 32 x 32 tile (a third fewer bytes per FMA) was measured ahead on 15 of the bench clip's 17 GEMM shapes, the 91-row
+    // coarse windows included although their 72 tiles leave SMs idle, and at most 2 % behind on the other two (DESIGN §4.5).
+    // f32 has only the 32 x 16 tile it has always had (DESIGN §4.5: at the fine-pass shapes it is 13-19 % faster than before).
+    if (variant == 0) variant = W.type == W_F16 ? 2 : 1;
+    if (W.type == W_F16) {
+        if (variant == 1) launch_tiled<__half, Tile32x16>(W, act, act_gs, rows, ep, n_sm, s);
+        else if (variant == 2) launch_tiled<__half, Tile32x32>(W, act, act_gs, rows, ep, n_sm, s);
+        else return 0;
+    } else if (W.type == W_F32) {
+        if (variant == 1) launch_tiled<float, Tile32x16>(W, act, act_gs, rows, ep, n_sm, s);
+        else return 0;
+    } else return 0;
+    return variant;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -62,7 +62,11 @@ void   qx_embed_fine(const GPTModel & m, const int32_t * d_ids, int nn, float * 
 void   qx_matmul(const DMat & W, const void * act_f32, int ld_act, int rows, const MatmulEpilogue & ep, cudaStream_t s);
 
 // ---- register-tiled multi-row kernels (gemm_kernels.cu) ------------------------------------------------------------
-void lane_gemm_tiled(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, cudaStream_t s);
+// W needs its group-major copy with o_pad a multiple of kGemmOPad (the widest block tile), the activation operand a row capacity
+// (act_gs / 128) that is a multiple of 32 (the tallest).  variant: 0 = the block tile picked for the weight type, 1 = 32 x 16 (8 warps,
+// two CTAs per SM), 2 = 32 x 32 (16 warps, one CTA per SM).  Returns the variant launched, 0 if it does not exist.
+constexpr int kGemmOPad = 32;
+int lane_gemm_tiled(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, cudaStream_t s, int variant = 0);
 
 // ---- fast mode (fast_kernels.cu, BARK_B200_MODE=fast): wgmma GEMM + flash-style attention for the dense passes -------------------
 enum { FEPI_F32 = 0, FEPI_RESID = 1, FEPI_GELU16 = 2, FEPI_QKV16 = 4 };

@@ -164,8 +164,8 @@ bool load_gpt(bark_context * ctx, std::ifstream & f, GPTModel & m, const char * 
             d.n_out = s.ne1; d.K = s.ne0; d.type = m.wtype; d.Kp = li_padded_k(d.K, m.wtype == W_F16 ? 2 : 4);
             d.p = ctx_alloc(ctx, (size_t) d.n_out * d.Kp * (m.wtype == W_F16 ? 2 : 4));
             permute_to_li(raw, d.p, d.n_out, d.K, m.wtype, ctx->stream);
-            if (s.gm) {                                  // second copy for the multi-row tiled mat-mul (group-major, rows padded to 16)
-                d.o_pad = (d.n_out + 15) / 16 * 16;
+            if (s.gm) {                                  // second copy for the multi-row tiled mat-mul (group-major, rows padded to the widest tile)
+                d.o_pad = (d.n_out + kGemmOPad - 1) / kGemmOPad * kGemmOPad;
                 const size_t gm_bytes = (size_t) gm_groups(d.K) * d.o_pad * kGmGroup * (m.wtype == W_F16 ? 2 : 4);
                 d.p_gm = ctx_alloc(ctx, gm_bytes);
                 permute_to_gm(raw, d.p_gm, d.n_out, d.o_pad, d.K, m.wtype, ctx->stream);

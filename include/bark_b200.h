@@ -115,6 +115,18 @@ BARK_API int  bark_b200_fast_attention(const uint16_t * q, const uint16_t * k, c
 BARK_API int  bark_b200_parity_attention(const float * q, const float * k, const float * v, float * out, int N, int n_kv, int n_past, int E, int H, int causal,
                                          int path);
 
+/* Parity-path tiled GEMM on host buffers without a context (tests, tools/gemm_bench.py): C = A W^T with every output the reference's
+ * vec_dot of its two rows, for A [M][K] and W [N][K] of wtype 0 (f32) or 1 (f16 bits), K % 32 == 0, through the multi-row passes'
+ * epilogue `epilogue`:
+ *   0 STORE     C = f32 [M][N]
+ *   1 RESID     C = f32 [M][N], holds the residual on entry and residual + A W^T on return
+ *   2 GELU_ACT  C = [M][N] in wtype: GELU of the product through gelu_tab (65536 f16 entries), as the next mat-mul's operand holds it
+ *   3 QKV       N % 3 == 0; C = f32 Q [M][N/3], then K [M][N/3], then V [M][N/3]
+ * variant: 0 = the block tile the library picks, 1 = 32 x 16 outputs (8 warps, two CTAs per SM), 2 = 32 x 32 (16 warps, one CTA
+ * per SM).  Returns the variant that ran, 0 on failure or invalid arguments, -1 if a store landed in the guard bands around the output. */
+BARK_API int  bark_b200_parity_gemm(const void * A, const void * W, void * C, int M, int N, int K, int wtype, int epilogue, int variant,
+                                    const uint16_t * gelu_tab);
+
 #ifdef __cplusplus
 }
 #endif
