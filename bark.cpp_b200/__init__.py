@@ -51,7 +51,7 @@ EXPORTS = [
     "bark_b200_profile_enable", "bark_b200_profile_report", "bark_b200_io_counters", "bark_b200_decode_timing",
     "bark_b200_shard_init", "bark_b200_shard_connect", "bark_b200_shard_nvlink_bytes",
     "bark_b200_fast_mode", "bark_b200_fast_gemm", "bark_b200_fast_attention", "bark_b200_parity_attention", "bark_b200_parity_gemm",
-    "bark_b200_generate_batch", "bark_b200_batch_audio", "bark_b200_batch_tokens", "bark_b200_gpt_eval_slot", "bark_b200_gpt_step_batch",
+    "bark_b200_parity_rows", "bark_b200_generate_batch", "bark_b200_batch_audio", "bark_b200_batch_tokens", "bark_b200_gpt_eval_slot", "bark_b200_gpt_step_batch",
     "ggml_time_init", "ggml_time_us", "ggml_time_ms", "ggml_init", "ggml_free",
 ]
 
@@ -131,6 +131,8 @@ def lib() -> C.CDLL:
     L.bark_b200_parity_attention.argtypes = [vp, vp, vp, vp] + [C.c_int] * 7
     L.bark_b200_parity_gemm.restype = C.c_int
     L.bark_b200_parity_gemm.argtypes = [vp, vp, vp] + [C.c_int] * 6 + [vp]
+    L.bark_b200_parity_rows.restype = C.c_int
+    L.bark_b200_parity_rows.argtypes = [C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, vp, vp, C.POINTER(C.c_uint)]
     L.bark_b200_generate_batch.restype = C.c_bool
     L.bark_b200_generate_batch.argtypes = [vp, C.POINTER(C.c_char_p), C.POINTER(C.c_uint32), C.c_int, C.c_int]
     L.bark_b200_batch_audio.restype = C.c_int
@@ -442,6 +444,33 @@ def parity_gemm(A: np.ndarray, W: np.ndarray, epilogue: str = "store", variant: 
         flat = out.reshape(-1)
         out = tuple(flat[i * M * (N // 3):(i + 1) * M * (N // 3)].reshape(M, N // 3) for i in range(3))
     return (out, r) if return_variant else out
+
+
+ROW_OPS = {"layernorm": 0, "softmax": 1}
+ROW_IMPLS = {"multi": 0, "decode": 1}
+
+
+def parity_rows(x: np.ndarray, op: str, impl: str, g: np.ndarray | None = None, b: np.ndarray | None = None):
+    """One of the parity path's row reductions on x [rows][n] float32, n <= 1024; returns (out [rows][n] float32, replays).
+
+    op "layernorm" (eps 1e-5, gain g required, bias b optional: the f32 value before any operand rounding) or "softmax" (the
+    probabilities as their consumers form them); impl "multi" (layernorm_act_kernel / softmax_row, the multi-row passes and the
+    attention kernels) or "decode" (block_layernorm / softmax_exp_rcp, the persistent decode kernels).  replays = how many bracket
+    decisions fell back to the sequential sum."""
+    x = np.ascontiguousarray(x, np.float32)
+    if x.ndim == 1:
+        x = x[None]
+    rows, n = x.shape
+    gp = bp = None
+    if g is not None:
+        g = np.ascontiguousarray(g, np.float32); assert g.shape == (n,), g.shape; gp = _p(g)
+    if b is not None:
+        b = np.ascontiguousarray(b, np.float32); assert b.shape == (n,), b.shape; bp = _p(b)
+    out = np.zeros((rows, n), np.float32)
+    rep = C.c_uint(0)
+    if not lib().bark_b200_parity_rows(ROW_OPS[op], ROW_IMPLS[impl], _p(x), rows, n, gp, bp, _p(out), C.byref(rep)):
+        raise RuntimeError(f"bark_b200_parity_rows ({op}, {impl}, {rows} x {n}) failed")
+    return out, rep.value
 
 
 def kernel_launches() -> int:

@@ -1055,6 +1055,43 @@ extern "C" int bark_b200_parity_attention(const float * q, const float * k, cons
     return guarded((int) 0, [&] { return bark_b200_parity_attention_impl(q, k, v, out, N, n_kv, n_past, E, H, causal, path); });
 }
 
+// the parity path's row reductions on host buffers (tests): op 0 LayerNorm, op 1 soft_max; impl 0 the multi-row kernels
+// (layernorm_act_kernel writing plain f32 rows, softmax_row), impl 1 the decode kernels' block_layernorm / softmax_exp_rcp
+static int bark_b200_parity_rows_impl(int op, int impl, const float * x, int rows, int n, const float * g, const float * b, float * out, unsigned * replays) {
+    if (!x || !out || !replays || op < 0 || op > 1 || impl < 0 || impl > 1 || rows < 1 || n < 1 || n > 1024 || (op == 0 && !g)) return 0;
+    struct Buffers {                                          // freed on every exit, including a CUDA failure thrown mid-way
+        void * p[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+        ~Buffers() { for (void * q : p) cudaFree(q); }
+    } d;
+    const size_t bytes = (size_t) rows * n * 4;
+    float * dx, * dout, * dg = nullptr, * db = nullptr; unsigned * dcnt;
+    BARK_CUDA_CHECK(cudaMalloc(&d.p[0], bytes)); dx = (float *) d.p[0];
+    BARK_CUDA_CHECK(cudaMalloc(&d.p[1], bytes)); dout = (float *) d.p[1];
+    BARK_CUDA_CHECK(cudaMalloc(&d.p[2], 2 * sizeof(unsigned))); dcnt = (unsigned *) d.p[2];
+    BARK_CUDA_CHECK(cudaMemcpy(dx, x, bytes, cudaMemcpyHostToDevice));
+    BARK_CUDA_CHECK(cudaMemset(dcnt, 0, 2 * sizeof(unsigned)));
+    BARK_CUDA_CHECK(cudaMemset(dout, 0xff, bytes));                       // NaN: a missing store shows up
+    if (op == 0) {
+        BARK_CUDA_CHECK(cudaMalloc(&d.p[3], (size_t) n * 4)); dg = (float *) d.p[3];
+        BARK_CUDA_CHECK(cudaMemcpy(dg, g, (size_t) n * 4, cudaMemcpyHostToDevice));
+        if (b) { BARK_CUDA_CHECK(cudaMalloc(&d.p[4], (size_t) n * 4)); db = (float *) d.p[4]; BARK_CUDA_CHECK(cudaMemcpy(db, b, (size_t) n * 4, cudaMemcpyHostToDevice)); }
+    }
+    if (impl == 1)    decode_rows(op, dx, rows, n, dg, db, dout, dcnt, 0);
+    else if (op == 0) layernorm_act(dx, rows, n, dg, db, dout, W_Q4_0, n, dcnt, 0);
+    else {            BARK_CUDA_CHECK(cudaMemcpy(dout, dx, bytes, cudaMemcpyDeviceToDevice)); softmax_rows(dout, rows, n, dcnt, 0); }
+    BARK_CUDA_CHECK(cudaGetLastError());                      // a launch the configuration rejects
+    const cudaError_t e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) { fprintf(stderr, "bark_b200_parity_rows: %s\n", cudaGetErrorString(e)); return 0; }
+    unsigned cnt[2];
+    BARK_CUDA_CHECK(cudaMemcpy(cnt, dcnt, sizeof(cnt), cudaMemcpyDeviceToHost));
+    BARK_CUDA_CHECK(cudaMemcpy(out, dout, bytes, cudaMemcpyDeviceToHost));
+    *replays = cnt[0] + cnt[1];
+    return 1;
+}
+extern "C" int bark_b200_parity_rows(int op, int impl, const float * x, int rows, int n, const float * g, const float * b, float * out, unsigned * replays) {
+    return guarded((int) 0, [&] { return bark_b200_parity_rows_impl(op, impl, x, rows, n, g, b, out, replays); });
+}
+
 // parity-path tiled GEMM on host buffers (tests, tools/gemm_bench.py): A [M][K] and W [N][K] go through permute_to_gm, as the loader
 // and the activation writers lay them out (row capacity and o_pad rounded up to the tallest / widest tile); the result comes back
 // row-major.  Every output region sits between guard bands and starts as NaN (RESID: as the residual from C).

@@ -209,7 +209,9 @@ __device__ __forceinline__ double approx_rcp(double x) {
 // takes the rounding decision itself (identical inputs, identical arithmetic -> identical result), instead of funnelling
 // through warp 0 and a second barrier.  red: [0,16) double mean partials, [16,24) 16 float |x| partials, [24,40) double
 // variance partials.
-template <bool ROUND16, bool TM, bool NATURAL = false>
+// COPY: 1 in decode_rows_kernel (the row tests) — the same source as a separate function, so that a second caller cannot change the
+// register allocation ptxas picks for the one the decode kernels call.
+template <bool ROUND16, bool TM, bool NATURAL = false, int COPY = 0>
 __device__ __noinline__ void block_layernorm(const float * xs, int E, double inv_E, const float * __restrict__ g, const float * __restrict__ b, float * act,
                                              double * red, unsigned * fallback_counter, int sb) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -1364,6 +1366,26 @@ void launch_decode_cluster(const DecodeArgs & args, WType wt, cudaStream_t s) {
     if (g_prof_on) prof_end(s);
     g_next_bytes = g_next_flops = 0.0;
     ++g_kernel_launches;
+}
+
+// The decode kernels' two row reductions on their own, one CTA of kThreads per row (bark_b200_parity_rows): op 0 = block_layernorm
+// (natural column order, no f16 rounding), op 1 = softmax_exp_rcp with the probabilities formed as P.V forms them.  counters[0] counts
+// LayerNorm replays, counters[1] soft_max replays.
+__global__ void __launch_bounds__(kThreads) decode_rows_kernel(int op, const float * __restrict__ x, int n, double inv_n, const float * __restrict__ g,
+                                                               const float * __restrict__ b, float * __restrict__ out, unsigned * counters) {
+    __shared__ double red[kWarps + kWarps / 2 + kWarps + 4];
+    __shared__ __align__(16) float p[1024];
+    const float * xr = x + (size_t) blockIdx.x * n;
+    float * orow = out + (size_t) blockIdx.x * n;
+    if (op == 0) { block_layernorm<false, false, true, 1>(xr, n, inv_n, g, b, orow, red, counters, 1); return; }
+    for (int i = threadIdx.x; i < n; i += kThreads) p[i] = xr[i];
+    __syncthreads();
+    const float sc_f = softmax_exp_rcp<false>(p, n, red, counters);
+    for (int i = threadIdx.x; i < n; i += kThreads) orow[i] = __fmul_rn(p[i], sc_f);
+}
+
+void decode_rows(int op, const float * x, int rows, int n, const float * g, const float * b, float * out, unsigned * counters, cudaStream_t s) {
+    BARK_LAUNCH(decode_rows_kernel, rows, kThreads, 0, s, op, x, n, 1.0 / n, g, b, out, counters);
 }
 
 static size_t decode_smem_bytes() { return (size_t) SmemLayout::total + 128; }

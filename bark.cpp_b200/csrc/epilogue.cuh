@@ -34,8 +34,9 @@ __device__ __forceinline__ float gelu_lookup(const __half * __restrict__ tab, fl
     return __half2float(tab[__half_as_ushort(__float2half_rn(x))]);
 }
 
-// soft_max over one row of n_kv <= 1024 by one warp (ggml.c:13953-14042 + ggml_vec_soft_max_f32 AVX2 branch ggml.c:2845-2888): in place
-__device__ __forceinline__ void softmax_row(float * __restrict__ p, int n_kv) {
+// soft_max over one row of n_kv <= 1024 by one warp (ggml.c:13953-14042 + ggml_vec_soft_max_f32 AVX2 branch ggml.c:2845-2888): in place.
+// replays (optional): counts the rows whose 1/sum needed the sequential replay (the row tests; the attention kernels pass none).
+__device__ __forceinline__ void softmax_row(float * __restrict__ p, int n_kv, unsigned * replays = nullptr) {
     const int lane = threadIdx.x & 31;
     float mx = __int_as_float(0xff800000);
     for (int i = lane; i < n_kv; i += 32) mx = fmaxf(mx, p[i]);
@@ -93,6 +94,7 @@ __device__ __forceinline__ void softmax_row(float * __restrict__ p, int n_kv) {
             }
             for (int i = nchunks * 8; i < n_kv; i++) sum = __dadd_rn(sum, (double) p[i]);
             sc = __double2float_rn(__ddiv_rn(1.0, sum));
+            if (replays && lane == 0) atomicAdd(replays, 1u);
         }
     }
     __syncwarp();

@@ -547,6 +547,17 @@ __global__ void attn_softmax_kernel(float * __restrict__ S, int rows, int n_kv) 
     softmax_row(S + (size_t) row * n_kv, n_kv);
 }
 
+// the same, counting the rows that took the sequential replay (bark_b200_parity_rows)
+__global__ void softmax_rows_kernel(float * __restrict__ S, int rows, int n, unsigned * __restrict__ replays) {
+    const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (row >= rows) return;
+    softmax_row(S + (size_t) row * n, n, replays);
+}
+
+void softmax_rows(float * S, int rows, int n, unsigned * replays, cudaStream_t s) {
+    BARK_LAUNCH(softmax_rows_kernel, (rows + 7) / 8, 256, 0, s, S, rows, n, replays);
+}
+
 int attn_tiled_max_rows(int H, int n_sm) { return kAttnQ * ((n_sm + H - 1) / H - 1); }
 
 void attention(const float * Q, const float * Kc, const float * Vc, int N, int n_kv, int n_past, int E, int H, bool causal,

@@ -38,6 +38,8 @@ enum AttnPath : int { ATTN_AUTO = 0, ATTN_FUSED = 1, ATTN_TILED = 2 };
 int  attn_tiled_max_rows(int H, int n_sm);
 void attention(const float * Q, const float * Kc, const float * Vc, int N, int n_kv, int n_past, int E, int H, bool causal,
                float * scores, void * act, WType wt, int Kp, cudaStream_t s, AttnPath path = ATTN_AUTO);
+// softmax_row on each of `rows` rows of n <= 1024 floats, in place, one warp per row; replays counts the sequential replays
+void softmax_rows(float * S, int rows, int n, unsigned * replays, cudaStream_t s);
 
 // Decode attention for B <= 8 rows of different sequences (batched step): row b's query is Q[b], its new K / V rows are staged in
 // Kst[b] / Vst[b] and are appended to its cache (kv.k[b], kv.v[b]: the layer's [block_size][E] slab) at position d_pos[b]; it attends
@@ -105,5 +107,8 @@ void launch_decode_step(const DecodeArgs & args, WType wt, int n_sm, cudaStream_
 // the same token inside one 16-CTA cluster (DSMEM exchanges, no polling); see decode_kernels.cu
 bool decode_cluster_supported(const DecodeArgs & args, WType wt, int max_row_bytes);
 void launch_decode_cluster(const DecodeArgs & args, WType wt, cudaStream_t s);
+// the decode kernels' LayerNorm (op 0) or soft_max (op 1) on `rows` rows of n <= 1024 floats, one CTA per row (tests):
+// counters[0] / counters[1] count the LayerNorm / soft_max rows that took the sequential replay
+void decode_rows(int op, const float * x, int rows, int n, const float * g, const float * b, float * out, unsigned * counters, cudaStream_t s);
 
 }  // namespace bark

@@ -93,13 +93,19 @@ def synth_vocab(cfg: Config):
 
 
 class _Writer:
-    def __init__(self, f, rng):
+    def __init__(self, f, rng, overrides=None):
         self.f, self.rng = f, rng
+        self.overrides = dict(overrides or {})
+        self.scope = ""                          # "semantic/", "coarse/", "fine/" while a GPT is written, "" for the codec
 
     def i32(self, *v):
         self.f.write(struct.pack("<%di" % len(v), *v))
 
     def tensor(self, name: str, arr: np.ndarray, ttype: int):
+        new = self.overrides.pop(self.scope + name, None)
+        if new is not None:                      # the seeded values are still drawn, so every other tensor keeps its bytes
+            assert np.shape(new) == arr.shape, (self.scope + name, np.shape(new), arr.shape)
+            arr = np.asarray(new)
         arr = np.ascontiguousarray(arr.astype(np.float16 if ttype == F16 else np.float32))
         nb = name.encode()
         self.i32(arr.ndim, len(nb), ttype)
@@ -196,10 +202,12 @@ def _write_codec(w: _Writer, ftype: int, with_encoder: bool):
         w.tensor(f"quantizer.vq.layers.{q}._codebook.embed", w.normal((n_bins, hidden), 1.0), F32)
 
 
-def write_weights(path: str, cfg: Config, seed: int = 1234, with_encoder: bool = True) -> str:
+def write_weights(path: str, cfg: Config, seed: int = 1234, with_encoder: bool = True, overrides: dict | None = None) -> str:
+    """overrides: tensor name -> array written instead of the seeded values (same shape); the names of the three GPTs' tensors
+    are prefixed with "semantic/", "coarse/" or "fine/" (e.g. "coarse/model/wpe"), the codec's are as in the file."""
     rng = np.random.Generator(np.random.PCG64(seed))
     with open(path, "wb") as f:
-        w = _Writer(f, rng)
+        w = _Writer(f, rng, overrides)
         f.write(struct.pack("<I", MAGIC))
         vocab = synth_vocab(cfg)
         w.i32(len(vocab))
@@ -207,11 +215,17 @@ def write_weights(path: str, cfg: Config, seed: int = 1234, with_encoder: bool =
             b = t.encode()
             f.write(struct.pack("<I", len(b)))
             f.write(b)
+        w.scope = "semantic/"
         _write_gpt(w, cfg.semantic, cfg.sem_in, cfg.sem_out, 1, 1, 0, cfg.gpt_ftype, cfg.lm_head_std)
+        w.scope = "coarse/"
         _write_gpt(w, cfg.coarse, cfg.coarse_vocab, cfg.coarse_vocab, 1, 1, 0, cfg.gpt_ftype, cfg.lm_head_std)
+        w.scope = "fine/"
         _write_gpt(w, cfg.fine, cfg.fine_vocab, cfg.fine_vocab, 7, 8, 1, cfg.gpt_ftype, cfg.lm_head_std)
         f.write(struct.pack("<I", MAGIC))
+        w.scope = ""
         _write_codec(w, cfg.codec_ftype, with_encoder)
+        if w.overrides:
+            raise KeyError(f"no tensor named {sorted(w.overrides)}")
     return path
 
 

@@ -115,6 +115,13 @@ BARK_API int  bark_b200_fast_attention(const uint16_t * q, const uint16_t * k, c
 BARK_API int  bark_b200_parity_attention(const float * q, const float * k, const float * v, float * out, int N, int n_kv, int n_past, int E, int H, int causal,
                                          int path);
 
+/* Parity-path row reductions on host buffers without a context (tests).  op 0: LayerNorm (eps 1e-5, g required, b may be NULL), the f32
+ * value before any operand rounding; op 1: soft_max, the probability as its consumers form it.  impl 0: the multi-row kernels
+ * (layernorm_act_kernel / softmax_row), impl 1: the decode kernels' device functions (block_layernorm / softmax_exp_rcp) in a
+ * one-CTA-per-row wrapper of 512 threads.  x, out: [rows][n] f32 row-major; n <= 1024.  *replays: number of bracket failures that took
+ * the sequential replay.  Returns 1 on success, 0 on invalid arguments or failure. */
+BARK_API int  bark_b200_parity_rows(int op, int impl, const float * x, int rows, int n, const float * g, const float * b, float * out, unsigned * replays);
+
 /* Parity-path tiled GEMM on host buffers without a context (tests, tools/gemm_bench.py): C = A W^T with every output the reference's
  * vec_dot of its two rows, for A [M][K] and W [N][K] of wtype 0 (f32) or 1 (f16 bits), K % 32 == 0, through the multi-row passes'
  * epilogue `epilogue`:
