@@ -51,7 +51,7 @@ EXPORTS = [
     "bark_b200_profile_enable", "bark_b200_profile_report", "bark_b200_io_counters", "bark_b200_decode_timing",
     "bark_b200_shard_init", "bark_b200_shard_connect", "bark_b200_shard_nvlink_bytes",
     "bark_b200_fast_mode", "bark_b200_fast_gemm", "bark_b200_fast_attention", "bark_b200_parity_attention", "bark_b200_parity_gemm",
-    "bark_b200_parity_rows", "bark_b200_generate_batch", "bark_b200_batch_audio", "bark_b200_batch_tokens", "bark_b200_gpt_eval_slot", "bark_b200_gpt_step_batch",
+    "bark_b200_parity_rows", "bark_b200_sample_given_u", "bark_b200_generate_batch", "bark_b200_batch_audio", "bark_b200_batch_tokens", "bark_b200_gpt_eval_slot", "bark_b200_gpt_step_batch",
     "ggml_time_init", "ggml_time_us", "ggml_time_ms", "ggml_init", "ggml_free",
 ]
 
@@ -133,6 +133,8 @@ def lib() -> C.CDLL:
     L.bark_b200_parity_gemm.argtypes = [vp, vp, vp] + [C.c_int] * 6 + [vp]
     L.bark_b200_parity_rows.restype = C.c_int
     L.bark_b200_parity_rows.argtypes = [C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, vp, vp, C.POINTER(C.c_uint)]
+    L.bark_b200_sample_given_u.restype = C.c_int
+    L.bark_b200_sample_given_u.argtypes = [f32p, C.c_int, C.c_int, C.c_float, vp, C.c_int, i32p, i32p, i32p, f32p]
     L.bark_b200_generate_batch.restype = C.c_bool
     L.bark_b200_generate_batch.argtypes = [vp, C.POINTER(C.c_char_p), C.POINTER(C.c_uint32), C.c_int, C.c_int]
     L.bark_b200_batch_audio.restype = C.c_int
@@ -471,6 +473,28 @@ def parity_rows(x: np.ndarray, op: str, impl: str, g: np.ndarray | None = None, 
     if not lib().bark_b200_parity_rows(ROW_OPS[op], ROW_IMPLS[impl], _p(x), rows, n, gp, bp, _p(out), C.byref(rep)):
         raise RuntimeError(f"bark_b200_parity_rows ({op}, {impl}, {rows} x {n}) failed")
     return out, rep.value
+
+
+def sample_given_u(logits: np.ndarray, temp: float, u=None, threads: int = 0):
+    """The device sampler on logits [rows][n] float32 with the uniform draws u [rows] given (not used when temp == 0); threads 0 runs
+    sample_rows_kernel as the library picks it, 256 or 1024 forces that instantiation.  Returns a dict: tokens (final), device_tokens
+    (the kernel's, before the host replay), flags, eos_p [rows] and replays (how many rows went to the host replay)."""
+    l = np.ascontiguousarray(logits, np.float32)
+    if l.ndim == 1:
+        l = l[None]
+    rows, n = l.shape
+    up = None
+    if u is not None:
+        u = np.ascontiguousarray(np.broadcast_to(np.asarray(u, np.float64), (rows,)))
+        up = _p(u)
+    out = {k: np.zeros(rows, np.int32) for k in ("tokens", "device_tokens", "flags")}
+    out["eos_p"] = np.zeros(rows, np.float32)
+    r = lib().bark_b200_sample_given_u(_p(l), n, rows, temp, up, threads, _p(out["tokens"]), _p(out["device_tokens"]), _p(out["flags"]),
+                                       _p(out["eos_p"]))
+    if r < 0:
+        raise RuntimeError(f"bark_b200_sample_given_u ({rows} x {n}, temp {temp}, threads {threads}) failed")
+    out["replays"] = r
+    return out
 
 
 def kernel_launches() -> int:

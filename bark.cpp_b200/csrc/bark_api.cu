@@ -1092,6 +1092,51 @@ extern "C" int bark_b200_parity_rows(int op, int impl, const float * x, int rows
     return guarded((int) 0, [&] { return bark_b200_parity_rows_impl(op, impl, x, rows, n, g, b, out, replays); });
 }
 
+// the device sampler on host rows with the uniforms given (tests): sample_rows_kernel at the instantiation asked for, then every
+// flagged row replayed with sample_token_given_u, as sample_device does it.  device_tokens keeps the kernel's tokens before the replay.
+static int bark_b200_sample_given_u_impl(const float * logits, int n, int rows, float temp, const double * u, int threads, int32_t * tokens,
+                                         int32_t * device_tokens, int32_t * flags, float * eos_p) {
+    if (!logits || !tokens || !device_tokens || !flags || !eos_p || (temp != 0.0f && !u)) return -1;
+    if (n < 2 || (size_t) n * 4 > 64 * 1024 || rows < 1 || rows > 1024 || !std::isfinite(temp) || temp < 0.0f) return -1;
+    if (threads != 0 && threads != 256 && threads != 1024) return -1;
+    if (temp != 0.0f) for (int r = 0; r < rows; r++) if (!(u[r] >= 0.0 && u[r] < 1.0)) return -1;
+    struct Buffers {                                          // freed on every exit, including a CUDA failure thrown mid-way
+        void * p[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+        ~Buffers() { for (void * q : p) cudaFree(q); }
+    } d;
+    const size_t bytes = (size_t) rows * n * 4;
+    BARK_CUDA_CHECK(cudaMalloc(&d.p[0], bytes));
+    BARK_CUDA_CHECK(cudaMalloc(&d.p[1], (size_t) rows * sizeof(double)));
+    BARK_CUDA_CHECK(cudaMalloc(&d.p[2], (size_t) rows * 4));
+    BARK_CUDA_CHECK(cudaMalloc(&d.p[3], (size_t) rows * 4));
+    BARK_CUDA_CHECK(cudaMalloc(&d.p[4], (size_t) rows * 4));
+    float * dl = (float *) d.p[0], * deos = (float *) d.p[4]; double * du = (double *) d.p[1]; int32_t * dtok = (int32_t *) d.p[2], * dflags = (int32_t *) d.p[3];
+    BARK_CUDA_CHECK(cudaMemcpy(dl, logits, bytes, cudaMemcpyHostToDevice));
+    if (temp != 0.0f) BARK_CUDA_CHECK(cudaMemcpy(du, u, (size_t) rows * sizeof(double), cudaMemcpyHostToDevice));
+    BARK_CUDA_CHECK(cudaMemset(dtok, 0xff, (size_t) rows * 4));                 // -1 / NaN: a missing store shows up
+    BARK_CUDA_CHECK(cudaMemset(dflags, 0xff, (size_t) rows * 4));
+    BARK_CUDA_CHECK(cudaMemset(deos, 0xff, (size_t) rows * 4));
+    sample_rows_threads(threads, dl, n, rows, temp, du, dtok, deos, dflags, 0);
+    BARK_CUDA_CHECK(cudaGetLastError());                      // a launch the configuration rejects
+    const cudaError_t e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) { fprintf(stderr, "bark_b200_sample_given_u: %s\n", cudaGetErrorString(e)); return -1; }
+    BARK_CUDA_CHECK(cudaMemcpy(device_tokens, dtok, (size_t) rows * 4, cudaMemcpyDeviceToHost));
+    BARK_CUDA_CHECK(cudaMemcpy(flags, dflags, (size_t) rows * 4, cudaMemcpyDeviceToHost));
+    BARK_CUDA_CHECK(cudaMemcpy(eos_p, deos, (size_t) rows * 4, cudaMemcpyDeviceToHost));
+    int replays = 0;
+    for (int r = 0; r < rows; r++) {
+        tokens[r] = device_tokens[r];
+        if (!flags[r]) continue;
+        tokens[r] = sample_token_given_u(logits + (size_t) r * n, n, temp, temp != 0.0f ? u[r] : 0.0, &eos_p[r]);
+        replays++;
+    }
+    return replays;
+}
+extern "C" int bark_b200_sample_given_u(const float * logits, int n, int rows, float temp, const double * u, int threads, int32_t * tokens,
+                                        int32_t * device_tokens, int32_t * flags, float * eos_p) {
+    return guarded((int) -1, [&] { return bark_b200_sample_given_u_impl(logits, n, rows, temp, u, threads, tokens, device_tokens, flags, eos_p); });
+}
+
 // parity-path tiled GEMM on host buffers (tests, tools/gemm_bench.py): A [M][K] and W [N][K] go through permute_to_gm, as the loader
 // and the activation writers lay them out (row capacity and o_pad rounded up to the tallest / widest tile); the result comes back
 // row-major.  Every output region sits between guard bands and starts as NaN (RESID: as the residual from C).

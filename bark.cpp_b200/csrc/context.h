@@ -119,6 +119,8 @@ bool codec_decode(bark_context * ctx, const int32_t * codes, int T, std::vector<
 // sampling.cu / gpt_forward.cu / bark_api.cu
 void sample_rows(const float * logits, int ld, int n, int rows, float temp, const double * d_u, int32_t * d_out_tok, int tok_add, int32_t * d_feed,
                  float * d_eos_p, int32_t * d_flags, int force_flag, cudaStream_t s);
+void sample_rows_threads(int threads, const float * logits, int n, int rows, float temp, const double * d_u, int32_t * d_out_tok, float * d_eos_p,
+                         int32_t * d_flags, cudaStream_t s);
 bool gpt_decode_chained(bark_context * ctx, GPTModel & m, const int32_t * d_token, int * n_past, int lm_lo, int lm_hi);
 bool sample_device(bark_context * ctx, GPTModel & m, std::mt19937 & rng, const float * d_logits, int ld, int n, int rows, float temp, int32_t * out_tok, float * out_eos);
 int32_t sample_token_given_u(const float * logits, int n, float temp, double u, float * eos_p);

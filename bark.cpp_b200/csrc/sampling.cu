@@ -14,8 +14,11 @@
 //   * the multinomial draw: the uniform u comes from the host's std::mt19937 stream (same two 32-bit draws per sample);
 //     the partial sums are formed in parallel in double and compared with u * total; if any partial sum lies within the
 //     rounding-error bound of the threshold the row is FLAGGED.
-// Flagged rows (probability ~1e-7 per row) are re-sampled on the host with the reference's exact sequence, using the same
-// u, so the token stream is identical to the host path in all cases.
+// Flagged rows are re-sampled on the host with the reference's exact sequence, using the same u, so the token stream is
+// identical to the host path in all cases.  How often real rows are flagged has not been measured.  tests/test_sampler_orders.py
+// restates both orders and brackets and builds rows on the decision edges; tests/test_sampler_gpu.py runs them through both
+// instantiations (bark_b200_sample_given_u).  eps = 0 fails test_threshold_rows and test_edge_rows; `>=` in the per-thread argmax
+// fails test_argmax_rows; dropping the exp check fails test_exp_rows and test_exp_rounding_against_glibc (DESIGN.md section 2).
 #include "gpt_kernels.h"
 
 namespace bark {
@@ -147,6 +150,21 @@ void sample_rows(const float * logits, int ld, int n, int rows, float temp, cons
     g_next_bytes = (double) rows * n * 4.0;
     if (rows == 1) BARK_LAUNCH(sample_rows_kernel<1024>, rows, 1024, smem, s, logits, ld, n, rows, temp, d_u, d_out_tok, tok_add, d_feed, d_eos_p, d_flags, force_flag);
     else           BARK_LAUNCH(sample_rows_kernel<256>, rows, 256, smem, s, logits, ld, n, rows, temp, d_u, d_out_tok, tok_add, d_feed, d_eos_p, d_flags, force_flag);
+}
+
+// The same kernels with the instantiation chosen by the caller (bark_b200_sample_given_u, tests): threads 0 picks as sample_rows does,
+// 256 or 1024 forces that one, so every row can be checked at both.  Rows are packed (ld = n), no offset, no feed, no forced flag.
+void sample_rows_threads(int threads, const float * logits, int n, int rows, float temp, const double * d_u, int32_t * d_out_tok, float * d_eos_p,
+                         int32_t * d_flags, cudaStream_t s) {
+    const size_t smem = ((size_t) n * sizeof(float) + 15) & ~(size_t) 15;
+    static std::atomic<unsigned long long> configured{0};
+    if (first_use_on_this_device(configured)) {
+        BARK_CUDA_CHECK(cudaFuncSetAttribute(sample_rows_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+        BARK_CUDA_CHECK(cudaFuncSetAttribute(sample_rows_kernel<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+    }
+    if (threads == 0) threads = rows == 1 ? 1024 : 256;
+    if (threads == 1024) BARK_LAUNCH(sample_rows_kernel<1024>, rows, 1024, smem, s, logits, n, n, rows, temp, d_u, d_out_tok, 0, nullptr, d_eos_p, d_flags, 0);
+    else                 BARK_LAUNCH(sample_rows_kernel<256>, rows, 256, smem, s, logits, n, n, rows, temp, d_u, d_out_tok, 0, nullptr, d_eos_p, d_flags, 0);
 }
 
 }  // namespace bark

@@ -122,6 +122,15 @@ BARK_API int  bark_b200_parity_attention(const float * q, const float * k, const
  * the sequential replay.  Returns 1 on success, 0 on invalid arguments or failure. */
 BARK_API int  bark_b200_parity_rows(int op, int impl, const float * x, int rows, int n, const float * g, const float * b, float * out, unsigned * replays);
 
+/* The device sampler on host rows without a context (tests): gpt_sample for each of `rows` logit rows of n (packed [rows][n] f32) with
+ * the uniform draw u[r] given (u may be NULL when temp == 0, where it is not used).  Runs sample_rows_kernel with `threads` threads per
+ * row (0: as the library picks, 1024 for a single row and 256 otherwise; or 256, or 1024), then replays every row the kernel flags on
+ * the host with the reference's sequence, as the library does.  tokens: the final tokens; device_tokens: the kernel's tokens before the
+ * replay; flags: 1 where the kernel could not prove its decision; eos_p: the probability of the last logit.  2 <= n, n * 4 <= 64 KB,
+ * 1 <= rows <= 1024, temp finite and >= 0, every u in [0, 1).  Returns the number of replayed rows, or -1 on invalid arguments or failure. */
+BARK_API int  bark_b200_sample_given_u(const float * logits, int n, int rows, float temp, const double * u, int threads, int32_t * tokens,
+                                       int32_t * device_tokens, int32_t * flags, float * eos_p);
+
 /* Parity-path tiled GEMM on host buffers without a context (tests, tools/gemm_bench.py): C = A W^T with every output the reference's
  * vec_dot of its two rows, for A [M][K] and W [N][K] of wtype 0 (f32) or 1 (f16 bits), K % 32 == 0, through the multi-row passes'
  * epilogue `epilogue`:

@@ -736,7 +736,8 @@ int orc_fine_eval(orc_ctx * c, const int32_t * in, int nn, float * logits) {
 /* ------------------------------------------------------------------------------------------ */
 /* sampling (bark.cpp:184-270)                                                                 */
 /* ------------------------------------------------------------------------------------------ */
-int orc_sample(orc_ctx * c, const float * logits_in, int n, float temp, float * eos_p) {
+/* gpt_sample with the uniform draw u already made (u is not used when temp == 0) */
+int orc_sample_u(const float * logits_in, int n, float temp, double u, float * eos_p) {
     float * l = malloc((size_t) n * 4);
     const float t = (temp == 0.0f) ? 0.7f : temp;                              /* bark.cpp:226-228 quirk */
     for (int i = 0; i < n; i++) l[i] = logits_in[i] / t;
@@ -756,15 +757,17 @@ int orc_sample(orc_ctx * c, const float * logits_in, int n, float temp, float * 
         double run = 0.0;
         for (int i = 0; i < n; i++) { double p = (double) l[i] / s; run = (i == 0) ? p : run + p; cp[i] = run; }
         cp[n - 1] = 1.0;
-        const double p = mt_canonical(c->rng);
-        int lo = 0, hi = n;                                                    /* lower_bound: first cp[i] >= p */
-        while (lo < hi) { int mid = lo + (hi - lo) / 2; if (cp[mid] < p) lo = mid + 1; else hi = mid; }
+        int lo = 0, hi = n;                                                    /* lower_bound: first cp[i] >= u */
+        while (lo < hi) { int mid = lo + (hi - lo) / 2; if (cp[mid] < u) lo = mid + 1; else hi = mid; }
         next = lo;
         free(cp);
     }
     if (eos_p) *eos_p = l[n - 1];
     free(l);
     return next;
+}
+int orc_sample(orc_ctx * c, const float * logits_in, int n, float temp, float * eos_p) {
+    return orc_sample_u(logits_in, n, temp, temp == 0.0f ? 0.0 : mt_canonical(c->rng), eos_p);   /* one draw per sample, none for argmax */
 }
 
 /* ------------------------------------------------------------------------------------------ */

@@ -40,6 +40,7 @@ int  orc_gpt_eval(orc_ctx * c, int which, const int32_t * tokens, int n, int * n
 int  orc_fine_eval(orc_ctx * c, const int32_t * in_buffer, int nn, float * logits_out);
 /* gpt_sample (bark.cpp:249) on the context's mt19937 */
 int  orc_sample(orc_ctx * c, const float * logits, int n, float temp, float * eos_p);
+int  orc_sample_u(const float * logits, int n, float temp, double u, float * eos_p);   /* the same with the uniform draw given */
 
 /* stage loops; return counts.  Buffers sized by the caller (<=768 semantic, frames<=1024) */
 int  orc_semantic(orc_ctx * c, const int32_t * prompt513, int32_t * out);

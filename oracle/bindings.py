@@ -204,6 +204,37 @@ class Ref:
         a = np.zeros(14, np.int64); self.L.ref_get_stats(self.ctx, _p(a)); return a
 
 
+_orc_lib = None
+
+
+def _oracle_lib():
+    global _orc_lib
+    if _orc_lib is None:
+        if not os.path.exists(ORACLE_SO):
+            build_oracle()
+        L = C.CDLL(ORACLE_SO)
+        L.orc_sample_u.restype = C.c_int
+        L.orc_sample_u.argtypes = [vp, C.c_int, C.c_float, C.c_double, C.POINTER(C.c_float)]
+        L.orc_mt_seed.argtypes = [vp, C.c_uint32]
+        L.orc_mt_next.restype = C.c_uint32
+        L.orc_mt_next.argtypes = [vp]
+        _orc_lib = L
+    return _orc_lib
+
+
+def sample_u(logits, temp, u):
+    """gpt_sample of one logit row with the uniform draw u given (orc_sample_u): (token, probability of the last logit)."""
+    l = np.ascontiguousarray(logits, np.float32); e = C.c_float(0)
+    return _oracle_lib().orc_sample_u(_p(l), l.size, temp, float(u), C.byref(e)), e.value
+
+
+def mt_words(seed, k):
+    """The first k 32-bit outputs of std::mt19937(seed) (orc_mt_seed / orc_mt_next)."""
+    L = _oracle_lib()
+    st = np.zeros(625, np.uint32); L.orc_mt_seed(_p(st), seed)
+    return np.array([L.orc_mt_next(_p(st)) for _ in range(k)], np.uint64)
+
+
 def gelu_tables():
     """(oracle table, reference table or None): gelu evaluated at every f16 input, as f16 bits."""
     if not os.path.exists(ORACLE_SO):
