@@ -770,7 +770,7 @@ extern "C" struct bark_context * bark_load_model(const char * model_path, struct
     { const char * e = getenv("BARK_B200_SAMPLE_FLAG_EVERY"); ctx->debug_flag_every = e ? atoi(e) : 0; }
     { const char * e = getenv("BARK_B200_SAMPLE"); ctx->sample_on_device = !(e && !strcmp(e, "host")); }      // "host": read logits back and sample on the CPU (A-B)
     { const char * e = getenv("BARK_B200_KV_REUSE"); ctx->kv_reuse = !(e && !strcmp(e, "0")); }              // "0": re-prefill every coarse window like the reference (A-B)
-    { const char * e = getenv("BARK_B200_DECODE"); ctx->use_decode_kernel = !(e && !strcmp(e, "multi")); ctx->decode_cluster = e && !strcmp(e, "cluster"); }   // "multi": one kernel per op (debug / A-B)
+    { const char * e = getenv("BARK_B200_DECODE"); ctx->use_decode_kernel = !(e && !strcmp(e, "multi")); }   // "multi": one kernel per op (debug / A-B)
     { const char * e = getenv("BARK_B200_DECODE_TIMING_TID"); if (e && atoi(e) >= 0 && atoi(e) < 512) ctx->timing_tid = atoi(e) & ~31; }
     { const char * e = getenv("BARK_B200_POLL_NS"); if (e && atoi(e) >= 0 && atoi(e) <= 100000) ctx->poll_ns = (unsigned) atoi(e); }
     { const char * e = getenv("BARK_B200_HEADSTART"); if (e) { unsigned v[6]; if (sscanf(e, "%u:%u:%u:%u:%u:%u", &v[0], &v[1], &v[2], &v[3], &v[4], &v[5]) == 6) for (int i = 0; i < 6; i++) ctx->headstart[i] = std::min(v[i], 100000u); } }

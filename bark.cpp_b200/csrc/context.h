@@ -53,7 +53,6 @@ struct bark_context {
     bool kv_reuse = true; unsigned long long n_kv_reused = 0;   // coarse windows start from the cached prefix (bark_api.cu run_coarse)
     // decode-kernel knobs (BARK_B200_DECODE_TIMING_TID / BARK_B200_POLL_NS / BARK_B200_HEADSTART); defaults:
     // 40 ns back-off between polls, 500 ns head start for the two residual exchanges
-    bool decode_cluster = false;                     // BARK_B200_DECODE=cluster: the decode step inside one 16-CTA cluster (decode_kernels.cu) where the model fits
     unsigned headstart[6] = {0, 2000, 500, 400, 500, 0};   // BARK_B200_HEADSTART=q:att:x1:ff:x2:scores (ns): sleep before the first poll of each exchange
     int timing_tid = 0; unsigned poll_ns = 40;
     unsigned long long * d_timing = nullptr;         // optional phase timestamps of the decode kernel (BARK_B200_DECODE_TIMING=1)

@@ -132,10 +132,7 @@ static void decode_step(bark_context * ctx, GPTModel & m, int token, const int32
     const double E = m.n_embd, L = m.n_layer;
     g_next_bytes = (12.0 * L * E * E + (double)(lm_hi - lm_lo) * E) * es + 2.0 * L * (double)(n_past + 1) * E * 4.0 + 2.0 * L * E * 4.0 + (double)(lm_hi - lm_lo) * 4.0;   // SURVEY §8d B_tok
     g_next_flops = 2.0 * (12.0 * L * E * E + (double)(lm_hi - lm_lo) * E) + 4.0 * L * (double)(n_past + 1) * E;
-    int max_row_bytes = 0;
-    for (const DMat * d : {&m.layers[0].c_attn, &m.layers[0].c_proj, &m.layers[0].fc, &m.layers[0].proj, &m.lm_head[0]}) max_row_bytes = std::max(max_row_bytes, (int)(d->Kp * (m.wtype == W_F16 ? 2 : 4)));   // (cluster kernel: f16 / f32 only)
-    if (ctx->decode_cluster && decode_cluster_supported(a, m.wtype, max_row_bytes)) launch_decode_cluster(a, m.wtype, ctx->stream);
-    else launch_decode_step(a, m.wtype, ctx->n_sm, ctx->stream);
+    launch_decode_step(a, m.wtype, ctx->n_sm, ctx->stream);
     ctx->tag_base += (unsigned) decode_tags_per_step(m.n_layer);
 }
 

@@ -224,8 +224,6 @@ __global__ void __launch_bounds__(256) lane_matmul_kernel(const T * __restrict__
     }
 }
 
-static bool use_tiled() { static const bool t = [] { const char * e = getenv("BARK_B200_GEMM"); return !(e && !strcmp(e, "simple")); }(); return t; }
-
 void lane_matmul(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, cudaStream_t s) {
     if (W.type == W_Q4_0) { q4_matmul(W, act, act_gs, rows, ep, s); return; }      // act_gs = f32 row stride for this type
     if (qx_supported(W.type)) { qx_matmul(W, act, act_gs, rows, ep, s); return; }
@@ -235,7 +233,7 @@ void lane_matmul(const DMat & W, const void * act, int act_gs, int rows, const M
         g_next_bytes = (double) W.n_out * W.K * es + (double) rows * (W.K * es + W.n_out * 4.0);
         g_next_flops = 2.0 * rows * (double) W.n_out * W.K;
     }
-    if (rows >= 16 && use_tiled() && (W.type == W_F16 || W.type == W_F32)) { lane_gemm_tiled(W, act, act_gs, rows, ep, s); return; }
+    if (rows >= 16 && (W.type == W_F16 || W.type == W_F32)) { lane_gemm_tiled(W, act, act_gs, rows, ep, s); return; }
     if (W.type == W_F16) {
         if (rows == 1) BARK_LAUNCH((lane_matmul_kernel<__half, 1>), dim3(gx, 1), 256, 0, s, (const __half *) W.p, W.K, W.Kp, W.n_out, (const __half *) act, act_gs, rows, ep);
         else           BARK_LAUNCH((lane_matmul_kernel<__half, 8>), dim3(gx, (rows + 7) / 8), 256, 0, s, (const __half *) W.p, W.K, W.Kp, W.n_out, (const __half *) act, act_gs, rows, ep);

@@ -104,9 +104,6 @@ struct DecodeArgs {
 };
 int  decode_tags_per_step(int n_layer);
 void launch_decode_step(const DecodeArgs & args, WType wt, int n_sm, cudaStream_t s);
-// the same token inside one 16-CTA cluster (DSMEM exchanges, no polling); see decode_kernels.cu
-bool decode_cluster_supported(const DecodeArgs & args, WType wt, int max_row_bytes);
-void launch_decode_cluster(const DecodeArgs & args, WType wt, cudaStream_t s);
 // the decode kernels' LayerNorm (op 0) or soft_max (op 1) on `rows` rows of n <= 1024 floats, one CTA per row (tests):
 // counters[0] / counters[1] count the LayerNorm / soft_max rows that took the sequential replay
 void decode_rows(int op, const float * x, int rows, int n, const float * g, const float * b, float * out, unsigned * counters, cudaStream_t s);

@@ -127,32 +127,6 @@ def test_sampler_paths_agree(pkg, weights_file, monkeypatch):
         assert np.array_equal(bits(a1), bits(runs[0][0])) and np.array_equal(bits(a2), bits(runs[0][2]))
 
 
-@pytest.mark.parametrize("config", ["mini", "small"])
-def test_cluster_decode_variant_is_bit_identical(pkg, weights_file, monkeypatch, config):
-    """BARK_B200_DECODE=cluster (each token inside one 16-CTA thread-block cluster, gpt_decode_cluster_kernel) against the default
-    grid-wide decode kernel on f16 models the cluster variant supports (mini; bark-small dimensions): same token ids, same waveform
-    bits, and the profile shows that the cluster kernel really evaluated the tokens."""
-    path = weights_file(config, "f16")
-    runs = {}
-    for mode in ("grid", "cluster"):
-        monkeypatch.delenv("BARK_B200_DECODE", raising=False)
-        if mode == "cluster":
-            monkeypatch.setenv("BARK_B200_DECODE", "cluster")
-        with pkg.Bark(path, seed=0, n_steps_text_encoder=24) as b:
-            pkg.profile_enable(True)
-            try:
-                audio = b.generate("hello world")
-                rep = pkg.profile_report()
-            finally:
-                pkg.profile_enable(False)
-            runs[mode] = (audio, [b.tokens(i).copy() for i in range(3)], rep)
-    assert any(k.startswith("gpt_decode_cluster_kernel") for k in runs["cluster"][2]), sorted(runs["cluster"][2])
-    assert not any(k.startswith("gpt_decode_cluster_kernel") for k in runs["grid"][2])
-    for a, c in zip(runs["grid"][1], runs["cluster"][1]):
-        assert np.array_equal(a, c)
-    assert np.array_equal(bits(runs["grid"][0]), bits(runs["cluster"][0]))
-
-
 def test_coarse_prefix_reuse_on_a_long_clip(pkg, weights_file, monkeypatch):
     """230 semantic tokens -> 690 coarse steps in 12 windows: the semantic window start moves (semantic_idx > 209) and the
     coarse history saturates at 630, so window prompts stop being extensions of the cache.  Prefix reuse (default) must give

@@ -180,9 +180,9 @@ def test_replay_in_a_coarse_prefill(pkg, orc, built_model):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("mode", ["grid", "cluster", "multi"])
+@pytest.mark.parametrize("mode", ["grid", "multi"])
 def test_replay_in_single_token_steps(pkg, orc, built_model, monkeypatch, mode):
-    """BARK_B200_DECODE unset: gpt_decode_step_kernel; cluster: gpt_decode_cluster_kernel; multi: one kernel per op"""
+    """BARK_B200_DECODE unset: gpt_decode_step_kernel; multi: one kernel per op"""
     monkeypatch.delenv("BARK_B200_DECODE", raising=False)
     if mode != "grid":
         monkeypatch.setenv("BARK_B200_DECODE", mode)

@@ -47,7 +47,7 @@ def main():
                     _, p = b.gpt_eval(1, np.array([10001], np.int32), p, False)
                 rep = pkg.profile_report()
                 pkg.profile_enable(False)
-                v = rep.get("gpt_decode_step_kernel") or rep["gpt_decode_cluster_kernel"]
+                v = rep["gpt_decode_step_kernel"]
                 us = v["ms"] * 1e3 / v["launches"]
                 out.append(dict(poll_ns=int(poll), headstart=headstart or "default", n_kv_start=n_past + 6, us_per_token=round(us, 2), launches=v["launches"]))
                 print(f"poll {poll:>5s} headstart {headstart or 'default'}  n_kv {n_past + 6:4d}..{p:4d}: {us:7.2f} us per decode step", flush=True)
