@@ -71,7 +71,7 @@ struct bark_context {
     int32_t * d_stok = nullptr, * h_stok = nullptr, * d_sflags = nullptr, * h_sflags = nullptr;
     float * d_seos = nullptr, * h_seos = nullptr;
     int32_t * d_feed = nullptr;                      // token handed from sample_rows_kernel to the next decode step
-    bool sample_on_device = true; long long n_sample_host_replays = 0;
+    long long n_sample_host_replays = 0;
     int debug_flag_every = 0; long long n_sample_calls = 0;   // BARK_B200_SAMPLE_FLAG_EVERY=k: force every k-th sample through the host replay (tests)
     float * h_logits = nullptr;                      // pinned, max(n_out) or 1024*fine_vocab
     int32_t * h_tok = nullptr;                       // pinned, 8*1024 ids
@@ -112,17 +112,24 @@ bool fine_eval(bark_context * ctx, const int32_t * in_buffer /*[8][1024]*/, int 
 bool fine_eval_shard(bark_context * ctx, const int32_t * in_buffer, int nn);                          // this rank's rows of one pass (shard.cu)
 bool sample_shard(bark_context * ctx, std::mt19937 & rng, int n, float temp, int32_t * out_all /*[1024]*/);
 bool fine_eval_fast(bark_context * ctx, const int32_t * in_buffer, int nn, float * logits_host);      // tensor-core variant (fast mode)
+bool gpt_decode_chained(bark_context * ctx, GPTModel & m, const int32_t * d_token, int * n_past, int lm_lo, int lm_hi);
 // EnCodec decode; codes [8][T] on the host; result in `audio`
 bool codec_decode(bark_context * ctx, const int32_t * codes, int T, std::vector<float> & audio);
 
-// sampling.cu / gpt_forward.cu / bark_api.cu
+// sampling.cu
+constexpr int kSampleMaxLogits = 16384;          // logits of one row: sample_rows_kernel holds the row in 64 KB of shared memory
+// sample_rows_kernel over `rows` rows of n logits (stride ld); threads 256 or 1024 per row, 0 picks 1024 for one row and 256 otherwise
 void sample_rows(const float * logits, int ld, int n, int rows, float temp, const double * d_u, int32_t * d_out_tok, int tok_add, int32_t * d_feed,
-                 float * d_eos_p, int32_t * d_flags, int force_flag, cudaStream_t s);
-void sample_rows_threads(int threads, const float * logits, int n, int rows, float temp, const double * d_u, int32_t * d_out_tok, float * d_eos_p,
-                         int32_t * d_flags, cudaStream_t s);
-bool gpt_decode_chained(bark_context * ctx, GPTModel & m, const int32_t * d_token, int * n_past, int lm_lo, int lm_hi);
-bool sample_device(bark_context * ctx, GPTModel & m, std::mt19937 & rng, const float * d_logits, int ld, int n, int rows, float temp, int32_t * out_tok, float * out_eos);
+                 float * d_eos_p, int32_t * d_flags, int force_flag, int threads, cudaStream_t s);
+// gpt_sample of one row on the host with the uniform u already drawn (unused when temp == 0)
 int32_t sample_token_given_u(const float * logits, int n, float temp, double u, float * eos_p);
+// Samples `rows` (<= 1024) rows of device logits, row r at d_logits + r * ld + lo, n <= kSampleMaxLogits wide, with the uniforms the
+// caller put in ctx->h_u[0, rows) (temp != 0).  One synchronisation reads the tokens (lo added), the flags and, with want_eos, the
+// probabilities of the last logit back to ctx->h_stok / h_sflags / h_seos; every flagged row is then replayed on the host with
+// sample_token_given_u and the same uniform.  Returns the number of rows replayed.
+int sample_and_replay(bark_context * ctx, const float * d_logits, int ld, int lo, int n, int rows, float temp, bool want_eos);
+// sample_and_replay with `rows` uniforms drawn from rng; tokens to out_tok, eos probabilities to out_eos when it is set
+bool sample_device(bark_context * ctx, GPTModel & m, std::mt19937 & rng, const float * d_logits, int ld, int n, int rows, float temp, int32_t * out_tok, float * out_eos);
 
 int64_t now_us();
 

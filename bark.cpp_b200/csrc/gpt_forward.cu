@@ -317,39 +317,6 @@ bool fine_eval_fast(bark_context * ctx, const int32_t * in_buffer, int nn, float
     return true;
 }
 
-// Sample `rows` tokens from device-resident logits (sampling.cu); rows the kernel could not decide bit-safely are replayed
-// on the host with the reference's exact arithmetic and the same uniform draw.  Leaves tokens (and optionally the
-// probability of the last logit) in out_tok / out_eos.  The RNG stream advances exactly as gpt_sample would advance it.
-bool sample_device(bark_context * ctx, GPTModel & m, std::mt19937 & rng, const float * d_logits, int ld, int n, int rows, float temp, int32_t * out_tok, float * out_eos) {
-    const int64_t t0 = now_us();
-    cudaStream_t s = ctx->stream;
-    if (rows < 1 || rows > 1024 || n < 2 || (size_t) n * 4 > 64 * 1024) { fprintf(stderr, "%s: unsupported shape (%d rows of %d)\n", __func__, rows, n); return false; }
-    if (temp != 0.0f) {
-        for (int r = 0; r < rows; r++) ctx->h_u[r] = std::generate_canonical<double, 53>(rng);   // what discrete_distribution::operator() draws
-        BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->d_u, ctx->h_u, (size_t) rows * sizeof(double), cudaMemcpyHostToDevice, s)); g_h2d_bytes += (size_t) rows * sizeof(double);
-    }
-    const int force = ctx->debug_flag_every > 0 && (ctx->n_sample_calls++ % ctx->debug_flag_every) == 0;
-    sample_rows(d_logits, ld, n, rows, temp, ctx->d_u, ctx->d_stok, 0, nullptr, ctx->d_seos, ctx->d_sflags, force, s);
-    BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->h_stok, ctx->d_stok, (size_t) rows * 4, cudaMemcpyDeviceToHost, s));
-    BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->h_sflags, ctx->d_sflags, (size_t) rows * 4, cudaMemcpyDeviceToHost, s));
-    BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->h_seos, ctx->d_seos, (size_t) rows * 4, cudaMemcpyDeviceToHost, s)); g_d2h_bytes += (size_t) rows * 12;
-    BARK_CUDA_CHECK(cudaStreamSynchronize(s));
-    std::vector<float> row;
-    for (int r = 0; r < rows; r++) {
-        if (ctx->h_sflags[r]) {
-            row.resize((size_t) n);
-            BARK_CUDA_CHECK(cudaMemcpy(row.data(), d_logits + (size_t) r * ld, (size_t) n * 4, cudaMemcpyDeviceToHost)); g_d2h_bytes += (size_t) n * 4;
-            ctx->h_stok[r] = sample_token_given_u(row.data(), n, temp, ctx->h_u[r], &ctx->h_seos[r]);
-            ctx->n_sample_host_replays++;
-        }
-        out_tok[r] = ctx->h_stok[r];
-        if (out_eos) out_eos[r] = ctx->h_seos[r];
-    }
-    m.t_sample_us += now_us() - t0;
-    m.n_sample += rows;
-    return true;
-}
-
 bool codec_decode(bark_context * ctx, const int32_t * codes, int T, std::vector<float> & audio) {
     if (T < 7) { fprintf(stderr, "%s: need at least 7 frames (reflect padding of the k=7 convolutions), got %d\n", __func__, T); return false; }
     CodecModel & cm = ctx->codec;

@@ -117,23 +117,13 @@ bool sample_shard(bark_context * ctx, std::mt19937 & rng, int n, float temp, int
     cudaStream_t s = ctx->stream;
     const int rows = 1024 / S.world, row0 = S.rank * rows;
     const int64_t t0 = now_us();
-    double u_all[1024];
-    if (temp != 0.0f) for (int r = 0; r < 1024; r++) u_all[r] = std::generate_canonical<double, 53>(rng);
-    memcpy(ctx->h_u, u_all + row0, (size_t) rows * sizeof(double));
-    BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->d_u, ctx->h_u, (size_t) rows * sizeof(double), cudaMemcpyHostToDevice, s)); g_h2d_bytes += (size_t) rows * sizeof(double);
-    sample_rows(ctx->last_logits, m.n_out_vocab, n, rows, temp, ctx->d_u, ctx->d_stok, 0, nullptr, ctx->d_seos, ctx->d_sflags, 0, s);
-    BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->h_stok, ctx->d_stok, (size_t) rows * 4, cudaMemcpyDeviceToHost, s));
-    BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->h_sflags, ctx->d_sflags, (size_t) rows * 4, cudaMemcpyDeviceToHost, s)); g_d2h_bytes += (size_t) rows * 8;
-    BARK_CUDA_CHECK(cudaStreamSynchronize(s));
-    bool replayed = false;
-    std::vector<float> row;
-    for (int r = 0; r < rows; r++) if (ctx->h_sflags[r]) {                    // too close to call on the device: the reference's exact sequence on the host
-        row.resize((size_t) n);
-        BARK_CUDA_CHECK(cudaMemcpy(row.data(), ctx->last_logits + (size_t) r * m.n_out_vocab, (size_t) n * 4, cudaMemcpyDeviceToHost));
-        ctx->h_stok[r] = sample_token_given_u(row.data(), n, temp, ctx->h_u[r], nullptr);
-        ctx->n_sample_host_replays++; replayed = true;
+    if (temp != 0.0f) for (int r = 0; r < 1024; r++) {
+        const double u = std::generate_canonical<double, 53>(rng);
+        if (r >= row0 && r < row0 + rows) ctx->h_u[r - row0] = u;
     }
-    if (replayed) BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->d_stok, ctx->h_stok, (size_t) rows * 4, cudaMemcpyHostToDevice, s));
+    if (sample_and_replay(ctx, ctx->last_logits, m.n_out_vocab, 0, n, rows, temp, false) > 0) {     // the peers must get the replayed ids
+        BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->d_stok, ctx->h_stok, (size_t) rows * 4, cudaMemcpyHostToDevice, s)); g_h2d_bytes += (size_t) rows * 4;
+    }
     PeerIds P{};
     for (int p = 0; p < S.world; p++) P.ids[p] = shard_ids(S.peer[p], m);
     BARK_LAUNCH(publish_ids_kernel, S.world, 128, 0, s, P, S.world, ctx->d_stok, row0, rows);

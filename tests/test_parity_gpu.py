@@ -107,13 +107,12 @@ def test_device_sampler_matches_oracle(pkg, orc, weights_file):
 
 
 def test_sampler_paths_agree(pkg, weights_file, monkeypatch):
-    """Device sampler (chained decode), forced host replays inside the chain, and the plain host sampler: same tokens and
-    same RNG state afterwards (second clip on the same context)."""
+    """Device sampler (chained decode), forced host replays inside the chain, the per-op decode and the full coarse re-prefill:
+    same tokens and same RNG state afterwards (second clip on the same context)."""
     path = weights_file("mini", "f16")
     runs = []
-    for env in ({}, {"BARK_B200_SAMPLE_FLAG_EVERY": "5"}, {"BARK_B200_SAMPLE": "host"}, {"BARK_B200_DECODE": "multi"}, {"BARK_B200_KV_REUSE": "0"},
-                {"BARK_B200_KV_REUSE": "0", "BARK_B200_SAMPLE": "host"}):
-        for k in ("BARK_B200_SAMPLE_FLAG_EVERY", "BARK_B200_SAMPLE", "BARK_B200_DECODE", "BARK_B200_KV_REUSE"):
+    for env in ({}, {"BARK_B200_SAMPLE_FLAG_EVERY": "5"}, {"BARK_B200_DECODE": "multi"}, {"BARK_B200_KV_REUSE": "0"}):
+        for k in ("BARK_B200_SAMPLE_FLAG_EVERY", "BARK_B200_DECODE", "BARK_B200_KV_REUSE"):
             monkeypatch.delenv(k, raising=False)
         for k, v in env.items():
             monkeypatch.setenv(k, v)
@@ -125,6 +124,36 @@ def test_sampler_paths_agree(pkg, weights_file, monkeypatch):
         for i in range(3):
             assert np.array_equal(t1[i], runs[0][1][i]) and np.array_equal(t2[i], runs[0][3][i])
         assert np.array_equal(bits(a1), bits(runs[0][0])) and np.array_equal(bits(a2), bits(runs[0][2]))
+
+
+@pytest.mark.parametrize("flag_every", [None, "3"])
+def test_sharded_fine_stage_on_one_gpu(pkg, weights_file, monkeypatch, flag_every):
+    """A context connected as a world of one rank samples its fine passes through fine_eval_shard / sample_shard: fine ids and
+    waveform must equal the unsharded context's.  With BARK_B200_SAMPLE_FLAG_EVERY=3 every third sampling launch flags all of
+    its rows, so sharded passes go through the host replay and publish the replayed ids."""
+    if flag_every:
+        monkeypatch.setenv("BARK_B200_SAMPLE_FLAG_EVERY", flag_every)
+    path = weights_file("mini", "f16")
+    runs = []
+    for sharded in (False, True):
+        with pkg.Bark(path, seed=3, n_steps_text_encoder=40) as b:
+            if sharded:
+                b.shard_connect(b.shard_init(0, 1))
+            a = b.generate("hello world")
+            runs.append((a, b.tokens(2).copy()))
+    assert runs[0][1].shape[0] > 0 and np.array_equal(runs[0][1], runs[1][1])
+    assert np.array_equal(bits(runs[0][0]), bits(runs[1][0]))
+
+
+def test_oversized_semantic_vocabulary_is_refused(pkg, weights_mod, tmp_path, capfd):
+    """More semantic logits than the device sampler's row holds: the model loads, generation fails with a message."""
+    import dataclasses
+    path = str(tmp_path / "tiny_sem_out_16392.bin")
+    weights_mod.write_weights(path, dataclasses.replace(weights_mod.tiny(), sem_out=16392))
+    with pkg.Bark(path, n_steps_text_encoder=12) as b:
+        with pytest.raises(RuntimeError):
+            b.generate("hello world")
+    assert "exceed the device sampler's row" in capfd.readouterr().err
 
 
 def test_coarse_prefix_reuse_on_a_long_clip(pkg, weights_file, monkeypatch):
