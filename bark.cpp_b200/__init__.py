@@ -45,6 +45,7 @@ EXPORTS = [
     "bark_context_default_params", "bark_load_model", "bark_generate_audio", "bark_get_audio_data", "bark_get_audio_data_size",
     "bark_get_load_time", "bark_get_eval_time", "bark_reset_statistics", "bark_model_quantize", "bark_free",
     "bark_b200_set_device", "bark_b200_version", "bark_b200_gpt_eval", "bark_b200_fine_eval", "bark_b200_encodec_decode",
+    "bark_b200_encodec_encode", "bark_b200_rvq_encode",
     "bark_b200_sample", "bark_b200_sample_rows", "bark_b200_reseed", "bark_b200_tokenize", "bark_b200_forward_text_encoder",
     "bark_b200_forward_coarse_encoder", "bark_b200_forward_fine_encoder", "bark_b200_get_tokens", "bark_b200_set_tokens",
     "bark_b200_get_stats", "bark_b200_get_hparams", "bark_b200_kernel_launches", "bark_b200_layernorm_fallbacks",
@@ -92,6 +93,10 @@ def lib() -> C.CDLL:
     L.bark_b200_fine_eval.argtypes = [vp, i32p, C.c_int, f32p]
     L.bark_b200_encodec_decode.restype = C.c_int
     L.bark_b200_encodec_decode.argtypes = [vp, i32p, C.c_int, f32p, C.c_int]
+    L.bark_b200_encodec_encode.restype = C.c_int
+    L.bark_b200_encodec_encode.argtypes = [vp, f32p, C.c_int, i32p, C.c_int, f32p, C.c_int]
+    L.bark_b200_rvq_encode.restype = C.c_int
+    L.bark_b200_rvq_encode.argtypes = [f32p, C.c_int, f32p, C.c_int, C.c_int, C.c_int, i32p]
     L.bark_b200_sample.restype = C.c_int
     L.bark_b200_sample.argtypes = [vp, C.c_int, f32p, C.c_int, C.c_float, C.POINTER(C.c_float)]
     L.bark_b200_sample_rows.restype = C.c_int
@@ -300,6 +305,18 @@ class Bark:
             raise RuntimeError("bark_b200_encodec_decode failed")
         return out[:n]
 
+    def encodec_encode(self, audio, return_latent: bool = False):
+        """Mono 24 kHz float32 samples (finite, at least 1921) -> codes [8][T] int32, T = ceil(n / 320), the layout encodec_decode
+        takes; with return_latent also the encoder output before quantisation, [128][T] float32."""
+        a = np.ascontiguousarray(audio, np.float32).ravel()
+        T = (a.size + 319) // 320
+        codes = np.zeros((8, max(T, 1)), np.int32); lat = np.zeros((128, max(T, 1)), np.float32)
+        r = lib().bark_b200_encodec_encode(self.ctx, _p(a), a.size, _p(codes), codes.size, _p(lat), lat.size)
+        if r < 0:
+            raise RuntimeError("bark_b200_encodec_encode failed (see stderr)")
+        assert r == T, (r, T)
+        return (codes, lat) if return_latent else codes
+
     def sample(self, which: int, logits, temp: float):
         l = np.ascontiguousarray(logits, np.float32)
         e = C.c_float(0)
@@ -495,6 +512,19 @@ def sample_given_u(logits: np.ndarray, temp: float, u=None, threads: int = 0):
         raise RuntimeError(f"bark_b200_sample_given_u ({rows} x {n}, temp {temp}, threads {threads}) failed")
     out["replays"] = r
     return out
+
+
+def rvq_encode(latent: np.ndarray, codebooks: np.ndarray) -> np.ndarray:
+    """The RVQ encode kernel on latent [hidden][T] and codebooks [n_q][n_bins][hidden] float32 (hidden % 32 == 0 and <= 128,
+    n_bins <= 1024, n_q <= 8); returns codes [n_q][T] int32, bit-identical to the reference's quantizer encode."""
+    lat = np.ascontiguousarray(latent, np.float32); cb = np.ascontiguousarray(codebooks, np.float32)
+    hidden, T = lat.shape
+    n_q, n_bins, h2 = cb.shape
+    assert h2 == hidden, (lat.shape, cb.shape)
+    codes = np.zeros((n_q, T), np.int32)
+    if not lib().bark_b200_rvq_encode(_p(lat), T, _p(cb), hidden, n_bins, n_q, _p(codes)):
+        raise RuntimeError(f"bark_b200_rvq_encode ({hidden} x {T}, {n_q} x {n_bins} codewords) failed")
+    return codes
 
 
 def kernel_launches() -> int:

@@ -9,6 +9,7 @@
 //   generate / lifecycle . bark.cpp:1165-1184, 2125-2232, 2379-2407
 #include "../../include/bark_b200.h"
 #include "context.h"
+#include "codec_kernels.h"
 #include "gpt_kernels.h"
 
 #include <algorithm>
@@ -792,6 +793,49 @@ static int bark_b200_encodec_decode_impl(struct bark_context * ctx, const int32_
     return n;
 }
 extern "C" int bark_b200_encodec_decode(struct bark_context * ctx, const int32_t * codes, int n_frames, float * out, int out_cap) { return guarded((int) -1, [&] { return bark_b200_encodec_decode_impl(ctx, codes, n_frames, out, out_cap); }); }
+static int bark_b200_encodec_encode_impl(struct bark_context * ctx, const float * audio, int n_samples, int32_t * codes, int codes_cap, float * latent,
+                                         int latent_cap) {
+    if (!ctx || !audio) { fprintf(stderr, "bark_b200_encodec_encode: null %s\n", ctx ? "audio" : "context"); return -1; }
+    BARK_CUDA_CHECK(cudaSetDevice(ctx->device));
+    std::vector<int32_t> c; std::vector<float> l;
+    if (!codec_encode(ctx, audio, n_samples, c, l)) return -1;
+    if (codes) memcpy(codes, c.data(), sizeof(int32_t) * std::min(c.size(), (size_t) std::max(codes_cap, 0)));
+    if (latent) memcpy(latent, l.data(), sizeof(float) * std::min(l.size(), (size_t) std::max(latent_cap, 0)));
+    return (int)(c.size() / 8);
+}
+extern "C" int bark_b200_encodec_encode(struct bark_context * ctx, const float * audio, int n_samples, int32_t * codes, int codes_cap, float * latent,
+                                        int latent_cap) {
+    return guarded((int) -1, [&] { return bark_b200_encodec_encode_impl(ctx, audio, n_samples, codes, codes_cap, latent, latent_cap); });
+}
+// the RVQ encode kernel on host buffers (tests): norms from rvq_norms_kernel, codes [n_q][T] from rvq_encode_kernel
+static int bark_b200_rvq_encode_impl(const float * latent, int T, const float * codebooks, int hidden, int n_bins, int n_q, int32_t * codes) {
+    if (!latent || !codebooks || !codes || T < 1 || hidden < 32 || hidden > 128 || hidden % 32 || n_bins < 1 || n_bins > 1024 || n_q < 1 || n_q > 8) return 0;
+    struct Buffers {                                          // freed on every exit, including a CUDA failure thrown mid-way
+        void * p[4] = {nullptr, nullptr, nullptr, nullptr};
+        ~Buffers() { for (void * q : p) cudaFree(q); }
+    } d;
+    const size_t cb_n = (size_t) n_q * n_bins * hidden;
+    BARK_CUDA_CHECK(cudaMalloc(&d.p[0], (size_t) hidden * T * 4)); BARK_CUDA_CHECK(cudaMalloc(&d.p[1], cb_n * 4));
+    BARK_CUDA_CHECK(cudaMalloc(&d.p[2], (size_t) n_q * n_bins * 4)); BARK_CUDA_CHECK(cudaMalloc(&d.p[3], (size_t) n_q * T * 4));
+    float * dl = (float *) d.p[0], * dcb = (float *) d.p[1], * dn = (float *) d.p[2]; int32_t * dc = (int32_t *) d.p[3];
+    BARK_CUDA_CHECK(cudaMemcpy(dl, latent, (size_t) hidden * T * 4, cudaMemcpyHostToDevice));
+    BARK_CUDA_CHECK(cudaMemcpy(dcb, codebooks, cb_n * 4, cudaMemcpyHostToDevice));
+    BARK_CUDA_CHECK(cudaMemset(dc, 0xff, (size_t) n_q * T * 4));              // -1: a missing store shows up
+    const float * emb[8], * nrm[8];
+    for (int q = 0; q < n_q; q++) {
+        emb[q] = dcb + (size_t) q * n_bins * hidden; nrm[q] = dn + (size_t) q * n_bins;
+        rvq_norms(emb[q], n_bins, hidden, dn + (size_t) q * n_bins, 0);
+    }
+    if (!rvq_encode(emb, nrm, n_q, n_bins, hidden, dl, T, dc, 0)) return 0;
+    BARK_CUDA_CHECK(cudaGetLastError());
+    const cudaError_t e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) { fprintf(stderr, "bark_b200_rvq_encode: %s\n", cudaGetErrorString(e)); return 0; }
+    BARK_CUDA_CHECK(cudaMemcpy(codes, dc, (size_t) n_q * T * 4, cudaMemcpyDeviceToHost));
+    return 1;
+}
+extern "C" int bark_b200_rvq_encode(const float * latent, int T, const float * codebooks, int hidden, int n_bins, int n_q, int32_t * codes) {
+    return guarded((int) 0, [&] { return bark_b200_rvq_encode_impl(latent, T, codebooks, hidden, n_bins, n_q, codes); });
+}
 extern "C" int bark_b200_sample(struct bark_context * ctx, int which, const float * logits, int n, float temp, float * eos_p) {
     if (!ctx || !logits || n < 1) return -1;
     GPTModel & m = *pick(ctx, which < 0 || which > 2 ? 0 : which);

@@ -1,8 +1,10 @@
-// EnCodec decoder kernels (24 kHz model, bandwidth 6 -> 8 codebooks, hop 320), bit-exact path.
+// EnCodec kernels (24 kHz model, bandwidth 6 -> 8 codebooks, hop 320), bit-exact path.
 //
 // Replaces encodec_forward_quantizer_decode (encodec.cpp/quantizer.h:78-111) and
 // encodec_forward_decoder (encodec.cpp/decoder.h:43-113):
-//   RVQ gather-sum -> conv k7 -> 2 x LSTM(512) + skip -> 4 x [ELU, ConvT(k=2s, s), resblock] -> ELU -> conv k7.
+//   RVQ gather-sum -> conv k7 -> 2 x LSTM(512) + skip -> 4 x [ELU, ConvT(k=2s, s), resblock] -> ELU -> conv k7,
+// and their inverse, encodec_forward_encoder (encoder.h:39-109) and encodec_forward_quantizer_encode (quantizer.h:20-76):
+//   conv k7 -> 4 x [resblock, ELU, conv(k=2r, stride r)] -> 2 x LSTM(512) + skip -> ELU -> conv k7 -> RVQ nearest codeword.
 // Activations are [C][T] with time contiguous (the reference's [T, C] ggml tensors).
 //
 // Every contraction in the reference's decoder is a ggml_vec_dot_f16 (ggml.c:2251): conv1d = im2col to f16
@@ -30,6 +32,113 @@ __global__ void rvq_decode_kernel(Codebooks cb, const int32_t * __restrict__ cod
 void rvq_decode(const CodecModel & cm, const int32_t * d_codes, int T, float * x, cudaStream_t s) {
     Codebooks cb; for (int q = 0; q < 8; q++) cb.e[q] = cm.embed[q];
     BARK_LAUNCH(rvq_decode_kernel, dim3((T + 127) / 128, cm.hidden_dim), 128, 0, s, cb, d_codes, T, cm.hidden_dim, x);
+}
+
+// ------------------------------------------------------------------------------------------------
+// quantizer encode (quantizer.h:20-76), codebooks q = 0..n_q-1 in order on the residual r (initially the latent column):
+//   v_j = -(e_j + (s + fl(-2 * vec_dot_f32(Hd, embed_q[j], r)))),  s = f32(sum_double fl(r_i^2)),  e_j = f32(sum_double fl(embed_q[j][i]^2))
+//   code = ggml_vec_argmax_f32(v) (ggml.c:2965-2973),  r <- r - embed_q[code]
+// ------------------------------------------------------------------------------------------------
+// e_j: ggml_sum_rows(ggml_sqr(embed)) = sequential double sum of the f32 squares (ggml.c:2912-2922); weights only, computed at load
+__global__ void rvq_norms_kernel(const float * __restrict__ e, int n_bins, int Hd, float * __restrict__ out) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n_bins) return;
+    double s = 0.0;
+    for (int i = 0; i < Hd; i++) { const float v = e[(size_t) j * Hd + i]; s = __dadd_rn(s, (double) __fmul_rn(v, v)); }
+    out[j] = __double2float_rn(s);
+}
+
+void rvq_norms(const float * embed, int n_bins, int Hd, float * out, cudaStream_t s) {
+    BARK_LAUNCH(rvq_norms_kernel, (n_bins + 127) / 128, 128, 0, s, embed, n_bins, Hd, out);
+}
+
+// One CTA per 8 frames, one warp per frame for the argmax; every warp walks codewords j = warp, warp + 8, ... with lane v holding
+// virtual lane v of the dot's chain (Hd / 32 steps), so each codeword row is read once per 8 frames.  The residuals stay in shared
+// memory through all codebooks.  The argmax takes the last index holding the row maximum (what the reference's running MAX and ==
+// select for rows without NaN); a row with a NaN goes through the reference's loop on one lane, where a NaN resets the maximum.
+constexpr int kRvqFrames = 8, kRvqMaxBins = 1024, kRvqMaxHidden = 128;
+__global__ void __launch_bounds__(256, 1) rvq_encode_kernel(const float * __restrict__ latent, int T, Codebooks cb, Codebooks norms, int n_q, int n_bins,
+                                                         int Hd, int32_t * __restrict__ codes) {
+    __shared__ float vals[kRvqFrames][kRvqMaxBins];
+    __shared__ float res[kRvqFrames][kRvqMaxHidden];
+    __shared__ float s_nrm[kRvqFrames];
+    __shared__ int s_code[kRvqFrames];
+    __shared__ const float * s_cb[8], * s_cn[8];         // indexing the parameter structs by q would copy them to the stack
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, f0 = blockIdx.x * kRvqFrames, nc = Hd >> 5;
+#pragma unroll
+    for (int q = 0; q < 8; q++) if (threadIdx.x == q) { s_cb[q] = cb.e[q]; s_cn[q] = norms.e[q]; }
+    for (int i = threadIdx.x; i < kRvqFrames * Hd; i += blockDim.x) {
+        const int f = i / Hd, d = i % Hd;
+        res[f][d] = f0 + f < T ? latent[(size_t) d * T + f0 + f] : 0.f;
+    }
+    __syncthreads();
+    for (int q = 0; q < n_q; q++) {
+        const float * E = s_cb[q], * nrm = s_cn[q];
+        if (lane == 0) {
+            double s = 0.0;
+            for (int d = 0; d < Hd; d++) s = __dadd_rn(s, (double) __fmul_rn(res[warp][d], res[warp][d]));
+            s_nrm[warp] = __double2float_rn(s);
+        }
+        __syncthreads();
+        float r[kRvqFrames][kRvqMaxHidden / 32], sn[kRvqFrames];
+#pragma unroll
+        for (int f = 0; f < kRvqFrames; f++) {
+            sn[f] = s_nrm[f];
+#pragma unroll
+            for (int c = 0; c < kRvqMaxHidden / 32; c++) r[f][c] = c < nc ? res[f][c * 32 + lane] : 0.f;
+        }
+        for (int j = warp; j < n_bins; j += 8) {
+            float ev[kRvqMaxHidden / 32];
+#pragma unroll
+            for (int c = 0; c < kRvqMaxHidden / 32; c++) ev[c] = c < nc ? __ldg(E + (size_t) j * Hd + c * 32 + lane) : 0.f;
+            const float ej = __ldg(nrm + j);
+#pragma unroll
+            for (int f = 0; f < kRvqFrames; f++) {
+                float acc = 0.f;
+#pragma unroll
+                for (int c = 0; c < kRvqMaxHidden / 32; c++) if (c < nc) acc = __fmaf_rn(ev[c], r[f][c], acc);
+                const float dot = lane_tree_reduce(acc);
+                if (lane == f) vals[f][j] = -__fadd_rn(ej, __fadd_rn(sn[f], __fmul_rn(dot, -2.0f)));
+            }
+        }
+        __syncthreads();
+        {
+            const float * v = vals[warp];
+            float m = -INFINITY; bool nan = false;
+            for (int j = lane; j < n_bins; j += 32) { const float a = v[j]; nan |= a != a; m = fmaxf(m, a); }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+            int idx = -1;
+            for (int j = lane; j < n_bins; j += 32) if (v[j] == m) idx = j;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) idx = max(idx, __shfl_xor_sync(0xffffffffu, idx, o));
+            if (__any_sync(0xffffffffu, nan) && lane == 0) {
+                float mx = -INFINITY; idx = 0;
+                for (int j = 0; j < n_bins; j++) { mx = mx > v[j] ? mx : v[j]; if (mx == v[j]) idx = j; }
+            }
+            if (lane == 0) {
+                const bool live = f0 + warp < T;
+                s_code[warp] = live ? idx : 0;
+                if (live) codes[(size_t) q * T + f0 + warp] = idx;
+            }
+        }
+        __syncthreads();
+        for (int i = threadIdx.x; i < kRvqFrames * Hd; i += blockDim.x) {
+            const int f = i / Hd, d = i % Hd;
+            res[f][d] = __fsub_rn(res[f][d], __ldg(E + (size_t) s_code[f] * Hd + d));
+        }
+        __syncthreads();
+    }
+}
+
+bool rvq_encode(const float * const * embed, const float * const * norms, int n_q, int n_bins, int Hd, const float * latent, int T, int32_t * codes,
+                cudaStream_t s) {
+    if (n_q < 1 || n_q > 8 || n_bins < 1 || n_bins > kRvqMaxBins || Hd < 32 || Hd > kRvqMaxHidden || Hd % 32 || T < 1) return false;
+    Codebooks cb, nr;
+    for (int q = 0; q < 8; q++) { cb.e[q] = q < n_q ? embed[q] : nullptr; nr.e[q] = q < n_q ? norms[q] : nullptr; }
+    g_next_flops = 2.0 * (double) T * n_q * n_bins * Hd;
+    BARK_LAUNCH(rvq_encode_kernel, (T + kRvqFrames - 1) / kRvqFrames, 256, 0, s, latent, T, cb, nr, n_q, n_bins, Hd, codes);
+    return true;
 }
 
 // chain of one virtual lane out of an LI16 row: up to NG groups of 8 f16 values
@@ -111,9 +220,173 @@ static int device_sms() {
     return n;
 }
 
-void conv1d(const float * x, int Cin, int T, const ConvW & cv, bool elu_in, const float * resid, float * y, cudaStream_t s) {
+// ------------------------------------------------------------------------------------------------
+// conv1d with K = Cin*k < 32 (the encoder's initial conv, K = 7; conv_2 of the first encoder block and of the last decoder block,
+// K = 16): ggml_vec_dot_f16 has no full lane step, so the whole dot is its leftover loop, f32 products summed in double from 0
+// (ggml.c:2281-2283).  One thread per output position; the block stages a tile of the input (ELU'd, f16-rounded) once.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(128) conv1d_short_kernel(const float * __restrict__ x, int Cin, int T, int k, const __half * __restrict__ w_li, int Kp,
+                                                           const float * __restrict__ bias, int Cout, int o_per_block, int elu_in,
+                                                           const float * __restrict__ resid, float * __restrict__ y) {
+    constexpr int TT = 128;
+    extern __shared__ float xs[];                        // [Cin][TT + k - 1]
+    const int W = TT + k - 1, t0 = blockIdx.x * TT;
+    for (int i = threadIdx.x; i < Cin * W; i += blockDim.x) {
+        const int c = i / W, j = i % W;
+        int t = t0 + j - (k - 1);
+        if (t < 0) t = -t;
+        float v = 0.f;
+        if (t < T) { v = x[(size_t) c * T + t]; if (elu_in) v = elu_exact(v); v = round_f16(v); }
+        xs[i] = v;
+    }
+    __syncthreads();
+    const int tl = threadIdx.x, t = t0 + tl;
+    if (t >= T) return;
+    const int K = Cin * k, o_lo = blockIdx.y * o_per_block, o_hi = min(Cout, o_lo + o_per_block);
+    for (int o = o_lo; o < o_hi; o++) {
+        const __half * wrow = w_li + (size_t) o * Kp;
+        double sd = 0.0;
+        for (int kk = 0; kk < K; kk++)
+            sd = __dadd_rn(sd, (double) __fmul_rn(__half2float(__ldg(wrow + li_offset(kk, 8))), xs[(kk / k) * W + (kk % k) + tl]));
+        float r = __fadd_rn(__ldg(bias + o), __double2float_rn(sd));                 // ops.cpp:72 add(repeat(b), dst)
+        if (resid) r = __fadd_rn(r, resid[(size_t) o * T + t]);
+        y[(size_t) o * T + t] = r;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// conv1d whose lane chains do not fit in registers (K = Cin*k up to 4096) and/or with a stride: the encoder's down-sampling convs
+// (k = 2r, stride r) and its final conv (k 7, K = 3584).  strided_conv_1d (ops.cpp:59-75) reflect-pads k - stride on the left and
+// `extra` on the right (ggml.c:15587-15588); output t reads padded positions t*stride .. t*stride + k - 1.
+// One block: TT output positions x a chunk of output channels, the padded input span in shared memory (ELU'd, f16-rounded).  A warp
+// owns OW output channels at a time and streams their LI16 rows 8 chain steps per 16-byte load; each lane keeps OW x TT accumulators,
+// so a weight word is used TT times.  Chain order, tree and bias add are conv1d_lane_kernel's (K % 32 == 0: no leftovers).
+// ------------------------------------------------------------------------------------------------
+template <int KW, int STRIDE>
+__global__ void __launch_bounds__(256) conv1d_stream_kernel(const float * __restrict__ x, int Cin, int L, int Lp, int Tout, const __half * __restrict__ w_li,
+                                                            int Kp, const float * __restrict__ bias, int Cout, int o_per_block, int elu_in, float * __restrict__ y) {
+    constexpr int TT = STRIDE >= 8 ? 8 : 16, OW = 2;
+    constexpr int SPAN = (TT - 1) * STRIDE + KW, SR = SPAN | 1, PADL = KW - STRIDE;
+    extern __shared__ float xs[];                        // [Cin][SR]
+    const int t0 = blockIdx.x * TT;
+    for (int i = threadIdx.x; i < Cin * SPAN; i += blockDim.x) {
+        const int c = i / SPAN, u = i % SPAN, p = t0 * STRIDE + u;
+        float v = 0.f;
+        if (p < Lp) {
+            int t = p - PADL;
+            if (t < 0) t = -t;                           // reflect left (ggml.c:15587)
+            if (t >= L) t = 2 * (L - 1) - t;             // reflect right (ggml.c:15588)
+            v = x[(size_t) c * L + t];
+            if (elu_in) v = elu_exact(v);
+            v = round_f16(v);
+        }
+        xs[c * SR + u] = v;
+    }
+    __syncthreads();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int nsteps = (Cin * KW) >> 5, ngroups = (nsteps + 7) >> 3;
+    const int o_lo = blockIdx.y * o_per_block, o_hi = min(Cout, o_lo + o_per_block);
+    for (int ob = o_lo + warp * OW; ob < o_hi; ob += 8 * OW) {
+        float acc[OW][TT];
+#pragma unroll
+        for (int q = 0; q < OW; q++)
+#pragma unroll
+            for (int t = 0; t < TT; t++) acc[q][t] = 0.f;
+        for (int g = 0; g < ngroups; g++) {
+            float w[OW][8];
+#pragma unroll
+            for (int q = 0; q < OW; q++) {
+                const int o = min(ob + q, o_hi - 1);    // a missing second channel repeats the first; its sums are not stored
+                const uint4 u = __ldg(reinterpret_cast<const uint4 *>(w_li + (size_t) o * Kp) + g * 32 + lane);
+                const __half2 * h = reinterpret_cast<const __half2 *>(&u);
+#pragma unroll
+                for (int i = 0; i < 4; i++) { const float2 f = __half22float2(h[i]); w[q][2 * i] = f.x; w[q][2 * i + 1] = f.y; }
+            }
+#pragma unroll
+            for (int st = 0; st < 8; st++) {
+                const int step = g * 8 + st;
+                if (step < nsteps) {
+                    const int kk = step * 32 + lane;
+                    const float * col = xs + (kk / KW) * SR + (kk % KW);
+#pragma unroll
+                    for (int t = 0; t < TT; t++) {
+                        const float xv = col[t * STRIDE];
+#pragma unroll
+                        for (int q = 0; q < OW; q++) acc[q][t] = __fmaf_rn(w[q][st], xv, acc[q][t]);
+                    }
+                }
+            }
+        }
+#pragma unroll
+        for (int q = 0; q < OW; q++) {
+            float mine = 0.f;
+#pragma unroll
+            for (int t = 0; t < TT; t++) { const float r = lane_tree_reduce(acc[q][t]); if (lane == t) mine = r; }
+            const int o = ob + q, t = t0 + lane;
+            if (o < o_hi && lane < TT && t < Tout) y[(size_t) o * Tout + t] = __fadd_rn(__ldg(bias + o), mine);
+        }
+    }
+}
+
+// output length of strided_conv_1d (ops.cpp:8-16, 59-66): extra right padding from get_extra_padding_for_conv_1d, evaluated in
+// float like the reference
+static void strided_conv_lengths(int L, int k, int stride, int * Lp, int * Tout) {
+    const float length = (float) L, ks = (float) k, st = (float) stride, pad_total = (float)(k - stride);
+    const float n_frames = (length - ks + pad_total) / st + 1.0f;
+    const int ideal_length = (int)((ceilf(n_frames) - 1.0f) * st + (ks - pad_total));
+    const int extra = (int)((float) ideal_length - length);
+    *Lp = L + (k - stride) + extra;
+    *Tout = (*Lp - k) / stride + 1;
+}
+
+int conv1d_out_len(int L, int k, int stride) { int Lp, Tout; strided_conv_lengths(L, k, stride, &Lp, &Tout); return Tout; }
+
+// shapes the stream kernel is instantiated for: the encoder's down-sampling convs (k = 2r, stride r) and its final conv
+static void conv1d_stream(const float * x, int Cin, int L, const ConvW & cv, int stride, bool elu_in, float * y, cudaStream_t s) {
+    const int K = Cin * cv.k;
+    int Lp, Tout;
+    strided_conv_lengths(L, cv.k, stride, &Lp, &Tout);
+    if (K % 32 != 0 || Lp - L - (cv.k - stride) > L - 1) {
+        fprintf(stderr, "bark_b200: unsupported conv shape Cin=%d k=%d stride=%d L=%d\n", Cin, cv.k, stride, L); throw std::runtime_error("unsupported configuration (see the message above)");
+    }
+    const int TT = stride >= 8 ? 8 : 16, SR = ((TT - 1) * stride + cv.k) | 1;
+    const size_t smem = (size_t) Cin * SR * sizeof(float);
+    const int tiles = (Tout + TT - 1) / TT;
+    int o_per_block = cv.cout;
+    const int n_sm = device_sms();
+    while (o_per_block > 16 && tiles * ((cv.cout + o_per_block - 1) / o_per_block) < 2 * n_sm) o_per_block = (o_per_block + 1) / 2;
+    const dim3 grid(tiles, (cv.cout + o_per_block - 1) / o_per_block);
+    g_next_flops = 2.0 * (double) Tout * cv.cout * K;
+#define STREAM_CASE(KW, ST)                                                                                                  \
+    if (cv.k == KW && stride == ST) {                                                                                        \
+        BARK_CUDA_CHECK(cudaFuncSetAttribute(conv1d_stream_kernel<KW, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem)); \
+        BARK_LAUNCH((conv1d_stream_kernel<KW, ST>), grid, 256, smem, s, x, Cin, L, Lp, Tout, cv.w, cv.Kp, cv.b, cv.cout, o_per_block, elu_in ? 1 : 0, y); \
+        return;                                                                                                              \
+    }
+    STREAM_CASE(4, 2) STREAM_CASE(8, 4) STREAM_CASE(10, 5) STREAM_CASE(16, 8) STREAM_CASE(7, 1)
+#undef STREAM_CASE
+    fprintf(stderr, "bark_b200: unsupported conv kernel size %d with stride %d\n", cv.k, stride); throw std::runtime_error("unsupported configuration (see the message above)");
+}
+
+void conv1d(const float * x, int Cin, int T, const ConvW & cv, bool elu_in, const float * resid, float * y, cudaStream_t s, int stride) {
     const int K = Cin * cv.k, nsteps = K / 32, ngroups = (nsteps + 7) / 8;
-    if (ngroups > 4) { fprintf(stderr, "bark_b200: unsupported conv shape Cin=%d k=%d\n", Cin, cv.k); throw std::runtime_error("unsupported configuration (see the message above)"); }
+    if (K < 32 && stride == 1) {
+        const int TT = 128, tiles = (T + TT - 1) / TT;
+        int o_per_block = cv.cout;
+        const int n_sm = device_sms();
+        while (o_per_block > 1 && tiles * ((cv.cout + o_per_block - 1) / o_per_block) < 4 * n_sm) o_per_block = (o_per_block + 1) / 2;
+        const size_t smem = (size_t) Cin * (TT + cv.k - 1) * sizeof(float);
+        g_next_flops = 2.0 * (double) T * cv.cout * K;
+        BARK_LAUNCH(conv1d_short_kernel, dim3(tiles, (cv.cout + o_per_block - 1) / o_per_block), TT, smem, s, x, Cin, T, cv.k, cv.w, cv.Kp, cv.b,
+                    cv.cout, o_per_block, elu_in ? 1 : 0, resid, y);
+        return;
+    }
+    const bool lane_fits = stride == 1 && ((cv.k == 1 && ngroups <= 2) || (cv.k == 3 && ngroups <= 3) || (cv.k == 7 && ngroups <= 4));
+    if (!lane_fits) {
+        if (resid) { fprintf(stderr, "bark_b200: unsupported conv shape Cin=%d k=%d stride=%d with a residual\n", Cin, cv.k, stride); throw std::runtime_error("unsupported configuration (see the message above)"); }
+        conv1d_stream(x, Cin, T, cv, stride, elu_in, y, s);
+        return;
+    }
     const int TT = 32;
     const int S = (TT + cv.k - 1) | 1;
     const size_t smem = (size_t) Cin * S * sizeof(float);

@@ -115,6 +115,9 @@ bool fine_eval_fast(bark_context * ctx, const int32_t * in_buffer, int nn, float
 bool gpt_decode_chained(bark_context * ctx, GPTModel & m, const int32_t * d_token, int * n_past, int lm_lo, int lm_hi);
 // EnCodec decode; codes [8][T] on the host; result in `audio`
 bool codec_decode(bark_context * ctx, const int32_t * codes, int T, std::vector<float> & audio);
+// EnCodec encode (encodec_compress_audio at 6 kbps): n mono 24 kHz samples -> codes [8][T] and the latent [128][T], T = ceil(n / 320);
+// false (message on stderr) without encoder tensors, for n < 1921 or a non-finite sample.  Leaves the generation state alone.
+bool codec_encode(bark_context * ctx, const float * audio, int n, std::vector<int32_t> & codes, std::vector<float> & latent);
 
 // sampling.cu
 constexpr int kSampleMaxLogits = 16384;          // logits of one row: sample_rows_kernel holds the row in 64 KB of shared memory

@@ -7,6 +7,7 @@
 #include "gpt_kernels.h"
 
 #include <algorithm>
+#include <cmath>
 #include <vector>
 #include <time.h>
 
@@ -317,6 +318,24 @@ bool fine_eval_fast(bark_context * ctx, const int32_t * in_buffer, int nn, float
     return true;
 }
 
+// codec scratch for a T-frame clip, grown on demand: three activation buffers of 10240*T floats (the decoder's largest activation is
+// [64][160T] = [32][320T]; the encoder's, [32][n_samples], is no larger), the LSTM input projections and the [8][T] codes
+static bool codec_scratch(bark_context * ctx, int T, const char * caller) {
+    const size_t need = (size_t) 10240 * T + 1024;
+    if (need > ctx->c_cap) {
+        // out of memory here is recoverable (a very long clip): report it and return false like the reference's failed encodec_eval
+        auto grow = [&](void ** p, size_t bytes) { if (*p) { cudaFree(*p); *p = nullptr; } return cudaMalloc(p, bytes) == cudaSuccess; };
+        ctx->c_cap = 0;
+        bool ok = true;
+        for (int i = 0; i < 3; i++) ok = ok && grow((void **) &ctx->c_buf[i], need * sizeof(float));
+        ok = ok && grow((void **) &ctx->c_gi, (size_t) T * 2048 * sizeof(float)) && grow((void **) &ctx->d_codes, (size_t) 8 * T * sizeof(int32_t));
+        if (!ok) { (void) cudaGetLastError(); fprintf(stderr, "%s: out of device memory for a %d-frame clip\n", caller, T); return false; }
+        if (!ctx->c_hbuf) { ctx->c_hbuf = (float *) ctx_alloc(ctx, 2 * 512 * sizeof(float)); ctx->c_counter = (unsigned *) ctx_alloc(ctx, sizeof(unsigned)); }
+        ctx->c_cap = need;
+    }
+    return true;
+}
+
 bool codec_decode(bark_context * ctx, const int32_t * codes, int T, std::vector<float> & audio) {
     if (T < 7) { fprintf(stderr, "%s: need at least 7 frames (reflect padding of the k=7 convolutions), got %d\n", __func__, T); return false; }
     CodecModel & cm = ctx->codec;
@@ -325,18 +344,7 @@ bool codec_decode(bark_context * ctx, const int32_t * codes, int T, std::vector<
     for (size_t i = 0; i < (size_t) 8 * T; i++) if (codes[i] < 0 || codes[i] >= cm.n_bins) {
         fprintf(stderr, "%s: code %d (codebook %zu, frame %zu) is outside the codebooks (%d bins)\n", __func__, codes[i], i / T, i % T, cm.n_bins); return false;
     }
-    const size_t need = (size_t) 10240 * T + 1024;             // largest activation: [64][160T] = [32][320T] = 10240*T floats
-    if (need > ctx->c_cap) {
-        // out of memory here is recoverable (a very long clip): report it and return false like the reference's failed encodec_eval
-        auto grow = [&](void ** p, size_t bytes) { if (*p) { cudaFree(*p); *p = nullptr; } return cudaMalloc(p, bytes) == cudaSuccess; };
-        ctx->c_cap = 0;
-        bool ok = true;
-        for (int i = 0; i < 3; i++) ok = ok && grow((void **) &ctx->c_buf[i], need * sizeof(float));
-        ok = ok && grow((void **) &ctx->c_gi, (size_t) T * 2048 * sizeof(float)) && grow((void **) &ctx->d_codes, (size_t) 8 * T * sizeof(int32_t));
-        if (!ok) { (void) cudaGetLastError(); fprintf(stderr, "%s: out of device memory for a %d-frame clip\n", __func__, T); return false; }
-        if (!ctx->c_hbuf) { ctx->c_hbuf = (float *) ctx_alloc(ctx, 2 * 512 * sizeof(float)); ctx->c_counter = (unsigned *) ctx_alloc(ctx, sizeof(unsigned)); }
-        ctx->c_cap = need;
-    }
+    if (!codec_scratch(ctx, T, __func__)) return false;
     float * a = ctx->c_buf[0], * b = ctx->c_buf[1], * c = ctx->c_buf[2];
     BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->d_codes, codes, (size_t) 8 * T * sizeof(int32_t), cudaMemcpyHostToDevice, s)); g_h2d_bytes += (size_t) 8 * T * sizeof(int32_t);
     rvq_decode(cm, ctx->d_codes, T, a, s);                                                // [128][T]
@@ -357,6 +365,45 @@ bool codec_decode(bark_context * ctx, const int32_t * codes, int T, std::vector<
     conv1d(cur, C, L, cm.final_conv, true, nullptr, t1, s);           // ELU -> k7 -> [1][320 T]
     audio.resize((size_t) L);
     BARK_CUDA_CHECK(cudaMemcpyAsync(audio.data(), t1, (size_t) L * sizeof(float), cudaMemcpyDeviceToHost, s)); g_d2h_bytes += (size_t) L * sizeof(float);
+    BARK_CUDA_CHECK(cudaStreamSynchronize(s));
+    return true;
+}
+
+bool codec_encode(bark_context * ctx, const float * audio, int n, std::vector<int32_t> & codes, std::vector<float> & latent) {
+    CodecModel & cm = ctx->codec;
+    const CodecModel::Encoder & e = cm.enc;
+    if (!e.present) { fprintf(stderr, "%s: the model file has no EnCodec encoder tensors (encoder.*)\n", __func__); return false; }
+    // the final k=7 conv reflect-pads 6 samples of a T-frame latent: T >= 7 (the reference reads out of bounds below that)
+    if (n < 1921) { fprintf(stderr, "%s: need at least 1921 samples (7 frames), got %d\n", __func__, n); return false; }
+    for (int i = 0; i < n; i++) if (!std::isfinite(audio[i])) { fprintf(stderr, "%s: sample %d is not finite (%g)\n", __func__, i, (double) audio[i]); return false; }
+    const int T = (n - 1) / 320 + 1;
+    if (!codec_scratch(ctx, T, __func__)) return false;
+    cudaStream_t s = ctx->stream;
+    static const int ratios[4] = {8, 5, 4, 2};
+    float * cur = ctx->c_buf[0], * t1 = ctx->c_buf[1], * t2 = ctx->c_buf[2];
+    BARK_CUDA_CHECK(cudaMemcpyAsync(t2, audio, (size_t) n * sizeof(float), cudaMemcpyHostToDevice, s)); g_h2d_bytes += (size_t) n * sizeof(float);
+    conv1d(t2, 1, n, e.init, false, nullptr, cur, s);                   // encoder.h:49 -> [32][n]
+    int C = e.init.cout, L = n;
+    for (int i = 0; i < 4; i++) {                                        // encoder.h:52-83
+        const int r = ratios[3 - i];
+        conv1d(cur, C, L, e.blk[i].sc, false, nullptr, t1, s);           // shortcut on the block input
+        conv1d(cur, C, L, e.blk[i].c1, true, nullptr, t2, s);            // ELU -> k3 -> [C/2][L]
+        conv1d(t2, C / 2, L, e.blk[i].c2, true, t1, cur, s);             // ELU -> k1, + shortcut
+        conv1d(cur, C, L, e.blk[i].ds, true, nullptr, t1, s, r);         // ELU -> k 2r, stride r -> [2C][ceil(L / r)]
+        L = conv1d_out_len(L, e.blk[i].ds.k, r); C *= 2;
+        std::swap(cur, t1);
+    }
+    if (L != T) { fprintf(stderr, "%s: internal error: %d latent frames for %d samples\n", __func__, L, n); return false; }
+    lstm_layer(cur, C, T, e.lstm_ih_w[0], e.lstm_hh_w[0], e.lstm_Kp, e.lstm_ih_b[0], e.lstm_hh_b[0], nullptr, ctx->c_gi, ctx->c_hbuf, ctx->c_counter, t1, s);
+    lstm_layer(t1, C, T, e.lstm_ih_w[1], e.lstm_hh_w[1], e.lstm_Kp, e.lstm_ih_b[1], e.lstm_hh_b[1], cur /*skip (encoder.h:98)*/, ctx->c_gi, ctx->c_hbuf, ctx->c_counter, t2, s);
+    conv1d(t2, C, T, e.final_conv, true, nullptr, t1, s);                // ELU -> k7 -> latent [128][T]
+    const float * emb[8], * nrm[8];
+    for (int q = 0; q < 8; q++) { emb[q] = cm.embed[q]; nrm[q] = cm.embed_norm[q]; }
+    if (!rvq_encode(emb, nrm, 8, cm.n_bins, cm.hidden_dim, t1, T, ctx->d_codes, s)) { fprintf(stderr, "%s: unsupported codebook shape (%d bins of %d)\n", __func__, cm.n_bins, cm.hidden_dim); return false; }
+    codes.resize((size_t) 8 * T); latent.resize((size_t) cm.hidden_dim * T);
+    BARK_CUDA_CHECK(cudaMemcpyAsync(codes.data(), ctx->d_codes, codes.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    BARK_CUDA_CHECK(cudaMemcpyAsync(latent.data(), t1, latent.size() * sizeof(float), cudaMemcpyDeviceToHost, s));
+    g_d2h_bytes += codes.size() * sizeof(int32_t) + latent.size() * sizeof(float);
     BARK_CUDA_CHECK(cudaStreamSynchronize(s));
     return true;
 }

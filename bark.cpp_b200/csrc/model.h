@@ -55,6 +55,15 @@ struct CodecModel {
     float  * lstm_ih_b[2] = {nullptr, nullptr}, * lstm_hh_b[2] = {nullptr, nullptr};
     struct Block { ConvW us, c1, c2, sc; } blk[4];   // us: transposed conv
     float * embed[8] = {nullptr};           // codebooks 0..7, [n_bins][hidden] f32
+    float * embed_norm[8] = {nullptr};      // their rows' sums of squares [n_bins] (RVQ encode)
+    struct Encoder {                        // encoder.* tensors (encodec.cpp/encoder.h:8-37); a file may lack them all
+        bool present = false;
+        ConvW init, final_conv;
+        struct Block { ConvW sc, c1, c2, ds; } blk[4];   // ds: down-sampling conv, k = 2r, stride r
+        __half * lstm_ih_w[2] = {nullptr, nullptr}, * lstm_hh_w[2] = {nullptr, nullptr};
+        int lstm_Kp = 0;
+        float  * lstm_ih_b[2] = {nullptr, nullptr}, * lstm_hh_b[2] = {nullptr, nullptr};
+    } enc;
 };
 
 // Scratch activations for one GPT evaluation of up to `max_rows` positions.

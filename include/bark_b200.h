@@ -6,6 +6,7 @@
  *   bark_b200_gpt_eval ........ one causal GPT evaluation  == bark_eval_encoder_internal      (bark.cpp:1586-1643)
  *   bark_b200_fine_eval ....... one fine pass              == bark_eval_fine_encoder_internal (bark.cpp:1907-1959)
  *   bark_b200_encodec_decode .. codes -> waveform          == encodec_decompress_audio        (encodec.cpp/encodec.cpp:902-924)
+ *   bark_b200_encodec_encode .. waveform -> codes          == encodec_compress_audio          (encodec.cpp/encodec.cpp:878-900)
  *   bark_b200_sample .......... gpt_sample on the context RNG                                 (bark.cpp:249-270)
  *   bark_b200_sample_rows ..... the same for `rows` logit rows, on the device sampler the stages use (host replay of rows it cannot decide)
  *   bark_b200_forward_* ....... extern "C" names for bark_forward_{text,coarse,fine}_encoder  (bark.cpp:1703,1865,2061)
@@ -31,6 +32,17 @@ BARK_API int  bark_b200_gpt_eval(struct bark_context * ctx, int which, const int
 BARK_API int  bark_b200_fine_eval(struct bark_context * ctx, const int32_t * in_buffer, int nn, float * logits_out);
 /* codes: [8][n_frames]; returns number of samples (320 * n_frames), copies min(n, out_cap) floats to out (may be NULL) */
 BARK_API int  bark_b200_encodec_decode(struct bark_context * ctx, const int32_t * codes, int n_frames, float * out, int out_cap);
+/* EnCodec encode == encodec_compress_audio (encodec.cpp/encodec.cpp:878-900) at 6 kbps, bit-identical to it; the context's generation
+ * state (RNG, ids, bark_get_audio_data) is not touched.
+ * audio: n_samples mono 24 kHz f32, finite, n_samples >= 1921.  codes: [8][T] codebook-major (the layout bark_b200_encodec_decode
+ * takes), T = ceil(n_samples / 320); copies min(8 T, codes_cap) values (codes may be NULL).  latent (may be NULL): the encoder output
+ * before quantisation, [128][T] f32, min(128 T, latent_cap) values.  Returns T, or -1 (message on stderr), also for a model file
+ * written without the encoder tensors. */
+BARK_API int  bark_b200_encodec_encode(struct bark_context * ctx, const float * audio, int n_samples, int32_t * codes, int codes_cap,
+                                       float * latent, int latent_cap);
+/* Test hook, no context: the RVQ encode kernel on host buffers.  latent [hidden][T], codebooks [n_q][n_bins][hidden] f32, codes [n_q][T];
+ * hidden % 32 == 0 and <= 128, n_bins <= 1024, n_q <= 8.  Returns 1 on success, 0 on invalid arguments or failure. */
+BARK_API int  bark_b200_rvq_encode(const float * latent, int T, const float * codebooks, int hidden, int n_bins, int n_q, int32_t * codes);
 BARK_API int  bark_b200_sample(struct bark_context * ctx, int which, const float * logits, int n, float temp, float * eos_p);
 BARK_API int  bark_b200_sample_rows(struct bark_context * ctx, const float * logits /*[rows][n], host*/, int n, int rows, float temp, int32_t * tokens_out,
                                      float * eos_p_out /*[rows] or NULL*/);   /* returns the number of rows replayed on the host, <0 on error */
