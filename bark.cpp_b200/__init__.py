@@ -40,6 +40,45 @@ class BarkStatistics(C.Structure):
                 ("t_fine_us", C.c_int64), ("n_sample_semantic", C.c_int32), ("n_sample_coarse", C.c_int32), ("n_sample_fine", C.c_int32)]
 
 
+class HistoryPromptStruct(C.Structure):
+    """struct bark_b200_history_prompt (include/bark_b200.h)."""
+    _fields_ = [("semantic", C.c_void_p), ("n_semantic", C.c_int), ("coarse", C.c_void_p), ("n_coarse_frames", C.c_int),
+                ("fine", C.c_void_p), ("n_fine_frames", C.c_int)]
+
+
+HISTORY_KEYS = ("semantic_prompt", "coarse_prompt", "fine_prompt")
+
+
+def load_history_prompt(src) -> dict:
+    """A speaker history prompt from an upstream Bark voice file (.npz path) or a mapping with its three keys: semantic_prompt [n_s],
+    coarse_prompt [2][n_c] and fine_prompt [8][n_f] (n_f may be 0).  Returns the three as contiguous int32 arrays; raises ValueError on
+    a missing key or a wrong rank or shape.  Id ranges and the semantic / coarse alignment are checked by bark_b200_set_history_prompt."""
+    if isinstance(src, (str, bytes, os.PathLike)):
+        with np.load(src) as f:
+            return load_history_prompt({k: f[k] for k in f.files})
+    out = {}
+    for k, lead in zip(HISTORY_KEYS, (None, 2, 8)):
+        try:
+            a = np.asarray(src[k])
+        except KeyError:
+            raise ValueError(f"history prompt: missing {k}") from None
+        if a.dtype.kind not in "iu":
+            raise ValueError(f"history prompt: {k} holds {a.dtype} values, not integer ids")
+        if lead is None and a.ndim != 1:
+            raise ValueError(f"history prompt: {k} has shape {a.shape}, expected [n]")
+        if lead is not None and (a.ndim != 2 or a.shape[0] != lead):
+            raise ValueError(f"history prompt: {k} has shape {a.shape}, expected [{lead}][n]")
+        out[k] = np.ascontiguousarray(a, np.int32)
+    return out
+
+
+def _history_struct(p):
+    """(struct bark_b200_history_prompt, the arrays it points into) for a prompt as load_history_prompt accepts it."""
+    p = load_history_prompt(p)
+    s, c, f = (p[k] for k in HISTORY_KEYS)
+    return HistoryPromptStruct(_p(s), s.size, _p(c), c.shape[1], _p(f) if f.size else None, f.shape[1]), p
+
+
 # every symbol the two public headers declare (tests check the library exports exactly these)
 EXPORTS = [
     "bark_context_default_params", "bark_load_model", "bark_generate_audio", "bark_get_audio_data", "bark_get_audio_data_size",
@@ -53,6 +92,7 @@ EXPORTS = [
     "bark_b200_shard_init", "bark_b200_shard_connect", "bark_b200_shard_nvlink_bytes",
     "bark_b200_fast_mode", "bark_b200_fast_gemm", "bark_b200_fast_attention", "bark_b200_parity_attention", "bark_b200_parity_gemm",
     "bark_b200_parity_rows", "bark_b200_sample_given_u", "bark_b200_generate_batch", "bark_b200_batch_audio", "bark_b200_batch_tokens", "bark_b200_gpt_eval_slot", "bark_b200_gpt_step_batch",
+    "bark_b200_set_history_prompt", "bark_b200_generate_batch_prompted",
     "ggml_time_init", "ggml_time_us", "ggml_time_ms", "ggml_init", "ggml_free",
 ]
 
@@ -150,6 +190,11 @@ def lib() -> C.CDLL:
     L.bark_b200_gpt_eval_slot.argtypes = [vp, C.c_int, C.c_int, i32p, C.c_int, C.POINTER(C.c_int), C.c_int, f32p]
     L.bark_b200_gpt_step_batch.restype = C.c_int
     L.bark_b200_gpt_step_batch.argtypes = [vp, C.c_int, C.c_int, i32p, i32p, i32p, f32p]
+    L.bark_b200_set_history_prompt.restype = C.c_int
+    L.bark_b200_set_history_prompt.argtypes = [vp, C.POINTER(HistoryPromptStruct)]
+    L.bark_b200_generate_batch_prompted.restype = C.c_bool
+    L.bark_b200_generate_batch_prompted.argtypes = [vp, C.POINTER(C.c_char_p), C.POINTER(C.c_uint32), C.POINTER(C.POINTER(HistoryPromptStruct)),
+                                                    C.c_int, C.c_int]
     L.ggml_time_us.restype = C.c_int64
     _lib = L
     return L
@@ -196,11 +241,35 @@ class Bark:
         self.close()
 
     # ---- bark.h ----
-    def generate(self, text: str, n_threads: int = 1) -> np.ndarray:
+    def generate(self, text: str, n_threads: int = 1, history_prompt=None) -> np.ndarray:
+        """The waveform for `text`.  history_prompt (a voice file or mapping, see load_history_prompt) conditions this call only: it
+        is set before and cleared after, also on failure.  Without it the context's prompt (set_history_prompt) applies."""
+        if history_prompt is not None:
+            self.set_history_prompt(history_prompt)
+            try:
+                return self.generate(text, n_threads)
+            finally:
+                self.set_history_prompt(None)
         if not lib().bark_generate_audio(self.ctx, text.encode(), n_threads):
             raise RuntimeError("bark_generate_audio failed")
         n = lib().bark_get_audio_data_size(self.ctx)
         return np.ctypeslib.as_array(lib().bark_get_audio_data(self.ctx), shape=(n,)).copy()
+
+    def set_history_prompt(self, prompt):
+        """Speaker history prompt of the later generations on this context (bark_b200_set_history_prompt); None clears it.  Raises
+        ValueError for a prompt the library rejects (the message is on stderr); the previous prompt then stays."""
+        if prompt is None:
+            lib().bark_b200_set_history_prompt(self.ctx, None)
+            return
+        st, _keep = _history_struct(prompt)
+        if not lib().bark_b200_set_history_prompt(self.ctx, C.byref(st)):
+            raise ValueError("bark_b200_set_history_prompt rejected the prompt (see stderr)")
+
+    def last_generation_prompt(self) -> dict:
+        """The last generation's ids as a history prompt: semantic_prompt [n], coarse_prompt [2][T], fine_prompt [8][T].  np.savez of it
+        writes a voice file upstream Bark also reads."""
+        return {"semantic_prompt": self.tokens(0).copy(), "coarse_prompt": np.ascontiguousarray(self.tokens(1).T),
+                "fine_prompt": np.ascontiguousarray(self.tokens(2).T)}
 
     @property
     def load_time_us(self):
@@ -260,15 +329,24 @@ class Bark:
             raise RuntimeError("bark_b200_gpt_step_batch failed")
         return out, npa
 
-    def generate_batch(self, texts, seeds, n_threads: int = 1) -> list:
-        """Up to 8 prompts decoded together; item i equals a fresh context's generate(texts[i]) with seed seeds[i].
+    def generate_batch(self, texts, seeds, n_threads: int = 1, history_prompts=None) -> list:
+        """Up to 8 prompts decoded together; item i equals a fresh context's generate(texts[i], history_prompt=history_prompts[i])
+        with seed seeds[i].  history_prompts: None, or one prompt or None per item; the context's own prompt does not apply.
         Returns the waveforms; batch_tokens(i, stage) gives the ids."""
         n = len(texts)
         if len(seeds) != n:
             raise RuntimeError(f"generate_batch: {n} prompts but {len(seeds)} seeds")
         arr = (C.c_char_p * max(n, 1))(*[t.encode() for t in texts])
         sd = (C.c_uint32 * max(n, 1))(*[int(s) for s in seeds])
-        if not lib().bark_b200_generate_batch(self.ctx, arr, sd, n, n_threads):
+        if history_prompts is None:
+            ok = lib().bark_b200_generate_batch(self.ctx, arr, sd, n, n_threads)
+        else:
+            if len(history_prompts) != n:
+                raise RuntimeError(f"generate_batch: {n} prompts but {len(history_prompts)} history prompts")
+            structs = [None if p is None else _history_struct(p) for p in history_prompts]
+            ptrs = (C.POINTER(HistoryPromptStruct) * max(n, 1))(*[C.pointer(s[0]) if s else None for s in structs])
+            ok = lib().bark_b200_generate_batch_prompted(self.ctx, arr, sd, ptrs, n, n_threads)
+        if not ok:
             raise RuntimeError("bark_b200_generate_batch failed")
         out = []
         for i in range(n):

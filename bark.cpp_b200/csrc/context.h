@@ -17,10 +17,20 @@ struct ShardState {
     unsigned long long nvlink_bytes = 0;             // bytes this rank stored into peer memory (K / V rows, sampled ids)
 };
 
-// What one generation reads and produces: its RNG, its token streams and its waveform.  The context holds one (bark.h's
-// single-prompt calls); every item of a batch (bark_b200_generate_batch) holds its own, so a batch leaves the context's untouched.
+// A speaker history prompt (bark_b200_set_history_prompt): upstream Bark's voice-file arrays, codebook-major, validated.
+// No semantic ids: no prompt.
+struct HistoryPrompt {
+    std::vector<int32_t> semantic;                   // [n_s]
+    std::vector<int32_t> coarse;                     // [2][n_c]
+    std::vector<int32_t> fine;                       // [8][n_f], n_f may be 0
+    bool empty() const { return semantic.empty(); }
+};
+
+// What one generation reads and produces: its RNG, its history prompt, its token streams and its waveform.  The context holds one
+// (bark.h's single-prompt calls); every item of a batch (bark_b200_generate_batch) holds its own, so a batch leaves the context's untouched.
 struct Generation {
     std::mt19937 rng;                                // seeded once at load (bark.cpp:1179), or per batch item
+    HistoryPrompt prompt;                            // conditions the three stages (bark_api.cu); empty: every generation starts from nothing
     std::vector<int32_t> tokens;                     // 513 prompt ids
     std::vector<int32_t> semantic_tokens;
     std::vector<int32_t> coarse_tokens;              // [T][2] flattened

@@ -104,6 +104,32 @@ BARK_API int  bark_b200_batch_tokens(struct bark_context * ctx, int i, int stage
 BARK_API int  bark_b200_gpt_eval_slot(struct bark_context * ctx, int which, int slot, const int32_t * tokens, int n, int * n_past, int merge_ctx, float * logits_out);
 BARK_API int  bark_b200_gpt_step_batch(struct bark_context * ctx, int which, int B, const int32_t * slots, const int32_t * tokens, int * n_past, float * logits_out);
 
+/* SPEAKER HISTORY PROMPTS: condition the semantic, coarse and fine stages on a voice prompt's ids, as upstream Bark's history_prompt
+ * (its semantic_prompt / coarse_prompt / fine_prompt voice-file arrays) does, so that consecutive generations keep one voice.  A
+ * finished generation's own ids are a valid prompt for the next one; bark_b200_encodec_encode's codes are a fine prompt.  C and F are
+ * codebook-major, the layout of the voice files and of bark_b200_encodec_encode.  A prompt is valid when n_semantic >= 1 and every
+ * semantic id is in [0, semantic_vocab_size); n_coarse_frames >= 1, n_fine_frames >= 0 and every code is in [0, codebook_size); and
+ * the two lengths align as upstream checks it, round(n_c / n_s, 1) == round(stc / n_coarse_codebooks, 1) with stc = coarse_rate_hz /
+ * semantic_rate_hz * n_coarse_codebooks: 29 n_s < 20 n_c < 31 n_s for the default rates.  What a prompt changes (DESIGN.md §12):
+ *   semantic  prompt positions [256, 512) hold the last 256 semantic ids, right-padded
+ *   coarse    each window starts from up to 209 prompt semantic ids and up to 628 prompt coarse ids before the generated ones
+ *   fine      the last min(n_fine_frames, 512) prompt frames precede the coarse frames in the fine windows
+ * The generated ids, bark_get_audio_data, the statistics and bark_b200_get_tokens stages 0-2 describe the generated part only; stage
+ * 3 returns the prompted 513 ids. */
+struct bark_b200_history_prompt {
+    const int32_t * semantic; int n_semantic;        /* [n_semantic] */
+    const int32_t * coarse;   int n_coarse_frames;   /* [2][n_coarse_frames] */
+    const int32_t * fine;     int n_fine_frames;     /* [8][n_fine_frames], may be 0 frames */
+};
+/* Validates and copies; NULL clears.  Applies to later bark_generate_audio, bark_b200_tokenize and bark_b200_forward_* calls
+ * on this context.  Returns 1, or 0 with a message; a rejected prompt leaves the previous one in place. */
+BARK_API int  bark_b200_set_history_prompt(struct bark_context * ctx, const struct bark_b200_history_prompt * prompt);
+/* bark_b200_generate_batch with one prompt per item: prompts may be NULL, and so may any entry (no prompt).  Item i equals a fresh
+ * context with seeds[i] and prompts[i] set, generating texts[i].  A rejected prompt fails the batch before anything runs.
+ * bark_b200_generate_batch itself ignores the context's prompt. */
+BARK_API bool bark_b200_generate_batch_prompted(struct bark_context * ctx, const char * const * texts, const uint32_t * seeds,
+                                                const struct bark_b200_history_prompt * const * prompts, int n, int n_threads);
+
 /* FAST MODE (BARK_B200_MODE=fast in the environment at load; opt-in, NOT bit-identical to the reference): the fine model's
  * 1024-row passes (bark.cpp:1416-1584) run as wgmma tensor-core GEMMs + flash-style attention (csrc/fast_kernels.cu).
  * The two kernel hooks below run on host buffers without a context, for the numerics tests:
