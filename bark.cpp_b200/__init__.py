@@ -40,6 +40,11 @@ class BarkStatistics(C.Structure):
                 ("t_fine_us", C.c_int64), ("n_sample_semantic", C.c_int32), ("n_sample_coarse", C.c_int32), ("n_sample_fine", C.c_int32)]
 
 
+class EncodecStatistics(C.Structure):
+    """struct encodec_statistics (include/encodec.h)."""
+    _fields_ = [("t_load_us", C.c_int64), ("t_compute_us", C.c_int64)]
+
+
 class HistoryPromptStruct(C.Structure):
     """struct bark_b200_history_prompt (include/bark_b200.h)."""
     _fields_ = [("semantic", C.c_void_p), ("n_semantic", C.c_int), ("coarse", C.c_void_p), ("n_coarse_frames", C.c_int),
@@ -94,6 +99,13 @@ EXPORTS = [
     "bark_b200_parity_rows", "bark_b200_sample_given_u", "bark_b200_generate_batch", "bark_b200_batch_audio", "bark_b200_batch_tokens", "bark_b200_gpt_eval_slot", "bark_b200_gpt_step_batch",
     "bark_b200_set_history_prompt", "bark_b200_generate_batch_prompted",
     "ggml_time_init", "ggml_time_us", "ggml_time_ms", "ggml_init", "ggml_free",
+]
+
+# encodec.cpp's API (include/encodec.h), exported by the same library; kept apart from EXPORTS, which lists the bark headers' symbols
+ENCODEC_EXPORTS = [
+    "encodec_load_model", "encodec_set_target_bandwidth", "encodec_set_sample_rate", "encodec_reconstruct_audio", "encodec_compress_audio",
+    "encodec_decompress_audio", "encodec_get_audio", "encodec_get_audio_size", "encodec_get_codes", "encodec_get_codes_size",
+    "encodec_get_statistics", "encodec_reset_statistics", "encodec_free",
 ]
 
 _lib = None
@@ -196,6 +208,23 @@ def lib() -> C.CDLL:
     L.bark_b200_generate_batch_prompted.argtypes = [vp, C.POINTER(C.c_char_p), C.POINTER(C.c_uint32), C.POINTER(C.POINTER(HistoryPromptStruct)),
                                                     C.c_int, C.c_int]
     L.ggml_time_us.restype = C.c_int64
+    L.encodec_load_model.restype = vp
+    L.encodec_load_model.argtypes = [C.c_char_p, C.c_int, C.c_int]
+    L.encodec_set_target_bandwidth.argtypes = [vp, C.c_int]
+    L.encodec_set_sample_rate.argtypes = [vp, C.c_int]
+    for n in ("encodec_reconstruct_audio", "encodec_compress_audio"):
+        getattr(L, n).restype = C.c_bool
+        getattr(L, n).argtypes = [vp, f32p, C.c_int, C.c_int]
+    L.encodec_decompress_audio.restype = C.c_bool
+    L.encodec_decompress_audio.argtypes = [vp, i32p, C.c_int, C.c_int]
+    L.encodec_get_audio.restype = C.POINTER(C.c_float)
+    L.encodec_get_codes.restype = C.POINTER(C.c_int32)
+    L.encodec_get_statistics.restype = C.POINTER(EncodecStatistics)
+    for n in ("encodec_get_audio_size", "encodec_get_codes_size"):
+        getattr(L, n).restype = C.c_int
+    for n in ("encodec_get_audio", "encodec_get_audio_size", "encodec_get_codes", "encodec_get_codes_size", "encodec_get_statistics",
+              "encodec_reset_statistics", "encodec_free"):
+        getattr(L, n).argtypes = [vp]
     _lib = L
     return L
 
@@ -592,9 +621,94 @@ def sample_given_u(logits: np.ndarray, temp: float, u=None, threads: int = 0):
     return out
 
 
+class Encodec:
+    """One encodec_context (include/encodec.h): the 24 kHz EnCodec of a weight file, at any bandwidth its codebooks allow.
+    offset: byte position of the codec section (0 for a standalone encodec.cpp file).  Mirrors encodec.cpp's examples."""
+
+    def __init__(self, model_path: str, offset: int = 0, device: int | None = None):
+        L = lib()
+        if device is not None:
+            L.bark_b200_set_device(device)
+        self.ctx = L.encodec_load_model(os.fsencode(model_path), offset, 0)
+        if not self.ctx:
+            raise RuntimeError(f"encodec_load_model failed for {model_path} at offset {offset} (see stderr); no CPU fallback exists")
+        self.ctx = C.c_void_p(self.ctx)
+        self._bandwidth, self._sample_rate = None, None
+
+    def close(self):
+        if getattr(self, "ctx", None):
+            lib().encodec_free(self.ctx)
+            self.ctx = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    @property
+    def bandwidth(self):
+        """Target bandwidth in kbps (encodec_set_target_bandwidth); None: the file's."""
+        return self._bandwidth
+
+    @bandwidth.setter
+    def bandwidth(self, kbps: int):
+        lib().encodec_set_target_bandwidth(self.ctx, int(kbps))
+        self._bandwidth = int(kbps)
+
+    @property
+    def sample_rate(self):
+        """Sample rate in Hz (encodec_set_sample_rate); it only changes n_q, as in the reference.  None: the file's."""
+        return self._sample_rate
+
+    @sample_rate.setter
+    def sample_rate(self, hz: int):
+        lib().encodec_set_sample_rate(self.ctx, int(hz))
+        self._sample_rate = int(hz)
+
+    @property
+    def n_q(self) -> int:
+        """Codebooks of the current bandwidth and sample rate, read from the codes of a minimal compress."""
+        return self.compress(np.zeros(1921, np.float32)).shape[0]
+
+    def compress(self, audio) -> np.ndarray:
+        """Mono float32 samples (finite, at least 1921) -> codes [n_q][T] int32, T = ceil(n / 320)."""
+        a = np.ascontiguousarray(audio, np.float32).ravel()
+        if not lib().encodec_compress_audio(self.ctx, _p(a), a.size, 1):
+            raise RuntimeError("encodec_compress_audio failed (see stderr)")
+        n = lib().encodec_get_codes_size(self.ctx)
+        T = (a.size + 319) // 320
+        return np.ctypeslib.as_array(lib().encodec_get_codes(self.ctx), shape=(n,)).copy().reshape(n // T, T)
+
+    def decompress(self, codes) -> np.ndarray:
+        """Codes [n_q][T] (n_q of the current bandwidth) -> 320 T float32 samples."""
+        c = np.ascontiguousarray(codes, np.int32)
+        if not lib().encodec_decompress_audio(self.ctx, _p(c), c.size, 1):
+            raise RuntimeError("encodec_decompress_audio failed (see stderr)")
+        return self._audio()
+
+    def reconstruct(self, audio) -> np.ndarray:
+        """compress then decompress on the device: 320 T float32 samples."""
+        a = np.ascontiguousarray(audio, np.float32).ravel()
+        if not lib().encodec_reconstruct_audio(self.ctx, _p(a), a.size, 1):
+            raise RuntimeError("encodec_reconstruct_audio failed (see stderr)")
+        return self._audio()
+
+    def _audio(self):
+        n = lib().encodec_get_audio_size(self.ctx)
+        return np.ctypeslib.as_array(lib().encodec_get_audio(self.ctx), shape=(n,)).copy()
+
+    def stats(self) -> dict:
+        s = lib().encodec_get_statistics(self.ctx).contents
+        return {"t_load_us": s.t_load_us, "t_compute_us": s.t_compute_us}
+
+    def reset_stats(self):
+        lib().encodec_reset_statistics(self.ctx)
+
+
 def rvq_encode(latent: np.ndarray, codebooks: np.ndarray) -> np.ndarray:
     """The RVQ encode kernel on latent [hidden][T] and codebooks [n_q][n_bins][hidden] float32 (hidden % 32 == 0 and <= 128,
-    n_bins <= 1024, n_q <= 8); returns codes [n_q][T] int32, bit-identical to the reference's quantizer encode."""
+    n_bins <= 1024, n_q <= 32); returns codes [n_q][T] int32, bit-identical to the reference's quantizer encode."""
     lat = np.ascontiguousarray(latent, np.float32); cb = np.ascontiguousarray(codebooks, np.float32)
     hidden, T = lat.shape
     n_q, n_bins, h2 = cb.shape

@@ -390,7 +390,7 @@ bool decode_audio(bark_context * ctx, Generation & g) {
     if (ctx->params.target_bandwidth != 6 || ctx->params.sample_rate != 24000) {
         fprintf(stderr, "%s: only target_bandwidth 6 / 24 kHz is implemented\n", __func__); return false;
     }
-    if (!codec_decode(ctx, codes.data(), T, g.audio)) { printf("%s: Could not generate waveform from tokens with Encodec\n", __func__); return false; }
+    if (!codec_decode(ctx->codec, ctx->codec_scratch, ctx->stream, codes.data(), 8, T, g.audio)) { printf("%s: Could not generate waveform from tokens with Encodec\n", __func__); return false; }
     return true;
 }
 
@@ -716,23 +716,29 @@ extern "C" struct bark_context_params bark_context_default_params(void) {
 
 extern "C" void bark_b200_set_device(int device) { g_device_override = device; }
 
-extern "C" struct bark_context * bark_load_model(const char * model_path, struct bark_context_params params, uint32_t seed) {
-    const int64_t t0 = now_us();
-    if (!model_path) { fprintf(stderr, "%s: null model path\n", __func__); return nullptr; }
+int bark::select_device(const char * caller, cudaDeviceProp * prop) {
     int n_dev = 0;
     if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0) {
-        fprintf(stderr, "%s: no CUDA device available — this library has no CPU path\n", __func__);
-        return nullptr;
+        fprintf(stderr, "%s: no CUDA device available — this library has no CPU path\n", caller);
+        return -1;
     }
     int dev = g_device_override;
     if (dev < 0) { const char * e = getenv("BARK_B200_DEVICE"); dev = e ? atoi(e) : 0; }
-    if (dev < 0 || dev >= n_dev) { fprintf(stderr, "%s: CUDA device %d out of range (%d present)\n", __func__, dev, n_dev); return nullptr; }
-    cudaDeviceProp prop;
-    if (cudaSetDevice(dev) != cudaSuccess || cudaGetDeviceProperties(&prop, dev) != cudaSuccess) { fprintf(stderr, "%s: cannot use CUDA device %d: %s\n", __func__, dev, cudaGetErrorString(cudaGetLastError())); return nullptr; }
-    if (prop.major != 9 || prop.minor != 0) {
-        fprintf(stderr, "%s: device %d is sm_%d%d; this library is built for sm_90a (H100) only\n", __func__, dev, prop.major, prop.minor);
-        return nullptr;
+    if (dev < 0 || dev >= n_dev) { fprintf(stderr, "%s: CUDA device %d out of range (%d present)\n", caller, dev, n_dev); return -1; }
+    if (cudaSetDevice(dev) != cudaSuccess || cudaGetDeviceProperties(prop, dev) != cudaSuccess) { fprintf(stderr, "%s: cannot use CUDA device %d: %s\n", caller, dev, cudaGetErrorString(cudaGetLastError())); return -1; }
+    if (prop->major != 9 || prop->minor != 0) {
+        fprintf(stderr, "%s: device %d is sm_%d%d; this library is built for sm_90a (H100) only\n", caller, dev, prop->major, prop->minor);
+        return -1;
     }
+    return dev;
+}
+
+extern "C" struct bark_context * bark_load_model(const char * model_path, struct bark_context_params params, uint32_t seed) {
+    const int64_t t0 = now_us();
+    if (!model_path) { fprintf(stderr, "%s: null model path\n", __func__); return nullptr; }
+    cudaDeviceProp prop;
+    const int dev = select_device(__func__, &prop);
+    if (dev < 0) return nullptr;
     bark_context * ctx = new bark_context();
     ctx->device = dev;
     ctx->n_sm = ctx->n_sm_total = prop.multiProcessorCount;
@@ -820,12 +826,10 @@ extern "C" void bark_free(struct bark_context * ctx) {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
-    for (void * p : ctx->device_allocs) cudaFree(p);
+    ctx->arena.release();
     for (int p = 0; p < ctx->shard.world; p++) if (p != ctx->shard.rank && ctx->shard.peer[p]) cudaIpcCloseMemHandle(ctx->shard.peer[p]);
     if (ctx->shard.local) cudaFree(ctx->shard.local);
-    for (int i = 0; i < 3; i++) if (ctx->c_buf[i]) cudaFree(ctx->c_buf[i]);
-    if (ctx->c_gi) cudaFree(ctx->c_gi);
-    if (ctx->d_codes) cudaFree(ctx->d_codes);
+    ctx->codec_scratch.release();
     if (ctx->h_logits) cudaFreeHost(ctx->h_logits);
     if (ctx->h_tok) cudaFreeHost(ctx->h_tok);
     if (ctx->h_u) cudaFreeHost(ctx->h_u);
@@ -860,7 +864,7 @@ extern "C" int bark_b200_fine_eval(struct bark_context * ctx, const int32_t * in
 static int bark_b200_encodec_decode_impl(struct bark_context * ctx, const int32_t * codes, int n_frames, float * out, int out_cap) {
     if (!ctx || !codes) return -1;
     BARK_CUDA_CHECK(cudaSetDevice(ctx->device));
-    if (!codec_decode(ctx, codes, n_frames, ctx->gen.audio)) return -1;
+    if (!codec_decode(ctx->codec, ctx->codec_scratch, ctx->stream, codes, 8, n_frames, ctx->gen.audio)) return -1;
     const int n = (int) ctx->gen.audio.size();
     if (out) memcpy(out, ctx->gen.audio.data(), sizeof(float) * (size_t) std::min(n, out_cap));
     return n;
@@ -871,7 +875,7 @@ static int bark_b200_encodec_encode_impl(struct bark_context * ctx, const float 
     if (!ctx || !audio) { fprintf(stderr, "bark_b200_encodec_encode: null %s\n", ctx ? "audio" : "context"); return -1; }
     BARK_CUDA_CHECK(cudaSetDevice(ctx->device));
     std::vector<int32_t> c; std::vector<float> l;
-    if (!codec_encode(ctx, audio, n_samples, c, l)) return -1;
+    if (!codec_encode(ctx->codec, ctx->codec_scratch, ctx->stream, audio, n_samples, 8, &c, &l)) return -1;
     if (codes) memcpy(codes, c.data(), sizeof(int32_t) * std::min(c.size(), (size_t) std::max(codes_cap, 0)));
     if (latent) memcpy(latent, l.data(), sizeof(float) * std::min(l.size(), (size_t) std::max(latent_cap, 0)));
     return (int)(c.size() / 8);
@@ -882,7 +886,7 @@ extern "C" int bark_b200_encodec_encode(struct bark_context * ctx, const float *
 }
 // the RVQ encode kernel on host buffers (tests): norms from rvq_norms_kernel, codes [n_q][T] from rvq_encode_kernel
 static int bark_b200_rvq_encode_impl(const float * latent, int T, const float * codebooks, int hidden, int n_bins, int n_q, int32_t * codes) {
-    if (!latent || !codebooks || !codes || T < 1 || hidden < 32 || hidden > 128 || hidden % 32 || n_bins < 1 || n_bins > 1024 || n_q < 1 || n_q > 8) return 0;
+    if (!latent || !codebooks || !codes || T < 1 || hidden < 32 || hidden > 128 || hidden % 32 || n_bins < 1 || n_bins > 1024 || n_q < 1 || n_q > kMaxCodebooks) return 0;
     struct Buffers {                                          // freed on every exit, including a CUDA failure thrown mid-way
         void * p[4] = {nullptr, nullptr, nullptr, nullptr};
         ~Buffers() { for (void * q : p) cudaFree(q); }
@@ -894,7 +898,7 @@ static int bark_b200_rvq_encode_impl(const float * latent, int T, const float * 
     BARK_CUDA_CHECK(cudaMemcpy(dl, latent, (size_t) hidden * T * 4, cudaMemcpyHostToDevice));
     BARK_CUDA_CHECK(cudaMemcpy(dcb, codebooks, cb_n * 4, cudaMemcpyHostToDevice));
     BARK_CUDA_CHECK(cudaMemset(dc, 0xff, (size_t) n_q * T * 4));              // -1: a missing store shows up
-    const float * emb[8], * nrm[8];
+    const float * emb[kMaxCodebooks], * nrm[kMaxCodebooks];
     for (int q = 0; q < n_q; q++) {
         emb[q] = dcb + (size_t) q * n_bins * hidden; nrm[q] = dn + (size_t) q * n_bins;
         rvq_norms(emb[q], n_bins, hidden, dn + (size_t) q * n_bins, 0);

@@ -1,4 +1,4 @@
-// EnCodec kernels (24 kHz model, bandwidth 6 -> 8 codebooks, hop 320), bit-exact path.
+// EnCodec kernels (24 kHz model, up to 32 codebooks, hop 320), bit-exact path.
 //
 // Replaces encodec_forward_quantizer_decode (encodec.cpp/quantizer.h:78-111) and
 // encodec_forward_decoder (encodec.cpp/decoder.h:43-113):
@@ -14,24 +14,29 @@
 // bit-identical to the CPU reference, not merely within the 1e-3 contract.
 #include "codec_kernels.h"
 
+#include <cooperative_groups.h>
+namespace cg = cooperative_groups;
+
 namespace bark {
 
 // ------------------------------------------------------------------------------------------------
-// quantizer decode: x[d][t] = sum_q embed_q[codes[q][t]][d], q = 0..7 in order onto a zeroed tensor
+// quantizer decode: x[d][t] = sum_q embed_q[codes[q][t]][d], q = 0..n_q-1 in order onto a zeroed tensor (quantizer.h:95-106)
 // ------------------------------------------------------------------------------------------------
-struct Codebooks { const float * e[8]; };
-__global__ void rvq_decode_kernel(Codebooks cb, const int32_t * __restrict__ codes, int T, int Hd, float * __restrict__ x) {
+struct Codebooks { const float * e[kMaxCodebooks]; };
+__global__ void rvq_decode_kernel(Codebooks cb, const int32_t * __restrict__ codes, int n_q, int T, int Hd, float * __restrict__ x) {
     const int t = blockIdx.x * blockDim.x + threadIdx.x, d = blockIdx.y;
     if (t >= T) return;
     float acc = 0.0f;
 #pragma unroll
-    for (int q = 0; q < 8; q++) acc = __fadd_rn(acc, cb.e[q][(size_t) codes[q * T + t] * Hd + d]);
+    for (int q = 0; q < kMaxCodebooks; q++)              // constant indices: the parameter struct stays in constant memory
+        if (q < n_q) acc = __fadd_rn(acc, cb.e[q][(size_t) codes[q * T + t] * Hd + d]);
     x[(size_t) d * T + t] = acc;
 }
 
-void rvq_decode(const CodecModel & cm, const int32_t * d_codes, int T, float * x, cudaStream_t s) {
-    Codebooks cb; for (int q = 0; q < 8; q++) cb.e[q] = cm.embed[q];
-    BARK_LAUNCH(rvq_decode_kernel, dim3((T + 127) / 128, cm.hidden_dim), 128, 0, s, cb, d_codes, T, cm.hidden_dim, x);
+void rvq_decode(const CodecModel & cm, const int32_t * d_codes, int n_q, int T, float * x, cudaStream_t s) {
+    Codebooks cb{};
+    for (int q = 0; q < n_q; q++) cb.e[q] = cm.embed[q];
+    BARK_LAUNCH(rvq_decode_kernel, dim3((T + 127) / 128, cm.hidden_dim), 128, 0, s, cb, d_codes, n_q, T, cm.hidden_dim, x);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -52,27 +57,38 @@ void rvq_norms(const float * embed, int n_bins, int Hd, float * out, cudaStream_
     BARK_LAUNCH(rvq_norms_kernel, (n_bins + 127) / 128, 128, 0, s, embed, n_bins, Hd, out);
 }
 
-// One CTA per 8 frames, one warp per frame for the argmax; every warp walks codewords j = warp, warp + 8, ... with lane v holding
-// virtual lane v of the dot's chain (Hd / 32 steps), so each codeword row is read once per 8 frames.  The residuals stay in shared
-// memory through all codebooks.  The argmax takes the last index holding the row maximum (what the reference's running MAX and ==
-// select for rows without NaN); a row with a NaN goes through the reference's loop on one lane, where a NaN resets the maximum.
-constexpr int kRvqFrames = 8, kRvqMaxBins = 1024, kRvqMaxHidden = 128;
-__global__ void __launch_bounds__(256, 1) rvq_encode_kernel(const float * __restrict__ latent, int T, Codebooks cb, Codebooks norms, int n_q, int n_bins,
-                                                         int Hd, int32_t * __restrict__ codes) {
-    __shared__ float vals[kRvqFrames][kRvqMaxBins];
+// One cluster of kRvqCtas CTAs per 8 frames.  CTA r owns codewords [r*S, min((r+1)*S, n_bins)), S = ceil(n_bins / kRvqCtas), and every
+// CTA keeps its own copy of the 8 residuals in shared memory through all codebooks.  Per codebook, warp w of a CTA walks its codewords
+// j = lo + w, lo + w + 8, ... with lane v holding virtual lane v of the dot's chain (Hd / 32 steps), so each codeword row is read once
+// per 8 frames; warp f then reduces frame f's slice to (maximum, last index holding it, NaN seen).  The CTAs exchange these through
+// distributed shared memory and each combines them in the same way: the last index holding the row maximum is what the reference's
+// running MAX and == select for rows without NaN.  A row with a NaN goes through the reference's loop on one lane, reading the peers'
+// slices in order through DSMEM, where a NaN resets the maximum.  Every CTA then applies the same residual update.
+// The values and partials are double-buffered by codebook parity, so one cluster barrier per codebook orders the writes of codebook
+// q + 2 after every peer's reads of codebook q.
+constexpr int kRvqFrames = 8, kRvqCtas = 8, kRvqMaxBins = 1024, kRvqMaxHidden = 128, kRvqSlice = kRvqMaxBins / kRvqCtas;
+__global__ void __cluster_dims__(kRvqCtas, 1, 1) __launch_bounds__(256) rvq_encode_kernel(
+        const float * __restrict__ latent, int T, Codebooks cb, Codebooks norms, int n_q, int n_bins, int Hd, int32_t * __restrict__ codes) {
+    __shared__ float vals[2][kRvqFrames][kRvqSlice];
+    __shared__ float p_max[2][kRvqFrames];
+    __shared__ int p_idx[2][kRvqFrames], p_nan[2][kRvqFrames];
     __shared__ float res[kRvqFrames][kRvqMaxHidden];
     __shared__ float s_nrm[kRvqFrames];
     __shared__ int s_code[kRvqFrames];
-    __shared__ const float * s_cb[8], * s_cn[8];         // indexing the parameter structs by q would copy them to the stack
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, f0 = blockIdx.x * kRvqFrames, nc = Hd >> 5;
+    __shared__ const float * s_cb[kMaxCodebooks], * s_cn[kMaxCodebooks];   // indexing the parameter structs by q would copy them to the stack
+    cg::cluster_group cluster = cg::this_cluster();
+    const int rank = (int) cluster.block_rank();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, f0 = (blockIdx.x / kRvqCtas) * kRvqFrames, nc = Hd >> 5;
+    const int S = (n_bins + kRvqCtas - 1) / kRvqCtas, lo = min(rank * S, n_bins), cnt = min(n_bins - lo, S);
 #pragma unroll
-    for (int q = 0; q < 8; q++) if (threadIdx.x == q) { s_cb[q] = cb.e[q]; s_cn[q] = norms.e[q]; }
+    for (int q = 0; q < kMaxCodebooks; q++) if (threadIdx.x == q) { s_cb[q] = cb.e[q]; s_cn[q] = norms.e[q]; }
     for (int i = threadIdx.x; i < kRvqFrames * Hd; i += blockDim.x) {
         const int f = i / Hd, d = i % Hd;
         res[f][d] = f0 + f < T ? latent[(size_t) d * T + f0 + f] : 0.f;
     }
     __syncthreads();
     for (int q = 0; q < n_q; q++) {
+        const int b = q & 1;
         const float * E = s_cb[q], * nrm = s_cn[q];
         if (lane == 0) {
             double s = 0.0;
@@ -87,7 +103,8 @@ __global__ void __launch_bounds__(256, 1) rvq_encode_kernel(const float * __rest
 #pragma unroll
             for (int c = 0; c < kRvqMaxHidden / 32; c++) r[f][c] = c < nc ? res[f][c * 32 + lane] : 0.f;
         }
-        for (int j = warp; j < n_bins; j += 8) {
+        for (int jl = warp; jl < cnt; jl += 8) {
+            const int j = lo + jl;
             float ev[kRvqMaxHidden / 32];
 #pragma unroll
             for (int c = 0; c < kRvqMaxHidden / 32; c++) ev[c] = c < nc ? __ldg(E + (size_t) j * Hd + c * 32 + lane) : 0.f;
@@ -98,28 +115,49 @@ __global__ void __launch_bounds__(256, 1) rvq_encode_kernel(const float * __rest
 #pragma unroll
                 for (int c = 0; c < kRvqMaxHidden / 32; c++) if (c < nc) acc = __fmaf_rn(ev[c], r[f][c], acc);
                 const float dot = lane_tree_reduce(acc);
-                if (lane == f) vals[f][j] = -__fadd_rn(ej, __fadd_rn(sn[f], __fmul_rn(dot, -2.0f)));
+                if (lane == f) vals[b][f][jl] = -__fadd_rn(ej, __fadd_rn(sn[f], __fmul_rn(dot, -2.0f)));
             }
         }
         __syncthreads();
-        {
-            const float * v = vals[warp];
+        {   // this CTA's slice of frame `warp`
+            const float * v = vals[b][warp];
             float m = -INFINITY; bool nan = false;
-            for (int j = lane; j < n_bins; j += 32) { const float a = v[j]; nan |= a != a; m = fmaxf(m, a); }
+            for (int j = lane; j < cnt; j += 32) { const float a = v[j]; nan |= a != a; m = fmaxf(m, a); }
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
             int idx = -1;
-            for (int j = lane; j < n_bins; j += 32) if (v[j] == m) idx = j;
+            for (int j = lane; j < cnt; j += 32) if (v[j] == m) idx = lo + j;
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) idx = max(idx, __shfl_xor_sync(0xffffffffu, idx, o));
+            const bool any_nan = __any_sync(0xffffffffu, nan);
+            if (lane == 0) { p_max[b][warp] = m; p_idx[b][warp] = idx; p_nan[b][warp] = any_nan; }
+        }
+        cluster.sync();                                  // every CTA's partials (and values) of codebook q are visible
+        {   // lane r < kRvqCtas reads rank r's partial of frame `warp`; ranks hold ascending codeword ranges
+            float m = -INFINITY; int idx = -1, nan = 0;
+            if (lane < kRvqCtas) {
+                m = *cluster.map_shared_rank(&p_max[b][warp], lane);
+                idx = *cluster.map_shared_rank(&p_idx[b][warp], lane);
+                nan = *cluster.map_shared_rank(&p_nan[b][warp], lane);
+            }
+            float mx = m;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+            int best = lane < kRvqCtas && m == mx ? idx : -1;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) best = max(best, __shfl_xor_sync(0xffffffffu, best, o));
             if (__any_sync(0xffffffffu, nan) && lane == 0) {
-                float mx = -INFINITY; idx = 0;
-                for (int j = 0; j < n_bins; j++) { mx = mx > v[j] ? mx : v[j]; if (mx == v[j]) idx = j; }
+                float run = -INFINITY; best = 0;
+                for (int pr = 0; pr < kRvqCtas; pr++) {
+                    const int plo = min(pr * S, n_bins), pcnt = min(n_bins - plo, S);
+                    const float * pv = cluster.map_shared_rank(&vals[b][warp][0], pr);
+                    for (int j = 0; j < pcnt; j++) { const float a = pv[j]; run = run > a ? run : a; if (run == a) best = plo + j; }
+                }
             }
             if (lane == 0) {
                 const bool live = f0 + warp < T;
-                s_code[warp] = live ? idx : 0;
-                if (live) codes[(size_t) q * T + f0 + warp] = idx;
+                s_code[warp] = live ? best : 0;
+                if (live && rank == 0) codes[(size_t) q * T + f0 + warp] = best;
             }
         }
         __syncthreads();
@@ -129,15 +167,16 @@ __global__ void __launch_bounds__(256, 1) rvq_encode_kernel(const float * __rest
         }
         __syncthreads();
     }
+    cluster.sync();                                      // a CTA's shared memory must outlive its peers' last reads
 }
 
 bool rvq_encode(const float * const * embed, const float * const * norms, int n_q, int n_bins, int Hd, const float * latent, int T, int32_t * codes,
                 cudaStream_t s) {
-    if (n_q < 1 || n_q > 8 || n_bins < 1 || n_bins > kRvqMaxBins || Hd < 32 || Hd > kRvqMaxHidden || Hd % 32 || T < 1) return false;
-    Codebooks cb, nr;
-    for (int q = 0; q < 8; q++) { cb.e[q] = q < n_q ? embed[q] : nullptr; nr.e[q] = q < n_q ? norms[q] : nullptr; }
+    if (n_q < 1 || n_q > kMaxCodebooks || n_bins < 1 || n_bins > kRvqMaxBins || Hd < 32 || Hd > kRvqMaxHidden || Hd % 32 || T < 1) return false;
+    Codebooks cb{}, nr{};
+    for (int q = 0; q < n_q; q++) { cb.e[q] = embed[q]; nr.e[q] = norms[q]; }
     g_next_flops = 2.0 * (double) T * n_q * n_bins * Hd;
-    BARK_LAUNCH(rvq_encode_kernel, (T + kRvqFrames - 1) / kRvqFrames, 256, 0, s, latent, T, cb, nr, n_q, n_bins, Hd, codes);
+    BARK_LAUNCH(rvq_encode_kernel, (T + kRvqFrames - 1) / kRvqFrames * kRvqCtas, 256, 0, s, latent, T, cb, nr, n_q, n_bins, Hd, codes);
     return true;
 }
 

@@ -4,11 +4,11 @@
 
 namespace bark {
 
-void rvq_decode(const CodecModel & cm, const int32_t * d_codes /*[8][T]*/, int T, float * x /*[hidden][T]*/, cudaStream_t s);
+void rvq_decode(const CodecModel & cm, const int32_t * d_codes /*[n_q][T]*/, int n_q, int T, float * x /*[hidden][T]*/, cudaStream_t s);
 // e_j = sum of squares of codeword j (the RVQ encode's codebook norms), embed [n_bins][Hd] -> out [n_bins]
 void rvq_norms(const float * embed, int n_bins, int Hd, float * out, cudaStream_t s);
 // codes [n_q][T] of latent [Hd][T] through codebooks embed[q] [n_bins][Hd] with their norms; false for shapes outside
-// n_q <= 8, n_bins <= 1024, Hd % 32 == 0 and Hd <= 128
+// n_q <= 32, n_bins <= 1024, Hd % 32 == 0 and Hd <= 128
 bool rvq_encode(const float * const * embed, const float * const * norms, int n_q, int n_bins, int Hd, const float * latent, int T, int32_t * codes,
                 cudaStream_t s);
 // strided_conv_1d (ops.cpp:59-75) on x [Cin][T]: ELU on the input when elu_in, resid added to the output (stride 1 only).

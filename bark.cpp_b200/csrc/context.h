@@ -4,6 +4,7 @@
 #include "../../include/bark.h"
 #include "model.h"
 
+#include <fstream>
 #include <map>
 #include <random>
 #include <string>
@@ -86,11 +87,7 @@ struct bark_context {
     float * h_logits = nullptr;                      // pinned, max(n_out) or 1024*fine_vocab
     int32_t * h_tok = nullptr;                       // pinned, 8*1024 ids
 
-    // codec scratch
-    float * c_buf[3] = {nullptr, nullptr, nullptr}; size_t c_cap = 0;   // ping-pong activations (floats)
-    float * c_gi = nullptr;                                            // LSTM input projections
-    float * c_hbuf = nullptr; unsigned * c_counter = nullptr;          // LSTM hidden-state exchange + grid barrier counter
-    int32_t * d_codes = nullptr;
+    bark::CodecScratch codec_scratch;
 
     Generation gen;                                  // the bark.h calls' generation state
     BatchSlots batch;
@@ -98,7 +95,7 @@ struct bark_context {
     bark_context_params params;
     bark_statistics stats{};
 
-    std::vector<void *> device_allocs;               // everything cudaMalloc'ed for this context
+    bark::DeviceArena arena;                         // everything else cudaMalloc'ed for this context
 };
 
 namespace bark {
@@ -123,11 +120,17 @@ bool fine_eval_shard(bark_context * ctx, const int32_t * in_buffer, int nn);    
 bool sample_shard(bark_context * ctx, std::mt19937 & rng, int n, float temp, int32_t * out_all /*[1024]*/);
 bool fine_eval_fast(bark_context * ctx, const int32_t * in_buffer, int nn, float * logits_host);      // tensor-core variant (fast mode)
 bool gpt_decode_chained(bark_context * ctx, GPTModel & m, const int32_t * d_token, int * n_past, int lm_lo, int lm_hi);
-// EnCodec decode; codes [8][T] on the host; result in `audio`
-bool codec_decode(bark_context * ctx, const int32_t * codes, int T, std::vector<float> & audio);
-// EnCodec encode (encodec_compress_audio at 6 kbps): n mono 24 kHz samples -> codes [8][T] and the latent [128][T], T = ceil(n / 320);
-// false (message on stderr) without encoder tensors, for n < 1921 or a non-finite sample.  Leaves the generation state alone.
-bool codec_encode(bark_context * ctx, const float * audio, int n, std::vector<int32_t> & codes, std::vector<float> & latent);
+// The EnCodec pipelines, shared by bark_context (8 codebooks) and encodec_context (encodec_api.cu).
+// Reads the codec section at f's position into c: every tensor, codebooks 0..max_q-1 (at least 8 must exist); buffers from arena.
+bool load_codec(std::ifstream & f, CodecModel & c, int max_q, DeviceArena & arena, cudaStream_t s, bool verbose);
+// Decode n_q x T codes to 320 T samples in `audio`.  codes: [n_q][T] on the host, checked against the codebooks; null: the codes already
+// in sc.codes (codec_encode's).
+bool codec_decode(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, const int32_t * codes, int n_q, int T, std::vector<float> & audio);
+// Encode (encodec_compress_audio): n mono 24 kHz samples -> codes [n_q][T] in sc.codes, T = ceil(n / 320), copied to `codes` and the
+// latent [128][T] to `latent` where they are set (then synchronised).  false (message on stderr) without encoder tensors, for
+// n < 1921, a non-finite sample or n_q outside the loaded codebooks.
+bool codec_encode(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, const float * audio, int n, int n_q, std::vector<int32_t> * codes,
+                  std::vector<float> * latent);
 
 // sampling.cu
 constexpr int kSampleMaxLogits = 16384;          // logits of one row: sample_rows_kernel holds the row in 64 KB of shared memory
@@ -145,5 +148,8 @@ int sample_and_replay(bark_context * ctx, const float * d_logits, int ld, int lo
 bool sample_device(bark_context * ctx, GPTModel & m, std::mt19937 & rng, const float * d_logits, int ld, int n, int rows, float temp, int32_t * out_tok, float * out_eos);
 
 int64_t now_us();
+// bark_api.cu: the device of the calling thread's next context (bark_b200_set_device, else BARK_B200_DEVICE, else 0), made current;
+// -1 with a message from `caller` when it is missing or not an sm_90 device
+int select_device(const char * caller, cudaDeviceProp * prop);
 
 }  // namespace bark

@@ -47,6 +47,8 @@ struct GPTModel {
 
 struct ConvW { __half * w = nullptr; float * b = nullptr; int k = 0, cin = 0, cout = 0, Kp = 0; };   // w: LI16 rows (conv: [Cout] x Cin*k; transposed conv: [Cout*k] x Cin)
 
+constexpr int kMaxCodebooks = 32;          // codebooks of the 24 kHz EnCodec (24 kbps)
+
 struct CodecModel {
     int hidden_dim = 128, n_filters = 32, kernel_size = 7, res_kernel = 3, n_bins = 1024;
     ConvW init, final_conv;
@@ -54,8 +56,10 @@ struct CodecModel {
     int lstm_Kp = 0;
     float  * lstm_ih_b[2] = {nullptr, nullptr}, * lstm_hh_b[2] = {nullptr, nullptr};
     struct Block { ConvW us, c1, c2, sc; } blk[4];   // us: transposed conv
-    float * embed[8] = {nullptr};           // codebooks 0..7, [n_bins][hidden] f32
-    float * embed_norm[8] = {nullptr};      // their rows' sums of squares [n_bins] (RVQ encode)
+    int bandwidth = 24, sample_rate = 24000;           // the file's hyper-parameters (kbps, Hz)
+    int n_q = 0;                            // codebooks loaded: 0..n_q-1
+    float * embed[kMaxCodebooks] = {nullptr};        // codebooks, [n_bins][hidden] f32
+    float * embed_norm[kMaxCodebooks] = {nullptr};   // their rows' sums of squares [n_bins] (RVQ encode)
     struct Encoder {                        // encoder.* tensors (encodec.cpp/encoder.h:8-37); a file may lack them all
         bool present = false;
         ConvW init, final_conv;
@@ -64,6 +68,22 @@ struct CodecModel {
         int lstm_Kp = 0;
         float  * lstm_ih_b[2] = {nullptr, nullptr}, * lstm_hh_b[2] = {nullptr, nullptr};
     } enc;
+};
+
+// Device buffers owned by one context, freed together by release()
+struct DeviceArena {
+    std::vector<void *> allocs;
+    void * alloc(size_t bytes);             // cudaMalloc'ed and recorded (loader.cu)
+    void release();
+};
+
+// EnCodec scratch for a T-frame clip, grown on demand by codec_scratch (gpt_forward.cu), freed by release()
+struct CodecScratch {
+    float * buf[3] = {nullptr, nullptr, nullptr}; size_t cap = 0;   // ping-pong activations (floats)
+    float * gi = nullptr;                                            // LSTM input projections
+    float * hbuf = nullptr; unsigned * counter = nullptr;            // LSTM hidden-state exchange + grid barrier counter
+    int32_t * codes = nullptr; size_t codes_cap = 0;                 // [n_q][T]
+    void release();
 };
 
 // Scratch activations for one GPT evaluation of up to `max_rows` positions.

@@ -14,7 +14,7 @@
  *
  * plus device selection for one-context-per-GPU batching (SURVEY.md §8e): bark_context_params must keep the
  * reference layout, so the device is chosen by bark_b200_set_device() or the BARK_B200_DEVICE environment
- * variable before bark_load_model.
+ * variable before bark_load_model (and before encodec_load_model, include/encodec.h).
  */
 #pragma once
 #include "bark.h"
@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-BARK_API void bark_b200_set_device(int cuda_device);                       /* applies to subsequent bark_load_model calls */
+BARK_API void bark_b200_set_device(int cuda_device);                       /* applies to subsequent bark_load_model / encodec_load_model calls */
 BARK_API const char * bark_b200_version(void);
 
 /* which: 0 semantic, 1 coarse.  Host pointers.  *n_past advances exactly like the reference (by 257 for the merged prompt). */
@@ -41,7 +41,7 @@ BARK_API int  bark_b200_encodec_decode(struct bark_context * ctx, const int32_t 
 BARK_API int  bark_b200_encodec_encode(struct bark_context * ctx, const float * audio, int n_samples, int32_t * codes, int codes_cap,
                                        float * latent, int latent_cap);
 /* Test hook, no context: the RVQ encode kernel on host buffers.  latent [hidden][T], codebooks [n_q][n_bins][hidden] f32, codes [n_q][T];
- * hidden % 32 == 0 and <= 128, n_bins <= 1024, n_q <= 8.  Returns 1 on success, 0 on invalid arguments or failure. */
+ * hidden % 32 == 0 and <= 128, n_bins <= 1024, n_q <= 32.  Returns 1 on success, 0 on invalid arguments or failure. */
 BARK_API int  bark_b200_rvq_encode(const float * latent, int T, const float * codebooks, int hidden, int n_bins, int n_q, int32_t * codes);
 BARK_API int  bark_b200_sample(struct bark_context * ctx, int which, const float * logits, int n, float temp, float * eos_p);
 BARK_API int  bark_b200_sample_rows(struct bark_context * ctx, const float * logits /*[rows][n], host*/, int n, int rows, float temp, int32_t * tokens_out,
