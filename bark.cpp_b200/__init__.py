@@ -77,6 +77,19 @@ def load_history_prompt(src) -> dict:
     return out
 
 
+class SamplingStruct(C.Structure):
+    """struct bark_b200_sampling (include/bark_b200.h)"""
+    _fields_ = [("top_k", C.c_int32), ("use_top_p", C.c_int32), ("top_p", C.c_float)]
+
+
+SAMPLING_STAGES = {"semantic": 0, "coarse": 1}
+
+
+def _sampling_struct(top_k=None, top_p=None):
+    """struct bark_b200_sampling for top_k (None or 0: off) and top_p (None: off)."""
+    return SamplingStruct(int(top_k or 0), int(top_p is not None), float(top_p) if top_p is not None else 1.0)
+
+
 def _history_struct(p):
     """(struct bark_b200_history_prompt, the arrays it points into) for a prompt as load_history_prompt accepts it."""
     p = load_history_prompt(p)
@@ -97,7 +110,7 @@ EXPORTS = [
     "bark_b200_shard_init", "bark_b200_shard_connect", "bark_b200_shard_nvlink_bytes",
     "bark_b200_fast_mode", "bark_b200_fast_gemm", "bark_b200_fast_attention", "bark_b200_parity_attention", "bark_b200_parity_gemm",
     "bark_b200_parity_rows", "bark_b200_sample_given_u", "bark_b200_generate_batch", "bark_b200_batch_audio", "bark_b200_batch_tokens", "bark_b200_gpt_eval_slot", "bark_b200_gpt_step_batch",
-    "bark_b200_set_history_prompt", "bark_b200_generate_batch_prompted",
+    "bark_b200_set_history_prompt", "bark_b200_generate_batch_prompted", "bark_b200_set_sampling", "bark_b200_sample_filtered_given_u",
     "ggml_time_init", "ggml_time_us", "ggml_time_ms", "ggml_init", "ggml_free",
 ]
 
@@ -202,6 +215,10 @@ def lib() -> C.CDLL:
     L.bark_b200_gpt_eval_slot.argtypes = [vp, C.c_int, C.c_int, i32p, C.c_int, C.POINTER(C.c_int), C.c_int, f32p]
     L.bark_b200_gpt_step_batch.restype = C.c_int
     L.bark_b200_gpt_step_batch.argtypes = [vp, C.c_int, C.c_int, i32p, i32p, i32p, f32p]
+    L.bark_b200_set_sampling.restype = C.c_int
+    L.bark_b200_set_sampling.argtypes = [vp, C.c_int, C.POINTER(SamplingStruct)]
+    L.bark_b200_sample_filtered_given_u.restype = C.c_int
+    L.bark_b200_sample_filtered_given_u.argtypes = [f32p, C.c_int, C.c_int, C.c_float, C.POINTER(SamplingStruct), vp, C.c_int, i32p, i32p, i32p, f32p, i32p]
     L.bark_b200_set_history_prompt.restype = C.c_int
     L.bark_b200_set_history_prompt.argtypes = [vp, C.POINTER(HistoryPromptStruct)]
     L.bark_b200_generate_batch_prompted.restype = C.c_bool
@@ -293,6 +310,16 @@ class Bark:
         st, _keep = _history_struct(prompt)
         if not lib().bark_b200_set_history_prompt(self.ctx, C.byref(st)):
             raise ValueError("bark_b200_set_history_prompt rejected the prompt (see stderr)")
+
+    def set_sampling(self, stage: str, top_k=None, top_p=None):
+        """Top-k / top-p filter of the "semantic" or "coarse" stage for the later generations and batches on this context
+        (bark_b200_set_sampling, DESIGN.md §14).  top_k: None or 0 for off, else k >= 1; top_p: None for off, else in [0, 1].  Both None
+        turn the stage's filter off.  Raises ValueError for settings the library rejects; the previous ones then stay."""
+        if stage not in SAMPLING_STAGES:
+            raise ValueError(f"stage {stage!r}: 'semantic' or 'coarse' (the fine stage has no filter)")
+        st = _sampling_struct(top_k, top_p)
+        if not lib().bark_b200_set_sampling(self.ctx, SAMPLING_STAGES[stage], C.byref(st)):
+            raise ValueError(f"bark_b200_set_sampling rejected top_k={top_k!r}, top_p={top_p!r} (see stderr)")
 
     def last_generation_prompt(self) -> dict:
         """The last generation's ids as a history prompt: semantic_prompt [n], coarse_prompt [2][T], fine_prompt [8][T].  np.savez of it
@@ -617,6 +644,29 @@ def sample_given_u(logits: np.ndarray, temp: float, u=None, threads: int = 0):
                                        _p(out["eos_p"]))
     if r < 0:
         raise RuntimeError(f"bark_b200_sample_given_u ({rows} x {n}, temp {temp}, threads {threads}) failed")
+    out["replays"] = r
+    return out
+
+
+def sample_filtered_given_u(logits: np.ndarray, temp: float, u=None, top_k=None, top_p=None, threads: int = 0):
+    """sample_given_u with the top-k / top-p filter first (bark_b200_sample_filtered_given_u): filter_rows_kernel, then the sampler on
+    its output, then the host replay of every flagged row from the raw logits.  Returns sample_given_u's dict plus kept [rows], the
+    number of logits the device filter kept; flags has bit 0 for the sampler and bit 1 for the filter."""
+    l = np.ascontiguousarray(logits, np.float32)
+    if l.ndim == 1:
+        l = l[None]
+    rows, n = l.shape
+    up = None
+    if u is not None:
+        u = np.ascontiguousarray(np.broadcast_to(np.asarray(u, np.float64), (rows,)))
+        up = _p(u)
+    out = {k: np.zeros(rows, np.int32) for k in ("tokens", "device_tokens", "flags", "kept")}
+    out["eos_p"] = np.zeros(rows, np.float32)
+    st = _sampling_struct(top_k, top_p)
+    r = lib().bark_b200_sample_filtered_given_u(_p(l), n, rows, temp, C.byref(st), up, threads, _p(out["tokens"]), _p(out["device_tokens"]),
+                                                _p(out["flags"]), _p(out["eos_p"]), _p(out["kept"]))
+    if r < 0:
+        raise RuntimeError(f"bark_b200_sample_filtered_given_u ({rows} x {n}, temp {temp}, top_k {top_k}, top_p {top_p}, threads {threads}) failed")
     out["replays"] = r
     return out
 

@@ -139,7 +139,7 @@ void print_stage_stats(const GPTModel & m) {                                    
 // the limits of the sampler (kSampleMaxLogits) and of the uniform / token buffers (1024 steps) are checked here.
 template <typename LoOf>
 bool run_chain(bark_context * ctx, std::mt19937 & rng, GPTModel & m, const std::vector<int32_t> & first_in, bool merge_ctx, int * n_past, int n, LoOf lo_of, int samp_n, float temp,
-               int32_t * out_tok, float * out_eos) {
+               const bark_b200_sampling & filt, int32_t * out_tok, float * out_eos) {
     if (n < 1 || n > 1024) { fprintf(stderr, "%s: %d steps in one chain (1 to 1024)\n", __func__, n); return false; }
     if (samp_n > kSampleMaxLogits) { fprintf(stderr, "%s: %d logits per sample exceed the device sampler's row of %d\n", __func__, samp_n, kSampleMaxLogits); return false; }
     const int64_t t_begin = now_us();
@@ -148,7 +148,7 @@ bool run_chain(bark_context * ctx, std::mt19937 & rng, GPTModel & m, const std::
         for (int j = 0; j < n; j++) ctx->h_u[j] = std::generate_canonical<double, 53>(rng);     // one draw per sample, as the discrete distribution's operator() makes
         BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->d_u, ctx->h_u, (size_t) n * sizeof(double), cudaMemcpyHostToDevice, s)); bark::g_h2d_bytes += (size_t) n * sizeof(double);
     }
-    const bool chain = ctx->use_decode_kernel && m.decode_ok;
+    const bool chain = ctx->use_decode_kernel && m.decode_ok, filtered = filter_on(filt);
     std::vector<int> past_before((size_t) n);
     std::vector<int32_t> cur_in = first_in;
     std::vector<float> host_logits;
@@ -161,15 +161,21 @@ bool run_chain(bark_context * ctx, std::mt19937 & rng, GPTModel & m, const std::
             if (j == start) { if (!gpt_eval(ctx, m, cur_in.data(), (int) cur_in.size(), n_past, merge_ctx && *n_past == 0, nullptr, lo, lo + samp_n)) return false; }
             const int force = ctx->debug_flag_every > 0 && (ctx->n_sample_calls++ % ctx->debug_flag_every) == 0;
             if (j > start && !gpt_decode_chained(ctx, m, ctx->d_feed, n_past, lo, lo + samp_n)) return false;
-            sample_rows(ctx->last_logits + lo, m.n_out_vocab, samp_n, 1, temp, ctx->d_u + j, ctx->d_stok + j, lo, ctx->d_feed, ctx->d_seos + j, ctx->d_sflags + j, force, 0, s);
+            if (filtered) {                              // the filter's row, then the sampler on it: still no host round trip
+                filter_rows(ctx->last_logits + lo, m.n_out_vocab, samp_n, 1, filt, ctx->d_frow, nullptr, ctx->d_fflags + j, 0, s);
+                sample_rows(ctx->d_frow, samp_n, samp_n, 1, temp, ctx->d_u + j, ctx->d_stok + j, lo, ctx->d_feed, ctx->d_seos + j, ctx->d_sflags + j, force, 0, s);
+            } else {
+                sample_rows(ctx->last_logits + lo, m.n_out_vocab, samp_n, 1, temp, ctx->d_u + j, ctx->d_stok + j, lo, ctx->d_feed, ctx->d_seos + j, ctx->d_sflags + j, force, 0, s);
+            }
         }
         const size_t cnt = (size_t)(stop - start);
         BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->h_stok + start, ctx->d_stok + start, cnt * 4, cudaMemcpyDeviceToHost, s));
         BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->h_sflags + start, ctx->d_sflags + start, cnt * 4, cudaMemcpyDeviceToHost, s));
         BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->h_seos + start, ctx->d_seos + start, cnt * 4, cudaMemcpyDeviceToHost, s)); bark::g_d2h_bytes += cnt * 12;
+        if (filtered) { BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->h_fflags + start, ctx->d_fflags + start, cnt * 4, cudaMemcpyDeviceToHost, s)); bark::g_d2h_bytes += cnt * 4; }
         BARK_CUDA_CHECK(cudaStreamSynchronize(s));
         int f = start;
-        while (f < stop && !ctx->h_sflags[f]) f++;
+        while (f < stop && !ctx->h_sflags[f] && !(filtered && ctx->h_fflags[f])) f++;
         if (f == stop) { start = stop; if (start < n) cur_in.assign(1, ctx->h_stok[start - 1]); continue; }
         // step f must be decided on the host: re-evaluate it with its logits read back (steps before f stand)
         if (f > start) cur_in.assign(1, ctx->h_stok[f - 1]);
@@ -177,6 +183,7 @@ bool run_chain(bark_context * ctx, std::mt19937 & rng, GPTModel & m, const std::
         const int lo = lo_of(f);
         host_logits.resize((size_t) m.n_out_vocab);
         if (!gpt_eval(ctx, m, cur_in.data(), (int) cur_in.size(), n_past, merge_ctx && *n_past == 0, host_logits.data(), lo, lo + samp_n)) return false;
+        if (filtered) filter_row_host(host_logits.data() + lo, samp_n, filt);
         ctx->h_stok[f] = lo + sample_token_given_u(host_logits.data() + lo, samp_n, temp, ctx->h_u[f], &ctx->h_seos[f]);
         ctx->n_sample_host_replays++;
         start = f + 1;
@@ -203,7 +210,7 @@ bool run_semantic(bark_context * ctx, Generation & g) {
         const int nb = std::min(kBatch, P.n_steps_text_encoder - i);
         const std::mt19937 saved = g.rng;
         // the reference samples over ALL n_out_vocab logits, not the 10001 "relevant" ones (quirk D.1)
-        if (!run_chain(ctx, g.rng, m, input, true, &n_past, nb, [](int) { return 0; }, m.n_out_vocab, P.temp, tok.data(), eos.data())) { fprintf(stderr, "%s: Could not generate token\n", __func__); return false; }
+        if (!run_chain(ctx, g.rng, m, input, true, &n_past, nb, [](int) { return 0; }, m.n_out_vocab, P.temp, ctx->sampling[0], tok.data(), eos.data())) { fprintf(stderr, "%s: Could not generate token\n", __func__); return false; }
         for (int j = 0; j < nb; j++) {
             if (P.progress_callback) P.progress_callback(ctx, SEMANTIC, 100 * (i + j + 1) / P.n_steps_text_encoder, P.progress_callback_user_data);
             if (tok[(size_t) j] == P.semantic_vocab_size || eos[(size_t) j] >= P.min_eos_p) {               // bark.cpp:1675-1677
@@ -325,7 +332,7 @@ bool run_coarse(bark_context * ctx, Generation & g) {
         const int nw = std::min(P.sliding_window_size, n_steps - step), step0 = step;
         std::vector<int32_t> tok((size_t) nw);
         auto lo_of = [&](int j) { return P.semantic_vocab_size + (((step0 + j) % P.n_coarse_codebooks == 0) ? 0 : 1) * P.codebook_size; };
-        if (!run_chain(ctx, g.rng, m, in_eval, false, &n_past, nw, lo_of, P.codebook_size, P.temp, tok.data(), nullptr)) { fprintf(stderr, "%s: Could not generate token\n", __func__); return false; }
+        if (!run_chain(ctx, g.rng, m, in_eval, false, &n_past, nw, lo_of, P.codebook_size, P.temp, ctx->sampling[1], tok.data(), nullptr)) { fprintf(stderr, "%s: Could not generate token\n", __func__); return false; }
         for (int j = 0; j < nw; j++) {
             if (P.progress_callback) P.progress_callback(ctx, COARSE, 100 * (step + 1) / n_steps, P.progress_callback_user_data);
             out.push_back(tok[(size_t) j]); step++;
@@ -455,12 +462,13 @@ bool batch_prefill(bark_context * ctx, GPTModel & m, int which, BatchItem & it, 
 // Samples row r of the batch logits (window [lo, lo + n)) for item act[r], with one uniform from that item's RNG, as run_chain draws
 // it.  The one host synchronisation of the step; rows the device kernel flags are replayed on the host from the same logits and
 // uniform.  tok[r] = lo + the sampled index, eos[r] = probability of the window's last logit.
-bool batch_sample(bark_context * ctx, GPTModel & m, std::vector<BatchItem> & items, const std::vector<int> & act, int lo, int n, float temp, int32_t * tok, float * eos) {
+bool batch_sample(bark_context * ctx, GPTModel & m, std::vector<BatchItem> & items, const std::vector<int> & act, int lo, int n, float temp,
+                  const bark_b200_sampling & filt, int32_t * tok, float * eos) {
     const int64_t t0 = now_us();
     const int B = (int) act.size();
     if (n > kSampleMaxLogits) { fprintf(stderr, "%s: %d logits per row exceed the device sampler's row of %d\n", __func__, n, kSampleMaxLogits); return false; }
     if (temp != 0.0f) for (int r = 0; r < B; r++) ctx->h_u[r] = std::generate_canonical<double, 53>(items[(size_t) act[(size_t) r]].g.rng);
-    sample_and_replay(ctx, ctx->batch.d_logits, m.n_out_vocab, lo, n, B, temp, true);
+    sample_and_replay(ctx, ctx->batch.d_logits, m.n_out_vocab, lo, n, B, temp, true, &filt);
     for (int r = 0; r < B; r++) { tok[r] = ctx->h_stok[r]; eos[r] = ctx->h_seos[r]; }
     m.n_sample += B;
     m.t_sample_us += now_us() - t0;
@@ -488,7 +496,7 @@ bool batch_semantic(bark_context * ctx, std::vector<BatchItem> & items) {
     }
     int32_t tok[kMaxBatch]; float eos[kMaxBatch];
     while (!act.empty()) {
-        if (!batch_sample(ctx, m, items, act, 0, m.n_out_vocab, P.temp, tok, eos)) return false;     // all n_out logits (quirk D.1)
+        if (!batch_sample(ctx, m, items, act, 0, m.n_out_vocab, P.temp, ctx->sampling[0], tok, eos)) return false;     // all n_out logits (quirk D.1)
         std::vector<int> next; int32_t next_tok[kMaxBatch];
         for (size_t r = 0; r < act.size(); r++) {
             Generation & g = items[(size_t) act[r]].g;
@@ -531,7 +539,7 @@ bool batch_coarse(bark_context * ctx, std::vector<BatchItem> & items) {
         }
         for (int j = 0; !act.empty(); j++) {
             const int lo = lo_of(step0 + j);
-            if (!batch_sample(ctx, m, items, act, lo, P.codebook_size, P.temp, tok, eos)) return false;
+            if (!batch_sample(ctx, m, items, act, lo, P.codebook_size, P.temp, ctx->sampling[1], tok, eos)) return false;
             std::vector<int> next; int32_t next_tok[kMaxBatch];
             for (size_t r = 0; r < act.size(); r++) {
                 BatchItem & it = items[(size_t) act[r]];
@@ -678,6 +686,8 @@ void alloc_workspace(bark_context * ctx) {
     ctx->d_u = (double *) ctx_alloc(ctx, 1024 * 8); ctx->d_stok = (int32_t *) ctx_alloc(ctx, 1024 * 4);
     ctx->d_sflags = (int32_t *) ctx_alloc(ctx, 1024 * 4); ctx->d_seos = (float *) ctx_alloc(ctx, 1024 * 4);
     ctx->d_feed = (int32_t *) ctx_alloc(ctx, 64); BARK_CUDA_CHECK(cudaMemset(ctx->d_feed, 0, 64));
+    ctx->d_frow = (float *) ctx_alloc(ctx, (size_t) kMaxFilterRows * kSampleMaxLogits * 4); ctx->d_fflags = (int32_t *) ctx_alloc(ctx, 1024 * 4);
+    BARK_CUDA_CHECK(cudaMallocHost(&ctx->h_fflags, 1024 * 4));
     BARK_CUDA_CHECK(cudaMemset(ctx->d_u, 0, 1024 * 8));
     BARK_CUDA_CHECK(cudaMallocHost(&ctx->h_u, 1024 * 8)); BARK_CUDA_CHECK(cudaMallocHost(&ctx->h_stok, 1024 * 4));
     BARK_CUDA_CHECK(cudaMallocHost(&ctx->h_sflags, 1024 * 4)); BARK_CUDA_CHECK(cudaMallocHost(&ctx->h_seos, 1024 * 4));
@@ -836,6 +846,7 @@ extern "C" void bark_free(struct bark_context * ctx) {
     if (ctx->h_stok) cudaFreeHost(ctx->h_stok);
     if (ctx->h_sflags) cudaFreeHost(ctx->h_sflags);
     if (ctx->h_seos) cudaFreeHost(ctx->h_seos);
+    if (ctx->h_fflags) cudaFreeHost(ctx->h_fflags);
     for (int w = 0; w < 2; w++) for (int b = 0; b < ctx->batch.cap; b++) { cudaFree(ctx->batch.k[w][b]); cudaFree(ctx->batch.v[w][b]); }
     if (ctx->batch.d_logits) cudaFree(ctx->batch.d_logits);
     if (ctx->batch.d_step) cudaFree(ctx->batch.d_step);
@@ -1160,6 +1171,77 @@ static int bark_b200_sample_given_u_impl(const float * logits, int n, int rows, 
 extern "C" int bark_b200_sample_given_u(const float * logits, int n, int rows, float temp, const double * u, int threads, int32_t * tokens,
                                         int32_t * device_tokens, int32_t * flags, float * eos_p) {
     return guarded((int) -1, [&] { return bark_b200_sample_given_u_impl(logits, n, rows, temp, u, threads, tokens, device_tokens, flags, eos_p); });
+}
+
+// top-k / top-p settings: false with a message for anything the rule does not define
+static bool sampling_valid(const char * fn, const bark_b200_sampling & s) {
+    if (s.top_k < 0) { fprintf(stderr, "%s: top_k %d (0 for off, or k >= 1)\n", fn, s.top_k); return false; }
+    if (s.use_top_p && !(std::isfinite(s.top_p) && s.top_p >= 0.0f && s.top_p <= 1.0f)) { fprintf(stderr, "%s: top_p %g is not in [0, 1]\n", fn, (double) s.top_p); return false; }
+    return true;
+}
+
+extern "C" int bark_b200_set_sampling(struct bark_context * ctx, int stage, const struct bark_b200_sampling * s) {
+    const char * fn = "bark_b200_set_sampling";
+    if (!ctx) { fprintf(stderr, "%s: invalid bark context\n", fn); return 0; }
+    if (stage != 0 && stage != 1) { fprintf(stderr, "%s: stage %d (0 semantic, 1 coarse; the fine stage has no filter)\n", fn, stage); return 0; }
+    if (s && !sampling_valid(fn, *s)) return 0;
+    ctx->sampling[stage] = s ? *s : bark_b200_sampling{0, 0, 1.0f};
+    return 1;
+}
+
+// the device filter and sampler on host rows (tests): filter_rows_kernel, then sample_rows_kernel on its output, then every row either
+// kernel flags replayed on the host from the raw logits (filter_row_host, sample_token_given_u), as sample_and_replay does it
+static int bark_b200_sample_filtered_given_u_impl(const float * logits, int n, int rows, float temp, const bark_b200_sampling * s, const double * u, int threads,
+                                                  int32_t * tokens, int32_t * device_tokens, int32_t * flags, float * eos_p, int32_t * kept) {
+    if (!logits || !tokens || !device_tokens || !flags || !eos_p || (temp != 0.0f && !u)) return -1;
+    if (n < 2 || n > kSampleMaxLogits || rows < 1 || rows > 1024 || !std::isfinite(temp) || temp < 0.0f) return -1;
+    if (threads != 0 && threads != 256 && threads != 1024) return -1;
+    if (temp != 0.0f) for (int r = 0; r < rows; r++) if (!(u[r] >= 0.0 && u[r] < 1.0)) return -1;
+    const bark_b200_sampling f = s ? *s : bark_b200_sampling{0, 0, 1.0f};
+    if (!sampling_valid("bark_b200_sample_filtered_given_u", f)) return -1;
+    struct Buffers {                                          // freed on every exit, including a CUDA failure thrown mid-way
+        void * p[8] = {};
+        ~Buffers() { for (void * q : p) cudaFree(q); }
+    } d;
+    const size_t bytes = (size_t) rows * n * 4;
+    for (int i = 0; i < 2; i++) BARK_CUDA_CHECK(cudaMalloc(&d.p[i], bytes));
+    BARK_CUDA_CHECK(cudaMalloc(&d.p[2], (size_t) rows * sizeof(double)));
+    for (int i = 3; i < 8; i++) BARK_CUDA_CHECK(cudaMalloc(&d.p[i], (size_t) rows * 4));
+    float * dl = (float *) d.p[0], * dfilt = (float *) d.p[1], * deos = (float *) d.p[7]; double * du = (double *) d.p[2];
+    int32_t * dtok = (int32_t *) d.p[3], * dsflags = (int32_t *) d.p[4], * dfflags = (int32_t *) d.p[5], * dkept = (int32_t *) d.p[6];
+    BARK_CUDA_CHECK(cudaMemcpy(dl, logits, bytes, cudaMemcpyHostToDevice));
+    if (temp != 0.0f) BARK_CUDA_CHECK(cudaMemcpy(du, u, (size_t) rows * sizeof(double), cudaMemcpyHostToDevice));
+    for (int i = 3; i < 8; i++) BARK_CUDA_CHECK(cudaMemset(d.p[i], 0xff, (size_t) rows * 4));      // -1 / NaN: a missing store shows up
+    BARK_CUDA_CHECK(cudaMemset(dfflags, 0, (size_t) rows * 4));
+    const bool filtered = filter_on(f);
+    if (filtered) filter_rows(dl, n, n, rows, f, dfilt, dkept, dfflags, threads, 0);
+    sample_rows(filtered ? dfilt : dl, n, n, rows, temp, du, dtok, 0, nullptr, deos, dsflags, 0, threads, 0);
+    BARK_CUDA_CHECK(cudaGetLastError());                      // a launch the configuration rejects
+    const cudaError_t e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) { fprintf(stderr, "bark_b200_sample_filtered_given_u: %s\n", cudaGetErrorString(e)); return -1; }
+    std::vector<int32_t> sf((size_t) rows), ff((size_t) rows), kp((size_t) rows, n);
+    BARK_CUDA_CHECK(cudaMemcpy(device_tokens, dtok, (size_t) rows * 4, cudaMemcpyDeviceToHost));
+    BARK_CUDA_CHECK(cudaMemcpy(sf.data(), dsflags, (size_t) rows * 4, cudaMemcpyDeviceToHost));
+    BARK_CUDA_CHECK(cudaMemcpy(ff.data(), dfflags, (size_t) rows * 4, cudaMemcpyDeviceToHost));
+    BARK_CUDA_CHECK(cudaMemcpy(eos_p, deos, (size_t) rows * 4, cudaMemcpyDeviceToHost));
+    if (filtered) BARK_CUDA_CHECK(cudaMemcpy(kp.data(), dkept, (size_t) rows * 4, cudaMemcpyDeviceToHost));
+    int replays = 0;
+    std::vector<float> row;
+    for (int r = 0; r < rows; r++) {
+        tokens[r] = device_tokens[r];
+        flags[r] = (sf[(size_t) r] ? 1 : 0) | (ff[(size_t) r] ? 2 : 0);
+        if (kept) kept[r] = kp[(size_t) r];
+        if (!flags[r]) continue;
+        row.assign(logits + (size_t) r * n, logits + (size_t) (r + 1) * n);
+        if (filtered) filter_row_host(row.data(), n, f);
+        tokens[r] = sample_token_given_u(row.data(), n, temp, temp != 0.0f ? u[r] : 0.0, &eos_p[r]);
+        replays++;
+    }
+    return replays;
+}
+extern "C" int bark_b200_sample_filtered_given_u(const float * logits, int n, int rows, float temp, const struct bark_b200_sampling * s, const double * u,
+                                                 int threads, int32_t * tokens, int32_t * device_tokens, int32_t * flags, float * eos_p, int32_t * kept) {
+    return guarded((int) -1, [&] { return bark_b200_sample_filtered_given_u_impl(logits, n, rows, temp, s, u, threads, tokens, device_tokens, flags, eos_p, kept); });
 }
 
 // parity-path tiled GEMM on host buffers (tests, tools/gemm_bench.py): A [M][K] and W [N][K] go through permute_to_gm, as the loader

@@ -1,7 +1,7 @@
 // bark_context: everything one generation needs, owned by bark_load_model / bark_free.
 // Host control plane in C++ (like the reference's bark.cpp:133-164), all tensors in HBM.
 #pragma once
-#include "../../include/bark.h"
+#include "../../include/bark_b200.h"
 #include "model.h"
 
 #include <fstream>
@@ -82,6 +82,10 @@ struct bark_context {
     int32_t * d_stok = nullptr, * h_stok = nullptr, * d_sflags = nullptr, * h_sflags = nullptr;
     float * d_seos = nullptr, * h_seos = nullptr;
     int32_t * d_feed = nullptr;                      // token handed from sample_rows_kernel to the next decode step
+    // top-k / top-p of the semantic [0] and coarse [1] stages (bark_b200_set_sampling), shared by every batch item; both off by default
+    bark_b200_sampling sampling[2] = {{0, 0, 1.0f}, {0, 0, 1.0f}};
+    float * d_frow = nullptr;                        // filter_rows_kernel's output: kMaxFilterRows filtered rows of kSampleMaxLogits
+    int32_t * d_fflags = nullptr, * h_fflags = nullptr;   // its flags, per sample (1024)
     long long n_sample_host_replays = 0;
     int debug_flag_every = 0; long long n_sample_calls = 0;   // BARK_B200_SAMPLE_FLAG_EVERY=k: force every k-th sample through the host replay (tests)
     float * h_logits = nullptr;                      // pinned, max(n_out) or 1024*fine_vocab
@@ -139,11 +143,22 @@ void sample_rows(const float * logits, int ld, int n, int rows, float temp, cons
                  float * d_eos_p, int32_t * d_flags, int force_flag, int threads, cudaStream_t s);
 // gpt_sample of one row on the host with the uniform u already drawn (unused when temp == 0)
 int32_t sample_token_given_u(const float * logits, int n, float temp, double u, float * eos_p);
-// Samples `rows` (<= 1024) rows of device logits, row r at d_logits + r * ld + lo, n <= kSampleMaxLogits wide, with the uniforms the
-// caller put in ctx->h_u[0, rows) (temp != 0).  One synchronisation reads the tokens (lo added), the flags and, with want_eos, the
-// probabilities of the last logit back to ctx->h_stok / h_sflags / h_seos; every flagged row is then replayed on the host with
-// sample_token_given_u and the same uniform.  Returns the number of rows replayed.
-int sample_and_replay(bark_context * ctx, const float * d_logits, int ld, int lo, int n, int rows, float temp, bool want_eos);
+// top-k / top-p (DESIGN.md §14): on when top_k >= 1 or use_top_p
+inline bool filter_on(const bark_b200_sampling & f) { return f.top_k > 0 || f.use_top_p != 0; }
+constexpr int kMaxFilterRows = 8;                // rows filtered at once: one decode step of a batch
+// filter_rows_kernel over `rows` rows of n <= kSampleMaxLogits raw logits (stride ld): d_out [rows][n] gets each row with the removed
+// logits set to -inf, d_kept (may be null) the number kept, d_flags 1 where the device cannot decide the row exactly (a NaN, a
+// non-finite maximum, an exp within rounding of a float boundary).  threads as sample_rows.
+void filter_rows(const float * logits, int ld, int n, int rows, const bark_b200_sampling & f, float * d_out, int32_t * d_kept, int32_t * d_flags, int threads,
+                 cudaStream_t s);
+// the same filter on the host with libm's exp, in place; returns the number of logits kept
+int filter_row_host(float * row, int n, const bark_b200_sampling & f);
+// Samples `rows` (<= 1024; <= kMaxFilterRows with a filter) rows of device logits, row r at d_logits + r * ld + lo, n <= kSampleMaxLogits
+// wide, with the uniforms the caller put in ctx->h_u[0, rows) (temp != 0).  With f set and on, filter_rows runs first and the sampler
+// reads its output.  One synchronisation reads the tokens (lo added), the flags and, with want_eos, the probabilities of the last logit
+// back to ctx->h_stok / h_sflags / h_seos; every row flagged by either kernel is then replayed on the host (filter_row_host from the raw
+// logits, then sample_token_given_u with the same uniform).  Returns the number of rows replayed.
+int sample_and_replay(bark_context * ctx, const float * d_logits, int ld, int lo, int n, int rows, float temp, bool want_eos, const bark_b200_sampling * f = nullptr);
 // sample_and_replay with `rows` uniforms drawn from rng; tokens to out_tok, eos probabilities to out_eos when it is set
 bool sample_device(bark_context * ctx, GPTModel & m, std::mt19937 & rng, const float * d_logits, int ld, int n, int rows, float temp, int32_t * out_tok, float * out_eos);
 

@@ -130,6 +130,29 @@ BARK_API int  bark_b200_set_history_prompt(struct bark_context * ctx, const stru
 BARK_API bool bark_b200_generate_batch_prompted(struct bark_context * ctx, const char * const * texts, const uint32_t * seeds,
                                                 const struct bark_b200_history_prompt * const * prompts, int n, int n_threads);
 
+/* TOP-K / TOP-P SAMPLING of the semantic and coarse stages, upstream Bark's generate_text_semantic / generate_coarse filter on the
+ * reference's arithmetic (DESIGN.md §14).  The row the stage samples (semantic: all n_out_vocab logits; coarse: the 1024-wide codebook
+ * window) is ordered by logit descending, equal logits (+0 and -0 included) by descending index.  top-p removes sorted position j >= 1
+ * when the float cumulative sum of the reference's softmax of the sorted row up to position j - 1 exceeds top_p; top-k then removes
+ * every logit below the k-th largest that remains (ties of the k-th value stay).  Removed logits become -inf before gpt_sample, which
+ * is otherwise unchanged: the same single uniform draw, the same RNG stream; eos_p is 0 when the last logit was removed.  The fine
+ * stage has no filter.  Both off: every stage is exactly what it is without this call. */
+struct bark_b200_sampling {
+    int32_t top_k;       /* 0: off; k >= 1 */
+    int32_t use_top_p;   /* 0: off */
+    float   top_p;       /* with use_top_p: finite, in [0, 1] (0 keeps only sorted position 0: of tied maxima, the highest index) */
+};
+/* stage 0 semantic, 1 coarse; s NULL turns both filters of the stage off.  Validates and copies; returns 1, or 0 with a message (the
+ * previous settings stay).  Applies to later bark_generate_audio and bark_b200_forward_text_encoder / _coarse_encoder calls, and to
+ * every item of bark_b200_generate_batch[_prompted]. */
+BARK_API int  bark_b200_set_sampling(struct bark_context * ctx, int stage, const struct bark_b200_sampling * s);
+/* Test hook, no context: bark_b200_sample_given_u with the filter s (NULL: off) applied first, on the device by filter_rows_kernel and,
+ * for a flagged row, on the host from the raw logits.  flags: bit 0 the sampler flagged the row, bit 1 the filter did; kept (may be
+ * NULL): the number of logits the device filter kept.  Returns the number of replayed rows, or -1 on invalid arguments or failure. */
+BARK_API int  bark_b200_sample_filtered_given_u(const float * logits, int n, int rows, float temp, const struct bark_b200_sampling * s,
+                                                const double * u, int threads, int32_t * tokens, int32_t * device_tokens, int32_t * flags,
+                                                float * eos_p, int32_t * kept);
+
 /* FAST MODE (BARK_B200_MODE=fast in the environment at load; opt-in, NOT bit-identical to the reference): the fine model's
  * 1024-row passes (bark.cpp:1416-1584) run as wgmma tensor-core GEMMs + flash-style attention (csrc/fast_kernels.cu).
  * The two kernel hooks below run on host buffers without a context, for the numerics tests:
