@@ -111,6 +111,7 @@ EXPORTS = [
     "bark_b200_fast_mode", "bark_b200_fast_gemm", "bark_b200_fast_attention", "bark_b200_parity_attention", "bark_b200_parity_gemm",
     "bark_b200_parity_rows", "bark_b200_sample_given_u", "bark_b200_generate_batch", "bark_b200_batch_audio", "bark_b200_batch_tokens", "bark_b200_gpt_eval_slot", "bark_b200_gpt_step_batch",
     "bark_b200_set_history_prompt", "bark_b200_generate_batch_prompted", "bark_b200_set_sampling", "bark_b200_sample_filtered_given_u",
+    "bark_b200_quant_matmul",
     "ggml_time_init", "ggml_time_us", "ggml_time_ms", "ggml_init", "ggml_free",
 ]
 
@@ -201,6 +202,8 @@ def lib() -> C.CDLL:
     L.bark_b200_parity_attention.argtypes = [vp, vp, vp, vp] + [C.c_int] * 7
     L.bark_b200_parity_gemm.restype = C.c_int
     L.bark_b200_parity_gemm.argtypes = [vp, vp, vp] + [C.c_int] * 6 + [vp]
+    L.bark_b200_quant_matmul.restype = C.c_int
+    L.bark_b200_quant_matmul.argtypes = [C.c_int, vp, vp, vp] + [C.c_int] * 5 + [vp, vp, vp, vp]
     L.bark_b200_parity_rows.restype = C.c_int
     L.bark_b200_parity_rows.argtypes = [C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, vp, vp, C.POINTER(C.c_uint)]
     L.bark_b200_sample_given_u.restype = C.c_int
@@ -597,6 +600,47 @@ def parity_gemm(A: np.ndarray, W: np.ndarray, epilogue: str = "store", variant: 
         flat = out.reshape(-1)
         out = tuple(flat[i * M * (N // 3):(i + 1) * M * (N // 3)].reshape(M, N // 3) for i in range(3))
     return (out, r) if return_variant else out
+
+
+QUANT_TYPES = {"q4_0": 2, "q4_1": 3, "q5_0": 6, "q5_1": 7, "q8_0": 8}     # enum ggml_type
+QUANT_BLOCK_BYTES = {"q4_0": 18, "q4_1": 20, "q5_0": 22, "q5_1": 24, "q8_0": 34}
+QUANT_PATHS = {"auto": 0, "decode_staged": 1, "decode_global": 2}
+
+
+def quant_matmul(qtype: str, W: np.ndarray, A: np.ndarray, epilogue: str = "store", path: str = "auto", resid: np.ndarray | None = None,
+                 gelu_tab: np.ndarray | None = None, return_q8: bool = False):
+    """Bit-exact A W^T on a quantised mat-mul; W [N][K/32 * block bytes] uint8, the weight rows as the model file stores them, A [M][K]
+    float32, K % 32 == 0.  Returns float32 [M][N] for "store", "resid" (resid + A W^T) and "gelu" (GELU through gelu_tab, 65536 uint16
+    f16 bits), the triple Q, K, V of [M][N/3] for "qkv".  path: "auto" (the per-op kernels the library runs for M rows), or for q4_0 with
+    M == 1 the decode step's kernels with the rows staged in shared memory ("decode_staged") or read from global memory ("decode_global").
+    With return_q8 the result is (outputs, q int8 [M][K], d float16 [M][K/32], s float16 [M][K/32] or None): the quantised activation."""
+    A = np.ascontiguousarray(A, np.float32); W = np.ascontiguousarray(W, np.uint8)
+    M, K = A.shape; N = W.shape[0]
+    assert K % 32 == 0 and W.shape[1] == K // 32 * QUANT_BLOCK_BYTES[qtype], (qtype, A.shape, W.shape)
+    if epilogue == "resid":
+        out = np.array(resid, np.float32, order="C", copy=True)
+        assert out.shape == (M, N), out.shape
+    else:
+        out = np.zeros((M, N), np.float32)
+    tab = None
+    if epilogue == "gelu":
+        tab = np.ascontiguousarray(gelu_tab, np.uint16)
+        assert tab.shape == (65536,), tab.shape
+    q = np.zeros((M, K), np.int8); d = np.zeros((M, K // 32), np.float32)
+    s = np.zeros((M, K // 32), np.float32) if qtype in ("q4_1", "q5_1") else None
+    r = lib().bark_b200_quant_matmul(QUANT_TYPES[qtype], _p(W), _p(A), _p(out), M, N, K, PARITY_EPILOGUES[epilogue], QUANT_PATHS[path],
+                                     None if tab is None else _p(tab), _p(q), _p(d), None if s is None else _p(s))
+    what = f"bark_b200_quant_matmul ({qtype}, {epilogue}, {M}x{N}x{K}, {path})"
+    if r == -1:
+        raise GuardBandError(f"{what} wrote outside its output")
+    if r != 1:
+        raise RuntimeError(f"{what} failed")
+    if epilogue == "qkv":
+        flat = out.reshape(-1)
+        out = tuple(flat[i * M * (N // 3):(i + 1) * M * (N // 3)].reshape(M, N // 3) for i in range(3))
+    if not return_q8:
+        return out
+    return out, q, d.astype(np.float16), None if s is None else s.astype(np.float16)
 
 
 ROW_OPS = {"layernorm": 0, "softmax": 1}

@@ -1309,6 +1309,85 @@ extern "C" int bark_b200_parity_gemm(const void * A, const void * W, void * C, i
     return guarded((int) 0, [&] { return bark_b200_parity_gemm_impl(A, W, C, M, N, K, wtype, epilogue, variant, gelu_tab); });
 }
 
+// quantised mat-muls on host buffers (tests): the weight rows arrive as the file's blocks and go through the loader's split (q4_split /
+// qx_split); the activation rows are f32, as store_act leaves them for a quantised model.  The q8 operand lives in this call's own
+// scratch: the calling thread's scratch pointers (a context's buffers) are put back on every exit.  The output sits between guard bands
+// and starts as NaN (RESID: as the residual from C).
+static int bark_b200_quant_matmul_impl(int wtype, const void * W, const float * A, float * C, int M, int N, int K, int epilogue, int path,
+                                       const uint16_t * gelu_tab, int8_t * q_out, float * d_out, float * s_out) {
+    const WType t = (WType) wtype;
+    if (!W || !A || !C || M < 1 || N < 1 || K < 32 || K % 32 || (t != W_Q4_0 && !qx_supported(t)) || path < 0 || path > 2) return 0;
+    if (epilogue < EPI_STORE || epilogue > EPI_QKV || (epilogue == EPI_QKV && N % 3) || (epilogue == EPI_GELU_ACT && !gelu_tab)) return 0;
+    const bool q81 = t == W_Q4_1 || t == W_Q5_1;
+    if ((path != 0 && (t != W_Q4_0 || M != 1 || K > 4096)) || (s_out && !q81)) return 0;
+    constexpr size_t kGuard = 4096;
+    constexpr unsigned char kPattern = 0x5a;
+    const int nb = K / 32;
+    const size_t n_blocks = (size_t) N * nb, raw_bytes = n_blocks * (t == W_Q4_0 ? 18 : qx_block_bytes(t)), out_bytes = (size_t) M * N * 4;
+    struct Scratch {                                          // the calling thread's q8 scratch, restored on every exit
+        void * q4[2], * qx[3];
+        Scratch() { q4_get_scratch(&q4[0], &q4[1]); qx_get_scratch(&qx[0], &qx[1], &qx[2]); }
+        ~Scratch() { q4_set_scratch(q4[0], q4[1]); qx_set_scratch(qx[0], qx[1], qx[2]); }
+    } keep;
+    struct Buffers {                                          // freed on every exit, including a CUDA failure thrown mid-way
+        void * p[11] = {};
+        ~Buffers() { for (void * b : p) cudaFree(b); }
+    } d;
+    void *& d_raw = d.p[0], *& d_qs = d.p[1], *& d_sc = d.p[2], *& d_min = d.p[3], *& d_qh = d.p[4], *& d_a = d.p[5], *& d_q8 = d.p[6], *& d_q8d = d.p[7],
+         *& d_q8s = d.p[8], *& d_c = d.p[9], *& d_tab = d.p[10];
+    BARK_CUDA_CHECK(cudaMalloc(&d_raw, raw_bytes));
+    BARK_CUDA_CHECK(cudaMemcpy(d_raw, W, raw_bytes, cudaMemcpyHostToDevice));
+    BARK_CUDA_CHECK(cudaMalloc(&d_qs, n_blocks * (t == W_Q8_0 ? 32 : 16))); BARK_CUDA_CHECK(cudaMalloc(&d_sc, n_blocks * 2));
+    DMat dm; dm.n_out = N; dm.K = K; dm.Kp = K; dm.type = t; dm.p = d_qs; dm.scales = d_sc;
+    if (t == W_Q4_0) q4_split(d_raw, n_blocks, d_qs, d_sc, 0);
+    else {
+        BARK_CUDA_CHECK(cudaMalloc(&d_min, n_blocks * 2)); BARK_CUDA_CHECK(cudaMalloc(&d_qh, n_blocks * 4));
+        dm.mins = d_min; dm.qh = d_qh;
+        qx_split(d_raw, n_blocks, t, d_qs, d_qh, d_sc, d_min, 0);
+    }
+    BARK_CUDA_CHECK(cudaMalloc(&d_a, (size_t) M * K * 4));
+    BARK_CUDA_CHECK(cudaMemcpy(d_a, A, (size_t) M * K * 4, cudaMemcpyHostToDevice));
+    BARK_CUDA_CHECK(cudaMalloc(&d_q8, (size_t) M * K)); BARK_CUDA_CHECK(cudaMalloc(&d_q8d, (size_t) M * nb * 4));
+    BARK_CUDA_CHECK(cudaMalloc(&d_q8s, (size_t) M * nb * 4));
+    BARK_CUDA_CHECK(cudaMalloc(&d_c, out_bytes + 2 * kGuard));
+    unsigned char * const reg = (unsigned char *) d_c;
+    BARK_CUDA_CHECK(cudaMemset(reg, kPattern, out_bytes + 2 * kGuard));
+    if (epilogue == EPI_RESID) BARK_CUDA_CHECK(cudaMemcpy(reg + kGuard, C, out_bytes, cudaMemcpyHostToDevice));
+    else                       BARK_CUDA_CHECK(cudaMemset(reg + kGuard, 0xff, out_bytes));
+    MatmulEpilogue ep; ep.mode = epilogue;
+    float * const out = (float *)(reg + kGuard);
+    if (epilogue == EPI_STORE || epilogue == EPI_RESID) { ep.out = out; ep.ldo = N; }
+    else if (epilogue == EPI_QKV) { const int E = N / 3; ep.out = out; ep.k_out = out + (size_t) M * E; ep.v_out = out + 2 * (size_t) M * E; ep.ldo = E; }
+    else {                                                    // f32 rows, as a quantised model's fc pass leaves its operand
+        BARK_CUDA_CHECK(cudaMalloc(&d_tab, 65536 * 2));
+        BARK_CUDA_CHECK(cudaMemcpy(d_tab, gelu_tab, 65536 * 2, cudaMemcpyHostToDevice));
+        ep.act_out = out; ep.act_wt = W_Q4_0; ep.act_Kp = N; ep.gelu_tab = (const __half *) d_tab;
+    }
+    if (path == 0) {
+        q4_set_scratch(d_q8, d_q8d); qx_set_scratch(d_q8, d_q8d, d_q8s);
+        lane_matmul(dm, d_a, K, M, ep, 0);
+    } else {
+        decode_q4_rows(path == 1, (const float *) d_a, K, d_qs, d_sc, N, ep, (int8_t *) d_q8, (float *) d_q8d, 0);
+    }
+    BARK_CUDA_CHECK(cudaGetLastError());
+    const cudaError_t e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) { fprintf(stderr, "bark_b200_quant_matmul: %s\n", cudaGetErrorString(e)); return 0; }
+    std::vector<unsigned char> h(out_bytes + 2 * kGuard);
+    BARK_CUDA_CHECK(cudaMemcpy(h.data(), reg, h.size(), cudaMemcpyDeviceToHost));
+    bool guards_intact = true;
+    for (size_t i = 0; i < kGuard; i++) guards_intact &= h[i] == kPattern && h[kGuard + out_bytes + i] == kPattern;
+    if (!guards_intact) { fprintf(stderr, "bark_b200_quant_matmul: a store landed outside the output (guard band overwritten)\n"); return -1; }
+    memcpy(C, h.data() + kGuard, out_bytes);
+    if (q_out) BARK_CUDA_CHECK(cudaMemcpy(q_out, d_q8, (size_t) M * K, cudaMemcpyDeviceToHost));
+    if (d_out) BARK_CUDA_CHECK(cudaMemcpy(d_out, d_q8d, (size_t) M * nb * 4, cudaMemcpyDeviceToHost));
+    if (s_out) BARK_CUDA_CHECK(cudaMemcpy(s_out, d_q8s, (size_t) M * nb * 4, cudaMemcpyDeviceToHost));
+    return 1;
+}
+extern "C" int bark_b200_quant_matmul(int wtype, const void * W, const float * A, float * C, int M, int N, int K, int epilogue, int path,
+                                      const uint16_t * gelu_tab, int8_t * q, float * d, float * s) {
+    return guarded((int) 0, [&] { return bark_b200_quant_matmul_impl(wtype, W, A, C, M, N, K, epilogue, path, gelu_tab, q, d, s); });
+}
+
 // batched generation (include/bark_b200.h)
 extern "C" bool bark_b200_generate_batch(struct bark_context * ctx, const char * const * texts, const uint32_t * seeds, int n, int n_threads) {
     (void) n_threads;

@@ -30,6 +30,7 @@
 //   P5  LN2 -> c_fc rows -> GELU table                                                 -> ff
 //   P6  mlp/c_proj rows + residual                                                     -> x
 // then LN_f -> lm_head rows [lm_lo, lm_hi) -> logits (plain stores; the kernel ends).
+#include "epilogue.cuh"
 #include "gpt_kernels.h"
 
 namespace bark {
@@ -399,7 +400,8 @@ struct Q4 {};
 template <typename WT> struct IsQ4 { static constexpr bool v = false; };
 template <> struct IsQ4<Q4> { static constexpr bool v = true; };
 
-// act (f32, natural order) -> int8 q[K] + f32 d[K/32] (the f16-rounded scale, widened back); block-wide, one warp per 32-element block
+// act (f32, natural order) -> int8 q[K] + f32 d[K/32] (the f16-rounded scale, widened back); block-wide, one warp per 32-element block.
+// A non-finite product gives -128 (cvtps_epi32 -> INT_MIN, then the saturating packs), as in quantize_q8_kernel.
 __device__ __forceinline__ void quantize_act_q8(const float * act, int K, int8_t * q, float * d) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (int b = warp; b < (K >> 5); b += kWarps) {
@@ -408,7 +410,8 @@ __device__ __forceinline__ void quantize_act_q8(const float * act, int K, int8_t
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
         const float id = amax != 0.0f ? __fdiv_rn(127.0f, amax) : 0.0f;
-        q[b * 32 + lane] = (int8_t) __float2int_rn(__fmul_rn(v, id));
+        const float p = __fmul_rn(v, id);
+        q[b * 32 + lane] = (int8_t)(isfinite(p) ? __float2int_rn(p) : -128);
         if (lane == 0) d[b] = __half2float(__float2half_rn(__fdiv_rn(amax, 127.0f)));
     }
     __syncthreads();
@@ -1065,6 +1068,54 @@ __global__ void __launch_bounds__(kThreads) decode_rows_kernel(int op, const flo
 
 void decode_rows(int op, const float * x, int rows, int n, const float * g, const float * b, float * out, unsigned * counters, cudaStream_t s) {
     BARK_LAUNCH(decode_rows_kernel, rows, kThreads, 0, s, op, x, n, 1.0 / n, g, b, out, counters);
+}
+
+// The decode step's q4_0 pieces on their own (bark_b200_quant_matmul paths 1 and 2), one CTA: quantize_act_q8 of one row into shared
+// memory, then every warp takes four rows at a time through row_dot_q4.  SH: the warp first copies them into its own slot in the layout
+// stage_rows leaves (the rows' nibble words, then their f16 scales); otherwise they are read from global memory.
+template <bool SH>
+__global__ void __launch_bounds__(kThreads) decode_q4_rows_kernel(const float * __restrict__ x, int K, const unsigned char * __restrict__ wq,
+                                                                  const unsigned char * __restrict__ ws, int n_out, MatmulEpilogue ep,
+                                                                  int8_t * __restrict__ q_out, float * __restrict__ d_out) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nb = K >> 5;
+    int8_t * aq = reinterpret_cast<int8_t *>(dsm);
+    float * ad = reinterpret_cast<float *>(dsm + K);
+    unsigned char * slot = dsm + K + nb * 4 + (size_t) warp * 4 * nb * 18;
+    quantize_act_q8(x, K, aq, ad);
+    for (int i = threadIdx.x; i < K; i += kThreads) q_out[i] = aq[i];
+    for (int i = threadIdx.x; i < nb; i += kThreads) d_out[i] = ad[i];
+    for (int r = warp * 4; r < n_out; r += kWarps * 4) {
+        const int n = min(4, n_out - r);
+        float t;
+        if constexpr (SH) {
+            const uint32_t * src = reinterpret_cast<const uint32_t *>(wq + (size_t) r * nb * 16);
+            const unsigned short * ssrc = reinterpret_cast<const unsigned short *>(ws + (size_t) r * nb * 2);
+            for (int i = lane; i < n * nb * 4; i += 32) reinterpret_cast<uint32_t *>(slot)[i] = src[i];
+            for (int i = lane; i < n * nb; i += 32) reinterpret_cast<unsigned short *>(slot + n * nb * 16)[i] = ssrc[i];
+            __syncwarp();
+            t = row_dot_q4<true>(slot, slot + n * nb * 16, n, nb, aq, ad, lane);
+            __syncwarp();
+        } else {
+            t = row_dot_q4<false>(wq + (size_t) r * nb * 16, ws + (size_t) r * nb * 2, n, nb, aq, ad, lane);
+        }
+#pragma unroll
+        for (int g = 0; g < 4; g++) {
+            const float v = __shfl_sync(0xffffffffu, t, g * 8);
+            if (lane == 0 && g < n) matmul_epilogue(ep, 0, r + g, v);
+        }
+    }
+}
+
+void decode_q4_rows(bool staged, const float * x, int K, const void * qs, const void * scales, int n_out, const MatmulEpilogue & ep, int8_t * q_out,
+                    float * d_out, cudaStream_t s) {
+    const size_t smem = (size_t) K + (K >> 5) * 4 + (staged ? (size_t) kWarps * 4 * (K >> 5) * 18 : 0);
+    const unsigned char * wq = (const unsigned char *) qs, * ws = (const unsigned char *) scales;
+    if (staged) {
+        BARK_CUDA_CHECK(cudaFuncSetAttribute(decode_q4_rows_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
+        BARK_LAUNCH(decode_q4_rows_kernel<true>, 1, kThreads, smem, s, x, K, wq, ws, n_out, ep, q_out, d_out);
+    } else {
+        BARK_LAUNCH(decode_q4_rows_kernel<false>, 1, kThreads, smem, s, x, K, wq, ws, n_out, ep, q_out, d_out);
+    }
 }
 
 static size_t decode_smem_bytes() { return (size_t) SmemLayout::total + 128; }

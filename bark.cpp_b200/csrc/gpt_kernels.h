@@ -52,6 +52,7 @@ void attention_batch(const float * Q, const float * Kst, const float * Vst, cons
 // ---- q4_0 weights (q4_kernels.cu) ---------------------------------------------------------------------------------
 void q4_split(const void * raw_blocks, size_t n_blocks, void * qs, void * scales, cudaStream_t s);
 void q4_set_scratch(void * q8, void * q8_scales);      // int8 [rows][K] + f32 [rows][K/32] for the activation operand, owned by the context
+void q4_get_scratch(void ** q8, void ** q8_scales);    // this host thread's current pointers (a test hook saves and restores them)
 void q4_matmul(const DMat & W, const void * act_f32, int ld_act, int rows, const MatmulEpilogue & ep, cudaStream_t s);
 
 // ---- q4_1 / q5_0 / q5_1 / q8_0 weights (qx_kernels.cu) ---------------------------------------------------------------------------
@@ -59,6 +60,7 @@ bool   qx_supported(WType t);
 size_t qx_block_bytes(WType t);
 void   qx_split(const void * raw_blocks, size_t n_blocks, WType t, void * qs, void * qh, void * d, void * m, cudaStream_t s);
 void   qx_set_scratch(void * q8, void * q8_scales, void * q8_sums);
+void   qx_get_scratch(void ** q8, void ** q8_scales, void ** q8_sums);
 void   qx_embed_causal(const GPTModel & m, const int32_t * d_tok, int N, int n_past, bool merge, float * x, cudaStream_t s, const int32_t * d_pos);
 void   qx_embed_fine(const GPTModel & m, const int32_t * d_ids, int nn, float * x, cudaStream_t s);
 void   qx_matmul(const DMat & W, const void * act_f32, int ld_act, int rows, const MatmulEpilogue & ep, cudaStream_t s);
@@ -107,5 +109,10 @@ void launch_decode_step(const DecodeArgs & args, WType wt, int n_sm, cudaStream_
 // the decode kernels' LayerNorm (op 0) or soft_max (op 1) on `rows` rows of n <= 1024 floats, one CTA per row (tests):
 // counters[0] / counters[1] count the LayerNorm / soft_max rows that took the sequential replay
 void decode_rows(int op, const float * x, int rows, int n, const float * g, const float * b, float * out, unsigned * counters, cudaStream_t s);
+// the decode kernels' q4_0 pieces on one f32 row x [K] (tests): quantize_act_q8, then row_dot_q4 over n_out rows (qs / scales as q4_split
+// leaves them) through the per-op epilogue ep (row 0), in one CTA; staged: the rows are copied into shared memory first (row_dot_q4<true>),
+// else read from global memory.  q_out [K] / d_out [K/32]: the q8 operand.  K <= 4096.
+void decode_q4_rows(bool staged, const float * x, int K, const void * qs, const void * scales, int n_out, const MatmulEpilogue & ep, int8_t * q_out,
+                    float * d_out, cudaStream_t s);
 
 }  // namespace bark

@@ -30,7 +30,8 @@ __global__ void split_q4_kernel(const unsigned char * __restrict__ raw, size_t n
     qs[b] = make_uint4(w[0], w[1], w[2], w[3]);
 }
 
-// one warp per (row, block), lane j = element j
+// one warp per (row, block), lane j = element j.  A non-finite product (a block holding an inf, or 0 < amax < 127 / FLT_MAX where
+// id = 127 / amax overflows) becomes -128: cvtps_epi32 turns it into INT_MIN and the saturating packs into -128.
 __global__ void quantize_q8_kernel(const float * __restrict__ x, int ldx, int rows, int K, int8_t * __restrict__ q, float * __restrict__ d_out) {
     const int nb = K >> 5;
     const size_t w = ((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -43,7 +44,8 @@ __global__ void quantize_q8_kernel(const float * __restrict__ x, int ldx, int ro
     for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
     const float d = __fdiv_rn(amax, 127.0f);
     const float id = amax != 0.0f ? __fdiv_rn(127.0f, amax) : 0.0f;
-    q[(size_t) r * K + b * 32 + lane] = (int8_t) __float2int_rn(__fmul_rn(v, id));          // _mm256_round_ps(nearest) + cvtps_epi32
+    const float p = __fmul_rn(v, id);
+    q[(size_t) r * K + b * 32 + lane] = (int8_t)(isfinite(p) ? __float2int_rn(p) : -128);   // _mm256_round_ps(nearest) + cvtps_epi32 + packs
     if (lane == 0) d_out[(size_t) r * nb + b] = __half2float(__float2half_rn(d));          // y[i].d = GGML_FP32_TO_FP16(d)
 }
 
@@ -110,6 +112,7 @@ void q4_split(const void * raw_blocks, size_t n_blocks, void * qs, void * scales
 }
 
 void q4_set_scratch(void * q8, void * q8_scales) { g_q8 = (int8_t *) q8; g_q8d = (float *) q8_scales; }
+void q4_get_scratch(void ** q8, void ** q8_scales) { *q8 = g_q8; *q8_scales = g_q8d; }
 
 // act: f32 rows [rows][ld_act] as store_act(W_Q4_0) leaves them
 void q4_matmul(const DMat & W, const void * act, int ld_act, int rows, const MatmulEpilogue & ep, cudaStream_t s) {

@@ -69,7 +69,9 @@ __global__ void split_qx_kernel(const unsigned char * __restrict__ raw, size_t n
     for (int i = 0; i < nq; i++) qs[b * nq + i] = src[i];
 }
 
-// q8_0 / q8_1 activation blocks (quantize_row_q8_0 / q8_1, AVX2 branches): one warp per (row, block); s = f16(d * sum(q)) with the unrounded d
+// q8_0 / q8_1 activation blocks (quantize_row_q8_0 / q8_1, AVX2 branches): one warp per (row, block); s = f16(d * sum(q)) with the unrounded d.
+// A non-finite product is INT_MIN after cvtps_epi32: the byte saturates to -128, and s sums the int32 values, wrapping as
+// _mm256_add_epi32 does.
 __global__ void quantize_q8x_kernel(const float * __restrict__ x, int ldx, int rows, int K, int8_t * __restrict__ q, float * __restrict__ d_out, float * __restrict__ s_out) {
     const int nb = K >> 5;
     const size_t w = ((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -82,14 +84,15 @@ __global__ void quantize_q8x_kernel(const float * __restrict__ x, int ldx, int r
     for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
     const float d = __fdiv_rn(amax, 127.0f);
     const float id = amax != 0.0f ? __fdiv_rn(127.0f, amax) : 0.0f;
-    const int qi = __float2int_rn(__fmul_rn(v, id));
-    q[(size_t) r * K + b * 32 + lane] = (int8_t) qi;
-    int sum = qi;
+    const float p = __fmul_rn(v, id);
+    const int qi = isfinite(p) ? __float2int_rn(p) : INT_MIN;
+    q[(size_t) r * K + b * 32 + lane] = (int8_t) max(qi, -128);
+    unsigned sum = (unsigned) qi;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
     if (lane == 0) {
         d_out[(size_t) r * nb + b] = __half2float(__float2half_rn(d));
-        if (s_out) s_out[(size_t) r * nb + b] = __half2float(__float2half_rn(__fmul_rn(d, (float) sum)));
+        if (s_out) s_out[(size_t) r * nb + b] = __half2float(__float2half_rn(__fmul_rn(d, (float)(int) sum)));
     }
 }
 
@@ -158,6 +161,7 @@ void qx_split(const void * raw_blocks, size_t n_blocks, WType t, void * qs, void
 }
 
 void qx_set_scratch(void * q8, void * q8_scales, void * q8_sums) { g_qx_q8 = (int8_t *) q8; g_qx_d = (float *) q8_scales; g_qx_s = (float *) q8_sums; }
+void qx_get_scratch(void ** q8, void ** q8_scales, void ** q8_sums) { *q8 = g_qx_q8; *q8_scales = g_qx_d; *q8_sums = g_qx_s; }
 
 void qx_embed_causal(const GPTModel & m, const int32_t * d_tok, int N, int n_past, bool merge, float * x, cudaStream_t s, const int32_t * d_pos) {
     BARK_LAUNCH(embed_causal_q_kernel, N, 256, 0, s, m.wte[0], (int) m.wtype, m.wpe, d_tok, N, n_past, merge ? 1 : 0, m.n_embd, x, d_pos);

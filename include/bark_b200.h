@@ -204,6 +204,19 @@ BARK_API int  bark_b200_sample_given_u(const float * logits, int n, int rows, fl
 BARK_API int  bark_b200_parity_gemm(const void * A, const void * W, void * C, int M, int N, int K, int wtype, int epilogue, int variant,
                                     const uint16_t * gelu_tab);
 
+/* Quantised mat-muls on host buffers without a context (tests): C = A W^T with every output the reference's ggml_vec_dot_<type>_q8_0 /
+ * _q8_1 of weight row o against activation row m after quantize_row_q8_0 / q8_1, for A [M][K] f32 and W [N][K/32] blocks as the model
+ * file stores them, wtype (enum ggml_type) 2 q4_0 (18-byte blocks), 3 q4_1 (20), 6 q5_0 (22), 7 q5_1 (24) or 8 q8_0 (34), K % 32 == 0.
+ * epilogue as bark_b200_parity_gemm (GELU_ACT: f32 [M][N], the operand a quantised model's next mat-mul quantises; QKV: N % 3 == 0).
+ *   path 0: the per-op kernels the library runs for M rows (quantize_q8_kernel + q4_matmul_kernel, or quantize_q8x_kernel + qx_matmul_kernel)
+ *   path 1 / 2: q4_0, M == 1, K <= 4096 only: the persistent decode step's quantize_act_q8 + row_dot_q4 in one CTA, the weight rows
+ *               staged in shared memory (1) or read from global memory (2)
+ * q [M][K] int8, d [M][K/32] f32 (the f16 scale, widened), s [M][K/32] f32 (q4_1 / q5_1 only, the f16 q8_1 sum): the quantised
+ * activation blocks; each may be NULL.  The calling thread's context is unaffected.  Returns 1, 0 on failure or invalid arguments, -1 if
+ * a store landed in the guard bands around the output. */
+BARK_API int  bark_b200_quant_matmul(int wtype, const void * W, const float * A, float * C, int M, int N, int K, int epilogue, int path,
+                                     const uint16_t * gelu_tab, int8_t * q, float * d, float * s);
+
 #ifdef __cplusplus
 }
 #endif

@@ -404,6 +404,11 @@ void orc_set_params(orc_ctx * c, float temp, float fine_temp, float min_eos_p, i
 /* ------------------------------------------------------------------------------------------ */
 typedef struct { uint16_t d; int8_t qs[32]; } q8_0_t;
 
+/* _mm256_round_ps(nearest-even) then _mm256_cvtps_epi32: a non-finite or out-of-range value becomes INT_MIN (the "integer
+ * indefinite"); the saturating packs (packs_epi32, packs_epi16) then clamp the int32 to a byte */
+static int32_t cvt_epi32(float v) { return isfinite(v) && fabsf(v) < 2147483648.0f ? (int32_t) nearbyintf(v) : INT32_MIN; }
+static int8_t packs8(int32_t i) { return (int8_t)(i < -128 ? -128 : i > 127 ? 127 : i); }
+
 static void quantize_row_q8_0(const float * x, q8_0_t * y, int k) {
     /* AVX2 branch: amax over the block, d = amax/127, id = 127/amax, q = round-to-nearest(x*id)
      * (ggml-quants.c:895-960: _mm256_round_ps nearest-even on x*id) */
@@ -413,7 +418,7 @@ static void quantize_row_q8_0(const float * x, q8_0_t * y, int k) {
         const float d = amax / 127.0f;
         const float id = (amax != 0.0f) ? 127.0f / amax : 0.0f;
         y[b].d = orc_f32_to_f16(d);
-        for (int j = 0; j < 32; j++) { float v = x[b * 32 + j] * id; y[b].qs[j] = (int8_t) nearbyintf(v); }
+        for (int j = 0; j < 32; j++) y[b].qs[j] = packs8(cvt_epi32(x[b * 32 + j] * id));
     }
 }
 
@@ -440,7 +445,8 @@ static float vec_dot_q4_0_q8_0(int n, const uint8_t * vx, const q8_0_t * y) {
     return s0 + s1;
 }
 
-/* q8_1 activation blocks (quantize_row_q8_1, AVX2 branch, ggml-quants.c:1305-1345): q as q8_0, plus s = f16(d * sum(q)) */
+/* q8_1 activation blocks (quantize_row_q8_1, AVX2 branch, ggml-quants.c:1305-1345): q as q8_0, plus s = f16(d * sum(q)), where the
+ * sum adds the int32 values before the packs (hsum_i32_8 of _mm256_add_epi32: wraps modulo 2^32) */
 typedef struct { uint16_t d, s; int8_t qs[32]; } q8_1_t;
 static void quantize_row_q8_1(const float * x, q8_1_t * y, int k) {
     for (int b = 0; b < k / 32; b++) {
@@ -449,9 +455,9 @@ static void quantize_row_q8_1(const float * x, q8_1_t * y, int k) {
         const float d = amax / 127.0f;
         const float id = (amax != 0.0f) ? 127.0f / amax : 0.0f;
         y[b].d = orc_f32_to_f16(d);
-        int sum = 0;
-        for (int j = 0; j < 32; j++) { float v = x[b * 32 + j] * id; int q = (int) nearbyintf(v); y[b].qs[j] = (int8_t) q; sum += q; }
-        y[b].s = orc_f32_to_f16(d * (float) sum);
+        uint32_t sum = 0;
+        for (int j = 0; j < 32; j++) { const int32_t q = cvt_epi32(x[b * 32 + j] * id); y[b].qs[j] = packs8(q); sum += (uint32_t) q; }
+        y[b].s = orc_f32_to_f16(d * (float)(int32_t) sum);
     }
 }
 
@@ -528,6 +534,43 @@ static float vec_dot_q8_0_q8_0(int n, const uint8_t * vx, const q8_0_t * y) {
         lanes8(q, y[b].qs, d, acc);
     }
     return hsum8(acc);
+}
+
+/* Exported for the kernel tests (oracle/bindings.py).  The activation quantisers on k floats (k % 32 == 0) into the reference's block
+ * layouts (block_q8_0: 34 bytes, block_q8_1: 36 bytes); one dot of n elements of weight blocks of wtype (enum ggml_type: 2 q4_0, 3 q4_1,
+ * 6 q5_0, 7 q5_1, 8 q8_0) against the blocks of its vec_dot_type; and out[m][o] = that dot of weight row o against row m of A [M][K]
+ * quantised, for W [N] rows of K/32 blocks. */
+void orc_quantize_row_q8_0(const float * x, void * y, int k) { quantize_row_q8_0(x, (q8_0_t *) y, k); }
+void orc_quantize_row_q8_1(const float * x, void * y, int k) { quantize_row_q8_1(x, (q8_1_t *) y, k); }
+static int q_block_bytes(int wtype) { return wtype == 2 ? 18 : wtype == 3 ? 20 : wtype == 6 ? 22 : wtype == 7 ? 24 : wtype == 8 ? 34 : 0; }
+float orc_vec_dot_q(int wtype, int n, const void * vx, const void * vy) {
+    init_f16_lut();
+    switch (wtype) {
+        case 2: return vec_dot_q4_0_q8_0(n, vx, vy);
+        case 3: return vec_dot_q4_1_q8_1(n, vx, vy);
+        case 6: return vec_dot_q5_0_q8_0(n, vx, vy);
+        case 7: return vec_dot_q5_1_q8_1(n, vx, vy);
+        case 8: return vec_dot_q8_0_q8_0(n, vx, vy);
+        default: return NAN;
+    }
+}
+int orc_quant_matmul(int wtype, const void * W, const float * A, int M, int N, int K, float * out) {
+    const int bb = q_block_bytes(wtype), nb = K / 32;
+    if (!bb || K % 32) return 0;
+    init_f16_lut();
+    const int q81 = wtype == 3 || wtype == 7;
+    const size_t ab = q81 ? sizeof(q8_1_t) : sizeof(q8_0_t);
+    unsigned char * aq = malloc((size_t) M * nb * ab);
+    for (int m = 0; m < M; m++) {
+        if (q81) quantize_row_q8_1(A + (size_t) m * K, (q8_1_t *) (aq + (size_t) m * nb * ab), K);
+        else     quantize_row_q8_0(A + (size_t) m * K, (q8_0_t *) (aq + (size_t) m * nb * ab), K);
+    }
+    #pragma omp parallel for schedule(static) collapse(2)
+    for (int m = 0; m < M; m++)
+        for (int o = 0; o < N; o++)
+            out[(size_t) m * N + o] = orc_vec_dot_q(wtype, K, (const unsigned char *) W + (size_t) o * nb * bb, aq + (size_t) m * nb * ab);
+    free(aq);
+    return 1;
 }
 
 /* ------------------------------------------------------------------------------------------ */

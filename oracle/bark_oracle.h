@@ -58,6 +58,13 @@ float    orc_vec_dot_f32(int n, const float * x, const float * y);
 uint16_t orc_f32_to_f16(float f);
 float    orc_f16_to_f32(uint16_t h);
 void     orc_gelu_table(uint16_t * out65536);
+/* quantised mat-muls (AVX2 branches of ggml-quants.c): quantize_row_q8_0 / q8_1 into block_q8_0 (34 B) / block_q8_1 (36 B); the dot
+ * of n elements of wtype (enum ggml_type 2, 3, 6, 7, 8) blocks against q8 blocks; out [M][N] = the dots of W's N rows of K/32 blocks
+ * against A [M][K] f32 quantised (returns 0 for an unknown type or K % 32 != 0) */
+void     orc_quantize_row_q8_0(const float * x, void * y, int k);
+void     orc_quantize_row_q8_1(const float * x, void * y, int k);
+float    orc_vec_dot_q(int wtype, int n, const void * vx, const void * vy);
+int      orc_quant_matmul(int wtype, const void * W, const float * A, int M, int N, int K, float * out);
 void     orc_norm(int n, const float * x, float * y, float eps);
 void     orc_soft_max(int n, const float * x, float * y);   /* row soft_max as ggml.c:13953 with scale 1 */
 float    orc_v_expf(float x);

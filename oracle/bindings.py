@@ -235,6 +235,52 @@ def mt_words(seed, k):
     return np.array([L.orc_mt_next(_p(st)) for _ in range(k)], np.uint64)
 
 
+QUANT_TYPES = {"q4_0": 2, "q4_1": 3, "q5_0": 6, "q5_1": 7, "q8_0": 8}     # enum ggml_type
+QUANT_BLOCK_BYTES = {"q4_0": 18, "q4_1": 20, "q5_0": 22, "q5_1": 24, "q8_0": 34}
+Q8_DTYPES = {   # block_q8_0 / block_q8_1 (ggml-common.h)
+    "q8_0": np.dtype([("d", "<u2"), ("qs", "i1", 32)]),
+    "q8_1": np.dtype([("d", "<u2"), ("s", "<u2"), ("qs", "i1", 32)]),
+}
+
+
+def vec_dot_type(qtype):
+    return "q8_1" if qtype in ("q4_1", "q5_1") else "q8_0"
+
+
+def _quant_lib(L):
+    L.orc_quantize_row_q8_0.argtypes = L.orc_quantize_row_q8_1.argtypes = [vp, vp, C.c_int]
+    L.orc_vec_dot_q.restype = C.c_float
+    L.orc_vec_dot_q.argtypes = [C.c_int, C.c_int, vp, vp]
+    L.orc_quant_matmul.restype = C.c_int
+    L.orc_quant_matmul.argtypes = [C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, vp]
+    return L
+
+
+def quantize_q8(x, kind):
+    """the oracle's quantize_row_q8_0 / q8_1 ("q8_0" / "q8_1") of float32 rows [..][K]: a structured array [..][K/32] of Q8_DTYPES[kind]"""
+    x = np.ascontiguousarray(x, np.float32)
+    y = np.zeros(x.shape[:-1] + (x.shape[-1] // 32,), Q8_DTYPES[kind])
+    getattr(_quant_lib(_oracle_lib()), f"orc_quantize_row_{kind}")(_p(x), _p(y), x.size)
+    return y
+
+
+def vec_dot_q(qtype, w_blocks, y_blocks):
+    """the oracle's ggml_vec_dot_<qtype>_<q8_0|q8_1> of one weight row (uint8 file blocks) against one q8 row (quantize_q8's blocks)"""
+    w = np.ascontiguousarray(w_blocks, np.uint8); y = np.ascontiguousarray(y_blocks)
+    assert y.dtype == Q8_DTYPES[vec_dot_type(qtype)] and w.size == y.size * QUANT_BLOCK_BYTES[qtype], (w.shape, y.shape)
+    return np.float32(_quant_lib(_oracle_lib()).orc_vec_dot_q(QUANT_TYPES[qtype], 32 * y.size, _p(w), _p(y)))
+
+
+def quant_matmul(qtype, W, A):
+    """out [M][N] float32: weight row o (W [N][K/32 * block bytes] uint8) against row m of A [M][K] float32 quantised, as the reference's mul_mat"""
+    W = np.ascontiguousarray(W, np.uint8); A = np.ascontiguousarray(A, np.float32)
+    M, K = A.shape; N = W.shape[0]
+    assert W.shape[1] == K // 32 * QUANT_BLOCK_BYTES[qtype], (W.shape, A.shape)
+    out = np.zeros((M, N), np.float32)
+    assert _quant_lib(_oracle_lib()).orc_quant_matmul(QUANT_TYPES[qtype], _p(W), _p(A), M, N, K, _p(out))
+    return out
+
+
 def gelu_tables():
     """(oracle table, reference table or None): gelu evaluated at every f16 input, as f16 bits."""
     if not os.path.exists(ORACLE_SO):
