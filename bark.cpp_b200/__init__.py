@@ -514,6 +514,29 @@ class GuardBandError(RuntimeError):
     """The GEMM stored outside its output."""
 
 
+def _gemm(what: str, run, epilogue: str, resid: np.ndarray | None, shape, dtype, parts=None):
+    """What the GEMM wrappers share: run(out) calls the hook on out, a float32 copy of resid [M][N] for the "resid" epilogue, else
+    zeros of shape and dtype.  Returns (out, the hook's return value); with parts, out is split into arrays of those shapes (the Q / K
+    / V blocks).  Raises GuardBandError when the hook stored outside its output, RuntimeError when it failed."""
+    if epilogue == "resid":
+        out = np.array(resid, np.float32, order="C", copy=True)
+        assert out.shape == shape, out.shape
+    else:
+        out = np.zeros(shape, dtype)
+    r = run(out)
+    if r == -1:
+        raise GuardBandError(f"{what} wrote outside its output")
+    if r <= 0:
+        raise RuntimeError(f"{what} failed")
+    if parts:
+        flat, o, blocks = out.reshape(-1), 0, []
+        for p in parts:
+            blocks.append(flat[o:o + p[0] * p[1]].reshape(p))
+            o += p[0] * p[1]
+        out = tuple(blocks)
+    return out, r
+
+
 def fast_gemm(A: np.ndarray, W: np.ndarray, epilogue: str = "f32", bn: int = 0, resid: np.ndarray | None = None, return_bn: bool = False):
     """A W^T on the wgmma path through one of the fine pass's epilogues; A [M][K], W [N][K] float16, K % 64 == 0.
 
@@ -523,21 +546,11 @@ def fast_gemm(A: np.ndarray, W: np.ndarray, epilogue: str = "f32", bn: int = 0, 
     A = np.ascontiguousarray(A, np.float16); W = np.ascontiguousarray(W, np.float16)
     M, K = A.shape; N = W.shape[0]
     assert W.shape[1] == K, (A.shape, W.shape)
-    if epilogue == "resid":
-        out = np.array(resid, np.float32, order="C", copy=True)
-        assert out.shape == (M, N), out.shape
-    elif epilogue == "qkv16":
-        assert N % 6 == 0, N
-        out = np.zeros(M * N, np.float16)
-    else:
-        out = np.zeros((M, N), np.float16 if epilogue == "gelu16" else np.float32)
-    r = lib().bark_b200_fast_gemm(_p(A), _p(W), _p(out), M, N, K, FAST_EPILOGUES[epilogue], bn)
-    if r == -1:
-        raise GuardBandError(f"bark_b200_fast_gemm ({epilogue}, {M}x{N}x{K}, bn {bn}) wrote outside its output")
-    if r <= 0:
-        raise RuntimeError(f"bark_b200_fast_gemm ({epilogue}, {M}x{N}x{K}, bn {bn}) failed")
     if epilogue == "qkv16":
-        out = (out[:M * 2 * N // 3].reshape(M, 2 * N // 3), out[M * 2 * N // 3:].reshape(N // 3, M))
+        assert N % 6 == 0, N
+    out, r = _gemm(f"bark_b200_fast_gemm ({epilogue}, {M}x{N}x{K}, bn {bn})",
+                   lambda out: lib().bark_b200_fast_gemm(_p(A), _p(W), _p(out), M, N, K, FAST_EPILOGUES[epilogue], bn), epilogue, resid,
+                   (M, N), np.float16 if epilogue in ("gelu16", "qkv16") else np.float32, ((M, 2 * N // 3), (N // 3, M)) if epilogue == "qkv16" else None)
     return (out, r) if return_bn else out
 
 
@@ -570,6 +583,15 @@ def parity_attention(q: np.ndarray, k: np.ndarray, v: np.ndarray, n_head: int, n
 PARITY_EPILOGUES = {"store": 0, "resid": 1, "gelu": 2, "qkv": 3}      # EPI_* (csrc/gpt_kernels.h)
 
 
+def _gelu_table(epilogue: str, gelu_tab):
+    """gelu_tab as the hooks take it for the "gelu" epilogue, 65536 uint16 f16 bits; None for the others."""
+    if epilogue != "gelu":
+        return None
+    tab = np.ascontiguousarray(gelu_tab, np.uint16)
+    assert tab.shape == (65536,), tab.shape
+    return tab
+
+
 def parity_gemm(A: np.ndarray, W: np.ndarray, epilogue: str = "store", variant: int = 0, resid: np.ndarray | None = None,
                 gelu_tab: np.ndarray | None = None, return_variant: bool = False):
     """Bit-exact A W^T on the parity path's tiled GEMM; A [M][K], W [N][K] both float16 or both float32, K % 32 == 0.
@@ -581,24 +603,11 @@ def parity_gemm(A: np.ndarray, W: np.ndarray, epilogue: str = "store", variant: 
     A = np.ascontiguousarray(A, dt); W = np.ascontiguousarray(W, dt)
     M, K = A.shape; N = W.shape[0]
     assert W.shape[1] == K, (A.shape, W.shape)
-    if epilogue == "resid":
-        out = np.array(resid, np.float32, order="C", copy=True)
-        assert out.shape == (M, N), out.shape
-    else:
-        out = np.zeros((M, N), dt if epilogue == "gelu" else np.float32)
-    tab = None
-    if epilogue == "gelu":
-        tab = np.ascontiguousarray(gelu_tab, np.uint16)
-        assert tab.shape == (65536,), tab.shape
-    r = lib().bark_b200_parity_gemm(_p(A), _p(W), _p(out), M, N, K, 1 if dt == np.float16 else 0, PARITY_EPILOGUES[epilogue], variant,
-                                    None if tab is None else _p(tab))
-    if r == -1:
-        raise GuardBandError(f"bark_b200_parity_gemm ({epilogue}, {M}x{N}x{K}, variant {variant}) wrote outside its output")
-    if r <= 0:
-        raise RuntimeError(f"bark_b200_parity_gemm ({epilogue}, {M}x{N}x{K}, variant {variant}) failed")
-    if epilogue == "qkv":
-        flat = out.reshape(-1)
-        out = tuple(flat[i * M * (N // 3):(i + 1) * M * (N // 3)].reshape(M, N // 3) for i in range(3))
+    tab = _gelu_table(epilogue, gelu_tab)
+    out, r = _gemm(f"bark_b200_parity_gemm ({epilogue}, {M}x{N}x{K}, variant {variant})",
+                   lambda out: lib().bark_b200_parity_gemm(_p(A), _p(W), _p(out), M, N, K, 1 if dt == np.float16 else 0, PARITY_EPILOGUES[epilogue],
+                                                           variant, None if tab is None else _p(tab)),
+                   epilogue, resid, (M, N), dt if epilogue == "gelu" else np.float32, ((M, N // 3),) * 3 if epilogue == "qkv" else None)
     return (out, r) if return_variant else out
 
 
@@ -617,27 +626,13 @@ def quant_matmul(qtype: str, W: np.ndarray, A: np.ndarray, epilogue: str = "stor
     A = np.ascontiguousarray(A, np.float32); W = np.ascontiguousarray(W, np.uint8)
     M, K = A.shape; N = W.shape[0]
     assert K % 32 == 0 and W.shape[1] == K // 32 * QUANT_BLOCK_BYTES[qtype], (qtype, A.shape, W.shape)
-    if epilogue == "resid":
-        out = np.array(resid, np.float32, order="C", copy=True)
-        assert out.shape == (M, N), out.shape
-    else:
-        out = np.zeros((M, N), np.float32)
-    tab = None
-    if epilogue == "gelu":
-        tab = np.ascontiguousarray(gelu_tab, np.uint16)
-        assert tab.shape == (65536,), tab.shape
+    tab = _gelu_table(epilogue, gelu_tab)
     q = np.zeros((M, K), np.int8); d = np.zeros((M, K // 32), np.float32)
     s = np.zeros((M, K // 32), np.float32) if qtype in ("q4_1", "q5_1") else None
-    r = lib().bark_b200_quant_matmul(QUANT_TYPES[qtype], _p(W), _p(A), _p(out), M, N, K, PARITY_EPILOGUES[epilogue], QUANT_PATHS[path],
-                                     None if tab is None else _p(tab), _p(q), _p(d), None if s is None else _p(s))
-    what = f"bark_b200_quant_matmul ({qtype}, {epilogue}, {M}x{N}x{K}, {path})"
-    if r == -1:
-        raise GuardBandError(f"{what} wrote outside its output")
-    if r != 1:
-        raise RuntimeError(f"{what} failed")
-    if epilogue == "qkv":
-        flat = out.reshape(-1)
-        out = tuple(flat[i * M * (N // 3):(i + 1) * M * (N // 3)].reshape(M, N // 3) for i in range(3))
+    out, _ = _gemm(f"bark_b200_quant_matmul ({qtype}, {epilogue}, {M}x{N}x{K}, {path})",
+                   lambda out: lib().bark_b200_quant_matmul(QUANT_TYPES[qtype], _p(W), _p(A), _p(out), M, N, K, PARITY_EPILOGUES[epilogue],
+                                                            QUANT_PATHS[path], None if tab is None else _p(tab), _p(q), _p(d), None if s is None else _p(s)),
+                   epilogue, resid, (M, N), np.float32, ((M, N // 3),) * 3 if epilogue == "qkv" else None)
     if not return_q8:
         return out
     return out, q, d.astype(np.float16), None if s is None else s.astype(np.float16)
@@ -670,10 +665,10 @@ def parity_rows(x: np.ndarray, op: str, impl: str, g: np.ndarray | None = None, 
     return out, rep.value
 
 
-def sample_given_u(logits: np.ndarray, temp: float, u=None, threads: int = 0):
-    """The device sampler on logits [rows][n] float32 with the uniform draws u [rows] given (not used when temp == 0); threads 0 runs
-    sample_rows_kernel as the library picks it, 256 or 1024 forces that instantiation.  Returns a dict: tokens (final), device_tokens
-    (the kernel's, before the host replay), flags, eos_p [rows] and replays (how many rows went to the host replay)."""
+def _given_u(hook: str, what: str, logits, u, extra: tuple, run) -> dict:
+    """What the sampler wrappers share: logits as float32 rows [rows][n], u as float64 [rows] (broadcast; None for temp 0) and the
+    result dict of int32 tokens, device_tokens, flags, the extra keys and float32 eos_p.  run(logits, n, rows, u, tokens, device_tokens,
+    flags, eos_p, *extra) calls the hook with pointers; its return value becomes replays, RuntimeError when it is negative."""
     l = np.ascontiguousarray(logits, np.float32)
     if l.ndim == 1:
         l = l[None]
@@ -682,37 +677,30 @@ def sample_given_u(logits: np.ndarray, temp: float, u=None, threads: int = 0):
     if u is not None:
         u = np.ascontiguousarray(np.broadcast_to(np.asarray(u, np.float64), (rows,)))
         up = _p(u)
-    out = {k: np.zeros(rows, np.int32) for k in ("tokens", "device_tokens", "flags")}
+    out = {k: np.zeros(rows, np.int32) for k in ("tokens", "device_tokens", "flags") + extra}
     out["eos_p"] = np.zeros(rows, np.float32)
-    r = lib().bark_b200_sample_given_u(_p(l), n, rows, temp, up, threads, _p(out["tokens"]), _p(out["device_tokens"]), _p(out["flags"]),
-                                       _p(out["eos_p"]))
+    r = run(_p(l), n, rows, up, *(_p(out[k]) for k in ("tokens", "device_tokens", "flags", "eos_p") + extra))
     if r < 0:
-        raise RuntimeError(f"bark_b200_sample_given_u ({rows} x {n}, temp {temp}, threads {threads}) failed")
+        raise RuntimeError(f"{hook} ({rows} x {n}, {what}) failed")
     out["replays"] = r
     return out
+
+
+def sample_given_u(logits: np.ndarray, temp: float, u=None, threads: int = 0):
+    """The device sampler on logits [rows][n] float32 with the uniform draws u [rows] given (not used when temp == 0); threads 0 runs
+    sample_rows_kernel as the library picks it, 256 or 1024 forces that instantiation.  Returns a dict: tokens (final), device_tokens
+    (the kernel's, before the host replay), flags, eos_p [rows] and replays (how many rows went to the host replay)."""
+    return _given_u("bark_b200_sample_given_u", f"temp {temp}, threads {threads}", logits, u, (),
+                    lambda l, n, rows, up, *o: lib().bark_b200_sample_given_u(l, n, rows, temp, up, threads, *o))
 
 
 def sample_filtered_given_u(logits: np.ndarray, temp: float, u=None, top_k=None, top_p=None, threads: int = 0):
     """sample_given_u with the top-k / top-p filter first (bark_b200_sample_filtered_given_u): filter_rows_kernel, then the sampler on
     its output, then the host replay of every flagged row from the raw logits.  Returns sample_given_u's dict plus kept [rows], the
     number of logits the device filter kept; flags has bit 0 for the sampler and bit 1 for the filter."""
-    l = np.ascontiguousarray(logits, np.float32)
-    if l.ndim == 1:
-        l = l[None]
-    rows, n = l.shape
-    up = None
-    if u is not None:
-        u = np.ascontiguousarray(np.broadcast_to(np.asarray(u, np.float64), (rows,)))
-        up = _p(u)
-    out = {k: np.zeros(rows, np.int32) for k in ("tokens", "device_tokens", "flags", "kept")}
-    out["eos_p"] = np.zeros(rows, np.float32)
     st = _sampling_struct(top_k, top_p)
-    r = lib().bark_b200_sample_filtered_given_u(_p(l), n, rows, temp, C.byref(st), up, threads, _p(out["tokens"]), _p(out["device_tokens"]),
-                                                _p(out["flags"]), _p(out["eos_p"]), _p(out["kept"]))
-    if r < 0:
-        raise RuntimeError(f"bark_b200_sample_filtered_given_u ({rows} x {n}, temp {temp}, top_k {top_k}, top_p {top_p}, threads {threads}) failed")
-    out["replays"] = r
-    return out
+    return _given_u("bark_b200_sample_filtered_given_u", f"temp {temp}, top_k {top_k}, top_p {top_p}, threads {threads}", logits, u, ("kept",),
+                    lambda l, n, rows, up, *o: lib().bark_b200_sample_filtered_given_u(l, n, rows, temp, C.byref(st), up, threads, *o))
 
 
 class Encodec:

@@ -895,35 +895,6 @@ extern "C" int bark_b200_encodec_encode(struct bark_context * ctx, const float *
                                         int latent_cap) {
     return guarded((int) -1, [&] { return bark_b200_encodec_encode_impl(ctx, audio, n_samples, codes, codes_cap, latent, latent_cap); });
 }
-// the RVQ encode kernel on host buffers (tests): norms from rvq_norms_kernel, codes [n_q][T] from rvq_encode_kernel
-static int bark_b200_rvq_encode_impl(const float * latent, int T, const float * codebooks, int hidden, int n_bins, int n_q, int32_t * codes) {
-    if (!latent || !codebooks || !codes || T < 1 || hidden < 32 || hidden > 128 || hidden % 32 || n_bins < 1 || n_bins > 1024 || n_q < 1 || n_q > kMaxCodebooks) return 0;
-    struct Buffers {                                          // freed on every exit, including a CUDA failure thrown mid-way
-        void * p[4] = {nullptr, nullptr, nullptr, nullptr};
-        ~Buffers() { for (void * q : p) cudaFree(q); }
-    } d;
-    const size_t cb_n = (size_t) n_q * n_bins * hidden;
-    BARK_CUDA_CHECK(cudaMalloc(&d.p[0], (size_t) hidden * T * 4)); BARK_CUDA_CHECK(cudaMalloc(&d.p[1], cb_n * 4));
-    BARK_CUDA_CHECK(cudaMalloc(&d.p[2], (size_t) n_q * n_bins * 4)); BARK_CUDA_CHECK(cudaMalloc(&d.p[3], (size_t) n_q * T * 4));
-    float * dl = (float *) d.p[0], * dcb = (float *) d.p[1], * dn = (float *) d.p[2]; int32_t * dc = (int32_t *) d.p[3];
-    BARK_CUDA_CHECK(cudaMemcpy(dl, latent, (size_t) hidden * T * 4, cudaMemcpyHostToDevice));
-    BARK_CUDA_CHECK(cudaMemcpy(dcb, codebooks, cb_n * 4, cudaMemcpyHostToDevice));
-    BARK_CUDA_CHECK(cudaMemset(dc, 0xff, (size_t) n_q * T * 4));              // -1: a missing store shows up
-    const float * emb[kMaxCodebooks], * nrm[kMaxCodebooks];
-    for (int q = 0; q < n_q; q++) {
-        emb[q] = dcb + (size_t) q * n_bins * hidden; nrm[q] = dn + (size_t) q * n_bins;
-        rvq_norms(emb[q], n_bins, hidden, dn + (size_t) q * n_bins, 0);
-    }
-    if (!rvq_encode(emb, nrm, n_q, n_bins, hidden, dl, T, dc, 0)) return 0;
-    BARK_CUDA_CHECK(cudaGetLastError());
-    const cudaError_t e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) { fprintf(stderr, "bark_b200_rvq_encode: %s\n", cudaGetErrorString(e)); return 0; }
-    BARK_CUDA_CHECK(cudaMemcpy(codes, dc, (size_t) n_q * T * 4, cudaMemcpyDeviceToHost));
-    return 1;
-}
-extern "C" int bark_b200_rvq_encode(const float * latent, int T, const float * codebooks, int hidden, int n_bins, int n_q, int32_t * codes) {
-    return guarded((int) 0, [&] { return bark_b200_rvq_encode_impl(latent, T, codebooks, hidden, n_bins, n_q, codes); });
-}
 extern "C" int bark_b200_sample(struct bark_context * ctx, int which, const float * logits, int n, float temp, float * eos_p) {
     if (!ctx || !logits || n < 1) return -1;
     GPTModel & m = *pick(ctx, which < 0 || which > 2 ? 0 : which);
@@ -987,198 +958,7 @@ static int bark_b200_decode_timing_impl(struct bark_context * ctx, unsigned long
     return std::min(n, 256 * 32);
 }
 extern "C" int bark_b200_decode_timing(struct bark_context * ctx, unsigned long long * out, int n) { return guarded((int) 0, [&] { return bark_b200_decode_timing_impl(ctx, out, n); }); }
-// fast-mode kernels on host buffers (tests): C = A[M][K] W[N][K]^T through one of the fine pass's GEMM epilogues (bark_b200.h), and
-// attention over [n][E] f16 q / k / v.  Every device output region of the GEMM sits between guard bands of a fixed byte pattern that
-// are checked after the kernel, and starts as NaN (RESID: as the residual from C), so a stray or a missing store shows up.
-static int bark_b200_fast_gemm_impl(const uint16_t * A, const uint16_t * W, void * C, int M, int N, int K, int epilogue, int bn) {
-    if (!A || !W || !C || M < 1 || N < 1 || K < 64 || K % 64) return 0;
-    if (epilogue != FEPI_F32 && epilogue != FEPI_RESID && epilogue != FEPI_GELU16 && epilogue != FEPI_QKV16) return 0;
-    if (epilogue == FEPI_QKV16 && N % 6) return 0;
-    constexpr size_t kGuard = 4096;
-    constexpr unsigned char kPattern = 0x5a;
-    // output regions in the order they are laid out in C: [M][N] f32 or f16; QKV16: Q|K [M][2N/3] f16, then V^T [N/3][M] f16
-    size_t bytes[2] = {(size_t) M * N * (epilogue == FEPI_GELU16 ? 2 : 4), 0};
-    if (epilogue == FEPI_QKV16) { bytes[0] = (size_t) M * (2 * N / 3) * 2; bytes[1] = (size_t) M * (N / 3) * 2; }
-    __half * dA, * dW; unsigned char * reg[2] = {nullptr, nullptr}; int dev = 0, n_sm = 0;
-    BARK_CUDA_CHECK(cudaGetDevice(&dev)); BARK_CUDA_CHECK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
-    BARK_CUDA_CHECK(cudaMalloc(&dA, (size_t) M * K * 2)); BARK_CUDA_CHECK(cudaMalloc(&dW, (size_t) N * K * 2));
-    BARK_CUDA_CHECK(cudaMemcpy(dA, A, (size_t) M * K * 2, cudaMemcpyHostToDevice)); BARK_CUDA_CHECK(cudaMemcpy(dW, W, (size_t) N * K * 2, cudaMemcpyHostToDevice));
-    for (int r = 0; r < 2 && bytes[r]; r++) {
-        BARK_CUDA_CHECK(cudaMalloc(&reg[r], bytes[r] + 2 * kGuard));
-        BARK_CUDA_CHECK(cudaMemset(reg[r], kPattern, bytes[r] + 2 * kGuard));
-        if (epilogue == FEPI_RESID) BARK_CUDA_CHECK(cudaMemcpy(reg[r] + kGuard, C, bytes[r], cudaMemcpyHostToDevice));
-        else                        BARK_CUDA_CHECK(cudaMemset(reg[r] + kGuard, 0xff, bytes[r]));
-    }
-    FastEpi ep; ep.mode = epilogue; ep.ldo = N;
-    if (epilogue == FEPI_F32 || epilogue == FEPI_RESID) ep.out32 = (float *)(reg[0] + kGuard);
-    else                                                ep.out16 = (__half *)(reg[0] + kGuard);
-    if (epilogue == FEPI_QKV16) { ep.ldo = 2 * N / 3; ep.vt = (__half *)(reg[1] + kGuard); ep.vt_ld = M; ep.v_col0 = 2 * N / 3; }     // the fine pass's arguments
-    const int ran = fast_gemm(dA, K, dW, K, M, N, K, ep, n_sm, bn, 0);
-    const cudaError_t e = cudaDeviceSynchronize();
-    bool guards_intact = true;
-    if (e != cudaSuccess) fprintf(stderr, "bark_b200_fast_gemm: %s\n", cudaGetErrorString(e));
-    else {
-        std::vector<unsigned char> g(kGuard);
-        size_t off = 0;
-        for (int r = 0; r < 2 && bytes[r]; r++) {
-            for (const unsigned char * band : {reg[r], reg[r] + kGuard + bytes[r]}) {
-                BARK_CUDA_CHECK(cudaMemcpy(g.data(), band, kGuard, cudaMemcpyDeviceToHost));
-                for (unsigned char b : g) guards_intact &= b == kPattern;
-            }
-            BARK_CUDA_CHECK(cudaMemcpy((unsigned char *) C + off, reg[r] + kGuard, bytes[r], cudaMemcpyDeviceToHost));
-            off += bytes[r];
-        }
-    }
-    cudaFree(dA); cudaFree(dW); cudaFree(reg[0]); cudaFree(reg[1]);
-    if (!ran || e != cudaSuccess) return 0;
-    if (!guards_intact) { fprintf(stderr, "bark_b200_fast_gemm: a store landed outside the output (guard band overwritten)\n"); return -1; }
-    return ran;
-}
-extern "C" int bark_b200_fast_gemm(const uint16_t * A, const uint16_t * W, void * C, int M, int N, int K, int epilogue, int bn) {
-    return guarded((int) 0, [&] { return bark_b200_fast_gemm_impl(A, W, C, M, N, K, epilogue, bn); });
-}
-static int bark_b200_fast_attention_impl(const uint16_t * q, const uint16_t * k, const uint16_t * v, uint16_t * out, int n, int E, int H) {
-    if (!q || !k || !v || !out || n < 128 || n % 128 || E != H * 64) return 0;
-    std::vector<uint16_t> qk((size_t) n * 2 * E), vt((size_t) E * n);
-    for (int r = 0; r < n; r++) {
-        memcpy(&qk[(size_t) r * 2 * E], q + (size_t) r * E, (size_t) E * 2); memcpy(&qk[(size_t) r * 2 * E + E], k + (size_t) r * E, (size_t) E * 2);
-        for (int c = 0; c < E; c++) vt[(size_t) c * n + r] = v[(size_t) r * E + c];
-    }
-    __half * dqk, * dvt, * dout;
-    BARK_CUDA_CHECK(cudaMalloc(&dqk, qk.size() * 2)); BARK_CUDA_CHECK(cudaMalloc(&dvt, vt.size() * 2)); BARK_CUDA_CHECK(cudaMalloc(&dout, (size_t) n * E * 2));
-    BARK_CUDA_CHECK(cudaMemcpy(dqk, qk.data(), qk.size() * 2, cudaMemcpyHostToDevice)); BARK_CUDA_CHECK(cudaMemcpy(dvt, vt.data(), vt.size() * 2, cudaMemcpyHostToDevice));
-    const bool ok = fast_attention(dqk, 2 * E, E, dvt, n, E, H, dout, 0);
-    const cudaError_t e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) fprintf(stderr, "bark_b200_fast_attention: %s\n", cudaGetErrorString(e));
-    else BARK_CUDA_CHECK(cudaMemcpy(out, dout, (size_t) n * E * 2, cudaMemcpyDeviceToHost));
-    cudaFree(dqk); cudaFree(dvt); cudaFree(dout);
-    return ok && e == cudaSuccess;
-}
-extern "C" int bark_b200_fast_attention(const uint16_t * q, const uint16_t * k, const uint16_t * v, uint16_t * out, int n, int E, int H) { return guarded((int) 0, [&] { return bark_b200_fast_attention_impl(q, k, v, out, n, E, H); }); }
 extern "C" int bark_b200_fast_mode(struct bark_context * ctx) { return ctx && ctx->fast_mode ? 1 : 0; }
-// parity-path attention on host f32 buffers (tests, tools/attn_bench.py): the result is written as f32 rows [N][E], the operand form
-// store_act produces for quantised weights.  path: 0 = as attention() chooses for this shape, 1 = attn_fused_kernel, 2 = three kernels.
-static int bark_b200_parity_attention_impl(const float * q, const float * k, const float * v, float * out, int N, int n_kv, int n_past, int E, int H,
-                                           int causal, int path) {
-    if (!q || !k || !v || !out || N < 1 || n_kv < 1 || n_kv > 1024 || n_past < 0 || H < 1 || E % H || path < 0 || path > 2) return 0;
-    const int D = E / H;
-    if (D % 32 || D > 128) return 0;
-    struct Buffers {                                          // freed on every exit, including a CUDA failure thrown mid-way
-        float * p[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-        ~Buffers() { for (float * b : p) cudaFree(b); }
-    } d;
-    float *& dq = d.p[0], *& dk = d.p[1], *& dv = d.p[2], *& dout = d.p[3], *& dsc = d.p[4];
-    BARK_CUDA_CHECK(cudaMalloc(&dq, (size_t) N * E * 4)); BARK_CUDA_CHECK(cudaMalloc(&dk, (size_t) n_kv * E * 4));
-    BARK_CUDA_CHECK(cudaMalloc(&dv, (size_t) n_kv * E * 4)); BARK_CUDA_CHECK(cudaMalloc(&dout, (size_t) N * E * 4));
-    BARK_CUDA_CHECK(cudaMalloc(&dsc, (size_t) H * N * n_kv * 4));
-    BARK_CUDA_CHECK(cudaMemcpy(dq, q, (size_t) N * E * 4, cudaMemcpyHostToDevice)); BARK_CUDA_CHECK(cudaMemcpy(dk, k, (size_t) n_kv * E * 4, cudaMemcpyHostToDevice));
-    BARK_CUDA_CHECK(cudaMemcpy(dv, v, (size_t) n_kv * E * 4, cudaMemcpyHostToDevice));
-    BARK_CUDA_CHECK(cudaMemset(dout, 0xff, (size_t) N * E * 4));          // NaN: a missing store shows up
-    if (path == ATTN_TILED) {                                 // the three kernels' row limit is the score buffer's, which this call sizes itself
-        int dev = 0, n_sm = 0;
-        BARK_CUDA_CHECK(cudaGetDevice(&dev)); BARK_CUDA_CHECK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
-        if (N > attn_tiled_max_rows(H, n_sm)) return 0;
-    }
-    attention(dq, dk, dv, N, n_kv, n_past, E, H, causal != 0, dsc, dout, W_Q4_0, E, 0, (AttnPath) path);
-    BARK_CUDA_CHECK(cudaGetLastError());                      // a launch the configuration rejects
-    const cudaError_t e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) { fprintf(stderr, "bark_b200_parity_attention: %s\n", cudaGetErrorString(e)); return 0; }
-    BARK_CUDA_CHECK(cudaMemcpy(out, dout, (size_t) N * E * 4, cudaMemcpyDeviceToHost));
-    return 1;
-}
-extern "C" int bark_b200_parity_attention(const float * q, const float * k, const float * v, float * out, int N, int n_kv, int n_past, int E, int H, int causal,
-                                          int path) {
-    return guarded((int) 0, [&] { return bark_b200_parity_attention_impl(q, k, v, out, N, n_kv, n_past, E, H, causal, path); });
-}
-
-// the parity path's row reductions on host buffers (tests): op 0 LayerNorm, op 1 soft_max; impl 0 the multi-row kernels
-// (layernorm_act_kernel writing plain f32 rows, softmax_row), impl 1 the decode kernels' block_layernorm / softmax_exp_rcp
-static int bark_b200_parity_rows_impl(int op, int impl, const float * x, int rows, int n, const float * g, const float * b, float * out, unsigned * replays) {
-    if (!x || !out || !replays || op < 0 || op > 1 || impl < 0 || impl > 1 || rows < 1 || n < 1 || n > 1024 || (op == 0 && !g)) return 0;
-    struct Buffers {                                          // freed on every exit, including a CUDA failure thrown mid-way
-        void * p[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-        ~Buffers() { for (void * q : p) cudaFree(q); }
-    } d;
-    const size_t bytes = (size_t) rows * n * 4;
-    float * dx, * dout, * dg = nullptr, * db = nullptr; unsigned * dcnt;
-    BARK_CUDA_CHECK(cudaMalloc(&d.p[0], bytes)); dx = (float *) d.p[0];
-    BARK_CUDA_CHECK(cudaMalloc(&d.p[1], bytes)); dout = (float *) d.p[1];
-    BARK_CUDA_CHECK(cudaMalloc(&d.p[2], 2 * sizeof(unsigned))); dcnt = (unsigned *) d.p[2];
-    BARK_CUDA_CHECK(cudaMemcpy(dx, x, bytes, cudaMemcpyHostToDevice));
-    BARK_CUDA_CHECK(cudaMemset(dcnt, 0, 2 * sizeof(unsigned)));
-    BARK_CUDA_CHECK(cudaMemset(dout, 0xff, bytes));                       // NaN: a missing store shows up
-    if (op == 0) {
-        BARK_CUDA_CHECK(cudaMalloc(&d.p[3], (size_t) n * 4)); dg = (float *) d.p[3];
-        BARK_CUDA_CHECK(cudaMemcpy(dg, g, (size_t) n * 4, cudaMemcpyHostToDevice));
-        if (b) { BARK_CUDA_CHECK(cudaMalloc(&d.p[4], (size_t) n * 4)); db = (float *) d.p[4]; BARK_CUDA_CHECK(cudaMemcpy(db, b, (size_t) n * 4, cudaMemcpyHostToDevice)); }
-    }
-    if (impl == 1)    decode_rows(op, dx, rows, n, dg, db, dout, dcnt, 0);
-    else if (op == 0) layernorm_act(dx, rows, n, dg, db, dout, W_Q4_0, n, dcnt, 0);
-    else {            BARK_CUDA_CHECK(cudaMemcpy(dout, dx, bytes, cudaMemcpyDeviceToDevice)); softmax_rows(dout, rows, n, dcnt, 0); }
-    BARK_CUDA_CHECK(cudaGetLastError());                      // a launch the configuration rejects
-    const cudaError_t e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) { fprintf(stderr, "bark_b200_parity_rows: %s\n", cudaGetErrorString(e)); return 0; }
-    unsigned cnt[2];
-    BARK_CUDA_CHECK(cudaMemcpy(cnt, dcnt, sizeof(cnt), cudaMemcpyDeviceToHost));
-    BARK_CUDA_CHECK(cudaMemcpy(out, dout, bytes, cudaMemcpyDeviceToHost));
-    *replays = cnt[0] + cnt[1];
-    return 1;
-}
-extern "C" int bark_b200_parity_rows(int op, int impl, const float * x, int rows, int n, const float * g, const float * b, float * out, unsigned * replays) {
-    return guarded((int) 0, [&] { return bark_b200_parity_rows_impl(op, impl, x, rows, n, g, b, out, replays); });
-}
-
-// the device sampler on host rows with the uniforms given (tests): sample_rows_kernel at the instantiation asked for, then every
-// flagged row replayed with sample_token_given_u, as sample_device does it.  device_tokens keeps the kernel's tokens before the replay.
-static int bark_b200_sample_given_u_impl(const float * logits, int n, int rows, float temp, const double * u, int threads, int32_t * tokens,
-                                         int32_t * device_tokens, int32_t * flags, float * eos_p) {
-    if (!logits || !tokens || !device_tokens || !flags || !eos_p || (temp != 0.0f && !u)) return -1;
-    if (n < 2 || n > kSampleMaxLogits || rows < 1 || rows > 1024 || !std::isfinite(temp) || temp < 0.0f) return -1;
-    if (threads != 0 && threads != 256 && threads != 1024) return -1;
-    if (temp != 0.0f) for (int r = 0; r < rows; r++) if (!(u[r] >= 0.0 && u[r] < 1.0)) return -1;
-    struct Buffers {                                          // freed on every exit, including a CUDA failure thrown mid-way
-        void * p[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-        ~Buffers() { for (void * q : p) cudaFree(q); }
-    } d;
-    const size_t bytes = (size_t) rows * n * 4;
-    BARK_CUDA_CHECK(cudaMalloc(&d.p[0], bytes));
-    BARK_CUDA_CHECK(cudaMalloc(&d.p[1], (size_t) rows * sizeof(double)));
-    BARK_CUDA_CHECK(cudaMalloc(&d.p[2], (size_t) rows * 4));
-    BARK_CUDA_CHECK(cudaMalloc(&d.p[3], (size_t) rows * 4));
-    BARK_CUDA_CHECK(cudaMalloc(&d.p[4], (size_t) rows * 4));
-    float * dl = (float *) d.p[0], * deos = (float *) d.p[4]; double * du = (double *) d.p[1]; int32_t * dtok = (int32_t *) d.p[2], * dflags = (int32_t *) d.p[3];
-    BARK_CUDA_CHECK(cudaMemcpy(dl, logits, bytes, cudaMemcpyHostToDevice));
-    if (temp != 0.0f) BARK_CUDA_CHECK(cudaMemcpy(du, u, (size_t) rows * sizeof(double), cudaMemcpyHostToDevice));
-    BARK_CUDA_CHECK(cudaMemset(dtok, 0xff, (size_t) rows * 4));                 // -1 / NaN: a missing store shows up
-    BARK_CUDA_CHECK(cudaMemset(dflags, 0xff, (size_t) rows * 4));
-    BARK_CUDA_CHECK(cudaMemset(deos, 0xff, (size_t) rows * 4));
-    sample_rows(dl, n, n, rows, temp, du, dtok, 0, nullptr, deos, dflags, 0, threads, 0);
-    BARK_CUDA_CHECK(cudaGetLastError());                      // a launch the configuration rejects
-    const cudaError_t e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) { fprintf(stderr, "bark_b200_sample_given_u: %s\n", cudaGetErrorString(e)); return -1; }
-    BARK_CUDA_CHECK(cudaMemcpy(device_tokens, dtok, (size_t) rows * 4, cudaMemcpyDeviceToHost));
-    BARK_CUDA_CHECK(cudaMemcpy(flags, dflags, (size_t) rows * 4, cudaMemcpyDeviceToHost));
-    BARK_CUDA_CHECK(cudaMemcpy(eos_p, deos, (size_t) rows * 4, cudaMemcpyDeviceToHost));
-    int replays = 0;
-    for (int r = 0; r < rows; r++) {
-        tokens[r] = device_tokens[r];
-        if (!flags[r]) continue;
-        tokens[r] = sample_token_given_u(logits + (size_t) r * n, n, temp, temp != 0.0f ? u[r] : 0.0, &eos_p[r]);
-        replays++;
-    }
-    return replays;
-}
-extern "C" int bark_b200_sample_given_u(const float * logits, int n, int rows, float temp, const double * u, int threads, int32_t * tokens,
-                                        int32_t * device_tokens, int32_t * flags, float * eos_p) {
-    return guarded((int) -1, [&] { return bark_b200_sample_given_u_impl(logits, n, rows, temp, u, threads, tokens, device_tokens, flags, eos_p); });
-}
-
-// top-k / top-p settings: false with a message for anything the rule does not define
-static bool sampling_valid(const char * fn, const bark_b200_sampling & s) {
-    if (s.top_k < 0) { fprintf(stderr, "%s: top_k %d (0 for off, or k >= 1)\n", fn, s.top_k); return false; }
-    if (s.use_top_p && !(std::isfinite(s.top_p) && s.top_p >= 0.0f && s.top_p <= 1.0f)) { fprintf(stderr, "%s: top_p %g is not in [0, 1]\n", fn, (double) s.top_p); return false; }
-    return true;
-}
 
 extern "C" int bark_b200_set_sampling(struct bark_context * ctx, int stage, const struct bark_b200_sampling * s) {
     const char * fn = "bark_b200_set_sampling";
@@ -1187,205 +967,6 @@ extern "C" int bark_b200_set_sampling(struct bark_context * ctx, int stage, cons
     if (s && !sampling_valid(fn, *s)) return 0;
     ctx->sampling[stage] = s ? *s : bark_b200_sampling{0, 0, 1.0f};
     return 1;
-}
-
-// the device filter and sampler on host rows (tests): filter_rows_kernel, then sample_rows_kernel on its output, then every row either
-// kernel flags replayed on the host from the raw logits (filter_row_host, sample_token_given_u), as sample_and_replay does it
-static int bark_b200_sample_filtered_given_u_impl(const float * logits, int n, int rows, float temp, const bark_b200_sampling * s, const double * u, int threads,
-                                                  int32_t * tokens, int32_t * device_tokens, int32_t * flags, float * eos_p, int32_t * kept) {
-    if (!logits || !tokens || !device_tokens || !flags || !eos_p || (temp != 0.0f && !u)) return -1;
-    if (n < 2 || n > kSampleMaxLogits || rows < 1 || rows > 1024 || !std::isfinite(temp) || temp < 0.0f) return -1;
-    if (threads != 0 && threads != 256 && threads != 1024) return -1;
-    if (temp != 0.0f) for (int r = 0; r < rows; r++) if (!(u[r] >= 0.0 && u[r] < 1.0)) return -1;
-    const bark_b200_sampling f = s ? *s : bark_b200_sampling{0, 0, 1.0f};
-    if (!sampling_valid("bark_b200_sample_filtered_given_u", f)) return -1;
-    struct Buffers {                                          // freed on every exit, including a CUDA failure thrown mid-way
-        void * p[8] = {};
-        ~Buffers() { for (void * q : p) cudaFree(q); }
-    } d;
-    const size_t bytes = (size_t) rows * n * 4;
-    for (int i = 0; i < 2; i++) BARK_CUDA_CHECK(cudaMalloc(&d.p[i], bytes));
-    BARK_CUDA_CHECK(cudaMalloc(&d.p[2], (size_t) rows * sizeof(double)));
-    for (int i = 3; i < 8; i++) BARK_CUDA_CHECK(cudaMalloc(&d.p[i], (size_t) rows * 4));
-    float * dl = (float *) d.p[0], * dfilt = (float *) d.p[1], * deos = (float *) d.p[7]; double * du = (double *) d.p[2];
-    int32_t * dtok = (int32_t *) d.p[3], * dsflags = (int32_t *) d.p[4], * dfflags = (int32_t *) d.p[5], * dkept = (int32_t *) d.p[6];
-    BARK_CUDA_CHECK(cudaMemcpy(dl, logits, bytes, cudaMemcpyHostToDevice));
-    if (temp != 0.0f) BARK_CUDA_CHECK(cudaMemcpy(du, u, (size_t) rows * sizeof(double), cudaMemcpyHostToDevice));
-    for (int i = 3; i < 8; i++) BARK_CUDA_CHECK(cudaMemset(d.p[i], 0xff, (size_t) rows * 4));      // -1 / NaN: a missing store shows up
-    BARK_CUDA_CHECK(cudaMemset(dfflags, 0, (size_t) rows * 4));
-    const bool filtered = filter_on(f);
-    if (filtered) filter_rows(dl, n, n, rows, f, dfilt, dkept, dfflags, threads, 0);
-    sample_rows(filtered ? dfilt : dl, n, n, rows, temp, du, dtok, 0, nullptr, deos, dsflags, 0, threads, 0);
-    BARK_CUDA_CHECK(cudaGetLastError());                      // a launch the configuration rejects
-    const cudaError_t e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) { fprintf(stderr, "bark_b200_sample_filtered_given_u: %s\n", cudaGetErrorString(e)); return -1; }
-    std::vector<int32_t> sf((size_t) rows), ff((size_t) rows), kp((size_t) rows, n);
-    BARK_CUDA_CHECK(cudaMemcpy(device_tokens, dtok, (size_t) rows * 4, cudaMemcpyDeviceToHost));
-    BARK_CUDA_CHECK(cudaMemcpy(sf.data(), dsflags, (size_t) rows * 4, cudaMemcpyDeviceToHost));
-    BARK_CUDA_CHECK(cudaMemcpy(ff.data(), dfflags, (size_t) rows * 4, cudaMemcpyDeviceToHost));
-    BARK_CUDA_CHECK(cudaMemcpy(eos_p, deos, (size_t) rows * 4, cudaMemcpyDeviceToHost));
-    if (filtered) BARK_CUDA_CHECK(cudaMemcpy(kp.data(), dkept, (size_t) rows * 4, cudaMemcpyDeviceToHost));
-    int replays = 0;
-    std::vector<float> row;
-    for (int r = 0; r < rows; r++) {
-        tokens[r] = device_tokens[r];
-        flags[r] = (sf[(size_t) r] ? 1 : 0) | (ff[(size_t) r] ? 2 : 0);
-        if (kept) kept[r] = kp[(size_t) r];
-        if (!flags[r]) continue;
-        row.assign(logits + (size_t) r * n, logits + (size_t) (r + 1) * n);
-        if (filtered) filter_row_host(row.data(), n, f);
-        tokens[r] = sample_token_given_u(row.data(), n, temp, temp != 0.0f ? u[r] : 0.0, &eos_p[r]);
-        replays++;
-    }
-    return replays;
-}
-extern "C" int bark_b200_sample_filtered_given_u(const float * logits, int n, int rows, float temp, const struct bark_b200_sampling * s, const double * u,
-                                                 int threads, int32_t * tokens, int32_t * device_tokens, int32_t * flags, float * eos_p, int32_t * kept) {
-    return guarded((int) -1, [&] { return bark_b200_sample_filtered_given_u_impl(logits, n, rows, temp, s, u, threads, tokens, device_tokens, flags, eos_p, kept); });
-}
-
-// parity-path tiled GEMM on host buffers (tests, tools/gemm_bench.py): A [M][K] and W [N][K] go through permute_to_gm, as the loader
-// and the activation writers lay them out (row capacity and o_pad rounded up to the tallest / widest tile); the result comes back
-// row-major.  Every output region sits between guard bands and starts as NaN (RESID: as the residual from C).
-static int bark_b200_parity_gemm_impl(const void * A, const void * W, void * C, int M, int N, int K, int wtype, int epilogue, int variant,
-                                      const uint16_t * gelu_tab) {
-    if (!A || !W || !C || M < 1 || N < 1 || K < 32 || K % 32 || (wtype != W_F32 && wtype != W_F16) || variant < 0) return 0;
-    if (epilogue < EPI_STORE || epilogue > EPI_QKV || (epilogue == EPI_QKV && N % 3) || (epilogue == EPI_GELU_ACT && !gelu_tab)) return 0;
-    constexpr size_t kGuard = 4096;
-    constexpr unsigned char kPattern = 0x5a;
-    const size_t es = wtype == W_F16 ? 2 : 4;
-    const int rows_cap = (M + 31) / 32 * 32, o_pad = (N + kGemmOPad - 1) / kGemmOPad * kGemmOPad;
-    const size_t a_bytes = (size_t) gm_groups(K) * rows_cap * kGmGroup * es, w_bytes = (size_t) gm_groups(K) * o_pad * kGmGroup * es;
-    // output: STORE / RESID / QKV f32 [M][N] (QKV: Q, K, V blocks of [M][N/3] each); GELU_ACT: the group-major operand of the next mul_mat
-    const size_t out_bytes = epilogue == EPI_GELU_ACT ? (size_t) gm_groups(N) * rows_cap * kGmGroup * es : (size_t) M * N * 4;
-    struct Buffers {                                          // freed on every exit, including a CUDA failure thrown mid-way
-        void * p[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-        ~Buffers() { for (void * b : p) cudaFree(b); }
-    } d;
-    void *& d_rm = d.p[0], *& d_a = d.p[1], *& d_w = d.p[2], *& d_out = d.p[3], *& d_tab = d.p[4];
-    BARK_CUDA_CHECK(cudaMalloc(&d_rm, (size_t) std::max(M, N) * K * es));
-    BARK_CUDA_CHECK(cudaMalloc(&d_a, a_bytes)); BARK_CUDA_CHECK(cudaMalloc(&d_w, w_bytes));
-    BARK_CUDA_CHECK(cudaMemcpy(d_rm, A, (size_t) M * K * es, cudaMemcpyHostToDevice));
-    permute_to_gm(d_rm, d_a, M, rows_cap, K, (WType) wtype, 0);
-    BARK_CUDA_CHECK(cudaStreamSynchronize(0));
-    BARK_CUDA_CHECK(cudaMemcpy(d_rm, W, (size_t) N * K * es, cudaMemcpyHostToDevice));
-    permute_to_gm(d_rm, d_w, N, o_pad, K, (WType) wtype, 0);
-    BARK_CUDA_CHECK(cudaMalloc(&d_out, out_bytes + 2 * kGuard));
-    unsigned char * const reg = (unsigned char *) d_out;
-    BARK_CUDA_CHECK(cudaMemset(reg, kPattern, out_bytes + 2 * kGuard));
-    if (epilogue == EPI_RESID) BARK_CUDA_CHECK(cudaMemcpy(reg + kGuard, C, out_bytes, cudaMemcpyHostToDevice));
-    else                       BARK_CUDA_CHECK(cudaMemset(reg + kGuard, 0xff, out_bytes));
-    DMat dm; dm.n_out = N; dm.K = K; dm.type = (WType) wtype; dm.p_gm = d_w; dm.o_pad = o_pad;
-    MatmulEpilogue ep; ep.mode = epilogue;
-    float * const out = (float *)(reg + kGuard);
-    if (epilogue == EPI_STORE || epilogue == EPI_RESID) { ep.out = out; ep.ldo = N; }
-    else if (epilogue == EPI_QKV) { const int E = N / 3; ep.out = out; ep.k_out = out + (size_t) M * E; ep.v_out = out + 2 * (size_t) M * E; ep.ldo = E; }
-    else {
-        BARK_CUDA_CHECK(cudaMalloc(&d_tab, 65536 * 2));
-        BARK_CUDA_CHECK(cudaMemcpy(d_tab, gelu_tab, 65536 * 2, cudaMemcpyHostToDevice));
-        ep.act_out = out; ep.act_wt = wtype; ep.act_Kp = rows_cap * kGmGroup; ep.gelu_tab = (const __half *) d_tab;
-    }
-    const int ran = lane_gemm_tiled(dm, d_a, rows_cap * kGmGroup, M, ep, 0, variant);
-    BARK_CUDA_CHECK(cudaGetLastError());
-    const cudaError_t e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) { fprintf(stderr, "bark_b200_parity_gemm: %s\n", cudaGetErrorString(e)); return 0; }
-    if (!ran) return 0;
-    std::vector<unsigned char> h(out_bytes + 2 * kGuard);
-    BARK_CUDA_CHECK(cudaMemcpy(h.data(), reg, h.size(), cudaMemcpyDeviceToHost));
-    bool guards_intact = true;
-    for (size_t i = 0; i < kGuard; i++) guards_intact &= h[i] == kPattern && h[kGuard + out_bytes + i] == kPattern;
-    if (!guards_intact) { fprintf(stderr, "bark_b200_parity_gemm: a store landed outside the output (guard band overwritten)\n"); return -1; }
-    const unsigned char * o = h.data() + kGuard;
-    if (epilogue != EPI_GELU_ACT) memcpy(C, o, out_bytes);
-    else {                                                    // group-major -> row-major [M][N]
-        const size_t gs = (size_t) rows_cap * kGmGroup;
-        for (int m = 0; m < M; m++)
-            for (int k = 0; k < N; k++) memcpy((unsigned char *) C + ((size_t) m * N + k) * es, o + gm_offset(m, k, gs) * es, es);
-    }
-    return ran;
-}
-extern "C" int bark_b200_parity_gemm(const void * A, const void * W, void * C, int M, int N, int K, int wtype, int epilogue, int variant,
-                                     const uint16_t * gelu_tab) {
-    return guarded((int) 0, [&] { return bark_b200_parity_gemm_impl(A, W, C, M, N, K, wtype, epilogue, variant, gelu_tab); });
-}
-
-// quantised mat-muls on host buffers (tests): the weight rows arrive as the file's blocks and go through the loader's split (q4_split /
-// qx_split); the activation rows are f32, as store_act leaves them for a quantised model.  The q8 operand lives in this call's own
-// scratch: the calling thread's scratch pointers (a context's buffers) are put back on every exit.  The output sits between guard bands
-// and starts as NaN (RESID: as the residual from C).
-static int bark_b200_quant_matmul_impl(int wtype, const void * W, const float * A, float * C, int M, int N, int K, int epilogue, int path,
-                                       const uint16_t * gelu_tab, int8_t * q_out, float * d_out, float * s_out) {
-    const WType t = (WType) wtype;
-    if (!W || !A || !C || M < 1 || N < 1 || K < 32 || K % 32 || (t != W_Q4_0 && !qx_supported(t)) || path < 0 || path > 2) return 0;
-    if (epilogue < EPI_STORE || epilogue > EPI_QKV || (epilogue == EPI_QKV && N % 3) || (epilogue == EPI_GELU_ACT && !gelu_tab)) return 0;
-    const bool q81 = t == W_Q4_1 || t == W_Q5_1;
-    if ((path != 0 && (t != W_Q4_0 || M != 1 || K > 4096)) || (s_out && !q81)) return 0;
-    constexpr size_t kGuard = 4096;
-    constexpr unsigned char kPattern = 0x5a;
-    const int nb = K / 32;
-    const size_t n_blocks = (size_t) N * nb, raw_bytes = n_blocks * (t == W_Q4_0 ? 18 : qx_block_bytes(t)), out_bytes = (size_t) M * N * 4;
-    struct Scratch {                                          // the calling thread's q8 scratch, restored on every exit
-        void * q4[2], * qx[3];
-        Scratch() { q4_get_scratch(&q4[0], &q4[1]); qx_get_scratch(&qx[0], &qx[1], &qx[2]); }
-        ~Scratch() { q4_set_scratch(q4[0], q4[1]); qx_set_scratch(qx[0], qx[1], qx[2]); }
-    } keep;
-    struct Buffers {                                          // freed on every exit, including a CUDA failure thrown mid-way
-        void * p[11] = {};
-        ~Buffers() { for (void * b : p) cudaFree(b); }
-    } d;
-    void *& d_raw = d.p[0], *& d_qs = d.p[1], *& d_sc = d.p[2], *& d_min = d.p[3], *& d_qh = d.p[4], *& d_a = d.p[5], *& d_q8 = d.p[6], *& d_q8d = d.p[7],
-         *& d_q8s = d.p[8], *& d_c = d.p[9], *& d_tab = d.p[10];
-    BARK_CUDA_CHECK(cudaMalloc(&d_raw, raw_bytes));
-    BARK_CUDA_CHECK(cudaMemcpy(d_raw, W, raw_bytes, cudaMemcpyHostToDevice));
-    BARK_CUDA_CHECK(cudaMalloc(&d_qs, n_blocks * (t == W_Q8_0 ? 32 : 16))); BARK_CUDA_CHECK(cudaMalloc(&d_sc, n_blocks * 2));
-    DMat dm; dm.n_out = N; dm.K = K; dm.Kp = K; dm.type = t; dm.p = d_qs; dm.scales = d_sc;
-    if (t == W_Q4_0) q4_split(d_raw, n_blocks, d_qs, d_sc, 0);
-    else {
-        BARK_CUDA_CHECK(cudaMalloc(&d_min, n_blocks * 2)); BARK_CUDA_CHECK(cudaMalloc(&d_qh, n_blocks * 4));
-        dm.mins = d_min; dm.qh = d_qh;
-        qx_split(d_raw, n_blocks, t, d_qs, d_qh, d_sc, d_min, 0);
-    }
-    BARK_CUDA_CHECK(cudaMalloc(&d_a, (size_t) M * K * 4));
-    BARK_CUDA_CHECK(cudaMemcpy(d_a, A, (size_t) M * K * 4, cudaMemcpyHostToDevice));
-    BARK_CUDA_CHECK(cudaMalloc(&d_q8, (size_t) M * K)); BARK_CUDA_CHECK(cudaMalloc(&d_q8d, (size_t) M * nb * 4));
-    BARK_CUDA_CHECK(cudaMalloc(&d_q8s, (size_t) M * nb * 4));
-    BARK_CUDA_CHECK(cudaMalloc(&d_c, out_bytes + 2 * kGuard));
-    unsigned char * const reg = (unsigned char *) d_c;
-    BARK_CUDA_CHECK(cudaMemset(reg, kPattern, out_bytes + 2 * kGuard));
-    if (epilogue == EPI_RESID) BARK_CUDA_CHECK(cudaMemcpy(reg + kGuard, C, out_bytes, cudaMemcpyHostToDevice));
-    else                       BARK_CUDA_CHECK(cudaMemset(reg + kGuard, 0xff, out_bytes));
-    MatmulEpilogue ep; ep.mode = epilogue;
-    float * const out = (float *)(reg + kGuard);
-    if (epilogue == EPI_STORE || epilogue == EPI_RESID) { ep.out = out; ep.ldo = N; }
-    else if (epilogue == EPI_QKV) { const int E = N / 3; ep.out = out; ep.k_out = out + (size_t) M * E; ep.v_out = out + 2 * (size_t) M * E; ep.ldo = E; }
-    else {                                                    // f32 rows, as a quantised model's fc pass leaves its operand
-        BARK_CUDA_CHECK(cudaMalloc(&d_tab, 65536 * 2));
-        BARK_CUDA_CHECK(cudaMemcpy(d_tab, gelu_tab, 65536 * 2, cudaMemcpyHostToDevice));
-        ep.act_out = out; ep.act_wt = W_Q4_0; ep.act_Kp = N; ep.gelu_tab = (const __half *) d_tab;
-    }
-    if (path == 0) {
-        q4_set_scratch(d_q8, d_q8d); qx_set_scratch(d_q8, d_q8d, d_q8s);
-        lane_matmul(dm, d_a, K, M, ep, 0);
-    } else {
-        decode_q4_rows(path == 1, (const float *) d_a, K, d_qs, d_sc, N, ep, (int8_t *) d_q8, (float *) d_q8d, 0);
-    }
-    BARK_CUDA_CHECK(cudaGetLastError());
-    const cudaError_t e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) { fprintf(stderr, "bark_b200_quant_matmul: %s\n", cudaGetErrorString(e)); return 0; }
-    std::vector<unsigned char> h(out_bytes + 2 * kGuard);
-    BARK_CUDA_CHECK(cudaMemcpy(h.data(), reg, h.size(), cudaMemcpyDeviceToHost));
-    bool guards_intact = true;
-    for (size_t i = 0; i < kGuard; i++) guards_intact &= h[i] == kPattern && h[kGuard + out_bytes + i] == kPattern;
-    if (!guards_intact) { fprintf(stderr, "bark_b200_quant_matmul: a store landed outside the output (guard band overwritten)\n"); return -1; }
-    memcpy(C, h.data() + kGuard, out_bytes);
-    if (q_out) BARK_CUDA_CHECK(cudaMemcpy(q_out, d_q8, (size_t) M * K, cudaMemcpyDeviceToHost));
-    if (d_out) BARK_CUDA_CHECK(cudaMemcpy(d_out, d_q8d, (size_t) M * nb * 4, cudaMemcpyDeviceToHost));
-    if (s_out) BARK_CUDA_CHECK(cudaMemcpy(s_out, d_q8s, (size_t) M * nb * 4, cudaMemcpyDeviceToHost));
-    return 1;
-}
-extern "C" int bark_b200_quant_matmul(int wtype, const void * W, const float * A, float * C, int M, int N, int K, int epilogue, int path,
-                                      const uint16_t * gelu_tab, int8_t * q, float * d, float * s) {
-    return guarded((int) 0, [&] { return bark_b200_quant_matmul_impl(wtype, W, A, C, M, N, K, epilogue, path, gelu_tab, q, d, s); });
 }
 
 // batched generation (include/bark_b200.h)

@@ -145,6 +145,8 @@ void sample_rows(const float * logits, int ld, int n, int rows, float temp, cons
 int32_t sample_token_given_u(const float * logits, int n, float temp, double u, float * eos_p);
 // top-k / top-p (DESIGN.md §14): on when top_k >= 1 or use_top_p
 inline bool filter_on(const bark_b200_sampling & f) { return f.top_k > 0 || f.use_top_p != 0; }
+// top-k / top-p settings: false with a message naming `fn` for anything the rule does not define
+bool sampling_valid(const char * fn, const bark_b200_sampling & s);
 constexpr int kMaxFilterRows = 8;                // rows filtered at once: one decode step of a batch
 // filter_rows_kernel over `rows` rows of n <= kSampleMaxLogits raw logits (stride ld): d_out [rows][n] gets each row with the removed
 // logits set to -inf, d_kept (may be null) the number kept, d_flags 1 where the device cannot decide the row exactly (a NaN, a

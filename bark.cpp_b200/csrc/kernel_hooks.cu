@@ -1,0 +1,339 @@
+// Kernel paths on host buffers (include/bark_b200.h), for the tests and the tools/ benchmarks: each entry point checks its arguments,
+// uploads them, runs one kernel path on the default stream, waits for it and copies the result back.  None touches a bark_context.
+#include "../../include/bark_b200.h"
+#include "context.h"
+#include "codec_kernels.h"
+#include "gpt_kernels.h"
+
+#include <algorithm>
+#include <cmath>
+#include <cstring>
+#include <optional>
+#include <vector>
+
+using namespace bark;
+
+namespace {
+
+// Every device allocation of one call, freed on every exit, including a CUDA failure thrown mid-way
+struct DeviceBuffers {
+    std::vector<void *> p;
+    ~DeviceBuffers() { for (void * q : p) cudaFree(q); }
+    template <typename T = void> T * alloc(size_t bytes) {
+        p.push_back(nullptr);
+        BARK_CUDA_CHECK(cudaMalloc(&p.back(), bytes));
+        return (T *) p.back();
+    }
+    template <typename T> T * upload(const T * host, size_t bytes) {
+        T * d = alloc<T>(bytes);
+        BARK_CUDA_CHECK(cudaMemcpy(d, host, bytes, cudaMemcpyHostToDevice));
+        return d;
+    }
+    template <typename T> T * poisoned(size_t bytes) {                 // 0xff bytes (-1 / NaN): a missing store shows up
+        T * d = alloc<T>(bytes);
+        BARK_CUDA_CHECK(cudaMemset(d, 0xff, bytes));
+        return d;
+    }
+};
+
+void download(void * host, const void * dev, size_t bytes) { BARK_CUDA_CHECK(cudaMemcpy(host, dev, bytes, cudaMemcpyDeviceToHost)); }
+
+constexpr size_t kGuard = 4096;                 // bytes of kPattern on each side of a guarded output
+constexpr unsigned char kPattern = 0x5a;
+
+// `bytes` of device output between two guard bands that are checked after the kernel, so a stray store shows up.  The output starts
+// as NaN, or for the RESID epilogues as the residual at `resid` (host), which the kernel adds to.
+struct GuardedOutput {
+    unsigned char * base; size_t bytes;
+    GuardedOutput(DeviceBuffers & mem, size_t bytes, const void * resid) : base(mem.alloc<unsigned char>(bytes + 2 * kGuard)), bytes(bytes) {
+        BARK_CUDA_CHECK(cudaMemset(base, kPattern, bytes + 2 * kGuard));
+        if (resid) BARK_CUDA_CHECK(cudaMemcpy(base + kGuard, resid, bytes, cudaMemcpyHostToDevice));
+        else       BARK_CUDA_CHECK(cudaMemset(base + kGuard, 0xff, bytes));
+    }
+    template <typename T> T * out() const { return (T *)(base + kGuard); }
+    // copies the output to `dst` (host); false, with a message naming `fn`, when a store landed in either band
+    bool read(const char * fn, void * dst) const {
+        std::vector<unsigned char> h(bytes + 2 * kGuard);
+        download(h.data(), base, h.size());
+        memcpy(dst, h.data() + kGuard, bytes);
+        for (size_t i = 0; i < kGuard; i++)
+            if (h[i] != kPattern || h[kGuard + bytes + i] != kPattern) {
+                fprintf(stderr, "%s: a store landed outside the output (guard band overwritten)\n", fn);
+                return false;
+            }
+        return true;
+    }
+};
+
+// After the launches: a launch the configuration rejects is thrown (the entry point's failure value); a fault while the kernels ran
+// is reported under `fn`.  True when the call's work completed.
+bool finish(const char * fn) {
+    BARK_CUDA_CHECK(cudaGetLastError());
+    const cudaError_t e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) fprintf(stderr, "%s: %s\n", fn, cudaGetErrorString(e));
+    return e == cudaSuccess;
+}
+
+int sm_count() {
+    int dev = 0, n_sm = 0;
+    BARK_CUDA_CHECK(cudaGetDevice(&dev)); BARK_CUDA_CHECK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
+    return n_sm;
+}
+
+// The epilogue of a parity-path or quantised mat-mul into `out`: rows [M][N] (STORE / RESID), Q, K and V blocks of [M][N/3] (QKV), or
+// GELU through gelu_tab (host, 65536 f16) into the next mat-mul's operand of type act_wt and group stride act_Kp (GELU_ACT).
+MatmulEpilogue matmul_epilogue(DeviceBuffers & mem, int mode, float * out, int M, int N, const uint16_t * gelu_tab, int act_wt, int act_Kp) {
+    MatmulEpilogue ep; ep.mode = mode;
+    if (mode == EPI_STORE || mode == EPI_RESID) { ep.out = out; ep.ldo = N; }
+    else if (mode == EPI_QKV) { const int E = N / 3; ep.out = out; ep.k_out = out + (size_t) M * E; ep.v_out = out + 2 * (size_t) M * E; ep.ldo = E; }
+    else { ep.act_out = out; ep.act_wt = act_wt; ep.act_Kp = act_Kp; ep.gelu_tab = mem.upload((const __half *) gelu_tab, 65536 * 2); }
+    return ep;
+}
+
+// The device filter and sampler on host rows with the uniforms given: filter_rows_kernel when the filter is on, then
+// sample_rows_kernel at the instantiation asked for, then every row either kernel flags replayed on the host from the raw logits
+// (filter_row_host, sample_token_given_u), as sample_and_replay does it.  device_tokens keeps the sampler's tokens before the replay;
+// flags has bit 0 for the sampler and bit 1 for the filter; kept (may be null) gets the logits the filter kept, n without a filter.
+int sample_given_u(const char * fn, const float * logits, int n, int rows, float temp, const bark_b200_sampling * s, const double * u, int threads,
+                   int32_t * tokens, int32_t * device_tokens, int32_t * flags, float * eos_p, int32_t * kept) {
+    if (!logits || !tokens || !device_tokens || !flags || !eos_p || (temp != 0.0f && !u)) return -1;
+    if (n < 2 || n > kSampleMaxLogits || rows < 1 || rows > 1024 || !std::isfinite(temp) || temp < 0.0f) return -1;
+    if (threads != 0 && threads != 256 && threads != 1024) return -1;
+    if (temp != 0.0f) for (int r = 0; r < rows; r++) if (!(u[r] >= 0.0 && u[r] < 1.0)) return -1;
+    const bark_b200_sampling f = s ? *s : bark_b200_sampling{0, 0, 1.0f};
+    if (!sampling_valid(fn, f)) return -1;
+    const bool filtered = filter_on(f);
+    DeviceBuffers mem;
+    const size_t bytes = (size_t) rows * n * 4, rb = (size_t) rows * 4;
+    const float * dl = mem.upload(logits, bytes);
+    const double * du = temp != 0.0f ? mem.upload(u, (size_t) rows * sizeof(double)) : nullptr;
+    int32_t * dtok = mem.poisoned<int32_t>(rb), * dsflags = mem.poisoned<int32_t>(rb);
+    float * deos = mem.poisoned<float>(rb);
+    float * dfilt = nullptr; int32_t * dkept = nullptr, * dfflags = nullptr;
+    if (filtered) {
+        dfilt = mem.alloc<float>(bytes); dkept = mem.poisoned<int32_t>(rb); dfflags = mem.poisoned<int32_t>(rb);
+        filter_rows(dl, n, n, rows, f, dfilt, dkept, dfflags, threads, 0);
+    }
+    sample_rows(filtered ? dfilt : dl, n, n, rows, temp, du, dtok, 0, nullptr, deos, dsflags, 0, threads, 0);
+    if (!finish(fn)) return -1;
+    std::vector<int32_t> ff((size_t) rows, 0);
+    download(device_tokens, dtok, rb); download(flags, dsflags, rb); download(eos_p, deos, rb);
+    if (filtered) download(ff.data(), dfflags, rb);
+    if (kept && filtered) download(kept, dkept, rb);
+    else if (kept) std::fill(kept, kept + rows, n);
+    int replays = 0;
+    std::vector<float> row;
+    for (int r = 0; r < rows; r++) {
+        tokens[r] = device_tokens[r];
+        flags[r] = (flags[r] ? 1 : 0) | (ff[(size_t) r] ? 2 : 0);
+        if (!flags[r]) continue;
+        row.assign(logits + (size_t) r * n, logits + (size_t) (r + 1) * n);
+        if (filtered) filter_row_host(row.data(), n, f);
+        tokens[r] = sample_token_given_u(row.data(), n, temp, temp != 0.0f ? u[r] : 0.0, &eos_p[r]);
+        replays++;
+    }
+    return replays;
+}
+
+}  // namespace
+
+// the RVQ encode kernel: norms from rvq_norms_kernel, codes [n_q][T] from rvq_encode_kernel
+extern "C" int bark_b200_rvq_encode(const float * latent, int T, const float * codebooks, int hidden, int n_bins, int n_q, int32_t * codes) {
+    return guarded(0, [&] {
+        if (!latent || !codebooks || !codes || T < 1 || hidden < 32 || hidden > 128 || hidden % 32 || n_bins < 1 || n_bins > 1024 || n_q < 1 || n_q > kMaxCodebooks) return 0;
+        DeviceBuffers mem;
+        const size_t n_cw = (size_t) n_q * n_bins;
+        const float * dl = mem.upload(latent, (size_t) hidden * T * 4), * dcb = mem.upload(codebooks, n_cw * hidden * 4);
+        float * dn = mem.alloc<float>(n_cw * 4);
+        int32_t * dc = mem.poisoned<int32_t>((size_t) n_q * T * 4);
+        const float * emb[kMaxCodebooks], * nrm[kMaxCodebooks];
+        for (int q = 0; q < n_q; q++) {
+            emb[q] = dcb + (size_t) q * n_bins * hidden; nrm[q] = dn + (size_t) q * n_bins;
+            rvq_norms(emb[q], n_bins, hidden, dn + (size_t) q * n_bins, 0);
+        }
+        if (!rvq_encode(emb, nrm, n_q, n_bins, hidden, dl, T, dc, 0) || !finish("bark_b200_rvq_encode")) return 0;
+        download(codes, dc, (size_t) n_q * T * 4);
+        return 1;
+    });
+}
+
+// fast mode: C = A[M][K] W[N][K]^T through one of the fine pass's GEMM epilogues, and attention over [n][E] f16 q / k / v
+extern "C" int bark_b200_fast_gemm(const uint16_t * A, const uint16_t * W, void * C, int M, int N, int K, int epilogue, int bn) {
+    return guarded(0, [&] {
+        if (!A || !W || !C || M < 1 || N < 1 || K < 64 || K % 64) return 0;
+        if (epilogue != FEPI_F32 && epilogue != FEPI_RESID && epilogue != FEPI_GELU16 && epilogue != FEPI_QKV16) return 0;
+        if (epilogue == FEPI_QKV16 && N % 6) return 0;
+        DeviceBuffers mem;
+        const __half * dA = mem.upload((const __half *) A, (size_t) M * K * 2), * dW = mem.upload((const __half *) W, (size_t) N * K * 2);
+        const bool qkv = epilogue == FEPI_QKV16;
+        // output regions in the order they are laid out in C: [M][N] f32 or f16; QKV16: Q|K [M][2N/3] f16, then V^T [N/3][M] f16
+        const GuardedOutput c(mem, qkv ? (size_t) M * (2 * N / 3) * 2 : (size_t) M * N * (epilogue == FEPI_GELU16 ? 2 : 4), epilogue == FEPI_RESID ? C : nullptr);
+        std::optional<GuardedOutput> vt;
+        FastEpi ep; ep.mode = epilogue; ep.ldo = N;
+        if (epilogue == FEPI_F32 || epilogue == FEPI_RESID) ep.out32 = c.out<float>();
+        else                                                ep.out16 = c.out<__half>();
+        if (qkv) {                                                     // the fine pass's arguments
+            vt.emplace(mem, (size_t) M * (N / 3) * 2, nullptr);
+            ep.ldo = 2 * N / 3; ep.vt = vt->out<__half>(); ep.vt_ld = M; ep.v_col0 = 2 * N / 3;
+        }
+        const int ran = fast_gemm(dA, K, dW, K, M, N, K, ep, sm_count(), bn, 0);
+        if (!finish("bark_b200_fast_gemm") || !ran) return 0;
+        if (!c.read("bark_b200_fast_gemm", C) || (vt && !vt->read("bark_b200_fast_gemm", (unsigned char *) C + c.bytes))) return -1;
+        return ran;
+    });
+}
+
+extern "C" int bark_b200_fast_attention(const uint16_t * q, const uint16_t * k, const uint16_t * v, uint16_t * out, int n, int E, int H) {
+    return guarded(0, [&] {
+        if (!q || !k || !v || !out || n < 128 || n % 128 || E != H * 64) return 0;
+        std::vector<uint16_t> qk((size_t) n * 2 * E), vt((size_t) E * n);
+        for (int r = 0; r < n; r++) {
+            memcpy(&qk[(size_t) r * 2 * E], q + (size_t) r * E, (size_t) E * 2); memcpy(&qk[(size_t) r * 2 * E + E], k + (size_t) r * E, (size_t) E * 2);
+            for (int c = 0; c < E; c++) vt[(size_t) c * n + r] = v[(size_t) r * E + c];
+        }
+        DeviceBuffers mem;
+        const __half * dqk = mem.upload((const __half *) qk.data(), qk.size() * 2), * dvt = mem.upload((const __half *) vt.data(), vt.size() * 2);
+        __half * dout = mem.alloc<__half>((size_t) n * E * 2);
+        const bool ok = fast_attention(dqk, 2 * E, E, dvt, n, E, H, dout, 0);
+        if (!finish("bark_b200_fast_attention") || !ok) return 0;
+        download(out, dout, (size_t) n * E * 2);
+        return 1;
+    });
+}
+
+// parity-path attention on f32 rows (tools/attn_bench.py too): the result is written as f32 rows [N][E], the operand form store_act
+// produces for quantised weights.  path: 0 = as attention() chooses for this shape, 1 = attn_fused_kernel, 2 = three kernels.
+extern "C" int bark_b200_parity_attention(const float * q, const float * k, const float * v, float * out, int N, int n_kv, int n_past, int E, int H, int causal,
+                                          int path) {
+    return guarded(0, [&] {
+        if (!q || !k || !v || !out || N < 1 || n_kv < 1 || n_kv > 1024 || n_past < 0 || H < 1 || E % H || path < 0 || path > 2) return 0;
+        const int D = E / H;
+        if (D % 32 || D > 128) return 0;
+        // the three kernels' row limit is the score buffer's, which this call sizes itself
+        if (path == ATTN_TILED && N > attn_tiled_max_rows(H, sm_count())) return 0;
+        DeviceBuffers mem;
+        const size_t q_bytes = (size_t) N * E * 4, kv_bytes = (size_t) n_kv * E * 4;
+        const float * dq = mem.upload(q, q_bytes), * dk = mem.upload(k, kv_bytes), * dv = mem.upload(v, kv_bytes);
+        float * dout = mem.poisoned<float>(q_bytes), * dsc = mem.alloc<float>((size_t) H * N * n_kv * 4);
+        attention(dq, dk, dv, N, n_kv, n_past, E, H, causal != 0, dsc, dout, W_Q4_0, E, 0, (AttnPath) path);
+        if (!finish("bark_b200_parity_attention")) return 0;
+        download(out, dout, q_bytes);
+        return 1;
+    });
+}
+
+// the parity path's row reductions: op 0 LayerNorm, op 1 soft_max; impl 0 the multi-row kernels (layernorm_act_kernel writing plain
+// f32 rows, softmax_row), impl 1 the decode kernels' block_layernorm / softmax_exp_rcp
+extern "C" int bark_b200_parity_rows(int op, int impl, const float * x, int rows, int n, const float * g, const float * b, float * out, unsigned * replays) {
+    return guarded(0, [&] {
+        if (!x || !out || !replays || op < 0 || op > 1 || impl < 0 || impl > 1 || rows < 1 || n < 1 || n > 1024 || (op == 0 && !g)) return 0;
+        DeviceBuffers mem;
+        const size_t bytes = (size_t) rows * n * 4;
+        const float * dx = mem.upload(x, bytes);
+        const float * dg = op == 0 ? mem.upload(g, (size_t) n * 4) : nullptr, * db = op == 0 && b ? mem.upload(b, (size_t) n * 4) : nullptr;
+        float * dout = mem.poisoned<float>(bytes);
+        unsigned * dcnt = mem.alloc<unsigned>(2 * sizeof(unsigned));
+        BARK_CUDA_CHECK(cudaMemset(dcnt, 0, 2 * sizeof(unsigned)));
+        if (impl == 1)    decode_rows(op, dx, rows, n, dg, db, dout, dcnt, 0);
+        else if (op == 0) layernorm_act(dx, rows, n, dg, db, dout, W_Q4_0, n, dcnt, 0);
+        else {            BARK_CUDA_CHECK(cudaMemcpy(dout, dx, bytes, cudaMemcpyDeviceToDevice)); softmax_rows(dout, rows, n, dcnt, 0); }
+        if (!finish("bark_b200_parity_rows")) return 0;
+        unsigned cnt[2];
+        download(cnt, dcnt, sizeof(cnt));
+        download(out, dout, bytes);
+        *replays = cnt[0] + cnt[1];
+        return 1;
+    });
+}
+
+// the device sampler, without and with the top-k / top-p filter (sample_given_u above)
+extern "C" int bark_b200_sample_given_u(const float * logits, int n, int rows, float temp, const double * u, int threads, int32_t * tokens,
+                                        int32_t * device_tokens, int32_t * flags, float * eos_p) {
+    return guarded(-1, [&] {
+        return sample_given_u("bark_b200_sample_given_u", logits, n, rows, temp, nullptr, u, threads, tokens, device_tokens, flags, eos_p, nullptr);
+    });
+}
+extern "C" int bark_b200_sample_filtered_given_u(const float * logits, int n, int rows, float temp, const struct bark_b200_sampling * s, const double * u,
+                                                 int threads, int32_t * tokens, int32_t * device_tokens, int32_t * flags, float * eos_p, int32_t * kept) {
+    return guarded(-1, [&] {
+        return sample_given_u("bark_b200_sample_filtered_given_u", logits, n, rows, temp, s, u, threads, tokens, device_tokens, flags, eos_p, kept);
+    });
+}
+
+// parity-path tiled GEMM (tools/gemm_bench.py too): A [M][K] and W [N][K] go through permute_to_gm, as the loader and the activation
+// writers lay them out (row capacity and o_pad rounded up to the tallest / widest tile); the result comes back row-major.
+extern "C" int bark_b200_parity_gemm(const void * A, const void * W, void * C, int M, int N, int K, int wtype, int epilogue, int variant,
+                                     const uint16_t * gelu_tab) {
+    return guarded(0, [&] {
+        if (!A || !W || !C || M < 1 || N < 1 || K < 32 || K % 32 || (wtype != W_F32 && wtype != W_F16) || variant < 0) return 0;
+        if (epilogue < EPI_STORE || epilogue > EPI_QKV || (epilogue == EPI_QKV && N % 3) || (epilogue == EPI_GELU_ACT && !gelu_tab)) return 0;
+        const size_t es = wtype == W_F16 ? 2 : 4;
+        const int rows_cap = (M + 31) / 32 * 32, o_pad = (N + kGemmOPad - 1) / kGemmOPad * kGemmOPad;
+        DeviceBuffers mem;
+        void * d_a = mem.alloc((size_t) gm_groups(K) * rows_cap * kGmGroup * es), * d_w = mem.alloc((size_t) gm_groups(K) * o_pad * kGmGroup * es);
+        permute_to_gm(mem.upload(A, (size_t) M * K * es), d_a, M, rows_cap, K, (WType) wtype, 0);
+        permute_to_gm(mem.upload(W, (size_t) N * K * es), d_w, N, o_pad, K, (WType) wtype, 0);
+        // output: STORE / RESID / QKV f32 [M][N] (QKV: Q, K, V blocks of [M][N/3] each); GELU_ACT: the group-major operand of the next mul_mat
+        const bool gm = epilogue == EPI_GELU_ACT;
+        const GuardedOutput c(mem, gm ? (size_t) gm_groups(N) * rows_cap * kGmGroup * es : (size_t) M * N * 4, epilogue == EPI_RESID ? C : nullptr);
+        DMat dm; dm.n_out = N; dm.K = K; dm.type = (WType) wtype; dm.p_gm = d_w; dm.o_pad = o_pad;
+        const MatmulEpilogue ep = matmul_epilogue(mem, epilogue, c.out<float>(), M, N, gelu_tab, wtype, rows_cap * kGmGroup);
+        const int ran = lane_gemm_tiled(dm, d_a, rows_cap * kGmGroup, M, ep, 0, variant);
+        if (!finish("bark_b200_parity_gemm") || !ran) return 0;
+        std::vector<unsigned char> h(gm ? c.bytes : 0);
+        if (!c.read("bark_b200_parity_gemm", gm ? h.data() : C)) return -1;
+        if (gm) {                                                      // group-major -> row-major [M][N]
+            const size_t gs = (size_t) rows_cap * kGmGroup;
+            for (int m = 0; m < M; m++)
+                for (int k = 0; k < N; k++) memcpy((unsigned char *) C + ((size_t) m * N + k) * es, h.data() + gm_offset(m, k, gs) * es, es);
+        }
+        return ran;
+    });
+}
+
+// quantised mat-muls: the weight rows arrive as the file's blocks and go through the loader's split (q4_split / qx_split); the
+// activation rows are f32, as store_act leaves them for a quantised model.  The q8 operand lives in this call's own scratch: the
+// calling thread's scratch pointers (a context's buffers) are put back on every exit.
+extern "C" int bark_b200_quant_matmul(int wtype, const void * W, const float * A, float * C, int M, int N, int K, int epilogue, int path,
+                                      const uint16_t * gelu_tab, int8_t * q_out, float * d_out, float * s_out) {
+    return guarded(0, [&] {
+        const WType t = (WType) wtype;
+        if (!W || !A || !C || M < 1 || N < 1 || K < 32 || K % 32 || (t != W_Q4_0 && !qx_supported(t)) || path < 0 || path > 2) return 0;
+        if (epilogue < EPI_STORE || epilogue > EPI_QKV || (epilogue == EPI_QKV && N % 3) || (epilogue == EPI_GELU_ACT && !gelu_tab)) return 0;
+        const bool q81 = t == W_Q4_1 || t == W_Q5_1;
+        if ((path != 0 && (t != W_Q4_0 || M != 1 || K > 4096)) || (s_out && !q81)) return 0;
+        struct Scratch {                                               // the calling thread's q8 scratch, restored on every exit
+            void * q4[2], * qx[3];
+            Scratch() { q4_get_scratch(&q4[0], &q4[1]); qx_get_scratch(&qx[0], &qx[1], &qx[2]); }
+            ~Scratch() { q4_set_scratch(q4[0], q4[1]); qx_set_scratch(qx[0], qx[1], qx[2]); }
+        } keep;
+        const int nb = K / 32;
+        const size_t n_blocks = (size_t) N * nb;
+        DeviceBuffers mem;
+        const void * d_raw = mem.upload(W, n_blocks * (t == W_Q4_0 ? 18 : qx_block_bytes(t)));
+        DMat dm; dm.n_out = N; dm.K = K; dm.Kp = K; dm.type = t; dm.p = mem.alloc(n_blocks * (t == W_Q8_0 ? 32 : 16)); dm.scales = mem.alloc(n_blocks * 2);
+        if (t == W_Q4_0) q4_split(d_raw, n_blocks, dm.p, dm.scales, 0);
+        else {
+            dm.mins = mem.alloc(n_blocks * 2); dm.qh = mem.alloc(n_blocks * 4);
+            qx_split(d_raw, n_blocks, t, dm.p, dm.qh, dm.scales, dm.mins, 0);
+        }
+        const float * d_a = mem.upload(A, (size_t) M * K * 4);
+        int8_t * d_q8 = mem.alloc<int8_t>((size_t) M * K);
+        float * d_q8d = mem.alloc<float>((size_t) M * nb * 4), * d_q8s = mem.alloc<float>((size_t) M * nb * 4);
+        const GuardedOutput c(mem, (size_t) M * N * 4, epilogue == EPI_RESID ? C : nullptr);
+        // GELU_ACT: f32 rows, as a quantised model's fc pass leaves its operand
+        const MatmulEpilogue ep = matmul_epilogue(mem, epilogue, c.out<float>(), M, N, gelu_tab, W_Q4_0, N);
+        if (path == 0) {
+            q4_set_scratch(d_q8, d_q8d); qx_set_scratch(d_q8, d_q8d, d_q8s);
+            lane_matmul(dm, d_a, K, M, ep, 0);
+        } else {
+            decode_q4_rows(path == 1, d_a, K, dm.p, dm.scales, N, ep, d_q8, d_q8d, 0);
+        }
+        if (!finish("bark_b200_quant_matmul")) return 0;
+        if (!c.read("bark_b200_quant_matmul", C)) return -1;
+        if (q_out) download(q_out, d_q8, (size_t) M * K);
+        if (d_out) download(d_out, d_q8d, (size_t) M * nb * 4);
+        if (s_out) download(s_out, d_q8s, (size_t) M * nb * 4);
+        return 1;
+    });
+}

@@ -265,6 +265,12 @@ __global__ void __launch_bounds__(kThreads, 1) filter_rows_kernel(const float * 
     if (tid == 0) { flags[blockIdx.x] = s_amb; if (kept) kept[blockIdx.x] = K; }
 }
 
+bool sampling_valid(const char * fn, const bark_b200_sampling & s) {
+    if (s.top_k < 0) { fprintf(stderr, "%s: top_k %d (0 for off, or k >= 1)\n", fn, s.top_k); return false; }
+    if (s.use_top_p && !(std::isfinite(s.top_p) && s.top_p >= 0.0f && s.top_p <= 1.0f)) { fprintf(stderr, "%s: top_p %g is not in [0, 1]\n", fn, (double) s.top_p); return false; }
+    return true;
+}
+
 static int filter_sort_width(int n) { int P = 2; while (P < n) P <<= 1; return P; }
 
 void filter_rows(const float * logits, int ld, int n, int rows, const bark_b200_sampling & f, float * d_out, int32_t * d_kept, int32_t * d_flags, int threads,
