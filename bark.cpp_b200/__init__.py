@@ -111,7 +111,7 @@ EXPORTS = [
     "bark_b200_fast_mode", "bark_b200_fast_gemm", "bark_b200_fast_attention", "bark_b200_parity_attention", "bark_b200_parity_gemm",
     "bark_b200_parity_rows", "bark_b200_sample_given_u", "bark_b200_generate_batch", "bark_b200_batch_audio", "bark_b200_batch_tokens", "bark_b200_gpt_eval_slot", "bark_b200_gpt_step_batch",
     "bark_b200_set_history_prompt", "bark_b200_generate_batch_prompted", "bark_b200_set_sampling", "bark_b200_sample_filtered_given_u",
-    "bark_b200_quant_matmul",
+    "bark_b200_quant_matmul", "bark_b200_fast_convert",
     "ggml_time_init", "ggml_time_us", "ggml_time_ms", "ggml_init", "ggml_free",
 ]
 
@@ -196,6 +196,8 @@ def lib() -> C.CDLL:
     L.bark_b200_fast_mode.argtypes = [vp]
     L.bark_b200_fast_gemm.restype = C.c_int
     L.bark_b200_fast_gemm.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
+    L.bark_b200_fast_convert.restype = C.c_int
+    L.bark_b200_fast_convert.argtypes = [C.c_int, vp, C.c_int, C.c_int, vp, C.POINTER(C.c_int)]
     L.bark_b200_fast_attention.restype = C.c_int
     L.bark_b200_fast_attention.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int]
     L.bark_b200_parity_attention.restype = C.c_int
@@ -636,6 +638,28 @@ def quant_matmul(qtype: str, W: np.ndarray, A: np.ndarray, epilogue: str = "stor
     if not return_q8:
         return out
     return out, q, d.astype(np.float16), None if s is None else s.astype(np.float16)
+
+
+def fast_convert(wtype: str, W: np.ndarray):
+    """Fast mode's load-time weight conversion to f16 (bark_b200_fast_convert).  W: [n_out][K] float32 for "f32", or for a quantised
+    type the weight rows as the model file stores them, uint8 [n_out][K/32 * block bytes]; K % 32 == 0.  Returns (float16 [n_out][K],
+    the number of results that are inf or NaN).  Raises GuardBandError when the kernel stored outside its output, RuntimeError when
+    the hook failed."""
+    if wtype == "f32":
+        W = np.ascontiguousarray(W, np.float32)
+        n_out, K = W.shape
+    else:
+        W = np.ascontiguousarray(W, np.uint8)
+        n_out, K = W.shape[0], W.shape[1] // QUANT_BLOCK_BYTES[wtype] * 32
+        assert W.shape[1] == K // 32 * QUANT_BLOCK_BYTES[wtype], (wtype, W.shape)
+    out = np.zeros((n_out, K), np.float16)
+    non_finite = C.c_int(0)
+    r = lib().bark_b200_fast_convert(0 if wtype == "f32" else QUANT_TYPES[wtype], _p(W), n_out, K, _p(out), C.byref(non_finite))
+    if r == -1:
+        raise GuardBandError(f"bark_b200_fast_convert ({wtype}, {n_out}x{K}) wrote outside its output")
+    if r != 1:
+        raise RuntimeError(f"bark_b200_fast_convert ({wtype}, {n_out}x{K}) failed")
+    return out, non_finite.value
 
 
 ROW_OPS = {"layernorm": 0, "softmax": 1}

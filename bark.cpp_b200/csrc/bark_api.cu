@@ -672,8 +672,8 @@ void alloc_workspace(bark_context * ctx) {
     }
     if (ctx->fast_mode) {
         const GPTModel & fm = ctx->fine;
-        if (fm.wtype != W_F16 || fm.n_embd / fm.n_head != 64 || fm.n_embd % 64 != 0 || fm.n_embd > 1024) {
-            fprintf(stderr, "bark_b200: BARK_B200_MODE=fast needs f16 fine-model weights with 64-wide heads; using the parity path\n");
+        if (fm.n_embd / fm.n_head != 64 || fm.n_embd % 64 != 0 || fm.n_embd > 1024) {
+            fprintf(stderr, "bark_b200: BARK_B200_MODE=fast needs a fine model with 64-wide heads; using the parity path\n");
             ctx->fast_mode = false;
         } else {
             const size_t FE = (size_t) fm.n_embd;

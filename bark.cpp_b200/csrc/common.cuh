@@ -88,6 +88,24 @@ extern thread_local double g_next_bytes, g_next_flops;
 enum WType : int { W_F32 = 0, W_F16 = 1, W_Q4_0 = 2, W_Q4_1 = 3, W_Q5_0 = 6, W_Q5_1 = 7, W_Q8_0 = 8 };   // 3..8: qx_kernels.cu
 inline bool is_quant(WType t) { return t != W_F32 && t != W_F16; }
 
+// Element e of a quantised matrix kept in the file's blocks (rows are whole blocks of 32): the f32 that dequantize_row_<t>
+// (ggml-quants.c:1522-1630) computes.  q5 codes take their fifth bit from bit j of qh.  x*d + m of q4_1 / q5_1 is one fused
+// multiply-add in the pinned build (vfmadd132ps); x*d is exact in f32 (a code below 32 times an f16), so a separate product and sum
+// would give the same value (tests/test_fast_weights.py checks both forms against tests/golden/ref_pairs/dequant.npz).
+__device__ __forceinline__ float dequant_element(const unsigned char * blocks, WType t, size_t e) {
+    const int bytes = t == W_Q4_0 ? 18 : t == W_Q4_1 ? 20 : t == W_Q5_0 ? 22 : t == W_Q5_1 ? 24 : 34;
+    const unsigned char * b = blocks + (e >> 5) * bytes;
+    const int j = (int)(e & 31);
+    const float d = __half2float(__ushort_as_half((unsigned short)(b[0] | (b[1] << 8))));
+    if (t == W_Q8_0) return __fmul_rn((float)(signed char) b[2 + j], d);
+    const bool has_m = t == W_Q4_1 || t == W_Q5_1, q5 = t == W_Q5_0 || t == W_Q5_1;
+    const unsigned char * qs = b + 2 + (has_m ? 2 : 0) + (q5 ? 4 : 0);
+    int q = j < 16 ? (qs[j] & 0x0f) : (qs[j - 16] >> 4);
+    if (q5) q |= ((b[2 + (has_m ? 2 : 0) + (j >> 3)] >> (j & 7)) & 1) << 4;
+    if (has_m) return __fmaf_rn((float) q, d, __half2float(__ushort_as_half((unsigned short)(b[2] | (b[3] << 8)))));
+    return __fmul_rn((float)(q - (q5 ? 16 : 8)), d);
+}
+
 // ---------------------------------------------------------------------------------------------
 // Lane-interleaved ("LI") matrix layout.
 // A row of K elements (K % 32 == 0) is cut into chain steps c = k / 32 for virtual lane v = k % 32.

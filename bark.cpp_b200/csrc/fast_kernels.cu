@@ -373,6 +373,26 @@ __global__ void __launch_bounds__(256) ln_rows_f16_kernel(const float * __restri
 }
 
 // ------------------------------------------------------------------------------------------------
+// weight conversion at load: one matrix of the file's type -> row-major f16 (the GEMMs' W operand)
+// ------------------------------------------------------------------------------------------------
+// Rows are whole blocks of 32, so the flat [n_out][K] index of an element is its index in the source as well.  The f16 is the round to
+// nearest even of the weight (f32) or of dequantize_row_<t>'s value (dequant_element).  non_finite (device) is increased by the number
+// of results that are inf or NaN: a source NaN / inf, or a value of magnitude >= 65520.
+__global__ void __launch_bounds__(256) convert_f16_kernel(const unsigned char * __restrict__ src, WType t, size_t n, __half * __restrict__ dst,
+                                                          int * __restrict__ non_finite) {
+    const size_t e = (size_t) blockIdx.x * 256 + threadIdx.x;
+    bool bad = false;
+    if (e < n) {
+        const float v = t == W_F32 ? reinterpret_cast<const float *>(src)[e] : dequant_element(src, t, e);
+        const __half h = __float2half_rn(v);
+        dst[e] = h;
+        bad = (__half_as_ushort(h) & 0x7c00) == 0x7c00;
+    }
+    const unsigned nb = __ballot_sync(0xffffffffu, bad);
+    if ((threadIdx.x & 31) == 0 && nb) atomicAdd(non_finite, __popc(nb));
+}
+
+// ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *, const cuuint32_t *,
@@ -457,6 +477,12 @@ bool fast_attention(const __half * qk, int ldq, int k_col0, const __half * vt, i
 
 void fast_layernorm(const float * x, int rows, int E, const float * g, const float * b, __half * out, cudaStream_t s) {
     BARK_LAUNCH_PDL(ln_rows_f16_kernel, dim3((rows + 7) / 8), dim3(256), (size_t) 0, s, x, rows, E, g, b, out);
+}
+
+void fast_convert(const void * src, WType t, int n_out, int K, __half * dst, int * non_finite, cudaStream_t s) {
+    const size_t n = (size_t) n_out * K;
+    g_next_bytes = (double) n * 2 + (t == W_F32 ? (double) n * 4 : (double)(n / 32) * (t == W_Q4_0 ? 18 : qx_block_bytes(t)));
+    BARK_LAUNCH(convert_f16_kernel, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, s, (const unsigned char *) src, t, n, dst, non_finite);
 }
 
 }  // namespace bark

@@ -57,12 +57,7 @@ void permute_to_gm(const void * src, void * dst, int n_out, int o_pad, int K, WT
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ float wte_value(const void * wte, int wt, int E, int row, int i) {
     if (wt == W_F16) return __half2float(((const __half *) wte)[(size_t) row * E + i]);
-    if (wt == W_Q4_0) {                                      // dequantize_row_q4_0 (ggml-quants.c:1515-1533): (nibble - 8) * d on the file's 18-byte blocks
-        const unsigned char * blk = (const unsigned char *) wte + ((size_t) row * (E >> 5) + (i >> 5)) * 18;
-        const float d = __half2float(__ushort_as_half((unsigned short)(blk[0] | (blk[1] << 8))));
-        const int j = i & 31, q = j < 16 ? (blk[2 + j] & 0x0f) : (blk[2 + j - 16] >> 4);
-        return __fmul_rn((float)(q - 8), d);
-    }
+    if (wt == W_Q4_0) return dequant_element((const unsigned char *) wte, W_Q4_0, (size_t) row * E + i);   // on the file's 18-byte blocks
     return ((const float *) wte)[(size_t) row * E + i];
 }
 

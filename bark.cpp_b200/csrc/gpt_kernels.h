@@ -83,6 +83,9 @@ struct FastEpi {
 int  fast_gemm(const __half * A, int lda, const __half * W, int ldw, int M, int N, int K, const FastEpi & ep, int n_sm, int bn, cudaStream_t s);
 bool fast_attention(const __half * qk, int ldq, int k_col0, const __half * vt, int n, int E, int H, __half * out, cudaStream_t s);
 void fast_layernorm(const float * x, int rows, int E, const float * g, const float * b, __half * out, cudaStream_t s);
+// [n_out][K] weights of type t (f32, or q4_0 / q4_1 / q5_0 / q5_1 / q8_0 blocks as the file stores them), K % 32 == 0 -> dst [n_out][K]
+// f16, the W operand of fast_gemm; *non_finite (device) grows by the number of inf / NaN results
+void fast_convert(const void * src, WType t, int n_out, int K, __half * dst, int * non_finite, cudaStream_t s);
 
 // ---- persistent decode step (decode_kernels.cu) -----------------------------------------------------------------
 constexpr int kDecodeReplicas = 8;        // copies of each all-to-all exchange vector (gx, gq, gatt, gff): CTA c reads copy c % 8

@@ -183,6 +183,25 @@ extern "C" int bark_b200_fast_gemm(const uint16_t * A, const uint16_t * W, void 
     });
 }
 
+// fast mode's weight conversion: W [n_out][K] in the file's type (f32, or the blocks of a quantised type) -> f16 [n_out][K]
+extern "C" int bark_b200_fast_convert(int wtype, const void * src, int n_out, int K, uint16_t * dst, int * non_finite) {
+    return guarded(0, [&] {
+        const WType t = (WType) wtype;
+        if (!src || !dst || !non_finite || n_out < 1 || K < 32 || K % 32 || (t != W_F32 && t != W_Q4_0 && !qx_supported(t))) return 0;
+        const size_t n = (size_t) n_out * K;
+        DeviceBuffers mem;
+        const void * d_src = mem.upload((const unsigned char *) src, t == W_F32 ? n * 4 : n / 32 * (t == W_Q4_0 ? 18 : qx_block_bytes(t)));
+        int * d_count = mem.alloc<int>(sizeof(int));
+        BARK_CUDA_CHECK(cudaMemset(d_count, 0, sizeof(int)));
+        const GuardedOutput c(mem, n * 2, nullptr);
+        fast_convert(d_src, t, n_out, K, c.out<__half>(), d_count, 0);
+        if (!finish("bark_b200_fast_convert")) return 0;
+        if (!c.read("bark_b200_fast_convert", dst)) return -1;
+        download(non_finite, d_count, sizeof(int));
+        return 1;
+    });
+}
+
 extern "C" int bark_b200_fast_attention(const uint16_t * q, const uint16_t * k, const uint16_t * v, uint16_t * out, int n, int E, int H) {
     return guarded(0, [&] {
         if (!q || !k || !v || !out || n < 128 || n % 128 || E != H * 64) return 0;

@@ -85,6 +85,26 @@ struct Slot {              // where a named GPT tensor goes
     bool gm = false;        // MATRIX: also keep a group-major copy (operand of the multi-row tiled mat-mul)
 };
 
+// Fast mode, fine model, a file that is not f16: d.p_rm = the f16 row-major copy of the raw upload (fast_convert) that the tensor cores
+// read.  A value that is not finite in f16 refuses fast mode for the context (the parity path runs instead), naming the tensor; copies
+// made before the refusal stay allocated until bark_free.
+void fast_copy(bark_context * ctx, const void * raw, WType t, DMat & d, const std::string & name) {
+    struct Buffers { __half * rm = nullptr; int * count = nullptr; ~Buffers() { cudaFree(rm); cudaFree(count); } } b;
+    BARK_CUDA_CHECK(cudaMalloc(&b.rm, (size_t) d.n_out * d.K * sizeof(__half)));
+    BARK_CUDA_CHECK(cudaMalloc(&b.count, sizeof(int)));
+    BARK_CUDA_CHECK(cudaMemsetAsync(b.count, 0, sizeof(int), ctx->stream));
+    fast_convert(raw, t, d.n_out, d.K, b.rm, b.count, ctx->stream);
+    int non_finite = 0;
+    BARK_CUDA_CHECK(cudaMemcpyAsync(&non_finite, b.count, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    BARK_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+    if (non_finite) {
+        fprintf(stderr, "bark_b200: BARK_B200_MODE=fast: fine-model weight '%s' has %d values that are not finite in f16; using the parity path\n", name.c_str(), non_finite);
+        ctx->fast_mode = false;
+        return;
+    }
+    d.p_rm = b.rm; ctx->arena.allocs.push_back(b.rm); b.rm = nullptr;
+}
+
 bool load_gpt(bark_context * ctx, std::ifstream & f, GPTModel & m, const char * what) {
     if (!rd(f, m.n_layer) || !rd(f, m.n_head) || !rd(f, m.n_embd) || !rd(f, m.block_size) || !rd(f, m.bias) || !rd(f, m.n_in_vocab) ||
         !rd(f, m.n_out_vocab) || !rd(f, m.n_lm_heads) || !rd(f, m.n_wtes) || !rd(f, m.ftype)) return false;
@@ -157,6 +177,7 @@ bool load_gpt(bark_context * ctx, std::ifstream & f, GPTModel & m, const char * 
                 d.mins = ctx_alloc(ctx, n_blocks * 2); d.qh = ctx_alloc(ctx, n_blocks * 4);
                 qx_split(raw, n_blocks, m.wtype, d.p, d.qh, d.scales, d.mins, ctx->stream);
                 BARK_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+                if (ctx->fast_mode && !causal) fast_copy(ctx, raw, m.wtype, d, h.name);
                 BARK_CUDA_CHECK(cudaFree(raw));
                 continue;
             }
@@ -166,6 +187,7 @@ bool load_gpt(bark_context * ctx, std::ifstream & f, GPTModel & m, const char * 
                 d.p = ctx_alloc(ctx, n_blocks * 16); d.scales = ctx_alloc(ctx, n_blocks * 2);
                 q4_split(raw, n_blocks, d.p, d.scales, ctx->stream);
                 BARK_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+                if (ctx->fast_mode && !causal) fast_copy(ctx, raw, W_Q4_0, d, h.name);
                 BARK_CUDA_CHECK(cudaFree(raw));
                 if (ctx->params.verbosity == HIGH) printf("%48s - [%5d, %5d], type = %d, %6.2f MB\n", h.name.c_str(), h.ne[0], h.ne[1], h.ttype, bytes / 1024.0 / 1024.0);
                 continue;
@@ -181,7 +203,10 @@ bool load_gpt(bark_context * ctx, std::ifstream & f, GPTModel & m, const char * 
             }
             BARK_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
             if (ctx->fast_mode && !causal && m.wtype == W_F16) { d.p_rm = raw; ctx->arena.allocs.push_back(raw); }   // fast mode: the tensor cores read the file's own row-major layout
-            else BARK_CUDA_CHECK(cudaFree(raw));
+            else {
+                if (ctx->fast_mode && !causal) fast_copy(ctx, raw, m.wtype, d, h.name);                             // f32: its f16 copy
+                BARK_CUDA_CHECK(cudaFree(raw));
+            }
         } else {
             void * raw = upload_raw(ctx->arena, ctx->stream, f, bytes, host, true);
             if (!raw) return false;

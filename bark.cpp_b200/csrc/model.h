@@ -16,7 +16,7 @@ struct DMat {                 // 2-D weight [n_out][K] in LI layout (f32 / f16) 
     void * scales = nullptr;        // quantised: f16 block scales [n_out][K/32]; p then holds the 16-byte nibble words (32 B for q8_0) [n_out][K/32]
     void * mins = nullptr, * qh = nullptr;   // experimental types: f16 block minima (q4_1, q5_1), fifth bits (q5_0, q5_1)
     void * p_gm = nullptr; int o_pad = 0;   // second copy in the group-major layout (common.cuh) for the tiled GEMM; rows padded to o_pad
-    void * p_rm = nullptr;                  // fast mode only: the file's row-major [n_out][K] f16 matrix = K-major wgmma operand (fast_kernels.cu)
+    void * p_rm = nullptr;                  // fast mode only: the row-major [n_out][K] f16 matrix = K-major wgmma operand (fast_kernels.cu); an f16 file's own upload, else its fast_convert copy
     WType type = W_F16;
 };
 

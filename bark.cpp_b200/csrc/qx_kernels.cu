@@ -12,22 +12,12 @@ namespace bark {
 
 namespace {
 
-__device__ __forceinline__ float f16_at(const unsigned char * p) { return __half2float(__ushort_as_half((unsigned short)(p[0] | (p[1] << 8)))); }
 __device__ __forceinline__ uint32_t u32_at(const unsigned char * p) { return (uint32_t) p[0] | ((uint32_t) p[1] << 8) | ((uint32_t) p[2] << 16) | ((uint32_t) p[3] << 24); }
 __host__ __device__ inline int block_bytes(int t) { return t == W_Q4_1 ? 20 : t == W_Q5_0 ? 22 : t == W_Q5_1 ? 24 : 34; }
 
-// get_rows on the file's blocks: dequantize_row_q4_1 / q5_0 / q5_1 / q8_0 (ggml-quants.c:1542-1630); x*d + m is one fused multiply-add there
+// get_rows on the file's blocks: dequantize_row_q4_1 / q5_0 / q5_1 / q8_0 (ggml-quants.c:1542-1630)
 __device__ __forceinline__ float wte_value_q(const void * wte, int t, int E, int row, int i) {
-    const int bb = block_bytes(t);
-    const unsigned char * blk = (const unsigned char *) wte + ((size_t) row * (E >> 5) + (i >> 5)) * bb;
-    const float d = f16_at(blk);
-    const int j = i & 31;
-    if (t == W_Q8_0) return __fmul_rn((float)(signed char) blk[2 + j], d);
-    const unsigned char * qs = blk + (t == W_Q4_1 ? 4 : t == W_Q5_0 ? 6 : 8);
-    int q = j < 16 ? (qs[j] & 0x0f) : (qs[j - 16] >> 4);
-    if (t != W_Q4_1) q |= (int)((u32_at(blk + (t == W_Q5_0 ? 2 : 4)) >> j) & 1u) << 4;
-    if (t == W_Q5_0) return __fmul_rn((float)(q - 16), d);
-    return __fmaf_rn((float) q, d, f16_at(blk + 2));
+    return dequant_element((const unsigned char *) wte, (WType) t, (size_t) row * E + i);
 }
 
 __global__ void embed_causal_q_kernel(const void * __restrict__ wte, int wt, const float * __restrict__ wpe, const int32_t * __restrict__ tok,

@@ -155,7 +155,11 @@ BARK_API int  bark_b200_sample_filtered_given_u(const float * logits, int n, int
 
 /* FAST MODE (BARK_B200_MODE=fast in the environment at load; opt-in, NOT bit-identical to the reference): the fine model's
  * 1024-row passes (bark.cpp:1416-1584) run as wgmma tensor-core GEMMs + flash-style attention (csrc/fast_kernels.cu).
- * The two kernel hooks below run on host buffers without a context, for the numerics tests:
+ * Every weight type the loader reads runs it: an f16 file's fine matrices are used as stored; those of an f32, q4_0, q4_1, q5_0, q5_1
+ * or q8_0 file are converted once at load to one f16 copy (bark_b200_fast_convert), each element the round to nearest even of the f32
+ * the reference's dequantize_row_<type> gives.  A fine weight that is not finite in f16 refuses fast mode for the context, with a
+ * message naming it: bark_b200_fast_mode then returns 0 and the parity path runs.
+ * The kernel hooks below run on host buffers without a context, for the numerics tests:
  *   bark_b200_fast_gemm ....... A[M][K] (f16 bits) * W[N][K]^T (f16 bits), K % 64 == 0, through the fine pass's epilogue `epilogue`:
  *                                 0 F32     C = f32 [M][N]
  *                                 1 RESID   C = f32 [M][N], holds the residual on entry and residual + A W^T on return
@@ -163,9 +167,14 @@ BARK_API int  bark_b200_sample_filtered_given_u(const float * logits, int n, int
  *                                 4 QKV16   N % 6 == 0; C = f16 [M][2N/3] (columns < 2N/3), then f16 [N/3][M] (columns >= 2N/3, transposed)
  *                               bn: 0 = the tile width the cost model picks, 64 / 128 / 256 = that width forced.
  *                               Returns the tile width that ran, 0 on failure, -1 if a store landed in the guard bands around the output.
- *   bark_b200_fast_attention .. out[n][E] (f16 bits) = soft_max(Q K^T / 8) V per 64-wide head, non-causal, n % 128 == 0 */
+ *   bark_b200_fast_attention .. out[n][E] (f16 bits) = soft_max(Q K^T / 8) V per 64-wide head, non-causal, n % 128 == 0
+ *   bark_b200_fast_convert .... the load-time conversion: src [n_out][K] of wtype (enum ggml_type) 0 f32, 2 q4_0 (18-byte blocks),
+ *                               3 q4_1 (20), 6 q5_0 (22), 7 q5_1 (24) or 8 q8_0 (34) as the model file stores it, K % 32 == 0 -> dst
+ *                               [n_out][K] f16 bits; *non_finite = the number of results that are inf or NaN.  Returns 1, 0 on invalid
+ *                               arguments or failure, -1 if a store landed in the guard bands around the output. */
 BARK_API int  bark_b200_fast_mode(struct bark_context * ctx);              /* 1 if this context runs the fast fine passes */
 BARK_API int  bark_b200_fast_gemm(const uint16_t * A, const uint16_t * W, void * C, int M, int N, int K, int epilogue, int bn);
+BARK_API int  bark_b200_fast_convert(int wtype, const void * src, int n_out, int K, uint16_t * dst, int * non_finite);
 BARK_API int  bark_b200_fast_attention(const uint16_t * q, const uint16_t * k, const uint16_t * v, uint16_t * out, int n, int E, int H);
 
 /* Parity-path attention on host buffers without a context (tests, tools/attn_bench.py): out[N][E] = soft_max(mask(Q K^T / sqrt(E/H))) V
