@@ -112,6 +112,8 @@ EXPORTS = [
     "bark_b200_parity_rows", "bark_b200_sample_given_u", "bark_b200_generate_batch", "bark_b200_batch_audio", "bark_b200_batch_tokens", "bark_b200_gpt_eval_slot", "bark_b200_gpt_step_batch",
     "bark_b200_set_history_prompt", "bark_b200_generate_batch_prompted", "bark_b200_set_sampling", "bark_b200_sample_filtered_given_u",
     "bark_b200_quant_matmul", "bark_b200_fast_convert",
+    "bark_b200_encodec_compress_batch", "bark_b200_encodec_decompress_batch", "bark_b200_encodec_reconstruct_batch",
+    "bark_b200_encodec_batch_codes", "bark_b200_encodec_batch_audio",
     "ggml_time_init", "ggml_time_us", "ggml_time_ms", "ggml_init", "ggml_free",
 ]
 
@@ -229,6 +231,12 @@ def lib() -> C.CDLL:
     L.bark_b200_generate_batch_prompted.restype = C.c_bool
     L.bark_b200_generate_batch_prompted.argtypes = [vp, C.POINTER(C.c_char_p), C.POINTER(C.c_uint32), C.POINTER(C.POINTER(HistoryPromptStruct)),
                                                     C.c_int, C.c_int]
+    for n in ("bark_b200_encodec_compress_batch", "bark_b200_encodec_decompress_batch", "bark_b200_encodec_reconstruct_batch"):
+        getattr(L, n).restype = C.c_bool
+        getattr(L, n).argtypes = [vp, vp, vp, C.c_int]
+    for n in ("bark_b200_encodec_batch_codes", "bark_b200_encodec_batch_audio"):
+        getattr(L, n).restype = C.c_int
+        getattr(L, n).argtypes = [vp, C.c_int, vp, C.c_int]
     L.ggml_time_us.restype = C.c_int64
     L.encodec_load_model.restype = vp
     L.encodec_load_model.argtypes = [C.c_char_p, C.c_int, C.c_int]
@@ -803,6 +811,43 @@ class Encodec:
     def _audio(self):
         n = lib().encodec_get_audio_size(self.ctx)
         return np.ctypeslib.as_array(lib().encodec_get_audio(self.ctx), shape=(n,)).copy()
+
+    # ---- batches (bark_b200_encodec_*_batch): item i equals the single call on clip i, bit for bit --------------------------------
+    def compress_batch(self, clips) -> list:
+        """Clips of mono float32 samples (each finite, at least 1921) -> codes [n_q][T_i] int32 per clip, in one batched call."""
+        xs = [np.ascontiguousarray(a, np.float32).ravel() for a in clips]
+        self._batch("bark_b200_encodec_compress_batch", xs)
+        out = []
+        for i, x in enumerate(xs):
+            c = self._item("bark_b200_encodec_batch_codes", i, np.int32)
+            T = (x.size + 319) // 320
+            out.append(c.reshape(c.size // T, T))
+        return out
+
+    def decompress_batch(self, codes) -> list:
+        """Codes [n_q][T_i] per item (n_q of the current bandwidth) -> 320 T_i float32 samples per item."""
+        cs = [np.ascontiguousarray(c, np.int32) for c in codes]
+        self._batch("bark_b200_encodec_decompress_batch", cs)
+        return [self._item("bark_b200_encodec_batch_audio", i, np.float32) for i in range(len(cs))]
+
+    def reconstruct_batch(self, clips) -> list:
+        """compress_batch then decompress_batch, the codes staying on the device: 320 T_i float32 samples per clip."""
+        xs = [np.ascontiguousarray(a, np.float32).ravel() for a in clips]
+        self._batch("bark_b200_encodec_reconstruct_batch", xs)
+        return [self._item("bark_b200_encodec_batch_audio", i, np.float32) for i in range(len(xs))]
+
+    def _batch(self, fn, arrays):
+        n = len(arrays)
+        ptrs = (C.c_void_p * max(n, 1))(*[a.ctypes.data for a in arrays])
+        lens = (C.c_int * max(n, 1))(*[a.size for a in arrays])
+        if not getattr(lib(), fn)(self.ctx, ptrs, lens, n):
+            raise RuntimeError(f"{fn} failed (see stderr)")
+
+    def _item(self, fn, i, dtype):
+        n = getattr(lib(), fn)(self.ctx, i, None, 0)
+        out = np.empty(n, dtype)
+        getattr(lib(), fn)(self.ctx, i, _p(out), n)
+        return out
 
     def stats(self) -> dict:
         s = lib().encodec_get_statistics(self.ctx).contents

@@ -14,18 +14,55 @@
 // bit-identical to the CPU reference, not merely within the 1e-3 contract.
 #include "codec_kernels.h"
 
+#include <algorithm>
+#include <vector>
+
 #include <cooperative_groups.h>
 namespace cg = cooperative_groups;
 
 namespace bark {
 
 // ------------------------------------------------------------------------------------------------
+// Items of one launch, passed by value (__grid_constant__: indexed in the parameter space, never copied).  Item b reads [C][L_in[b]] at
+// C * base_in[b] and writes [C'][L_out[b]] at C' * base_out[b]; base_* are prefix sums of the lengths, base_*[n] their total.  Grids are
+// one flattened run of tiles: item b owns tiles [tile0[b], tile0[b+1]) of the kernel's tile size, so a launch costs the sum of the
+// items' tiles, not n times the longest.  Lp: the stream kernel's padded input length.
+// ------------------------------------------------------------------------------------------------
+struct CodecItems {
+    int n;
+    int L_in[kCodecMaxItems], L_out[kCodecMaxItems], Lp[kCodecMaxItems];
+    int base_in[kCodecMaxItems + 1], base_out[kCodecMaxItems + 1], tile0[kCodecMaxItems + 1];
+};
+
+// tiled[b]: the positions item b's tiles of TT cover (its input or output length, as the kernel walks them)
+static CodecItems codec_items(int n, const int * L_in, const int * L_out, const int * tiled, int TT) {
+    if (n < 1 || n > kCodecMaxItems) { fprintf(stderr, "bark_b200: %d codec items in one launch (1 to %d)\n", n, kCodecMaxItems); throw std::runtime_error("unsupported configuration (see the message above)"); }
+    CodecItems it{};
+    it.n = n;
+    for (int b = 0; b < n; b++) {
+        it.L_in[b] = L_in[b]; it.L_out[b] = L_out[b];
+        it.base_in[b + 1] = it.base_in[b] + L_in[b]; it.base_out[b + 1] = it.base_out[b] + L_out[b];
+        it.tile0[b + 1] = it.tile0[b] + (tiled[b] + TT - 1) / TT;
+    }
+    return it;
+}
+
+// the last b in [0, n) with a[b] <= v (a ascending, a[0] = 0): the item of a flattened tile or of a concatenated position
+__device__ __forceinline__ int item_at(const int * a, int n, int v) {
+    int lo = 0, hi = n - 1;
+    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (a[mid] <= v) lo = mid; else hi = mid - 1; }
+    return lo;
+}
+
+// ------------------------------------------------------------------------------------------------
 // quantizer decode: x[d][t] = sum_q embed_q[codes[q][t]][d], q = 0..n_q-1 in order onto a zeroed tensor (quantizer.h:95-106)
 // ------------------------------------------------------------------------------------------------
 struct Codebooks { const float * e[kMaxCodebooks]; };
-__global__ void rvq_decode_kernel(Codebooks cb, const int32_t * __restrict__ codes, int n_q, int T, int Hd, float * __restrict__ x) {
-    const int t = blockIdx.x * blockDim.x + threadIdx.x, d = blockIdx.y;
+__global__ void rvq_decode_kernel(Codebooks cb, const int32_t * __restrict__ codes, int n_q, int Hd, float * __restrict__ x, const __grid_constant__ CodecItems it) {
+    const int b = item_at(it.tile0, it.n, blockIdx.x), T = it.L_in[b];
+    const int t = (blockIdx.x - it.tile0[b]) * blockDim.x + threadIdx.x, d = blockIdx.y;
     if (t >= T) return;
+    codes += (size_t) n_q * it.base_in[b]; x += (size_t) Hd * it.base_in[b];
     float acc = 0.0f;
 #pragma unroll
     for (int q = 0; q < kMaxCodebooks; q++)              // constant indices: the parameter struct stays in constant memory
@@ -33,10 +70,11 @@ __global__ void rvq_decode_kernel(Codebooks cb, const int32_t * __restrict__ cod
     x[(size_t) d * T + t] = acc;
 }
 
-void rvq_decode(const CodecModel & cm, const int32_t * d_codes, int n_q, int T, float * x, cudaStream_t s) {
+void rvq_decode(const CodecModel & cm, const int32_t * d_codes, int n_q, const int * T, int n, float * x, cudaStream_t s) {
     Codebooks cb{};
     for (int q = 0; q < n_q; q++) cb.e[q] = cm.embed[q];
-    BARK_LAUNCH(rvq_decode_kernel, dim3((T + 127) / 128, cm.hidden_dim), 128, 0, s, cb, d_codes, n_q, T, cm.hidden_dim, x);
+    const CodecItems it = codec_items(n, T, T, T, 128);
+    BARK_LAUNCH(rvq_decode_kernel, dim3(it.tile0[n], cm.hidden_dim), 128, 0, s, cb, d_codes, n_q, cm.hidden_dim, x, it);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -66,15 +104,19 @@ void rvq_norms(const float * embed, int n_bins, int Hd, float * out, cudaStream_
 // slices in order through DSMEM, where a NaN resets the maximum.  Every CTA then applies the same residual update.
 // The values and partials are double-buffered by codebook parity, so one cluster barrier per codebook orders the writes of codebook
 // q + 2 after every peer's reads of codebook q.
+// The 8 frames of a cluster are consecutive positions of the items' concatenated frames, so clusters fill across items: position g is
+// frame g - base[b] of item b, whose latent is [Hd][T_b] at Hd * base[b] and whose codes are [n_q][T_b] at n_q * base[b].
 constexpr int kRvqFrames = 8, kRvqCtas = 8, kRvqMaxBins = 1024, kRvqMaxHidden = 128, kRvqSlice = kRvqMaxBins / kRvqCtas;
-__global__ void __cluster_dims__(kRvqCtas, 1, 1) __launch_bounds__(256) rvq_encode_kernel(
-        const float * __restrict__ latent, int T, Codebooks cb, Codebooks norms, int n_q, int n_bins, int Hd, int32_t * __restrict__ codes) {
+__global__ void __cluster_dims__(kRvqCtas, 1, 1) __launch_bounds__(256, 4) rvq_encode_kernel(
+        const float * __restrict__ latent, Codebooks cb, Codebooks norms, int n_q, int n_bins, int Hd, int32_t * __restrict__ codes,
+        const __grid_constant__ CodecItems it) {
     __shared__ float vals[2][kRvqFrames][kRvqSlice];
     __shared__ float p_max[2][kRvqFrames];
     __shared__ int p_idx[2][kRvqFrames], p_nan[2][kRvqFrames];
     __shared__ float res[kRvqFrames][kRvqMaxHidden];
     __shared__ float s_nrm[kRvqFrames];
     __shared__ int s_code[kRvqFrames];
+    __shared__ int s_T[kRvqFrames], s_base[kRvqFrames], s_t[kRvqFrames];   // item length, item base, frame within the item (s_T 0: no frame)
     __shared__ const float * s_cb[kMaxCodebooks], * s_cn[kMaxCodebooks];   // indexing the parameter structs by q would copy them to the stack
     cg::cluster_group cluster = cg::this_cluster();
     const int rank = (int) cluster.block_rank();
@@ -82,9 +124,15 @@ __global__ void __cluster_dims__(kRvqCtas, 1, 1) __launch_bounds__(256) rvq_enco
     const int S = (n_bins + kRvqCtas - 1) / kRvqCtas, lo = min(rank * S, n_bins), cnt = min(n_bins - lo, S);
 #pragma unroll
     for (int q = 0; q < kMaxCodebooks; q++) if (threadIdx.x == q) { s_cb[q] = cb.e[q]; s_cn[q] = norms.e[q]; }
+    if (threadIdx.x < kRvqFrames) {
+        const int g = f0 + threadIdx.x, b = item_at(it.base_in, it.n, g);
+        const bool live = g < it.base_in[it.n];
+        s_T[threadIdx.x] = live ? it.L_in[b] : 0; s_base[threadIdx.x] = it.base_in[b]; s_t[threadIdx.x] = g - it.base_in[b];
+    }
+    __syncthreads();
     for (int i = threadIdx.x; i < kRvqFrames * Hd; i += blockDim.x) {
         const int f = i / Hd, d = i % Hd;
-        res[f][d] = f0 + f < T ? latent[(size_t) d * T + f0 + f] : 0.f;
+        res[f][d] = s_T[f] ? latent[(size_t) Hd * s_base[f] + (size_t) d * s_T[f] + s_t[f]] : 0.f;
     }
     __syncthreads();
     for (int q = 0; q < n_q; q++) {
@@ -155,9 +203,9 @@ __global__ void __cluster_dims__(kRvqCtas, 1, 1) __launch_bounds__(256) rvq_enco
                 }
             }
             if (lane == 0) {
-                const bool live = f0 + warp < T;
-                s_code[warp] = live ? best : 0;
-                if (live && rank == 0) codes[(size_t) q * T + f0 + warp] = best;
+                const int T = s_T[warp];
+                s_code[warp] = T ? best : 0;
+                if (T && rank == 0) codes[(size_t) n_q * s_base[warp] + (size_t) q * T + s_t[warp]] = best;
             }
         }
         __syncthreads();
@@ -170,13 +218,16 @@ __global__ void __cluster_dims__(kRvqCtas, 1, 1) __launch_bounds__(256) rvq_enco
     cluster.sync();                                      // a CTA's shared memory must outlive its peers' last reads
 }
 
-bool rvq_encode(const float * const * embed, const float * const * norms, int n_q, int n_bins, int Hd, const float * latent, int T, int32_t * codes,
-                cudaStream_t s) {
-    if (n_q < 1 || n_q > kMaxCodebooks || n_bins < 1 || n_bins > kRvqMaxBins || Hd < 32 || Hd > kRvqMaxHidden || Hd % 32 || T < 1) return false;
+bool rvq_encode(const float * const * embed, const float * const * norms, int n_q, int n_bins, int Hd, const float * latent, const int * T, int n,
+                int32_t * codes, cudaStream_t s) {
+    if (n_q < 1 || n_q > kMaxCodebooks || n_bins < 1 || n_bins > kRvqMaxBins || Hd < 32 || Hd > kRvqMaxHidden || Hd % 32) return false;
+    for (int b = 0; b < n; b++) if (T[b] < 1) return false;
     Codebooks cb{}, nr{};
     for (int q = 0; q < n_q; q++) { cb.e[q] = embed[q]; nr.e[q] = norms[q]; }
-    g_next_flops = 2.0 * (double) T * n_q * n_bins * Hd;
-    BARK_LAUNCH(rvq_encode_kernel, (T + kRvqFrames - 1) / kRvqFrames * kRvqCtas, 256, 0, s, latent, T, cb, nr, n_q, n_bins, Hd, codes);
+    const CodecItems it = codec_items(n, T, T, T, 1);
+    const int frames = it.base_in[n];
+    g_next_flops = 2.0 * (double) frames * n_q * n_bins * Hd;
+    BARK_LAUNCH(rvq_encode_kernel, (frames + kRvqFrames - 1) / kRvqFrames * kRvqCtas, 256, 0, s, latent, cb, nr, n_q, n_bins, Hd, codes, it);
     return true;
 }
 
@@ -202,13 +253,15 @@ __device__ __forceinline__ void load_chain(const __half * __restrict__ row, int 
 // already ELU'd and f16-rounded; a warp keeps one filter's lane chains in registers and walks its positions.
 // ------------------------------------------------------------------------------------------------
 template <int KW, int NG>
-__global__ void __launch_bounds__(256) conv1d_lane_kernel(const float * __restrict__ x, int Cin, int T, const __half * __restrict__ w_li, int Kp,
+__global__ void __launch_bounds__(256) conv1d_lane_kernel(const float * __restrict__ x, int Cin, const __half * __restrict__ w_li, int Kp,
                                                           const float * __restrict__ bias, int Cout, int o_per_block, int elu_in,
-                                                          const float * __restrict__ resid, float * __restrict__ y) {
+                                                          const float * __restrict__ resid, float * __restrict__ y, const __grid_constant__ CodecItems it) {
     constexpr int TT = 32;
     constexpr int S = ((TT + KW - 1) | 1);               // odd row stride: conflict-free lane -> (c, j) gathers
     extern __shared__ float xs[];                        // [Cin][S]
-    const int t0 = blockIdx.x * TT;
+    const int b = item_at(it.tile0, it.n, blockIdx.x), T = it.L_in[b], t0 = (blockIdx.x - it.tile0[b]) * TT;
+    x += (size_t) Cin * it.base_in[b]; y += (size_t) Cout * it.base_in[b];
+    if (resid) resid += (size_t) Cout * it.base_in[b];
     for (int i = threadIdx.x; i < Cin * (TT + KW - 1); i += blockDim.x) {
         const int c = i / (TT + KW - 1), j = i % (TT + KW - 1);
         int t = t0 + j - (KW - 1);
@@ -264,12 +317,15 @@ static int device_sms() {
 // K = 16): ggml_vec_dot_f16 has no full lane step, so the whole dot is its leftover loop, f32 products summed in double from 0
 // (ggml.c:2281-2283).  One thread per output position; the block stages a tile of the input (ELU'd, f16-rounded) once.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128) conv1d_short_kernel(const float * __restrict__ x, int Cin, int T, int k, const __half * __restrict__ w_li, int Kp,
+__global__ void __launch_bounds__(128) conv1d_short_kernel(const float * __restrict__ x, int Cin, int k, const __half * __restrict__ w_li, int Kp,
                                                            const float * __restrict__ bias, int Cout, int o_per_block, int elu_in,
-                                                           const float * __restrict__ resid, float * __restrict__ y) {
+                                                           const float * __restrict__ resid, float * __restrict__ y, const __grid_constant__ CodecItems it) {
     constexpr int TT = 128;
     extern __shared__ float xs[];                        // [Cin][TT + k - 1]
-    const int W = TT + k - 1, t0 = blockIdx.x * TT;
+    const int b = item_at(it.tile0, it.n, blockIdx.x), T = it.L_in[b];
+    const int W = TT + k - 1, t0 = (blockIdx.x - it.tile0[b]) * TT;
+    x += (size_t) Cin * it.base_in[b]; y += (size_t) Cout * it.base_in[b];
+    if (resid) resid += (size_t) Cout * it.base_in[b];
     for (int i = threadIdx.x; i < Cin * W; i += blockDim.x) {
         const int c = i / W, j = i % W;
         int t = t0 + j - (k - 1);
@@ -302,12 +358,15 @@ __global__ void __launch_bounds__(128) conv1d_short_kernel(const float * __restr
 // so a weight word is used TT times.  Chain order, tree and bias add are conv1d_lane_kernel's (K % 32 == 0: no leftovers).
 // ------------------------------------------------------------------------------------------------
 template <int KW, int STRIDE>
-__global__ void __launch_bounds__(256) conv1d_stream_kernel(const float * __restrict__ x, int Cin, int L, int Lp, int Tout, const __half * __restrict__ w_li,
-                                                            int Kp, const float * __restrict__ bias, int Cout, int o_per_block, int elu_in, float * __restrict__ y) {
+__global__ void __launch_bounds__(256) conv1d_stream_kernel(const float * __restrict__ x, int Cin, const __half * __restrict__ w_li,
+                                                            int Kp, const float * __restrict__ bias, int Cout, int o_per_block, int elu_in, float * __restrict__ y,
+                                                            const __grid_constant__ CodecItems it) {
     constexpr int TT = STRIDE >= 8 ? 8 : 16, OW = 2;
     constexpr int SPAN = (TT - 1) * STRIDE + KW, SR = SPAN | 1, PADL = KW - STRIDE;
     extern __shared__ float xs[];                        // [Cin][SR]
-    const int t0 = blockIdx.x * TT;
+    const int b = item_at(it.tile0, it.n, blockIdx.x), L = it.L_in[b], Lp = it.Lp[b], Tout = it.L_out[b];
+    const int t0 = (blockIdx.x - it.tile0[b]) * TT;
+    x += (size_t) Cin * it.base_in[b]; y += (size_t) Cout * it.base_out[b];
     for (int i = threadIdx.x; i < Cin * SPAN; i += blockDim.x) {
         const int c = i / SPAN, u = i % SPAN, p = t0 * STRIDE + u;
         float v = 0.f;
@@ -381,25 +440,29 @@ static void strided_conv_lengths(int L, int k, int stride, int * Lp, int * Tout)
 int conv1d_out_len(int L, int k, int stride) { int Lp, Tout; strided_conv_lengths(L, k, stride, &Lp, &Tout); return Tout; }
 
 // shapes the stream kernel is instantiated for: the encoder's down-sampling convs (k = 2r, stride r) and its final conv
-static void conv1d_stream(const float * x, int Cin, int L, const ConvW & cv, int stride, bool elu_in, float * y, cudaStream_t s) {
+static void conv1d_stream(const float * x, int Cin, const int * L, int n, const ConvW & cv, int stride, bool elu_in, float * y, cudaStream_t s) {
     const int K = Cin * cv.k;
-    int Lp, Tout;
-    strided_conv_lengths(L, cv.k, stride, &Lp, &Tout);
-    if (K % 32 != 0 || Lp - L - (cv.k - stride) > L - 1) {
-        fprintf(stderr, "bark_b200: unsupported conv shape Cin=%d k=%d stride=%d L=%d\n", Cin, cv.k, stride, L); throw std::runtime_error("unsupported configuration (see the message above)");
+    std::vector<int> Lp((size_t) n), Tout((size_t) n);
+    for (int b = 0; b < n; b++) {
+        strided_conv_lengths(L[b], cv.k, stride, &Lp[b], &Tout[b]);
+        if (K % 32 != 0 || Lp[b] - L[b] - (cv.k - stride) > L[b] - 1) {
+            fprintf(stderr, "bark_b200: unsupported conv shape Cin=%d k=%d stride=%d L=%d\n", Cin, cv.k, stride, L[b]); throw std::runtime_error("unsupported configuration (see the message above)");
+        }
     }
     const int TT = stride >= 8 ? 8 : 16, SR = ((TT - 1) * stride + cv.k) | 1;
+    CodecItems it = codec_items(n, L, Tout.data(), Tout.data(), TT);
+    for (int b = 0; b < n; b++) it.Lp[b] = Lp[b];
     const size_t smem = (size_t) Cin * SR * sizeof(float);
-    const int tiles = (Tout + TT - 1) / TT;
+    const int tiles = it.tile0[n];
     int o_per_block = cv.cout;
     const int n_sm = device_sms();
     while (o_per_block > 16 && tiles * ((cv.cout + o_per_block - 1) / o_per_block) < 2 * n_sm) o_per_block = (o_per_block + 1) / 2;
     const dim3 grid(tiles, (cv.cout + o_per_block - 1) / o_per_block);
-    g_next_flops = 2.0 * (double) Tout * cv.cout * K;
+    g_next_flops = 2.0 * (double) it.base_out[n] * cv.cout * K;
 #define STREAM_CASE(KW, ST)                                                                                                  \
     if (cv.k == KW && stride == ST) {                                                                                        \
         BARK_CUDA_CHECK(cudaFuncSetAttribute(conv1d_stream_kernel<KW, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem)); \
-        BARK_LAUNCH((conv1d_stream_kernel<KW, ST>), grid, 256, smem, s, x, Cin, L, Lp, Tout, cv.w, cv.Kp, cv.b, cv.cout, o_per_block, elu_in ? 1 : 0, y); \
+        BARK_LAUNCH((conv1d_stream_kernel<KW, ST>), grid, 256, smem, s, x, Cin, cv.w, cv.Kp, cv.b, cv.cout, o_per_block, elu_in ? 1 : 0, y, it); \
         return;                                                                                                              \
     }
     STREAM_CASE(4, 2) STREAM_CASE(8, 4) STREAM_CASE(10, 5) STREAM_CASE(16, 8) STREAM_CASE(7, 1)
@@ -407,38 +470,41 @@ static void conv1d_stream(const float * x, int Cin, int L, const ConvW & cv, int
     fprintf(stderr, "bark_b200: unsupported conv kernel size %d with stride %d\n", cv.k, stride); throw std::runtime_error("unsupported configuration (see the message above)");
 }
 
-void conv1d(const float * x, int Cin, int T, const ConvW & cv, bool elu_in, const float * resid, float * y, cudaStream_t s, int stride) {
+void conv1d(const float * x, int Cin, const int * L, int n, const ConvW & cv, bool elu_in, const float * resid, float * y, cudaStream_t s, int stride) {
     const int K = Cin * cv.k, nsteps = K / 32, ngroups = (nsteps + 7) / 8;
     if (K < 32 && stride == 1) {
-        const int TT = 128, tiles = (T + TT - 1) / TT;
+        const int TT = 128;
+        const CodecItems it = codec_items(n, L, L, L, TT);
+        const int tiles = it.tile0[n];
         int o_per_block = cv.cout;
         const int n_sm = device_sms();
         while (o_per_block > 1 && tiles * ((cv.cout + o_per_block - 1) / o_per_block) < 4 * n_sm) o_per_block = (o_per_block + 1) / 2;
         const size_t smem = (size_t) Cin * (TT + cv.k - 1) * sizeof(float);
-        g_next_flops = 2.0 * (double) T * cv.cout * K;
-        BARK_LAUNCH(conv1d_short_kernel, dim3(tiles, (cv.cout + o_per_block - 1) / o_per_block), TT, smem, s, x, Cin, T, cv.k, cv.w, cv.Kp, cv.b,
-                    cv.cout, o_per_block, elu_in ? 1 : 0, resid, y);
+        g_next_flops = 2.0 * (double) it.base_in[n] * cv.cout * K;
+        BARK_LAUNCH(conv1d_short_kernel, dim3(tiles, (cv.cout + o_per_block - 1) / o_per_block), TT, smem, s, x, Cin, cv.k, cv.w, cv.Kp, cv.b,
+                    cv.cout, o_per_block, elu_in ? 1 : 0, resid, y, it);
         return;
     }
     const bool lane_fits = stride == 1 && ((cv.k == 1 && ngroups <= 2) || (cv.k == 3 && ngroups <= 3) || (cv.k == 7 && ngroups <= 4));
     if (!lane_fits) {
         if (resid) { fprintf(stderr, "bark_b200: unsupported conv shape Cin=%d k=%d stride=%d with a residual\n", Cin, cv.k, stride); throw std::runtime_error("unsupported configuration (see the message above)"); }
-        conv1d_stream(x, Cin, T, cv, stride, elu_in, y, s);
+        conv1d_stream(x, Cin, L, n, cv, stride, elu_in, y, s);
         return;
     }
     const int TT = 32;
     const int S = (TT + cv.k - 1) | 1;
     const size_t smem = (size_t) Cin * S * sizeof(float);
-    const int tiles = (T + TT - 1) / TT;
+    const CodecItems it = codec_items(n, L, L, L, TT);
+    const int tiles = it.tile0[n];
     // enough blocks to fill the machine: split the output channels when there are few time tiles
     int o_per_block = cv.cout;
     const int n_sm = device_sms();
     while (o_per_block > 8 && tiles * ((cv.cout + o_per_block - 1) / o_per_block) < 4 * n_sm) o_per_block = (o_per_block + 1) / 2;
     const dim3 grid(tiles, (cv.cout + o_per_block - 1) / o_per_block);
-    g_next_flops = 2.0 * (double) T * cv.cout * K;
+    g_next_flops = 2.0 * (double) it.base_in[n] * cv.cout * K;
 #define CONV_CASE(KW, NG)                                                                                                   \
     { BARK_CUDA_CHECK(cudaFuncSetAttribute(conv1d_lane_kernel<KW, NG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024)); \
-      BARK_LAUNCH((conv1d_lane_kernel<KW, NG>), grid, 256, smem, s, x, Cin, T, cv.w, cv.Kp, cv.b, cv.cout, o_per_block, elu_in ? 1 : 0, resid, y); }
+      BARK_LAUNCH((conv1d_lane_kernel<KW, NG>), grid, 256, smem, s, x, Cin, cv.w, cv.Kp, cv.b, cv.cout, o_per_block, elu_in ? 1 : 0, resid, y, it); }
     if (cv.k == 1)      { if (ngroups <= 1) CONV_CASE(1, 1) else CONV_CASE(1, 2) }
     else if (cv.k == 3) { if (ngroups <= 1) CONV_CASE(3, 1) else if (ngroups <= 2) CONV_CASE(3, 2) else CONV_CASE(3, 3) }
     else if (cv.k == 7) { if (ngroups <= 1) CONV_CASE(7, 1) else CONV_CASE(7, 4) }
@@ -454,12 +520,14 @@ void conv1d(const float * x, int Cin, int T, const ConvW & cv, bool elu_in, cons
 // into a zeroed buffer, then adds the bias.  Weights arrive re-laid-out as rows [o][tap][Cin] in LI16.
 // ------------------------------------------------------------------------------------------------
 template <int NG>
-__global__ void __launch_bounds__(256) convtr1d_lane_kernel(const float * __restrict__ x, int Cin, int T, const __half * __restrict__ w_li, int Kp,
-                                                            const float * __restrict__ bias, int Cout, int stride, float * __restrict__ y) {
+__global__ void __launch_bounds__(256) convtr1d_lane_kernel(const float * __restrict__ x, int Cin, const __half * __restrict__ w_li, int Kp,
+                                                            const float * __restrict__ bias, int Cout, int stride, float * __restrict__ y,
+                                                            const __grid_constant__ CodecItems its) {
     constexpr int TF = 16;                               // input frames per block
     constexpr int S = TF + 1 + ((TF + 1) % 2 == 0);      // odd stride
     extern __shared__ float xs[];                        // [Cin][S]: frames t0-1 .. t0+TF-1, ELU'd, f16-rounded
-    const int t0 = blockIdx.x * TF;
+    const int b = item_at(its.tile0, its.n, blockIdx.x), T = its.L_in[b], t0 = (blockIdx.x - its.tile0[b]) * TF;
+    x += (size_t) Cin * its.base_in[b]; y += (size_t) Cout * its.base_out[b];
     for (int i = threadIdx.x; i < Cin * (TF + 1); i += blockDim.x) {
         const int c = i / (TF + 1), j = i % (TF + 1);
         const int t = t0 + j - 1;
@@ -497,18 +565,21 @@ __global__ void __launch_bounds__(256) convtr1d_lane_kernel(const float * __rest
     }
 }
 
-void convtr1d(const float * x, int Cin, int T, const ConvW & cv, int stride, float * y, cudaStream_t s) {
+void convtr1d(const float * x, int Cin, const int * T, int n, const ConvW & cv, int stride, float * y, cudaStream_t s) {
     const int nsteps = Cin / 32, ngroups = (nsteps + 7) / 8;
     if (Cin % 32 != 0 || ngroups > 2 || cv.k != 2 * stride) { fprintf(stderr, "bark_b200: unsupported transposed conv Cin=%d k=%d s=%d\n", Cin, cv.k, stride); throw std::runtime_error("unsupported configuration (see the message above)"); }
     const int TF = 16, S = TF + 1 + ((TF + 1) % 2 == 0);
     const size_t smem = (size_t) Cin * S * sizeof(float);
-    const int tiles = (T + TF - 1) / TF;
+    std::vector<int> L((size_t) n);
+    for (int b = 0; b < n; b++) L[(size_t) b] = T[b] * stride;
+    const CodecItems it = codec_items(n, T, L.data(), T, TF);
+    const int tiles = it.tile0[n];
     int gy = (cv.cout * stride + 7) / 8;
     const int n_sm = device_sms();
     while (gy > 1 && tiles * gy > 8 * n_sm) gy = (gy + 1) / 2;
-    g_next_flops = 2.0 * 2.0 * (double) T * stride * cv.cout * Cin;
-    if (ngroups <= 1) BARK_LAUNCH(convtr1d_lane_kernel<1>, dim3(tiles, gy), 256, smem, s, x, Cin, T, cv.w, cv.Kp, cv.b, cv.cout, stride, y);
-    else              BARK_LAUNCH(convtr1d_lane_kernel<2>, dim3(tiles, gy), 256, smem, s, x, Cin, T, cv.w, cv.Kp, cv.b, cv.cout, stride, y);
+    g_next_flops = 2.0 * 2.0 * (double) it.base_out[n] * cv.cout * Cin;
+    if (ngroups <= 1) BARK_LAUNCH(convtr1d_lane_kernel<1>, dim3(tiles, gy), 256, smem, s, x, Cin, cv.w, cv.Kp, cv.b, cv.cout, stride, y, it);
+    else              BARK_LAUNCH(convtr1d_lane_kernel<2>, dim3(tiles, gy), 256, smem, s, x, Cin, cv.w, cv.Kp, cv.b, cv.cout, stride, y, it);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -517,11 +588,12 @@ void convtr1d(const float * x, int Cin, int T, const ConvW & cv, int stride, flo
 //   c = f*c + i*g;  h = o * tanh(c)
 // ------------------------------------------------------------------------------------------------
 // gi[t][g] = vec_dot_f16(C, w_ih[g], f16(x[:, t])) + b_ih[g];   one warp per (t, gate row) pair, weights chain reused over 8 steps
-__global__ void __launch_bounds__(256) lstm_inproj_lane_kernel(const float * __restrict__ x, int C, int T, const __half * __restrict__ wih_li, int Kp,
-                                                               const float * __restrict__ bih, int G4, float * __restrict__ gi) {
+__global__ void __launch_bounds__(256) lstm_inproj_lane_kernel(const float * __restrict__ x, int C, const __half * __restrict__ wih_li, int Kp,
+                                                               const float * __restrict__ bih, int G4, float * __restrict__ gi, const __grid_constant__ CodecItems it) {
     constexpr int TT = 8;
     extern __shared__ float xs[];                        // [TT][C] f16-rounded
-    const int t0 = blockIdx.x * TT;
+    const int b = item_at(it.tile0, it.n, blockIdx.x), T = it.L_in[b], t0 = (blockIdx.x - it.tile0[b]) * TT;
+    x += (size_t) C * it.base_in[b]; gi += (size_t) G4 * it.base_in[b];
     for (int i = threadIdx.x; i < TT * C; i += blockDim.x) {
         const int tl = i / C, c = i % C;
         xs[i] = (t0 + tl < T) ? round_f16(x[(size_t) c * T + t0 + tl]) : 0.f;
@@ -557,10 +629,13 @@ __device__ __forceinline__ void grid_barrier(unsigned * counter, unsigned target
     __syncthreads();
 }
 
+// One sequence (every single-clip call): CTA b owns UPB hidden units; every step it reads h_{t-1}, computes its 4*UPB gates, updates its
+// units and publishes h_t.  Kept beside the batched kernel below because that one, run with one item, is measurably slower per step
+// (DESIGN.md §15); lstm_layer picks between them by the number of items.
 template <int UPB>
-__global__ void __launch_bounds__(UPB * 4 * 32) lstm_recur_kernel(const float * __restrict__ gi, int T, int Hn, const __half * __restrict__ whh_li, int Kp,
-                                                                  const float * __restrict__ bhh, const float * __restrict__ skip,
-                                                                  float * __restrict__ hbuf /*[2][Hn]*/, unsigned * __restrict__ counter, float * __restrict__ out) {
+__global__ void __launch_bounds__(UPB * 4 * 32) lstm_recur_one_kernel(const float * __restrict__ gi, int T, int Hn, const __half * __restrict__ whh_li, int Kp,
+                                                                      const float * __restrict__ bhh, const float * __restrict__ skip,
+                                                                      float * __restrict__ hbuf /*[2][Hn]*/, unsigned * __restrict__ counter, float * __restrict__ out) {
     extern __shared__ float hs[];                        // [Hn] f16-rounded h_{t-1}; then [4*UPB] gate pre-activations
     float * gates = hs + Hn;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;       // warp = local gate row: unit u = warp % UPB, gate q = warp / UPB
@@ -571,7 +646,7 @@ __global__ void __launch_bounds__(UPB * 4 * 32) lstm_recur_kernel(const float * 
     float wch[16];
     load_chain<2>(whh_li + (size_t) row * Kp, lane, (nsteps + 7) >> 3, wch);
     const float bg = bhh[row];
-    float c_state = 0.f;                                 // meaningful in thread (warp = u, lane 0)... kept by threads 0..UPB-1 instead
+    float c_state = 0.f;                                 // kept by threads 0..UPB-1, one per unit
     for (int t = 0; t < T; t++) {
         const float * hprev = hbuf + (size_t)((t + 1) & 1) * Hn;
         for (int j = threadIdx.x; j < Hn; j += blockDim.x) hs[j] = (t == 0) ? 0.f : round_f16(__ldcg(hprev + j));
@@ -597,19 +672,96 @@ __global__ void __launch_bounds__(UPB * 4 * 32) lstm_recur_kernel(const float * 
     }
 }
 
-void lstm_layer(const float * x, int C, int T, const __half * wih_li, const __half * whh_li, int Kp, const float * bih, const float * bhh,
+// Several items: every step carries all B items of the launch; a warp computes its gate row's dot for each item still inside its own
+// sequence (t < T_b), in that item's order and arithmetic (lstm_recur_one_kernel's), so an item's values do not depend on the others.
+// The loop runs max T_b steps with one grid barrier per step; an item past its T_b neither updates nor stores.  Thread (u, b) =
+// (tid % UPB, tid / UPB) keeps unit u's cell state of item b, so B <= blockDim / UPB.
+template <int UPB>
+__global__ void __launch_bounds__(UPB * 4 * 32) lstm_recur_kernel(const float * __restrict__ gi, int T_max, int Hn, const __half * __restrict__ whh_li, int Kp,
+                                                                  const float * __restrict__ bhh, const float * __restrict__ skip,
+                                                                  float * __restrict__ hbuf /*[2][B][Hn]*/, unsigned * __restrict__ counter, float * __restrict__ out,
+                                                                  const __grid_constant__ CodecItems its) {
+    extern __shared__ float hs[];                        // [B][Hn] f16-rounded h_{t-1} of every item; then [B][4*UPB] gate pre-activations
+    __shared__ int s_T[kCodecMaxItems], s_base[kCodecMaxItems];   // the items' lengths and offsets, read every step
+    const int B = its.n;
+    float * gates = hs + (size_t) B * Hn;
+    if ((int) threadIdx.x < B) { s_T[threadIdx.x] = its.L_in[threadIdx.x]; s_base[threadIdx.x] = its.base_in[threadIdx.x]; }
+    __syncthreads();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;       // warp = local gate row: unit u = warp % UPB, gate q = warp / UPB
+    const int u = warp % UPB, q = warp / UPB;
+    const int unit = blockIdx.x * UPB + u;
+    const int row = q * Hn + unit;
+    const int G4 = 4 * Hn, nsteps = Hn >> 5;
+    float wch[16];
+    load_chain<2>(whh_li + (size_t) row * Kp, lane, (nsteps + 7) >> 3, wch);
+    const float bg = bhh[row];
+    float c_state = 0.f;                                 // kept by thread (u, b) for unit u of item b
+    const bool owner = (int) threadIdx.x < UPB * B;
+    const int my_T = owner ? s_T[threadIdx.x / UPB] : 0, my_base = owner ? s_base[threadIdx.x / UPB] : 0;
+    for (int t = 0; t < T_max; t++) {
+        const float * hprev = hbuf + (size_t)((t + 1) & 1) * B * Hn;
+        for (int b = 0; b < B; b++)
+            if (t < s_T[b])
+                for (int j = threadIdx.x; j < Hn; j += blockDim.x) hs[b * Hn + j] = (t == 0) ? 0.f : round_f16(__ldcg(hprev + (size_t) b * Hn + j));
+        __syncthreads();
+        for (int b = 0; b < B; b++) {
+            if (t >= s_T[b]) continue;
+            float acc = 0.f;
+#pragma unroll
+            for (int c = 0; c < 16; c++) if (c < nsteps) acc = __fmaf_rn(wch[c], hs[b * Hn + c * 32 + lane], acc);
+            const float r = lane_tree_reduce(acc);
+            if (lane == 0)                                                                               // (ih + b_ih) + (hh + b_hh)
+                gates[b * 4 * UPB + warp] = __fadd_rn(__ldg(gi + (size_t) G4 * s_base[b] + (size_t) t * G4 + row), __fadd_rn(r, bg));
+        }
+        __syncthreads();
+        if (t < my_T) {                                  // owners only (my_T is 0 for the others)
+            const int uu = threadIdx.x % UPB, b = threadIdx.x / UPB, un = blockIdx.x * UPB + uu;
+            const float * g = gates + b * 4 * UPB;
+            const float it = sigmoid_exact(g[0 * UPB + uu]);
+            const float ft = sigmoid_exact(g[1 * UPB + uu]);
+            const float gt = glibc_tanhf_dev(g[2 * UPB + uu]);
+            const float ot = sigmoid_exact(g[3 * UPB + uu]);
+            c_state = __fadd_rn(__fmul_rn(ft, c_state), __fmul_rn(it, gt));
+            const float h = __fmul_rn(ot, glibc_tanhf_dev(c_state));
+            __stcg(hbuf + (size_t)(t & 1) * B * Hn + (size_t) b * Hn + un, h);
+            const size_t o = (size_t) Hn * my_base + (size_t) un * my_T + t;
+            out[o] = skip ? __fadd_rn(skip[o], h) : h;                                                     // decoder.h:72 inpL + out
+        }
+        grid_barrier(counter, (unsigned)(t + 1) * gridDim.x);
+    }
+}
+
+void lstm_layer(const float * x, int C, const int * T, int n, const __half * wih_li, const __half * whh_li, int Kp, const float * bih, const float * bhh,
                 const float * skip, float * gi_scratch, float * hbuf, unsigned * counter, float * out, cudaStream_t s) {
     const int Hn = C, G4 = 4 * Hn;
     if (Hn % 32 != 0 || Hn > 512 || Hn % 4 != 0) { fprintf(stderr, "bark_b200: unsupported LSTM width %d\n", Hn); throw std::runtime_error("unsupported configuration (see the message above)"); }
-    g_next_flops = 2.0 * (double) T * G4 * C;
-    BARK_LAUNCH(lstm_inproj_lane_kernel, dim3((T + 7) / 8, 32), 256, (size_t) 8 * C * sizeof(float), s, x, C, T, wih_li, Kp, bih, G4, gi_scratch);
+    const CodecItems it = codec_items(n, T, T, T, 8);
+    const int frames = it.base_in[n];
+    int T_max = 0;
+    for (int b = 0; b < n; b++) T_max = std::max(T_max, T[b]);
+    g_next_flops = 2.0 * (double) frames * G4 * C;
+    BARK_LAUNCH(lstm_inproj_lane_kernel, dim3(it.tile0[n], 32), 256, (size_t) 8 * C * sizeof(float), s, x, C, wih_li, Kp, bih, G4, gi_scratch, it);
     BARK_CUDA_CHECK(cudaMemsetAsync(counter, 0, sizeof(unsigned), s));
     constexpr int UPB = 4;
+    static_assert(UPB * kCodecMaxItems <= UPB * 4 * 32, "one thread per (unit, item) holds the cell state");
     const int blocks = Hn / UPB;                         // 128 CTAs for H = 512: co-resident on the 132 SMs of an H100 (cooperative launch checks it)
-    const size_t smem = (size_t)(Hn + 4 * UPB) * sizeof(float);
-    void * args[] = {(void *) &gi_scratch, (void *) &T, (void *) &Hn, (void *) &whh_li, (void *) &Kp, (void *) &bhh, (void *) &skip, (void *) &hbuf, (void *) &counter, (void *) &out};
-    if (g_prof_on) prof_begin("lstm_recur_kernel", s, 0.0, 2.0 * (double) T * G4 * Hn);
-    BARK_CUDA_CHECK(cudaLaunchCooperativeKernel((const void *) lstm_recur_kernel<UPB>, dim3(blocks), dim3(UPB * 4 * 32), args, smem, s));
+    const size_t smem = (size_t) n * (Hn + 4 * UPB) * sizeof(float);
+    if (g_prof_on) prof_begin("lstm_recur_kernel", s, 0.0, 2.0 * (double) frames * G4 * Hn);
+    if (n == 1) {
+        void * args[] = {(void *) &gi_scratch, (void *) &T_max, (void *) &Hn, (void *) &whh_li, (void *) &Kp, (void *) &bhh, (void *) &skip, (void *) &hbuf,
+                         (void *) &counter, (void *) &out};
+        BARK_CUDA_CHECK(cudaLaunchCooperativeKernel((const void *) lstm_recur_one_kernel<UPB>, dim3(blocks), dim3(UPB * 4 * 32), args, smem, s));
+    } else {
+        // The attribute belongs to the function on the device, shared by every context and thread: set once, to the largest launch
+        // (kCodecMaxItems items of the widest LSTM), never per launch.
+        static std::atomic<unsigned long long> configured{0};
+        if (first_use_on_this_device(configured))
+            BARK_CUDA_CHECK(cudaFuncSetAttribute(lstm_recur_kernel<UPB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                 (int)((size_t) kCodecMaxItems * (512 + 4 * UPB) * sizeof(float))));
+        void * args[] = {(void *) &gi_scratch, (void *) &T_max, (void *) &Hn, (void *) &whh_li, (void *) &Kp, (void *) &bhh, (void *) &skip, (void *) &hbuf,
+                         (void *) &counter, (void *) &out, (void *) &it};
+        BARK_CUDA_CHECK(cudaLaunchCooperativeKernel((const void *) lstm_recur_kernel<UPB>, dim3(blocks), dim3(UPB * 4 * 32), args, smem, s));
+    }
     if (g_prof_on) prof_end(s);
     ++g_kernel_launches;
 }

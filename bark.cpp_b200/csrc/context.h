@@ -127,14 +127,21 @@ bool gpt_decode_chained(bark_context * ctx, GPTModel & m, const int32_t * d_toke
 // The EnCodec pipelines, shared by bark_context (8 codebooks) and encodec_context (encodec_api.cu).
 // Reads the codec section at f's position into c: every tensor, codebooks 0..max_q-1 (at least 8 must exist); buffers from arena.
 bool load_codec(std::ifstream & f, CodecModel & c, int max_q, DeviceArena & arena, cudaStream_t s, bool verbose);
-// Decode n_q x T codes to 320 T samples in `audio`.  codes: [n_q][T] on the host, checked against the codebooks; null: the codes already
-// in sc.codes (codec_encode's).
-bool codec_decode(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, const int32_t * codes, int n_q, int T, std::vector<float> & audio);
-// Encode (encodec_compress_audio): n mono 24 kHz samples -> codes [n_q][T] in sc.codes, T = ceil(n / 320), copied to `codes` and the
-// latent [128][T] to `latent` where they are set (then synchronised).  false (message on stderr) without encoder tensors, for
-// n < 1921, a non-finite sample or n_q outside the loaded codebooks.
-bool codec_encode(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, const float * audio, int n, int n_q, std::vector<int32_t> * codes,
-                  std::vector<float> * latent);
+// Both take n clips of independent lengths.  Every item is validated before anything is enqueued; batch_fn: the public batch call, whose
+// name the messages carry and which name the item (null: a single call's messages, under the pipeline's own name);
+// the items then run in consecutive launches, each one pass of the codec kernels over all its items with one
+// synchronisation at its end.  Item i's results are bit-identical to the same clip run alone.
+// Frames of one launch (about 320 s of audio): its scratch is 131 KB per frame, 3.1 GB at the budget.  A longer clip runs alone.
+constexpr int kCodecLaunchFrames = 24000;
+// Decode codes[i] ([n_q][T[i]] on the host, checked against the codebooks, T[i] >= 7) to 320 T[i] samples in audio[i].
+bool codec_decode(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, int n, const int32_t * const * codes, const int * T, int n_q,
+                  std::vector<float> * audio, const char * batch_fn = nullptr);
+// Encode (encodec_compress_audio): audio[i], n_samples[i] mono 24 kHz samples -> codes [n_q][T_i], T_i = ceil(n_samples[i] / 320), copied to
+// codes[i], the latent [128][T_i] to latent[i] and the decoder's waveform of those codes (encodec_reconstruct_audio) to decoded[i] where
+// the arrays are set.  false (message on stderr) without encoder tensors, for n_samples < 1921, a non-finite sample or n_q outside the
+// loaded codebooks.
+bool codec_encode(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, int n, const float * const * audio, const int * n_samples, int n_q,
+                  std::vector<int32_t> * codes, std::vector<float> * latent, std::vector<float> * decoded, const char * batch_fn = nullptr);
 
 // sampling.cu
 constexpr int kSampleMaxLogits = 16384;          // logits of one row: sample_rows_kernel holds the row in 64 KB of shared memory

@@ -151,7 +151,7 @@ extern "C" int bark_b200_rvq_encode(const float * latent, int T, const float * c
             emb[q] = dcb + (size_t) q * n_bins * hidden; nrm[q] = dn + (size_t) q * n_bins;
             rvq_norms(emb[q], n_bins, hidden, dn + (size_t) q * n_bins, 0);
         }
-        if (!rvq_encode(emb, nrm, n_q, n_bins, hidden, dl, T, dc, 0) || !finish("bark_b200_rvq_encode")) return 0;
+        if (!rvq_encode(emb, nrm, n_q, n_bins, hidden, dl, &T, 1, dc, 0) || !finish("bark_b200_rvq_encode")) return 0;
         download(codes, dc, (size_t) n_q * T * 4);
         return 1;
     });

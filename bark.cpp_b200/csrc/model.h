@@ -77,12 +77,12 @@ struct DeviceArena {
     void release();
 };
 
-// EnCodec scratch for a T-frame clip, grown on demand by codec_scratch (gpt_forward.cu), freed by release()
+// EnCodec scratch for one launch's items (T frames in all), grown on demand by codec_scratch (gpt_forward.cu), freed by release()
 struct CodecScratch {
-    float * buf[3] = {nullptr, nullptr, nullptr}; size_t cap = 0;   // ping-pong activations (floats)
+    float * buf[3] = {nullptr, nullptr, nullptr}; size_t cap = 0;   // ping-pong activations (floats), item-major
     float * gi = nullptr;                                            // LSTM input projections
-    float * hbuf = nullptr; unsigned * counter = nullptr;            // LSTM hidden-state exchange + grid barrier counter
-    int32_t * codes = nullptr; size_t codes_cap = 0;                 // [n_q][T]
+    float * hbuf = nullptr; unsigned * counter = nullptr;            // LSTM hidden-state exchange [2][items][512] + grid barrier counter
+    int32_t * codes = nullptr; size_t codes_cap = 0;                 // [n_q][T_b] per item
     void release();
 };
 

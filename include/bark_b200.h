@@ -153,6 +153,28 @@ BARK_API int  bark_b200_sample_filtered_given_u(const float * logits, int n, int
                                                 const double * u, int threads, int32_t * tokens, int32_t * device_tokens, int32_t * flags,
                                                 float * eos_p, int32_t * kept);
 
+/* BATCHED ENCODEC on an encodec_context (include/encodec.h): n clips of independent lengths in one call, for tokenising a dataset.
+ * Item i's codes and waveform are bit-identical to encodec_compress_audio / _decompress_audio / _reconstruct_audio of that clip alone on
+ * the same context: they do not depend on n, on i's place in the batch or on the other items.  The context's current bandwidth and
+ * sample rate apply to every item.  1 <= n <= BARK_B200_ENCODEC_MAX_BATCH.  Every item is checked before anything runs, by the single
+ * calls' rules (audio: n_samples[i] >= 1921 and finite; codes: n_codes[i] a multiple of n_q, n_codes[i] / n_q >= 7 frames, each code in
+ * [0, n_bins)); a null array or entry, n out of range or a bad item returns false with a message naming the item, and changes nothing.
+ * Inside the library the items run in consecutive launches of at most 32 items and 24000 frames (320 s of audio) each, a longer clip
+ * alone; the codec scratch grows to the largest launch (131 KB per frame) and stays with the context.
+ * A batch leaves encodec_get_codes / encodec_get_audio as they were; encodec_get_statistics' t_compute_us is the batch's wall time.
+ *   bark_b200_encodec_compress_batch ..... audio[i]: n_samples[i] mono samples -> codes [n_q][T_i], T_i = ceil(n_samples[i] / 320)
+ *   bark_b200_encodec_decompress_batch ... codes[i]: n_codes[i] codes [n_q][T_i] -> 320 T_i samples
+ *   bark_b200_encodec_reconstruct_batch .. compress then decompress, the codes staying on the device -> 320 T_i samples
+ *   bark_b200_encodec_batch_codes ........ codes of item i of the last successful compress batch; copies min(count, cap) to out (may
+ *                                          be NULL); returns the count, or -1 if there is no such item
+ *   bark_b200_encodec_batch_audio ........ samples of item i of the last successful decompress or reconstruct batch, the same way */
+#define BARK_B200_ENCODEC_MAX_BATCH 1024
+BARK_API bool bark_b200_encodec_compress_batch(struct encodec_context * e, const float * const * audio, const int * n_samples, int n);
+BARK_API bool bark_b200_encodec_decompress_batch(struct encodec_context * e, const int32_t * const * codes, const int * n_codes, int n);
+BARK_API bool bark_b200_encodec_reconstruct_batch(struct encodec_context * e, const float * const * audio, const int * n_samples, int n);
+BARK_API int  bark_b200_encodec_batch_codes(struct encodec_context * e, int i, int32_t * out, int cap);
+BARK_API int  bark_b200_encodec_batch_audio(struct encodec_context * e, int i, float * out, int cap);
+
 /* FAST MODE (BARK_B200_MODE=fast in the environment at load; opt-in, NOT bit-identical to the reference): the fine model's
  * 1024-row passes (bark.cpp:1416-1584) run as wgmma tensor-core GEMMs + flash-style attention (csrc/fast_kernels.cu).
  * Every weight type the loader reads runs it: an f16 file's fine matrices are used as stored; those of an f32, q4_0, q4_1, q5_0, q5_1
