@@ -162,11 +162,16 @@ void filter_rows(const float * logits, int ld, int n, int rows, const bark_b200_
                  cudaStream_t s);
 // the same filter on the host with libm's exp, in place; returns the number of logits kept
 int filter_row_host(float * row, int n, const bark_b200_sampling & f);
+// Copies the sampler's outputs of rows [start, stop) back to the host — tokens to ctx->h_stok, flags to h_sflags, with want_eos the
+// probabilities of the last logit to h_seos, with filtered the filter's flags to h_fflags — and synchronises the stream.
+void read_back_samples(bark_context * ctx, int start, int stop, bool want_eos, bool filtered);
+// after read_back_samples: row r must be decided on the host (flagged by the sampler, or by the filter when one ran)
+inline bool sample_flagged(const bark_context * ctx, int r, bool filtered) { return ctx->h_sflags[r] || (filtered && ctx->h_fflags[r]); }
 // Samples `rows` (<= 1024; <= kMaxFilterRows with a filter) rows of device logits, row r at d_logits + r * ld + lo, n <= kSampleMaxLogits
 // wide, with the uniforms the caller put in ctx->h_u[0, rows) (temp != 0).  With f set and on, filter_rows runs first and the sampler
-// reads its output.  One synchronisation reads the tokens (lo added), the flags and, with want_eos, the probabilities of the last logit
-// back to ctx->h_stok / h_sflags / h_seos; every row flagged by either kernel is then replayed on the host (filter_row_host from the raw
-// logits, then sample_token_given_u with the same uniform).  Returns the number of rows replayed.
+// reads its output.  One read_back_samples brings the tokens (lo added), the flags and, with want_eos, the probabilities of the last
+// logit back; every row flagged by either kernel is then replayed on the host (filter_row_host from the raw logits, then
+// sample_token_given_u with the same uniform).  Returns the number of rows replayed.
 int sample_and_replay(bark_context * ctx, const float * d_logits, int ld, int lo, int n, int rows, float temp, bool want_eos, const bark_b200_sampling * f = nullptr);
 // sample_and_replay with `rows` uniforms drawn from rng; tokens to out_tok, eos probabilities to out_eos when it is set
 bool sample_device(bark_context * ctx, GPTModel & m, std::mt19937 & rng, const float * d_logits, int ld, int n, int rows, float temp, int32_t * out_tok, float * out_eos);

@@ -356,6 +356,17 @@ int32_t sample_token_given_u(const float * logits, int n, float temp, double u, 
     return (int32_t)(std::lower_bound(cp.begin(), cp.end(), u) - cp.begin());
 }
 
+void read_back_samples(bark_context * ctx, int start, int stop, bool want_eos, bool filtered) {
+    cudaStream_t s = ctx->stream;
+    const size_t cnt = (size_t)(stop - start);
+    if (filtered) { BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->h_fflags + start, ctx->d_fflags + start, cnt * 4, cudaMemcpyDeviceToHost, s)); g_d2h_bytes += cnt * 4; }
+    BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->h_stok + start, ctx->d_stok + start, cnt * 4, cudaMemcpyDeviceToHost, s));
+    BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->h_sflags + start, ctx->d_sflags + start, cnt * 4, cudaMemcpyDeviceToHost, s));
+    if (want_eos) BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->h_seos + start, ctx->d_seos + start, cnt * 4, cudaMemcpyDeviceToHost, s));
+    g_d2h_bytes += cnt * (want_eos ? 12 : 8);
+    BARK_CUDA_CHECK(cudaStreamSynchronize(s));
+}
+
 int sample_and_replay(bark_context * ctx, const float * d_logits, int ld, int lo, int n, int rows, float temp, bool want_eos, const bark_b200_sampling * f) {
     cudaStream_t s = ctx->stream;
     if (temp != 0.0f) { BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->d_u, ctx->h_u, (size_t) rows * sizeof(double), cudaMemcpyHostToDevice, s)); g_h2d_bytes += (size_t) rows * sizeof(double); }
@@ -365,18 +376,13 @@ int sample_and_replay(bark_context * ctx, const float * d_logits, int ld, int lo
         if (rows > kMaxFilterRows) throw std::logic_error("sample_and_replay: more rows than the filter workspace holds");
         filter_rows(d_logits + lo, ld, n, rows, *f, ctx->d_frow, nullptr, ctx->d_fflags, 0, s);
         sample_rows(ctx->d_frow, n, n, rows, temp, ctx->d_u, ctx->d_stok, lo, nullptr, ctx->d_seos, ctx->d_sflags, force, 0, s);
-        BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->h_fflags, ctx->d_fflags, (size_t) rows * 4, cudaMemcpyDeviceToHost, s)); g_d2h_bytes += (size_t) rows * 4;
     } else {
         sample_rows(d_logits + lo, ld, n, rows, temp, ctx->d_u, ctx->d_stok, lo, nullptr, ctx->d_seos, ctx->d_sflags, force, 0, s);
     }
-    BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->h_stok, ctx->d_stok, (size_t) rows * 4, cudaMemcpyDeviceToHost, s));
-    BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->h_sflags, ctx->d_sflags, (size_t) rows * 4, cudaMemcpyDeviceToHost, s));
-    if (want_eos) BARK_CUDA_CHECK(cudaMemcpyAsync(ctx->h_seos, ctx->d_seos, (size_t) rows * 4, cudaMemcpyDeviceToHost, s));
-    g_d2h_bytes += (size_t) rows * (want_eos ? 12 : 8);
-    BARK_CUDA_CHECK(cudaStreamSynchronize(s));
+    read_back_samples(ctx, 0, rows, want_eos, filtered);
     int replays = 0;
     std::vector<float> row;
-    for (int r = 0; r < rows; r++) if (ctx->h_sflags[r] || (filtered && ctx->h_fflags[r])) {
+    for (int r = 0; r < rows; r++) if (sample_flagged(ctx, r, filtered)) {
         row.resize((size_t) n);
         BARK_CUDA_CHECK(cudaMemcpy(row.data(), d_logits + (size_t) r * ld + lo, (size_t) n * 4, cudaMemcpyDeviceToHost)); g_d2h_bytes += (size_t) n * 4;
         if (filtered) filter_row_host(row.data(), n, *f);             // the raw logits are still on the device: restate the filter from them
