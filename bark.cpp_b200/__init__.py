@@ -11,6 +11,7 @@ The directory name contains a dot, so import it through `__graft_entry__.load_pa
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 
 import numpy as np
@@ -114,6 +115,8 @@ EXPORTS = [
     "bark_b200_quant_matmul", "bark_b200_fast_convert",
     "bark_b200_encodec_compress_batch", "bark_b200_encodec_decompress_batch", "bark_b200_encodec_reconstruct_batch",
     "bark_b200_encodec_batch_codes", "bark_b200_encodec_batch_audio",
+    "bark_b200_encodec_compress_resampled", "bark_b200_encodec_reconstruct_resampled", "bark_b200_encodec_compress_batch_resampled",
+    "bark_b200_encodec_reconstruct_batch_resampled", "bark_b200_encodec_encode_resampled", "bark_b200_resample",
     "ggml_time_init", "ggml_time_us", "ggml_time_ms", "ggml_init", "ggml_free",
 ]
 
@@ -237,6 +240,16 @@ def lib() -> C.CDLL:
     for n in ("bark_b200_encodec_batch_codes", "bark_b200_encodec_batch_audio"):
         getattr(L, n).restype = C.c_int
         getattr(L, n).argtypes = [vp, C.c_int, vp, C.c_int]
+    for n in ("bark_b200_encodec_compress_resampled", "bark_b200_encodec_reconstruct_resampled"):
+        getattr(L, n).restype = C.c_bool
+        getattr(L, n).argtypes = [vp, f32p, C.c_int, C.c_int, C.c_int]
+    for n in ("bark_b200_encodec_compress_batch_resampled", "bark_b200_encodec_reconstruct_batch_resampled"):
+        getattr(L, n).restype = C.c_bool
+        getattr(L, n).argtypes = [vp, vp, vp, vp, vp, C.c_int]
+    L.bark_b200_encodec_encode_resampled.restype = C.c_int
+    L.bark_b200_encodec_encode_resampled.argtypes = [vp, f32p, C.c_int, C.c_int, C.c_int, i32p, C.c_int, f32p, C.c_int]
+    L.bark_b200_resample.restype = C.c_int
+    L.bark_b200_resample.argtypes = [f32p, C.c_int, C.c_int, C.c_int, C.c_int, f32p, C.c_int]
     L.ggml_time_us.restype = C.c_int64
     L.encodec_load_model.restype = vp
     L.encodec_load_model.argtypes = [C.c_char_p, C.c_int, C.c_int]
@@ -261,6 +274,41 @@ def lib() -> C.CDLL:
 
 def _p(a: np.ndarray):
     return a.ctypes.data_as(C.c_void_p)
+
+
+CODEC_RATE = 24000          # the EnCodec model's sample rate
+
+
+def _frames(audio):
+    """(interleaved float32 frames [n][C] flattened, n, C) of mono samples [n] or of [channels][n_frames], the layout torchaudio.load
+    returns and upstream EnCodec's convert_audio takes."""
+    a = np.asarray(audio, np.float32)
+    if a.ndim == 1:
+        return np.ascontiguousarray(a), a.size, 1
+    if a.ndim != 2:
+        raise ValueError(f"audio of shape {a.shape}: [n_frames] or [channels][n_frames]")
+    return np.ascontiguousarray(a.T).ravel(), a.shape[1], a.shape[0]
+
+
+def resampled_length(n_frames: int, sr: int, new_sr: int = CODEC_RATE) -> int:
+    """L = ceil(new_sr n / sr), exactly: the samples of n frames at sr resampled to new_sr (0 for a rate below 1, which the library
+    refuses)."""
+    if sr < 1 or new_sr < 1:
+        return 0
+    g = math.gcd(sr, new_sr)
+    return -(-(new_sr // g) * n_frames // (sr // g))
+
+
+def resample(audio, sr: int, new_sr: int) -> np.ndarray:
+    """audio (mono [n] or [channels][n]) at sr Hz down-mixed and resampled to new_sr Hz on the GPU (bark_b200_resample, DESIGN.md
+    §16): torchaudio.functional.resample's default filter with an exact summation order, bit-reproducible.  Both rates in [4000,
+    384000].  Returns float32 [ceil(new_sr n / sr)]."""
+    x, n, ch = _frames(audio)
+    out = np.zeros(max(resampled_length(n, int(sr), int(new_sr)), 1), np.float32)
+    r = lib().bark_b200_resample(_p(x), n, ch, int(sr), int(new_sr), _p(out), out.size)
+    if r < 0:
+        raise RuntimeError(f"bark_b200_resample ({n} frames of {ch} channels, {sr} -> {new_sr} Hz) failed (see stderr)")
+    return out[:r]
 
 
 class Bark:
@@ -452,15 +500,25 @@ class Bark:
             raise RuntimeError("bark_b200_encodec_decode failed")
         return out[:n]
 
-    def encodec_encode(self, audio, return_latent: bool = False):
+    def encodec_encode(self, audio, return_latent: bool = False, sample_rate: int | None = None):
         """Mono 24 kHz float32 samples (finite, at least 1921) -> codes [8][T] int32, T = ceil(n / 320), the layout encodec_decode
-        takes; with return_latent also the encoder output before quantisation, [128][T] float32."""
-        a = np.ascontiguousarray(audio, np.float32).ravel()
-        T = (a.size + 319) // 320
+        takes; with return_latent also the encoder output before quantisation, [128][T] float32.  With sample_rate, audio is mono [n] or
+        [channels][n] at that rate, down-mixed and resampled to 24 kHz on the GPU first (bark_b200_encodec_encode_resampled): a fine
+        prompt from a speaker clip; T then counts the resampled samples."""
+        if sample_rate is None:
+            a = np.ascontiguousarray(audio, np.float32).ravel()
+            n = a.size
+        else:
+            a, nf, ch = _frames(audio)
+            n = resampled_length(nf, int(sample_rate))
+        T = (n + 319) // 320
         codes = np.zeros((8, max(T, 1)), np.int32); lat = np.zeros((128, max(T, 1)), np.float32)
-        r = lib().bark_b200_encodec_encode(self.ctx, _p(a), a.size, _p(codes), codes.size, _p(lat), lat.size)
+        if sample_rate is None:
+            r = lib().bark_b200_encodec_encode(self.ctx, _p(a), a.size, _p(codes), codes.size, _p(lat), lat.size)
+        else:
+            r = lib().bark_b200_encodec_encode_resampled(self.ctx, _p(a), nf, ch, int(sample_rate), _p(codes), codes.size, _p(lat), lat.size)
         if r < 0:
-            raise RuntimeError("bark_b200_encodec_encode failed (see stderr)")
+            raise RuntimeError(f"bark_b200_encodec_encode{'' if sample_rate is None else '_resampled'} failed (see stderr)")
         assert r == T, (r, T)
         return (codes, lat) if return_latent else codes
 
@@ -785,13 +843,22 @@ class Encodec:
         """Codebooks of the current bandwidth and sample rate, read from the codes of a minimal compress."""
         return self.compress(np.zeros(1921, np.float32)).shape[0]
 
-    def compress(self, audio) -> np.ndarray:
-        """Mono float32 samples (finite, at least 1921) -> codes [n_q][T] int32, T = ceil(n / 320)."""
-        a = np.ascontiguousarray(audio, np.float32).ravel()
-        if not lib().encodec_compress_audio(self.ctx, _p(a), a.size, 1):
-            raise RuntimeError("encodec_compress_audio failed (see stderr)")
+    def compress(self, audio, sample_rate: int | None = None) -> np.ndarray:
+        """Mono float32 samples (finite, at least 1921) -> codes [n_q][T] int32, T = ceil(n / 320).  With sample_rate, audio is mono
+        [n] or [channels][n] at that rate, down-mixed and resampled to 24 kHz on the GPU first (bark_b200_encodec_compress_resampled);
+        n then counts the resampled samples."""
+        if sample_rate is None:
+            a = np.ascontiguousarray(audio, np.float32).ravel()
+            if not lib().encodec_compress_audio(self.ctx, _p(a), a.size, 1):
+                raise RuntimeError("encodec_compress_audio failed (see stderr)")
+            L = a.size
+        else:
+            a, nf, ch = _frames(audio)
+            if not lib().bark_b200_encodec_compress_resampled(self.ctx, _p(a), nf, ch, int(sample_rate)):
+                raise RuntimeError("bark_b200_encodec_compress_resampled failed (see stderr)")
+            L = resampled_length(nf, int(sample_rate))
         n = lib().encodec_get_codes_size(self.ctx)
-        T = (a.size + 319) // 320
+        T = (L + 319) // 320
         return np.ctypeslib.as_array(lib().encodec_get_codes(self.ctx), shape=(n,)).copy().reshape(n // T, T)
 
     def decompress(self, codes) -> np.ndarray:
@@ -801,11 +868,16 @@ class Encodec:
             raise RuntimeError("encodec_decompress_audio failed (see stderr)")
         return self._audio()
 
-    def reconstruct(self, audio) -> np.ndarray:
-        """compress then decompress on the device: 320 T float32 samples."""
-        a = np.ascontiguousarray(audio, np.float32).ravel()
-        if not lib().encodec_reconstruct_audio(self.ctx, _p(a), a.size, 1):
-            raise RuntimeError("encodec_reconstruct_audio failed (see stderr)")
+    def reconstruct(self, audio, sample_rate: int | None = None) -> np.ndarray:
+        """compress then decompress on the device: 320 T float32 samples (24 kHz).  sample_rate as for compress."""
+        if sample_rate is None:
+            a = np.ascontiguousarray(audio, np.float32).ravel()
+            if not lib().encodec_reconstruct_audio(self.ctx, _p(a), a.size, 1):
+                raise RuntimeError("encodec_reconstruct_audio failed (see stderr)")
+        else:
+            a, nf, ch = _frames(audio)
+            if not lib().bark_b200_encodec_reconstruct_resampled(self.ctx, _p(a), nf, ch, int(sample_rate)):
+                raise RuntimeError("bark_b200_encodec_reconstruct_resampled failed (see stderr)")
         return self._audio()
 
     def _audio(self):
@@ -813,14 +885,20 @@ class Encodec:
         return np.ctypeslib.as_array(lib().encodec_get_audio(self.ctx), shape=(n,)).copy()
 
     # ---- batches (bark_b200_encodec_*_batch): item i equals the single call on clip i, bit for bit --------------------------------
-    def compress_batch(self, clips) -> list:
-        """Clips of mono float32 samples (each finite, at least 1921) -> codes [n_q][T_i] int32 per clip, in one batched call."""
-        xs = [np.ascontiguousarray(a, np.float32).ravel() for a in clips]
-        self._batch("bark_b200_encodec_compress_batch", xs)
+    def compress_batch(self, clips, sample_rate=None) -> list:
+        """Clips of mono float32 samples (each finite, at least 1921) -> codes [n_q][T_i] int32 per clip, in one batched call.  With
+        sample_rate (one rate, or a list of one per clip), each clip is mono [n] or [channels][n] at its rate, down-mixed and resampled
+        to 24 kHz on the GPU first (bark_b200_encodec_compress_batch_resampled)."""
+        if sample_rate is None:
+            xs = [np.ascontiguousarray(a, np.float32).ravel() for a in clips]
+            self._batch("bark_b200_encodec_compress_batch", xs)
+            lens = [x.size for x in xs]
+        else:
+            lens = self._batch_resampled("bark_b200_encodec_compress_batch_resampled", clips, sample_rate)
         out = []
-        for i, x in enumerate(xs):
+        for i, n in enumerate(lens):
             c = self._item("bark_b200_encodec_batch_codes", i, np.int32)
-            T = (x.size + 319) // 320
+            T = (n + 319) // 320
             out.append(c.reshape(c.size // T, T))
         return out
 
@@ -830,11 +908,30 @@ class Encodec:
         self._batch("bark_b200_encodec_decompress_batch", cs)
         return [self._item("bark_b200_encodec_batch_audio", i, np.float32) for i in range(len(cs))]
 
-    def reconstruct_batch(self, clips) -> list:
-        """compress_batch then decompress_batch, the codes staying on the device: 320 T_i float32 samples per clip."""
-        xs = [np.ascontiguousarray(a, np.float32).ravel() for a in clips]
-        self._batch("bark_b200_encodec_reconstruct_batch", xs)
+    def reconstruct_batch(self, clips, sample_rate=None) -> list:
+        """compress_batch then decompress_batch, the codes staying on the device: 320 T_i float32 samples per clip.  sample_rate as for
+        compress_batch."""
+        if sample_rate is None:
+            xs = [np.ascontiguousarray(a, np.float32).ravel() for a in clips]
+            self._batch("bark_b200_encodec_reconstruct_batch", xs)
+        else:
+            xs = self._batch_resampled("bark_b200_encodec_reconstruct_batch_resampled", clips, sample_rate)
         return [self._item("bark_b200_encodec_batch_audio", i, np.float32) for i in range(len(xs))]
+
+    def _batch_resampled(self, fn, clips, sample_rate):
+        """Runs a resampled batch call; returns the clips' resampled lengths."""
+        fr = [_frames(a) for a in clips]
+        n = len(fr)
+        rates = [int(sample_rate)] * n if np.ndim(sample_rate) == 0 else [int(r) for r in sample_rate]
+        if len(rates) != n:
+            raise ValueError(f"{fn}: {n} clips but {len(rates)} sample rates")
+        ptrs = (C.c_void_p * max(n, 1))(*[x.ctypes.data for x, _, _ in fr])
+        frames = (C.c_int * max(n, 1))(*[nf for _, nf, _ in fr])
+        chans = (C.c_int * max(n, 1))(*[ch for _, _, ch in fr])
+        srs = (C.c_int * max(n, 1))(*rates)
+        if not getattr(lib(), fn)(self.ctx, ptrs, frames, chans, srs, n):
+            raise RuntimeError(f"{fn} failed (see stderr)")
+        return [resampled_length(nf, r) for (_, nf, _), r in zip(fr, rates)]
 
     def _batch(self, fn, arrays):
         n = len(arrays)

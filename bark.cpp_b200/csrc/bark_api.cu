@@ -884,11 +884,12 @@ static int bark_b200_encodec_decode_impl(struct bark_context * ctx, const int32_
 }
 extern "C" int bark_b200_encodec_decode(struct bark_context * ctx, const int32_t * codes, int n_frames, float * out, int out_cap) { return guarded((int) -1, [&] { return bark_b200_encodec_decode_impl(ctx, codes, n_frames, out, out_cap); }); }
 static int bark_b200_encodec_encode_impl(struct bark_context * ctx, const float * audio, int n_samples, int32_t * codes, int codes_cap, float * latent,
-                                         int latent_cap) {
-    if (!ctx || !audio) { fprintf(stderr, "bark_b200_encodec_encode: null %s\n", ctx ? "audio" : "context"); return -1; }
+                                         int latent_cap, const AudioFormat * fmt = nullptr) {
+    const char * fn = fmt ? "bark_b200_encodec_encode_resampled" : "bark_b200_encodec_encode";
+    if (!ctx || !audio) { fprintf(stderr, "%s: null %s\n", fn, ctx ? "audio" : "context"); return -1; }
     BARK_CUDA_CHECK(cudaSetDevice(ctx->device));
     std::vector<int32_t> c; std::vector<float> l;
-    if (!codec_encode(ctx->codec, ctx->codec_scratch, ctx->stream, 1, &audio, &n_samples, 8, &c, &l, nullptr)) return -1;
+    if (!codec_encode(ctx->codec, ctx->codec_scratch, ctx->stream, 1, &audio, &n_samples, 8, &c, &l, nullptr, nullptr, fmt)) return -1;
     if (codes) memcpy(codes, c.data(), sizeof(int32_t) * std::min(c.size(), (size_t) std::max(codes_cap, 0)));
     if (latent) memcpy(latent, l.data(), sizeof(float) * std::min(l.size(), (size_t) std::max(latent_cap, 0)));
     return (int)(c.size() / 8);
@@ -896,6 +897,11 @@ static int bark_b200_encodec_encode_impl(struct bark_context * ctx, const float 
 extern "C" int bark_b200_encodec_encode(struct bark_context * ctx, const float * audio, int n_samples, int32_t * codes, int codes_cap, float * latent,
                                         int latent_cap) {
     return guarded((int) -1, [&] { return bark_b200_encodec_encode_impl(ctx, audio, n_samples, codes, codes_cap, latent, latent_cap); });
+}
+extern "C" int bark_b200_encodec_encode_resampled(struct bark_context * ctx, const float * audio, int n_frames, int channels, int sample_rate, int32_t * codes,
+                                                  int codes_cap, float * latent, int latent_cap) {
+    const AudioFormat f{channels, sample_rate};
+    return guarded((int) -1, [&] { return bark_b200_encodec_encode_impl(ctx, audio, n_frames, codes, codes_cap, latent, latent_cap, &f); });
 }
 extern "C" int bark_b200_sample(struct bark_context * ctx, int which, const float * logits, int n, float temp, float * eos_p) {
     if (!ctx || !logits || n < 1) return -1;

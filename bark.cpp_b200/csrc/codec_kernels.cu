@@ -15,6 +15,10 @@
 #include "codec_kernels.h"
 
 #include <algorithm>
+#include <climits>
+#include <cmath>
+#include <cstring>
+#include <numeric>
 #include <vector>
 
 #include <cooperative_groups.h>
@@ -776,6 +780,116 @@ __global__ void convtr_rows_kernel(const __half * __restrict__ src, __half * __r
 }
 void convtr_rows(const __half * src, __half * dst, int Cin, int Cout, int k, cudaStream_t s) {
     BARK_LAUNCH(convtr_rows_kernel, 592, 256, 0, s, src, dst, Cin, Cout, k);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Resampling (DESIGN.md §16): torchaudio.functional.resample(u, sr, new_sr) with sinc_interp_hann, width W = 6, rolloff 0.99, on the
+// down-mix u[i] = (x[i][0] + ... + x[i][C-1]) / C of upstream EnCodec's convert_audio.  Output k q + j is
+//   y = (float) sum_m u[k o + m - w] h[j][m],
+// a double accumulator from +0 in increasing m over phase j's nonzero f32 taps (each product is exact in double, so the fma is the
+// multiply-then-add), zeros outside [0, n).  The ±0 taps left out cannot change it: the accumulator is never -0.
+// ------------------------------------------------------------------------------------------------
+constexpr int kResampleW = 6, kResampleTile = 256, kResampleSmemFloats = 12224;     // outputs per CTA at most; input window within 48 KB
+
+long long resample_len(long long n, int sr, int new_sr) {
+    const long long g = std::gcd(sr, new_sr), o = sr / g, q = new_sr / g;
+    return (q * n + o - 1) / o;
+}
+
+std::vector<unsigned char> resample_table(int sr, int new_sr, ResampleTable * t) {
+    ResampleTable r;
+    r.sr = sr; r.new_sr = new_sr;
+    std::vector<unsigned char> bytes;
+    if (sr == new_sr) { r.tile = r.smem = kResampleTile; *t = r; return bytes; }
+    const int g = std::gcd(sr, new_sr), o = sr / g, q = new_sr / g;
+    const double pi = 3.141592653589793, base = std::min(o, q) * 0.99, reach = (double)(kResampleW * o) / base, scale = base / o;
+    const int w = (int) std::ceil(reach);
+    r.o = o; r.q = q; r.w = w;
+    // h[j][m] in torchaudio's expression order (_get_sinc_resample_kernel) with the C library's sin and cos
+    auto tap = [&](int j, int m) {
+        double x = ((double) -j / q + (double)(m - w) / o) * base;
+        x = std::min(std::max(x, (double) -kResampleW), (double) kResampleW);
+        const double c = std::cos(x * pi / kResampleW / 2), win = c * c;
+        x *= pi;
+        const double s = x == 0 ? 1.0 : std::sin(x) / x;
+        return (float)(s * (win * scale));
+    };
+    // Outside |x| < W every tap is the clamped sinc(±6 pi) cos^2(±pi/2), about 1e-49, so ±0 in f32: phase j's nonzero taps lie within
+    // reach of its centre w + o j / q, and the candidates are that range plus one index on each side
+    std::vector<int4> phase((size_t) q);
+    std::vector<float> taps;
+    for (int j = 0; j < q; j++) {
+        const double centre = w + (double)((long long) o * j) / q;
+        int lo = std::max(0, (int) std::floor(centre - reach) - 1), hi = std::min(2 * w + o - 1, (int) std::ceil(centre + reach) + 1);
+        while (lo <= hi && tap(j, lo) == 0.0f) lo++;
+        while (hi >= lo && tap(j, hi) == 0.0f) hi--;
+        phase[(size_t) j] = make_int4(lo, std::max(hi - lo + 1, 0), (int) taps.size(), 0);
+        for (int m = lo; m <= hi; m++) taps.push_back(tap(j, m));
+    }
+    // a CTA's window: its outputs' inputs lie within reach + 2 of o i / q
+    for (r.tile = kResampleTile; ; r.tile -= 32) {
+        r.smem = (int) std::ceil((r.tile - 1) * (double) o / q + 2 * reach) + 6;
+        if (r.smem <= kResampleSmemFloats || r.tile == 32) break;
+    }
+    bytes.resize(phase.size() * sizeof(int4) + taps.size() * sizeof(float));
+    memcpy(bytes.data(), phase.data(), phase.size() * sizeof(int4));
+    memcpy(bytes.data() + phase.size() * sizeof(int4), taps.data(), taps.size() * sizeof(float));
+    *t = r;
+    return bytes;
+}
+
+void resample_bind(ResampleTable & t, const void * dev) {
+    if (t.sr == t.new_sr) return;
+    t.phase = (const int4 *) dev;
+    t.taps = (const float *)((const int4 *) dev + t.q);
+}
+
+// One CTA per `tile` consecutive outputs.  The CTA finds the span of input its outputs read (the first input and tap count of each
+// output's phase), loads it once, down-mixed, into shared memory, and each thread then sums one output over its phase's taps, which
+// are read from global memory (the table stays in L2).  phase null: the identity, y = u.
+__global__ void __launch_bounds__(kResampleTile) resample_kernel(const float * __restrict__ x, long long n, int C, const int4 * __restrict__ phase,
+                                                                 const float * __restrict__ taps, int o, int q, int w, int tile, int L, float * __restrict__ y) {
+    extern __shared__ float su[];
+    __shared__ int window[2];
+    const long long i0 = (long long) blockIdx.x * tile, i = i0 + threadIdx.x, k0 = i0 / q;
+    const bool active = (int) threadIdx.x < tile && i < L;
+    if (threadIdx.x == 0) { window[0] = INT_MAX; window[1] = INT_MIN; }
+    __syncthreads();
+    int4 p = make_int4(0, 1, 0, 0);
+    int r = (int) threadIdx.x;                                  // output i's first input, relative to k0 o
+    if (active && phase) {
+        const long long k = i / q;
+        p = phase[i - k * q];
+        r = (int)((k - k0) * o) + p.x - w;
+    }
+    if (active && p.y > 0) { atomicMin(&window[0], r); atomicMax(&window[1], r + p.y); }
+    __syncthreads();
+    const int lo = window[0], span = window[1] - window[0];
+    const long long g0 = k0 * o + lo;
+    for (int s = threadIdx.x; s < span; s += blockDim.x) {
+        const long long g = g0 + s;
+        float v = 0.0f;
+        if (g >= 0 && g < n) {
+            const float * f = x + g * C;
+            v = f[0];
+            for (int c = 1; c < C; c++) v = __fadd_rn(v, f[c]);
+            if (C > 1) v = __fdiv_rn(v, (float) C);
+        }
+        su[s] = v;
+    }
+    __syncthreads();
+    if (!active) return;
+    if (!phase) { y[i] = su[r - lo]; return; }
+    const float * u = su + (r - lo), * h = taps + p.z;
+    double acc = 0.0;
+    for (int c = 0; c < p.y; c++) acc = __fma_rn((double) u[c], (double) h[c], acc);
+    y[i] = __double2float_rn(acc);
+}
+
+void resample(const float * x, long long n, int C, const ResampleTable & t, float * y, int L, cudaStream_t s) {
+    if (L < 1) return;
+    const long long grid = ((long long) L + t.tile - 1) / t.tile;
+    BARK_LAUNCH(resample_kernel, (unsigned) grid, kResampleTile, (size_t) t.smem * sizeof(float), s, x, n, C, t.phase, t.taps, t.o, t.q, t.w, t.tile, L, y);
 }
 
 }  // namespace bark

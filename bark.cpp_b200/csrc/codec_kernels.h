@@ -30,4 +30,17 @@ void lstm_layer(const float * x, int C, const int * T, int n, const __half * wih
 // load-time re-layout of a transposed-conv weight: [Cin][Cout][k] -> rows [Cout][k][Cin]
 void convtr_rows(const __half * src, __half * dst, int Cin, int Cout, int k, cudaStream_t s);
 
+// Resampling (DESIGN.md §16): torchaudio.functional.resample's default sinc_interp_hann filter with an exact summation order, after
+// upstream EnCodec's channel down-mix.  Both rates lie in [kResampleMinRate, kResampleMaxRate].
+constexpr int kResampleMinRate = 4000, kResampleMaxRate = 384000, kResampleMaxChannels = 8;
+// L = ceil(q n / o): samples of n frames at sr resampled to new_sr
+long long resample_len(long long n, int sr, int new_sr);
+// The taps of sr -> new_sr in double by the rule, rounded to f32, each phase trimmed to its nonzero span; fills t's sizes and returns
+// the bytes to upload (phases, then taps; empty for the identity)
+std::vector<unsigned char> resample_table(int sr, int new_sr, ResampleTable * t);
+// points t at its uploaded bytes
+void resample_bind(ResampleTable & t, const void * dev);
+// x: n interleaved frames [n][C] (device) -> y [L] (device), L = resample_len(n, t.sr, t.new_sr)
+void resample(const float * x, long long n, int C, const ResampleTable & t, float * y, int L, cudaStream_t s);
+
 }  // namespace bark

@@ -140,8 +140,16 @@ bool codec_decode(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, int 
 // codes[i], the latent [128][T_i] to latent[i] and the decoder's waveform of those codes (encodec_reconstruct_audio) to decoded[i] where
 // the arrays are set.  false (message on stderr) without encoder tensors, for n_samples < 1921, a non-finite sample or n_q outside the
 // loaded codebooks.
+// With fmt, item i is n_samples[i] interleaved frames [n][fmt[i].channels] at fmt[i].sample_rate, down-mixed and resampled to 24 kHz on
+// the device first (DESIGN.md §16); its resampled length L_i then stands for n_samples[i].  Mono 24 kHz items go in unchanged.
+constexpr int kCodecSampleRate = 24000;
+struct AudioFormat { int channels, sample_rate; };
 bool codec_encode(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, int n, const float * const * audio, const int * n_samples, int n_q,
-                  std::vector<int32_t> * codes, std::vector<float> * latent, std::vector<float> * decoded, const char * batch_fn = nullptr);
+                  std::vector<int32_t> * codes, std::vector<float> * latent, std::vector<float> * decoded, const char * batch_fn = nullptr,
+                  const AudioFormat * fmt = nullptr);
+// false (message naming fn, and the item for a batch) for a format or clip outside the resampler's limits: 1 to 8 channels, 4000 to
+// 384000 Hz, fewer than 2^31 samples, every sample finite with |x| <= 2^64
+bool resample_input_ok(const char * fn, const std::string & item, const float * x, int n_frames, int channels, int sample_rate);
 
 // sampling.cu
 constexpr int kSampleMaxLogits = 16384;          // logits of one row: sample_rows_kernel holds the row in 64 KB of shared memory

@@ -184,6 +184,77 @@ extern "C" bool bark_b200_encodec_reconstruct_batch(struct encodec_context * e, 
     });
 }
 
+// ---- resampled calls (include/bark_b200.h, RESAMPLED ENCODEC) -------------------------------------------------------------------
+extern "C" bool bark_b200_encodec_compress_resampled(struct encodec_context * e, const float * audio, int n_frames, int channels, int sample_rate) {
+    return run(e, __func__, [&] {
+        const char * fn = "bark_b200_encodec_compress_resampled";
+        int n_q;
+        if (!audio) { fprintf(stderr, "%s: null input audio\n", fn); return false; }
+        if (!codebooks_for(e, fn, &n_q)) return false;
+        const AudioFormat f{channels, sample_rate};
+        std::vector<int32_t> codes;
+        if (!codec_encode(e->model, e->scratch, e->stream, 1, &audio, &n_frames, n_q, &codes, nullptr, nullptr, nullptr, &f)) return false;
+        e->codes.swap(codes);
+        return true;
+    });
+}
+
+extern "C" bool bark_b200_encodec_reconstruct_resampled(struct encodec_context * e, const float * audio, int n_frames, int channels, int sample_rate) {
+    return run(e, __func__, [&] {
+        const char * fn = "bark_b200_encodec_reconstruct_resampled";
+        int n_q;
+        if (!audio) { fprintf(stderr, "%s: null input audio\n", fn); return false; }
+        if (!codebooks_for(e, fn, &n_q)) return false;
+        const AudioFormat f{channels, sample_rate};
+        std::vector<float> out;
+        if (!codec_encode(e->model, e->scratch, e->stream, 1, &audio, &n_frames, n_q, nullptr, nullptr, &out, nullptr, &f)) return false;
+        e->audio.swap(out);
+        return true;
+    });
+}
+
+namespace {
+
+// a batch call with per-item formats: batch_args' checks, then the two format arrays
+bool resampled_batch_formats(const char * fn, const float * const * audio, const int * n_frames, const int * channels, const int * sample_rates, int n,
+                             std::vector<AudioFormat> * fmt) {
+    if (!batch_args(fn, audio, n_frames, n)) return false;
+    if (!channels || !sample_rates) { fprintf(stderr, "%s: null %s\n", fn, channels ? "sample rate array" : "channel array"); return false; }
+    fmt->resize((size_t) n);
+    for (int i = 0; i < n; i++) (*fmt)[(size_t) i] = AudioFormat{channels[i], sample_rates[i]};
+    return true;
+}
+
+}  // namespace
+
+extern "C" bool bark_b200_encodec_compress_batch_resampled(struct encodec_context * e, const float * const * audio, const int * n_frames, const int * channels,
+                                                           const int * sample_rates, int n) {
+    return run(e, __func__, [&] {
+        const char * fn = "bark_b200_encodec_compress_batch_resampled";
+        int n_q;
+        std::vector<AudioFormat> fmt;
+        if (!resampled_batch_formats(fn, audio, n_frames, channels, sample_rates, n, &fmt) || !codebooks_for(e, fn, &n_q)) return false;
+        std::vector<std::vector<int32_t>> codes((size_t) n);
+        if (!codec_encode(e->model, e->scratch, e->stream, n, audio, n_frames, n_q, codes.data(), nullptr, nullptr, fn, fmt.data())) return false;
+        e->batch_codes.swap(codes);
+        return true;
+    });
+}
+
+extern "C" bool bark_b200_encodec_reconstruct_batch_resampled(struct encodec_context * e, const float * const * audio, const int * n_frames, const int * channels,
+                                                              const int * sample_rates, int n) {
+    return run(e, __func__, [&] {
+        const char * fn = "bark_b200_encodec_reconstruct_batch_resampled";
+        int n_q;
+        std::vector<AudioFormat> fmt;
+        if (!resampled_batch_formats(fn, audio, n_frames, channels, sample_rates, n, &fmt) || !codebooks_for(e, fn, &n_q)) return false;
+        std::vector<std::vector<float>> out((size_t) n);
+        if (!codec_encode(e->model, e->scratch, e->stream, n, audio, n_frames, n_q, nullptr, nullptr, out.data(), fn, fmt.data())) return false;
+        e->batch_audio.swap(out);
+        return true;
+    });
+}
+
 extern "C" int bark_b200_encodec_batch_codes(struct encodec_context * e, int i, int32_t * out, int cap) {
     if (!e) { fprintf(stderr, "%s: null context\n", __func__); return -1; }
     return batch_item(e->batch_codes, i, out, cap);

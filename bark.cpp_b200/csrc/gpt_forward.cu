@@ -7,6 +7,7 @@
 #include "gpt_kernels.h"
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <string>
 #include <vector>
@@ -341,8 +342,47 @@ static bool codec_scratch(CodecScratch & sc, size_t frames, int n_q, const char 
 
 void CodecScratch::release() {
     for (int i = 0; i < 3; i++) if (buf[i]) cudaFree(buf[i]);
-    for (void * p : {(void *) gi, (void *) hbuf, (void *) counter, (void *) codes}) if (p) cudaFree(p);
+    for (void * p : {(void *) gi, (void *) hbuf, (void *) counter, (void *) codes, (void *) stage}) if (p) cudaFree(p);
+    for (auto & t : tables) if (t.second) cudaFree(t.second);
     *this = CodecScratch();
+}
+
+// Rate pairs whose taps a scratch keeps; a launch needs at most kCodecMaxItems of them, and the cache is emptied between launches
+// when a new one would pass this
+constexpr size_t kResampleTablesKept = 64;
+
+// the taps of sr -> kCodecSampleRate, built and uploaded on first use
+static ResampleTable scratch_table(CodecScratch & sc, int sr) {
+    for (const auto & t : sc.tables) if (t.first.sr == sr) return t.first;
+    ResampleTable t;
+    const std::vector<unsigned char> bytes = resample_table(sr, kCodecSampleRate, &t);
+    void * d = nullptr;
+    if (!bytes.empty()) {
+        BARK_CUDA_CHECK(cudaMalloc(&d, bytes.size()));
+        sc.tables.emplace_back(t, d);                    // owned from here, so a failed copy does not leak it
+        BARK_CUDA_CHECK(cudaMemcpy(d, bytes.data(), bytes.size(), cudaMemcpyHostToDevice)); g_h2d_bytes += bytes.size();
+        resample_bind(sc.tables.back().first, d);
+        return sc.tables.back().first;
+    }
+    sc.tables.emplace_back(t, nullptr);
+    return t;
+}
+
+bool resample_input_ok(const char * fn, const std::string & item, const float * x, int n_frames, int channels, int sample_rate) {
+    if (channels < 1 || channels > kResampleMaxChannels) { fprintf(stderr, "%s: %s%d channels (1 to %d)\n", fn, item.c_str(), channels, kResampleMaxChannels); return false; }
+    if (sample_rate < kResampleMinRate || sample_rate > kResampleMaxRate) {
+        fprintf(stderr, "%s: %ssample rate %d Hz (%d to %d)\n", fn, item.c_str(), sample_rate, kResampleMinRate, kResampleMaxRate); return false;
+    }
+    if (n_frames < 1 || (long long) n_frames * channels > INT_MAX) {
+        fprintf(stderr, "%s: %s%d frames of %d channels (1 frame to 2^31 - 1 samples)\n", fn, item.c_str(), n_frames, channels); return false;
+    }
+    // |x| <= 2^64: neither the channel sum nor the filter's double sum can overflow
+    for (long long k = 0; k < (long long) n_frames * channels; k++) if (!(std::fabs(x[k]) <= 0x1p64f)) {
+        fprintf(stderr, "%s: %ssample %lld (frame %lld, channel %lld) is not finite or exceeds 2^64 in magnitude (%g)\n", fn, item.c_str(), k, k / channels,
+                k % channels, (double) x[k]);
+        return false;
+    }
+    return true;
 }
 
 // [first, last) item ranges of the launches: consecutive items, at most kCodecMaxItems and kCodecLaunchFrames frames, at least one item
@@ -447,31 +487,68 @@ bool codec_decode(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, int 
 }
 
 bool codec_encode(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, int n, const float * const * audio, const int * n_samples, int n_q,
-                  std::vector<int32_t> * codes, std::vector<float> * latent, std::vector<float> * decoded, const char * batch_fn) {
+                  std::vector<int32_t> * codes, std::vector<float> * latent, std::vector<float> * decoded, const char * batch_fn,
+                  const AudioFormat * fmt) {
     const char * fn = batch_fn ? batch_fn : __func__;
     const CodecModel::Encoder & e = cm.enc;
     if (!e.present) { fprintf(stderr, "%s: the model file has no EnCodec encoder tensors (encoder.*)\n", fn); return false; }
     if (n_q < 1 || n_q > cm.n_q) { fprintf(stderr, "%s: %d codebooks requested, %d loaded\n", fn, n_q, cm.n_q); return false; }
+    // the encoder's input samples per item, and whether the item goes through the resampler (mono 24 kHz does not)
+    std::vector<int> len(n_samples, n_samples + n);
+    std::vector<char> resampled((size_t) n, 0);
+    size_t stage = 0;                                    // floats of the largest resampled item's source
     for (int i = 0; i < n; i++) {
+        if (fmt) {
+            const std::string item = item_tag(batch_fn, i);
+            if (!resample_input_ok(fn, item, audio[i], n_samples[i], fmt[i].channels, fmt[i].sample_rate)) return false;
+            const long long L = resample_len(n_samples[i], fmt[i].sample_rate, kCodecSampleRate);
+            if (L < 1921 || L > INT_MAX) {
+                fprintf(stderr, "%s: %s%d frames at %d Hz resample to %lld samples at %d Hz (1921 to 2^31 - 1: at least 7 frames)\n", fn, item.c_str(),
+                        n_samples[i], fmt[i].sample_rate, L, kCodecSampleRate);
+                return false;
+            }
+            len[(size_t) i] = (int) L;
+            resampled[(size_t) i] = fmt[i].channels != 1 || fmt[i].sample_rate != kCodecSampleRate;
+            if (resampled[(size_t) i]) stage = std::max(stage, (size_t) n_samples[i] * fmt[i].channels);
+            continue;
+        }
         // the final k=7 conv reflect-pads 6 samples of a T-frame latent: T >= 7 (the reference reads out of bounds below that)
         if (n_samples[i] < 1921) { fprintf(stderr, "%s: %sneed at least 1921 samples (7 frames), got %d\n", fn, item_tag(batch_fn, i).c_str(), n_samples[i]); return false; }
         for (int k = 0; k < n_samples[i]; k++) if (!std::isfinite(audio[i][k])) {
             fprintf(stderr, "%s: %ssample %d is not finite (%g)\n", fn, item_tag(batch_fn, i).c_str(), k, (double) audio[i][k]); return false;
         }
     }
+    if (stage > sc.stage_cap) {
+        if (sc.stage) { cudaFree(sc.stage); sc.stage = nullptr; }
+        sc.stage_cap = 0;
+        if (cudaMalloc((void **) &sc.stage, stage * sizeof(float)) != cudaSuccess) {
+            (void) cudaGetLastError(); fprintf(stderr, "%s: out of device memory for %zu source samples\n", fn, stage); return false;
+        }
+        sc.stage_cap = stage;
+    }
     std::vector<int> T((size_t) n);
-    for (int i = 0; i < n; i++) T[(size_t) i] = (n_samples[i] - 1) / 320 + 1;
+    for (int i = 0; i < n; i++) T[(size_t) i] = (len[(size_t) i] - 1) / 320 + 1;
     const size_t Hd = (size_t) cm.hidden_dim;
     for (const auto & g : codec_launches(T.data(), n)) {
         size_t frames = 0, off = 0;
         for (int i = g.first; i < g.second; i++) frames += (size_t) T[(size_t) i];
         if (!codec_scratch(sc, frames, n_q, fn)) return false;
-        for (int i = g.first; i < g.second; off += (size_t) n_samples[i], i++) {
+        if (fmt && sc.tables.size() + (size_t)(g.second - g.first) > kResampleTablesKept) {
+            for (auto & t : sc.tables) if (t.second) cudaFree(t.second);          // no launch in flight: the last one synchronised
+            sc.tables.clear();
+        }
+        for (int i = g.first; i < g.second; off += (size_t) len[(size_t) i], i++) {
+            if (resampled[(size_t) i]) {                 // the source through the staging buffer, reused item by item on the stream
+                const size_t nb = (size_t) n_samples[i] * fmt[i].channels * sizeof(float);
+                BARK_CUDA_CHECK(cudaMemcpyAsync(sc.stage, audio[i], nb, cudaMemcpyHostToDevice, s)); g_h2d_bytes += nb;
+                resample(sc.stage, n_samples[i], fmt[i].channels, scratch_table(sc, fmt[i].sample_rate), sc.buf[2] + off, len[(size_t) i], s);
+                continue;
+            }
             const size_t nb = (size_t) n_samples[i] * sizeof(float);
             BARK_CUDA_CHECK(cudaMemcpyAsync(sc.buf[2] + off, audio[i], nb, cudaMemcpyHostToDevice, s)); g_h2d_bytes += nb;
         }
         const int m = g.second - g.first;
-        const float * lat = encode_launch(cm, sc, s, n_samples + g.first, m, n_q, fn);
+        const float * lat = encode_launch(cm, sc, s, len.data() + g.first, m, n_q, fn);
         if (!lat) return false;
         size_t f = 0;
         for (int i = g.first; i < g.second; f += (size_t) T[(size_t) i], i++) {

@@ -6,6 +6,7 @@
 #include "gpt_kernels.h"
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstring>
 #include <optional>
@@ -154,6 +155,29 @@ extern "C" int bark_b200_rvq_encode(const float * latent, int T, const float * c
         if (!rvq_encode(emb, nrm, n_q, n_bins, hidden, dl, &T, 1, dc, 0) || !finish("bark_b200_rvq_encode")) return 0;
         download(codes, dc, (size_t) n_q * T * 4);
         return 1;
+    });
+}
+
+// resample_kernel on interleaved host frames, its taps table built as the codec scratch builds it; L samples to out
+extern "C" int bark_b200_resample(const float * in, int n_frames, int channels, int in_rate, int out_rate, float * out, int cap) {
+    return guarded(-1, [&] {
+        const char * fn = "bark_b200_resample";
+        if (!in) { fprintf(stderr, "%s: null input\n", fn); return -1; }
+        if (!resample_input_ok(fn, "", in, n_frames, channels, in_rate)) return -1;
+        if (out_rate < kResampleMinRate || out_rate > kResampleMaxRate) { fprintf(stderr, "%s: output rate %d Hz (%d to %d)\n", fn, out_rate, kResampleMinRate, kResampleMaxRate); return -1; }
+        const long long L = resample_len(n_frames, in_rate, out_rate);
+        if (L > INT_MAX) { fprintf(stderr, "%s: %lld output samples (at most 2^31 - 1)\n", fn, L); return -1; }
+        if (!out) return (int) L;
+        if (cap < L) { fprintf(stderr, "%s: output capacity %d for %lld samples\n", fn, cap, L); return -1; }
+        ResampleTable t;
+        const std::vector<unsigned char> bytes = resample_table(in_rate, out_rate, &t);
+        DeviceBuffers mem;
+        if (!bytes.empty()) resample_bind(t, mem.upload(bytes.data(), bytes.size()));
+        const float * d_in = mem.upload(in, (size_t) n_frames * channels * sizeof(float));
+        const GuardedOutput y(mem, (size_t) L * sizeof(float), nullptr);
+        resample(d_in, n_frames, channels, t, y.out<float>(), (int) L, 0);
+        if (!finish(fn) || !y.read(fn, out)) return -1;
+        return (int) L;
     });
 }
 

@@ -77,12 +77,24 @@ struct DeviceArena {
     void release();
 };
 
+// The taps of one rate pair sr -> new_sr (DESIGN.md §16), built on the host by resample_table and bound to device memory by
+// resample_bind (codec_kernels.cu).  o = sr / g, q = new_sr / g (g = gcd), w the filter's half width in input samples; phase j has
+// phase[j] = {first m, count, offset into taps, 0}.  sr == new_sr is the identity (the down-mix alone) and has no taps.  Outputs go
+// tile per CTA with smem floats of shared memory: the tile's input window.
+struct ResampleTable {
+    int sr = 0, new_sr = 0, o = 1, q = 1, w = 0, tile = 0, smem = 0;
+    const int4 * phase = nullptr;
+    const float * taps = nullptr;
+};
+
 // EnCodec scratch for one launch's items (T frames in all), grown on demand by codec_scratch (gpt_forward.cu), freed by release()
 struct CodecScratch {
     float * buf[3] = {nullptr, nullptr, nullptr}; size_t cap = 0;   // ping-pong activations (floats), item-major
     float * gi = nullptr;                                            // LSTM input projections
     float * hbuf = nullptr; unsigned * counter = nullptr;            // LSTM hidden-state exchange [2][items][512] + grid barrier counter
     int32_t * codes = nullptr; size_t codes_cap = 0;                 // [n_q][T_b] per item
+    float * stage = nullptr; size_t stage_cap = 0;                   // one resampled item's interleaved source frames (floats)
+    std::vector<std::pair<ResampleTable, void *>> tables;            // resampling taps per rate pair, with their device allocation
     void release();
 };
 

@@ -175,6 +175,36 @@ BARK_API bool bark_b200_encodec_reconstruct_batch(struct encodec_context * e, co
 BARK_API int  bark_b200_encodec_batch_codes(struct encodec_context * e, int i, int32_t * out, int cap);
 BARK_API int  bark_b200_encodec_batch_audio(struct encodec_context * e, int i, float * out, int cap);
 
+/* RESAMPLED ENCODEC: audio at any sample rate and channel count, down-mixed and resampled to the encoder's 24 kHz on the GPU first
+ * (DESIGN.md §16).  Audio is interleaved frames [n_frames][channels] (WAV order) at sample_rate Hz.  The rule is upstream EnCodec's
+ * convert_audio order with torchaudio's resampler: the frame's channels summed in order in f32 and divided by channels, then
+ * torchaudio.functional.resample(mono, sample_rate, 24000) with its defaults (sinc_interp_hann, lowpass_filter_width 6, rolloff 0.99),
+ * taps in double rounded to f32 and each output a double sum in tap order, rounded once (upstream EnCodec resamples with julius, whose
+ * filter differs).  The resampled length is L = ceil(24000 n_frames / sample_rate) (exactly, in integers); mono 24 kHz goes in
+ * unchanged, so these calls then equal their mono 24 kHz counterparts bit for bit.  Limits: 1 <= channels <= 8, 4000 <= sample_rate <=
+ * 384000, n_frames * channels < 2^31, every sample finite with |x| <= 2^64, L >= 1921 (7 frames).  None of these calls changes the
+ * context's sample rate (encodec_set_sample_rate, which only sets n_q) or its bandwidth.
+ *   bark_b200_encodec_compress_resampled ......... encodec_compress_audio of the resampled clip: codes from encodec_get_codes
+ *   bark_b200_encodec_reconstruct_resampled ...... encodec_reconstruct_audio of it: samples (24 kHz) from encodec_get_audio
+ *   bark_b200_encodec_compress_batch_resampled ... bark_b200_encodec_compress_batch with a format per item: channels[i], sample_rates[i];
+ *                                                  results from bark_b200_encodec_batch_codes, refusals as for that call
+ *   bark_b200_encodec_reconstruct_batch_resampled  the same for bark_b200_encodec_reconstruct_batch: bark_b200_encodec_batch_audio
+ *   bark_b200_encodec_encode_resampled ........... bark_b200_encodec_encode on a bark context (a fine prompt from a speaker clip); it
+ *                                                  leaves the generation state alone
+ *   bark_b200_resample ........................... no context, host buffers: writes the L resampled samples at out_rate to out (cap >=
+ *                                                  L; out NULL only asks for L) and returns L, or -1 on invalid arguments or failure.
+ *                                                  Both rates in [4000, 384000]; for the tests, and for Bark's 24 kHz output at 44.1 or
+ *                                                  48 kHz. */
+BARK_API bool bark_b200_encodec_compress_resampled(struct encodec_context * e, const float * audio, int n_frames, int channels, int sample_rate);
+BARK_API bool bark_b200_encodec_reconstruct_resampled(struct encodec_context * e, const float * audio, int n_frames, int channels, int sample_rate);
+BARK_API bool bark_b200_encodec_compress_batch_resampled(struct encodec_context * e, const float * const * audio, const int * n_frames, const int * channels,
+                                                         const int * sample_rates, int n);
+BARK_API bool bark_b200_encodec_reconstruct_batch_resampled(struct encodec_context * e, const float * const * audio, const int * n_frames, const int * channels,
+                                                            const int * sample_rates, int n);
+BARK_API int  bark_b200_encodec_encode_resampled(struct bark_context * ctx, const float * audio, int n_frames, int channels, int sample_rate, int32_t * codes,
+                                                 int codes_cap, float * latent, int latent_cap);
+BARK_API int  bark_b200_resample(const float * in, int n_frames, int channels, int in_rate, int out_rate, float * out, int cap);
+
 /* FAST MODE (BARK_B200_MODE=fast in the environment at load; opt-in, NOT bit-identical to the reference): the fine model's
  * 1024-row passes (bark.cpp:1416-1584) run as wgmma tensor-core GEMMs + flash-style attention (csrc/fast_kernels.cu).
  * Every weight type the loader reads runs it: an f16 file's fine matrices are used as stored; those of an f32, q4_0, q4_1, q5_0, q5_1
