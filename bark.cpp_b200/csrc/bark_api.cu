@@ -668,8 +668,8 @@ void alloc_workspace(bark_context * ctx) {
     ws.logits = (float *) ctx_alloc(ctx, n_logits * 4);
     ws.tok  = (int32_t *) ctx_alloc(ctx, 8 * 1024 * 4);
     if (is_quant(ctx->semantic.wtype) || is_quant(ctx->coarse.wtype) || is_quant(ctx->fine.wtype)) {
-        ctx->d_q8 = ctx_alloc(ctx, R * (size_t) 4 * E); ctx->d_q8_scales = ctx_alloc(ctx, R * (size_t)(4 * E / 32) * 4);
-        ctx->d_q8_sums = ctx_alloc(ctx, R * (size_t)(4 * E / 32) * 4);
+        ctx->q8.q = (int8_t *) ctx_alloc(ctx, R * (size_t) 4 * E); ctx->q8.d = (float *) ctx_alloc(ctx, R * (size_t)(4 * E / 32) * 4);
+        ctx->q8.s = (float *) ctx_alloc(ctx, R * (size_t)(4 * E / 32) * 4);
     }
     if (ctx->fast_mode) {
         const GPTModel & fm = ctx->fine;

@@ -2,7 +2,7 @@
 // Host control plane in C++ (like the reference's bark.cpp:133-164), all tensors in HBM.
 #pragma once
 #include "../../include/bark_b200.h"
-#include "model.h"
+#include "gpt_kernels.h"
 
 #include <fstream>
 #include <map>
@@ -75,8 +75,7 @@ struct bark_context {
     ShardState shard;
 
     bark::Workspace ws;
-    void * d_q8_sums = nullptr;                       // experimental q4_1 / q5_1: q8_1 block sums s = f16(d * sum(q))
-    void * d_q8 = nullptr, * d_q8_scales = nullptr;  // q4_0 models: q8_0 activation operand (int8 [rows][4E], f32 scales [rows][4E/32])
+    bark::Q8Scratch q8;                              // quantised models: the q8 activation operand ([rows][4E] codes, [rows][4E/32] d and s)
     const float * last_logits = nullptr;             // device logits of the latest gpt_eval / fine_eval
     double * d_u = nullptr, * h_u = nullptr;         // device sampling: uniforms, tokens, flags, eos probabilities (1024 rows)
     int32_t * d_stok = nullptr, * h_stok = nullptr, * d_sflags = nullptr, * h_sflags = nullptr;
@@ -124,6 +123,26 @@ bool fine_eval_shard(bark_context * ctx, const int32_t * in_buffer, int nn);    
 bool sample_shard(bark_context * ctx, std::mt19937 & rng, int n, float temp, int32_t * out_all /*[1024]*/);
 bool fine_eval_fast(bark_context * ctx, const int32_t * in_buffer, int nn, float * logits_host);      // tensor-core variant (fast mode)
 bool gpt_decode_chained(bark_context * ctx, GPTModel & m, const int32_t * d_token, int * n_past, int lm_lo, int lm_hi);
+// The first step of every fine pass: nn and each code of the window checked (messages name fn), the [8][1024] ids uploaded and
+// rows [row0, row0 + rows) of the window embedded into ws.x
+bool fine_embed(bark_context * ctx, const int32_t * in_buffer, int nn, int row0, int rows, const char * fn);
+// final LayerNorm + lm_head (bark.cpp:1391-1405) on `rows` rows from x: the logits of head's outputs land at logits + lo, rows
+// n_out_vocab apart, and logits becomes the context's last_logits
+void output_head(bark_context * ctx, const GPTModel & m, const float * x, int rows, const DMat & head, float * logits, int lo = 0);
+
+// The activation operand of a model's per-op mat-muls (gpt_forward.cu act_layout): what the producers are told, and its group stride
+// in front of the E-wide and the 4E-wide mat-muls
+struct ActLayout { WType wt; int kpE, kp4E; };
+// The per-op transformer body on `rows` rows of ws.x, updated in place (gpt_forward.cu).  kv keeps the pass's K and V:
+// kv.store(ctx, m, il, rows, qkv) points the QKV epilogue's K / V stores at layer il's rows, and kv.attend(ctx, m, il, rows, a)
+// runs that layer's attention from ws.q into ws.act.
+template <class KV> void run_layers(bark_context * ctx, const GPTModel & m, int rows, const KV & kv);
+// K / V of the row-sharded fine pass (shard.cu)
+struct ShardKV {
+    int row0;
+    void store(bark_context * ctx, const GPTModel & m, int il, int rows, MatmulEpilogue & qkv) const;
+    void attend(bark_context * ctx, const GPTModel & m, int il, int rows, const ActLayout & a) const;
+};
 // The EnCodec pipelines, shared by bark_context (8 codebooks) and encodec_context (encodec_api.cu).
 // Reads the codec section at f's position into c: every tensor, codebooks 0..max_q-1 (at least 8 must exist); buffers from arena.
 bool load_codec(std::ifstream & f, CodecModel & c, int max_q, DeviceArena & arena, cudaStream_t s, bool verbose);

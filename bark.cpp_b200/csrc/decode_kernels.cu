@@ -401,7 +401,7 @@ template <typename WT> struct IsQ4 { static constexpr bool v = false; };
 template <> struct IsQ4<Q4> { static constexpr bool v = true; };
 
 // act (f32, natural order) -> int8 q[K] + f32 d[K/32] (the f16-rounded scale, widened back); block-wide, one warp per 32-element block.
-// A non-finite product gives -128 (cvtps_epi32 -> INT_MIN, then the saturating packs), as in quantize_q8_kernel.
+// A non-finite product gives -128 (cvtps_epi32 -> INT_MIN, then the saturating packs), as in quantize_q8x_kernel.
 __device__ __forceinline__ void quantize_act_q8(const float * act, int K, int8_t * q, float * d) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (int b = warp; b < (K >> 5); b += kWarps) {

@@ -10,7 +10,7 @@ namespace bark {
 // mul_mat consumes (the reference converts src1 to the weight's vec_dot_type, ggml.c:12530-12558)
 // ------------------------------------------------------------------------------------------------
 // activations are written in the group-major layout (common.cuh), gs = group stride in elements (= row capacity * 128)
-// (q4_0 weights: plain f32 rows, gs = row stride; quantize_q8_kernel turns them into q8_0 blocks in front of the mat-mul)
+// (q4_0 weights: plain f32 rows, gs = row stride; quantize_q8x_kernel turns them into q8_0 blocks in front of the mat-mul)
 __device__ __forceinline__ void store_act(void * act, int wt, int gs, int m, int k, float v) {
     if (wt == W_Q4_0) { ((float *) act)[(size_t) m * gs + k] = v; return; }
     const size_t off = gm_offset(m, k, (size_t) gs);

@@ -219,9 +219,9 @@ __global__ void __launch_bounds__(256) lane_matmul_kernel(const T * __restrict__
     }
 }
 
-void lane_matmul(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, cudaStream_t s) {
-    if (W.type == W_Q4_0) { q4_matmul(W, act, act_gs, rows, ep, s); return; }      // act_gs = f32 row stride for this type
-    if (qx_supported(W.type)) { qx_matmul(W, act, act_gs, rows, ep, s); return; }
+void lane_matmul(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, const Q8Scratch * q8, cudaStream_t s) {
+    if (W.type == W_Q4_0) { q4_matmul(W, act, act_gs, rows, ep, q8, s); return; }      // act_gs = f32 row stride for this type
+    if (qx_supported(W.type)) { qx_matmul(W, act, act_gs, rows, ep, q8, s); return; }
     const int gx = (W.n_out + 7) / 8;
     {   // roofline annotation: algorithmic HBM bytes (weights once + operands) and flops of this mat-mul
         const double es = W.type == W_F16 ? 2.0 : 4.0;

@@ -28,7 +28,12 @@ void gpt_embed_fine(const GPTModel & m, const int32_t * d_ids, int nn, float * x
 void layernorm_act(const float * x, int rows, int E, const float * g, const float * b, void * act, WType wt, int Kp,
                    unsigned * fallback_counter, cudaStream_t s);
 
-void lane_matmul(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, cudaStream_t s);
+// q8 activation operand of the quantised mat-muls, owned by the caller: int8 [rows][K], f32 block scales d and q8_1 block sums s
+// [rows][K/32] (sums for q4_1 / q5_1 only)
+struct Q8Scratch { int8_t * q = nullptr; float * d = nullptr, * s = nullptr; };
+
+// q8: the scratch a quantised W needs (null for f32 / f16 weights)
+void lane_matmul(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, const Q8Scratch * q8, cudaStream_t s);
 
 // Multi-row attention (gemm_kernels.cu): N query rows Q[N][E] against n_kv <= 1024 key / value rows Kc, Vc [n_kv][E], H heads of 32, 64,
 // 96 or 128; causal masks key k for query q when k > n_past + q.  Result -> activation operand for c_proj.
@@ -51,19 +56,17 @@ void attention_batch(const float * Q, const float * Kst, const float * Vst, cons
 
 // ---- q4_0 weights (q4_kernels.cu) ---------------------------------------------------------------------------------
 void q4_split(const void * raw_blocks, size_t n_blocks, void * qs, void * scales, cudaStream_t s);
-void q4_set_scratch(void * q8, void * q8_scales);      // int8 [rows][K] + f32 [rows][K/32] for the activation operand, owned by the context
-void q4_get_scratch(void ** q8, void ** q8_scales);    // this host thread's current pointers (a test hook saves and restores them)
-void q4_matmul(const DMat & W, const void * act_f32, int ld_act, int rows, const MatmulEpilogue & ep, cudaStream_t s);
+void q4_matmul(const DMat & W, const void * act_f32, int ld_act, int rows, const MatmulEpilogue & ep, const Q8Scratch * q8, cudaStream_t s);
 
 // ---- q4_1 / q5_0 / q5_1 / q8_0 weights (qx_kernels.cu) ---------------------------------------------------------------------------
 bool   qx_supported(WType t);
 size_t qx_block_bytes(WType t);
 void   qx_split(const void * raw_blocks, size_t n_blocks, WType t, void * qs, void * qh, void * d, void * m, cudaStream_t s);
-void   qx_set_scratch(void * q8, void * q8_scales, void * q8_sums);
-void   qx_get_scratch(void ** q8, void ** q8_scales, void ** q8_sums);
+// quantize_q8x_kernel: f32 rows x [rows][ldx] -> q8 blocks, K per row, into q / d, and the block sums into s unless it is null
+void   quantize_q8(const float * x, int ldx, int rows, int K, int8_t * q, float * d, float * s, cudaStream_t stream);
 void   qx_embed_causal(const GPTModel & m, const int32_t * d_tok, int N, int n_past, bool merge, float * x, cudaStream_t s, const int32_t * d_pos);
 void   qx_embed_fine(const GPTModel & m, const int32_t * d_ids, int nn, float * x, cudaStream_t s);
-void   qx_matmul(const DMat & W, const void * act_f32, int ld_act, int rows, const MatmulEpilogue & ep, cudaStream_t s);
+void   qx_matmul(const DMat & W, const void * act_f32, int ld_act, int rows, const MatmulEpilogue & ep, const Q8Scratch * q8, cudaStream_t s);
 
 // ---- register-tiled multi-row kernels (gemm_kernels.cu) ------------------------------------------------------------
 // W needs its group-major copy with o_pad a multiple of kGemmOPad (the widest block tile), the activation operand a row capacity

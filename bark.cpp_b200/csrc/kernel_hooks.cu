@@ -335,8 +335,7 @@ extern "C" int bark_b200_parity_gemm(const void * A, const void * W, void * C, i
 }
 
 // quantised mat-muls: the weight rows arrive as the file's blocks and go through the loader's split (q4_split / qx_split); the
-// activation rows are f32, as store_act leaves them for a quantised model.  The q8 operand lives in this call's own scratch: the
-// calling thread's scratch pointers (a context's buffers) are put back on every exit.
+// activation rows are f32, as store_act leaves them for a quantised model.  The q8 operand lives in this call's own scratch.
 extern "C" int bark_b200_quant_matmul(int wtype, const void * W, const float * A, float * C, int M, int N, int K, int epilogue, int path,
                                       const uint16_t * gelu_tab, int8_t * q_out, float * d_out, float * s_out) {
     return guarded(0, [&] {
@@ -345,11 +344,6 @@ extern "C" int bark_b200_quant_matmul(int wtype, const void * W, const float * A
         if (epilogue < EPI_STORE || epilogue > EPI_QKV || (epilogue == EPI_QKV && N % 3) || (epilogue == EPI_GELU_ACT && !gelu_tab)) return 0;
         const bool q81 = t == W_Q4_1 || t == W_Q5_1;
         if ((path != 0 && (t != W_Q4_0 || M != 1 || K > 4096)) || (s_out && !q81)) return 0;
-        struct Scratch {                                               // the calling thread's q8 scratch, restored on every exit
-            void * q4[2], * qx[3];
-            Scratch() { q4_get_scratch(&q4[0], &q4[1]); qx_get_scratch(&qx[0], &qx[1], &qx[2]); }
-            ~Scratch() { q4_set_scratch(q4[0], q4[1]); qx_set_scratch(qx[0], qx[1], qx[2]); }
-        } keep;
         const int nb = K / 32;
         const size_t n_blocks = (size_t) N * nb;
         DeviceBuffers mem;
@@ -361,22 +355,18 @@ extern "C" int bark_b200_quant_matmul(int wtype, const void * W, const float * A
             qx_split(d_raw, n_blocks, t, dm.p, dm.qh, dm.scales, dm.mins, 0);
         }
         const float * d_a = mem.upload(A, (size_t) M * K * 4);
-        int8_t * d_q8 = mem.alloc<int8_t>((size_t) M * K);
-        float * d_q8d = mem.alloc<float>((size_t) M * nb * 4), * d_q8s = mem.alloc<float>((size_t) M * nb * 4);
+        Q8Scratch q8;
+        q8.q = mem.alloc<int8_t>((size_t) M * K); q8.d = mem.alloc<float>((size_t) M * nb * 4); q8.s = mem.alloc<float>((size_t) M * nb * 4);
         const GuardedOutput c(mem, (size_t) M * N * 4, epilogue == EPI_RESID ? C : nullptr);
         // GELU_ACT: f32 rows, as a quantised model's fc pass leaves its operand
         const MatmulEpilogue ep = matmul_epilogue(mem, epilogue, c.out<float>(), M, N, gelu_tab, W_Q4_0, N);
-        if (path == 0) {
-            q4_set_scratch(d_q8, d_q8d); qx_set_scratch(d_q8, d_q8d, d_q8s);
-            lane_matmul(dm, d_a, K, M, ep, 0);
-        } else {
-            decode_q4_rows(path == 1, d_a, K, dm.p, dm.scales, N, ep, d_q8, d_q8d, 0);
-        }
+        if (path == 0) lane_matmul(dm, d_a, K, M, ep, &q8, 0);
+        else           decode_q4_rows(path == 1, d_a, K, dm.p, dm.scales, N, ep, q8.q, q8.d, 0);
         if (!finish("bark_b200_quant_matmul")) return 0;
         if (!c.read("bark_b200_quant_matmul", C)) return -1;
-        if (q_out) download(q_out, d_q8, (size_t) M * K);
-        if (d_out) download(d_out, d_q8d, (size_t) M * nb * 4);
-        if (s_out) download(s_out, d_q8s, (size_t) M * nb * 4);
+        if (q_out) download(q_out, q8.q, (size_t) M * K);
+        if (d_out) download(d_out, q8.d, (size_t) M * nb * 4);
+        if (s_out) download(s_out, q8.s, (size_t) M * nb * 4);
         return 1;
     });
 }

@@ -9,8 +9,8 @@
 // executable spec, pinned against the reference in tests/test_quantize.py.
 //
 // Layout: the 18-byte blocks of the file are split at load into qs [n_out][K/32] x 16 B (aligned 16-byte words) and
-// scales [n_out][K/32] f16.  Activations arrive as f32 rows (store_act, W_Q4_0) and are quantised by quantize_q8_kernel into
-// int8 [rows][K] + f32 scales [rows][K/32] (the f16-rounded d, widened back).
+// scales [n_out][K/32] f16.  Activations arrive as f32 rows (store_act, W_Q4_0) and are quantised by quantize_q8x_kernel
+// (qx_kernels.cu, without block sums) into int8 [rows][K] + f32 scales [rows][K/32] (the f16-rounded d, widened back).
 #include "epilogue.cuh"
 #include "gpt_kernels.h"
 
@@ -28,25 +28,6 @@ __global__ void split_q4_kernel(const unsigned char * __restrict__ raw, size_t n
 #pragma unroll
     for (int i = 0; i < 4; i++) w[i] = (uint32_t) p[2 + 4 * i] | ((uint32_t) p[3 + 4 * i] << 8) | ((uint32_t) p[4 + 4 * i] << 16) | ((uint32_t) p[5 + 4 * i] << 24);
     qs[b] = make_uint4(w[0], w[1], w[2], w[3]);
-}
-
-// one warp per (row, block), lane j = element j.  A non-finite product (a block holding an inf, or 0 < amax < 127 / FLT_MAX where
-// id = 127 / amax overflows) becomes -128: cvtps_epi32 turns it into INT_MIN and the saturating packs into -128.
-__global__ void quantize_q8_kernel(const float * __restrict__ x, int ldx, int rows, int K, int8_t * __restrict__ q, float * __restrict__ d_out) {
-    const int nb = K >> 5;
-    const size_t w = ((size_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int lane = threadIdx.x & 31;
-    if (w >= (size_t) rows * nb) return;
-    const int r = (int)(w / nb), b = (int)(w % nb);
-    const float v = x[(size_t) r * ldx + b * 32 + lane];
-    float amax = fabsf(v);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
-    const float d = __fdiv_rn(amax, 127.0f);
-    const float id = amax != 0.0f ? __fdiv_rn(127.0f, amax) : 0.0f;
-    const float p = __fmul_rn(v, id);
-    q[(size_t) r * K + b * 32 + lane] = (int8_t)(isfinite(p) ? __float2int_rn(p) : -128);   // _mm256_round_ps(nearest) + cvtps_epi32 + packs
-    if (lane == 0) d_out[(size_t) r * nb + b] = __half2float(__float2half_rn(d));          // y[i].d = GGML_FP32_TO_FP16(d)
 }
 
 // out[m][o] = vec_dot_q4_0_q8_0(W[o], A[m]).  Eight lanes own the eight float accumulators of one output; an 8-lane group walks OPW
@@ -103,27 +84,21 @@ __global__ void __launch_bounds__(256) q4_matmul_kernel(const uint4 * __restrict
         }
 }
 
-thread_local int8_t * g_q8 = nullptr; thread_local float * g_q8d = nullptr;   // per host thread: one thread drives one context
-
 }  // namespace
 
 void q4_split(const void * raw_blocks, size_t n_blocks, void * qs, void * scales, cudaStream_t s) {
     BARK_LAUNCH(split_q4_kernel, (unsigned)((n_blocks + 255) / 256), 256, 0, s, (const unsigned char *) raw_blocks, n_blocks, (uint4 *) qs, (__half *) scales);
 }
 
-void q4_set_scratch(void * q8, void * q8_scales) { g_q8 = (int8_t *) q8; g_q8d = (float *) q8_scales; }
-void q4_get_scratch(void ** q8, void ** q8_scales) { *q8 = g_q8; *q8_scales = g_q8d; }
-
 // act: f32 rows [rows][ld_act] as store_act(W_Q4_0) leaves them
-void q4_matmul(const DMat & W, const void * act, int ld_act, int rows, const MatmulEpilogue & ep, cudaStream_t s) {
-    if (!g_q8 || !g_q8d) { fprintf(stderr, "bark_b200: q4_0 scratch buffers are not set\n"); throw std::runtime_error("unsupported configuration (see the message above)"); }
+void q4_matmul(const DMat & W, const void * act, int ld_act, int rows, const MatmulEpilogue & ep, const Q8Scratch * q8, cudaStream_t s) {
+    if (!q8 || !q8->q || !q8->d) { fprintf(stderr, "bark_b200: q4_0 scratch buffers are not set\n"); throw std::runtime_error("unsupported configuration (see the message above)"); }
     const int nb = W.K / 32;
-    const size_t warps = (size_t) rows * nb;
-    BARK_LAUNCH(quantize_q8_kernel, (unsigned)((warps * 32 + 255) / 256), 256, 0, s, (const float *) act, ld_act, rows, W.K, g_q8, g_q8d);
+    quantize_q8((const float *) act, ld_act, rows, W.K, q8->q, q8->d, nullptr, s);          // q8_0 blocks: no sums
     g_next_bytes = (double) W.n_out * nb * 18.0 + (double) rows * (W.K * 1.0 + nb * 4.0 + W.n_out * 4.0);
     g_next_flops = 2.0 * rows * (double) W.n_out * W.K;
-    if (rows == 1) BARK_LAUNCH((q4_matmul_kernel<1, 1>), dim3((W.n_out + 31) / 32, 1), 256, 0, s, (const uint4 *) W.p, (const __half *) W.scales, W.K, W.n_out, g_q8, g_q8d, rows, ep);
-    else           BARK_LAUNCH((q4_matmul_kernel<8, 4>), dim3((W.n_out + 127) / 128, (rows + 7) / 8), 256, 0, s, (const uint4 *) W.p, (const __half *) W.scales, W.K, W.n_out, g_q8, g_q8d, rows, ep);
+    if (rows == 1) BARK_LAUNCH((q4_matmul_kernel<1, 1>), dim3((W.n_out + 31) / 32, 1), 256, 0, s, (const uint4 *) W.p, (const __half *) W.scales, W.K, W.n_out, q8->q, q8->d, rows, ep);
+    else           BARK_LAUNCH((q4_matmul_kernel<8, 4>), dim3((W.n_out + 127) / 128, (rows + 7) / 8), 256, 0, s, (const uint4 *) W.p, (const __half *) W.scales, W.K, W.n_out, q8->q, q8->d, rows, ep);
 }
 
 }  // namespace bark

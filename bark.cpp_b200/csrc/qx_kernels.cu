@@ -4,7 +4,7 @@
 // build (ggml-quants.c): q5 codes take their fifth bit from qh, q4_1 / q5_1 add `m_w * s_a` per block in ONE scalar fused chain
 // (summs) where s_a = f16(d_a * sum(q_a)) comes from the q8_1 activation blocks, q8_0 weights are plain int8.  oracle/bark_oracle.c
 // (vec_dot_q4_1_q8_1 ... vec_dot_q8_0_q8_0, pinned against the reference in tests/test_quantize.py) is the executable spec.
-// Everything here is NEW code: the kernels the f32 / f16 / q4_0 paths run are not touched (their SASS is unchanged).
+// The activation quantiser here also serves q4_0 (q4_kernels.cu), without the block sums.
 #include "epilogue.cuh"
 #include "gpt_kernels.h"
 
@@ -138,8 +138,6 @@ __global__ void __launch_bounds__(256) qx_matmul_kernel(const unsigned char * __
     }
 }
 
-thread_local int8_t * g_qx_q8 = nullptr; thread_local float * g_qx_d = nullptr, * g_qx_s = nullptr;
-
 }  // namespace
 
 bool qx_supported(WType t) { return t == W_Q4_1 || t == W_Q5_0 || t == W_Q5_1 || t == W_Q8_0; }
@@ -150,8 +148,10 @@ void qx_split(const void * raw_blocks, size_t n_blocks, WType t, void * qs, void
                 (__half *) d, (__half *) m);
 }
 
-void qx_set_scratch(void * q8, void * q8_scales, void * q8_sums) { g_qx_q8 = (int8_t *) q8; g_qx_d = (float *) q8_scales; g_qx_s = (float *) q8_sums; }
-void qx_get_scratch(void ** q8, void ** q8_scales, void ** q8_sums) { *q8 = g_qx_q8; *q8_scales = g_qx_d; *q8_sums = g_qx_s; }
+void quantize_q8(const float * x, int ldx, int rows, int K, int8_t * q, float * d, float * s, cudaStream_t stream) {
+    const size_t warps = (size_t) rows * (K / 32);
+    BARK_LAUNCH(quantize_q8x_kernel, (unsigned)((warps * 32 + 255) / 256), 256, 0, stream, x, ldx, rows, K, q, d, s);
+}
 
 void qx_embed_causal(const GPTModel & m, const int32_t * d_tok, int N, int n_past, bool merge, float * x, cudaStream_t s, const int32_t * d_pos) {
     BARK_LAUNCH(embed_causal_q_kernel, N, 256, 0, s, m.wte[0], (int) m.wtype, m.wpe, d_tok, N, n_past, merge ? 1 : 0, m.n_embd, x, d_pos);
@@ -162,21 +162,20 @@ void qx_embed_fine(const GPTModel & m, const int32_t * d_ids, int nn, float * x,
 }
 
 // act: f32 rows [rows][ld_act] as store_act(W_Q4_0) leaves them
-void qx_matmul(const DMat & W, const void * act, int ld_act, int rows, const MatmulEpilogue & ep, cudaStream_t s) {
-    if (!g_qx_q8 || !g_qx_d || !g_qx_s) { fprintf(stderr, "bark_b200: quantised-weight scratch buffers are not set\n"); throw std::runtime_error("unsupported configuration (see the message above)"); }
+void qx_matmul(const DMat & W, const void * act, int ld_act, int rows, const MatmulEpilogue & ep, const Q8Scratch * q8, cudaStream_t s) {
+    if (!q8 || !q8->q || !q8->d || !q8->s) { fprintf(stderr, "bark_b200: quantised-weight scratch buffers are not set\n"); throw std::runtime_error("unsupported configuration (see the message above)"); }
     const int nb = W.K / 32;
-    const size_t warps = (size_t) rows * nb;
     const bool q81 = W.type == W_Q4_1 || W.type == W_Q5_1;
-    BARK_LAUNCH(quantize_q8x_kernel, (unsigned)((warps * 32 + 255) / 256), 256, 0, s, (const float *) act, ld_act, rows, W.K, g_qx_q8, g_qx_d, q81 ? g_qx_s : nullptr);
+    quantize_q8((const float *) act, ld_act, rows, W.K, q8->q, q8->d, q81 ? q8->s : nullptr, s);
     g_next_bytes = (double) W.n_out * nb * (double) block_bytes((int) W.type) + (double) rows * (W.K * 1.0 + nb * 8.0 + W.n_out * 4.0);
     g_next_flops = 2.0 * rows * (double) W.n_out * W.K;
     const dim3 grid((W.n_out + 31) / 32, (rows + kQxMT - 1) / kQxMT);
     const unsigned char * qs = (const unsigned char *) W.p; const uint32_t * qh = (const uint32_t *) W.qh; const __half * wd = (const __half *) W.scales, * wm = (const __half *) W.mins;
     switch (W.type) {
-        case W_Q4_1: BARK_LAUNCH((qx_matmul_kernel<W_Q4_1>), grid, 256, 0, s, qs, qh, wd, wm, W.K, W.n_out, g_qx_q8, g_qx_d, g_qx_s, rows, ep); break;
-        case W_Q5_0: BARK_LAUNCH((qx_matmul_kernel<W_Q5_0>), grid, 256, 0, s, qs, qh, wd, wm, W.K, W.n_out, g_qx_q8, g_qx_d, g_qx_s, rows, ep); break;
-        case W_Q5_1: BARK_LAUNCH((qx_matmul_kernel<W_Q5_1>), grid, 256, 0, s, qs, qh, wd, wm, W.K, W.n_out, g_qx_q8, g_qx_d, g_qx_s, rows, ep); break;
-        case W_Q8_0: BARK_LAUNCH((qx_matmul_kernel<W_Q8_0>), grid, 256, 0, s, qs, qh, wd, wm, W.K, W.n_out, g_qx_q8, g_qx_d, g_qx_s, rows, ep); break;
+        case W_Q4_1: BARK_LAUNCH((qx_matmul_kernel<W_Q4_1>), grid, 256, 0, s, qs, qh, wd, wm, W.K, W.n_out, q8->q, q8->d, q8->s, rows, ep); break;
+        case W_Q5_0: BARK_LAUNCH((qx_matmul_kernel<W_Q5_0>), grid, 256, 0, s, qs, qh, wd, wm, W.K, W.n_out, q8->q, q8->d, q8->s, rows, ep); break;
+        case W_Q5_1: BARK_LAUNCH((qx_matmul_kernel<W_Q5_1>), grid, 256, 0, s, qs, qh, wd, wm, W.K, W.n_out, q8->q, q8->d, q8->s, rows, ep); break;
+        case W_Q8_0: BARK_LAUNCH((qx_matmul_kernel<W_Q8_0>), grid, 256, 0, s, qs, qh, wd, wm, W.K, W.n_out, q8->q, q8->d, q8->s, rows, ep); break;
         default: fprintf(stderr, "bark_b200: unsupported quantised type %d\n", (int) W.type); throw std::runtime_error("unsupported configuration (see the message above)");
     }
 }

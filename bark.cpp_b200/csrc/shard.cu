@@ -65,46 +65,34 @@ static bool shard_barrier(bark_context * ctx) {
     return true;
 }
 
+// This rank's rows [row0, row0 + rows) store layer il's K / V rows into the local buffer and every peer's (buffer pair il & 1); the
+// barrier after the QKV mat-mul orders those stores before any rank's attention reads all 1024 rows.
+void ShardKV::store(bark_context * ctx, const GPTModel & m, int il, int rows, MatmulEpilogue & qkv) const {
+    ShardState & S = ctx->shard;
+    const size_t at = (size_t) row0 * m.n_embd;
+    qkv.k_out = shard_k(S.local, m, il & 1) + at; qkv.v_out = shard_v(S.local, m, il & 1) + at;
+    for (int p = 0; p < S.world; p++) if (p != S.rank) {
+        qkv.k_peer[qkv.n_peer] = shard_k(S.peer[p], m, il & 1) + at; qkv.v_peer[qkv.n_peer] = shard_v(S.peer[p], m, il & 1) + at; qkv.n_peer++;
+    }
+    S.nvlink_bytes += (unsigned long long) qkv.n_peer * 2ull * rows * m.n_embd * 4ull;         // the fused all-gather
+}
+
+void ShardKV::attend(bark_context * ctx, const GPTModel & m, int il, int rows, const ActLayout & a) const {
+    ShardState & S = ctx->shard;
+    Workspace & ws = ctx->ws;
+    shard_barrier(ctx);
+    attention(ws.q, shard_k(S.local, m, il & 1), shard_v(S.local, m, il & 1), rows, 1024, 0, m.n_embd, m.n_head, false, ws.scores, ws.act, a.wt, a.kpE, ctx->stream);
+}
+
 // One pass over this rank's rows; logits of those rows are left in ws.logits [rows][n_out].
 bool fine_eval_shard(bark_context * ctx, const int32_t * in_buffer, int nn) {
     GPTModel & m = ctx->fine;
-    ShardState & S = ctx->shard;
-    Workspace & ws = ctx->ws;
-    cudaStream_t s = ctx->stream;
-    const int E = m.n_embd, H = m.n_head, rows = 1024 / S.world, row0 = S.rank * rows;
-    const bool q4 = is_quant(m.wtype);
-    if (q4) { fprintf(stderr, "%s: the row-sharded fine pass runs f32 / f16 weights\n", __func__); return false; }
+    const int rows = 1024 / ctx->shard.world, row0 = ctx->shard.rank * rows;
+    if (is_quant(m.wtype)) { fprintf(stderr, "%s: the row-sharded fine pass runs f32 / f16 weights\n", __func__); return false; }
     const int64_t t0 = now_us();
-    for (int i = 0; i < (nn + 1) * 1024; i++) if (in_buffer[i] < 0 || in_buffer[i] >= m.n_in_vocab) { fprintf(stderr, "%s: code out of range\n", __func__); return false; }
-    memcpy(ctx->h_tok, in_buffer, (size_t) 8 * 1024 * sizeof(int32_t));
-    BARK_CUDA_CHECK(cudaMemcpyAsync(ws.tok, ctx->h_tok, (size_t) 8 * 1024 * sizeof(int32_t), cudaMemcpyHostToDevice, s)); g_h2d_bytes += (size_t) 8 * 1024 * sizeof(int32_t);
-    gpt_embed_fine(m, ws.tok, nn, ws.x, s, row0, rows);
-    const WType awt = m.wtype;
-    const int kpE = ws.max_rows * kGmGroup;
-    for (int il = 0; il < m.n_layer; il++) {
-        const GPTLayer & L = m.layers[(size_t) il];
-        const int par = il & 1;
-        layernorm_act(ws.x, rows, E, L.ln_1_g, L.ln_1_b, ws.act, awt, kpE, ctx->d_ln_fallbacks, s);
-        MatmulEpilogue qkv; qkv.mode = EPI_QKV; qkv.out = ws.q; qkv.ldo = E;
-        qkv.k_out = shard_k(S.local, m, par) + (size_t) row0 * E; qkv.v_out = shard_v(S.local, m, par) + (size_t) row0 * E;
-        for (int p = 0; p < S.world; p++) if (p != S.rank) {
-            qkv.k_peer[qkv.n_peer] = shard_k(S.peer[p], m, par) + (size_t) row0 * E; qkv.v_peer[qkv.n_peer] = shard_v(S.peer[p], m, par) + (size_t) row0 * E; qkv.n_peer++;
-        }
-        S.nvlink_bytes += (unsigned long long) qkv.n_peer * 2ull * rows * E * 4ull;
-        lane_matmul(L.c_attn, ws.act, kpE, rows, qkv, s);                       // K / V rows land in every rank's buffer (fused all-gather)
-        shard_barrier(ctx);
-        attention(ws.q, shard_k(S.local, m, par), shard_v(S.local, m, par), rows, 1024, 0, E, H, false, ws.scores, ws.act, awt, kpE, s);
-        MatmulEpilogue res; res.mode = EPI_RESID; res.out = ws.x; res.ldo = E;
-        lane_matmul(L.c_proj, ws.act, kpE, rows, res, s);
-        layernorm_act(ws.x, rows, E, L.ln_2_g, L.ln_2_b, ws.act, awt, kpE, ctx->d_ln_fallbacks, s);
-        MatmulEpilogue ge; ge.mode = EPI_GELU_ACT; ge.act_out = ws.act2; ge.act_wt = (int) awt; ge.act_Kp = kpE; ge.gelu_tab = ctx->d_gelu_tab;
-        lane_matmul(L.fc, ws.act, kpE, rows, ge, s);
-        lane_matmul(L.proj, ws.act2, kpE, rows, res, s);
-    }
-    layernorm_act(ws.x, rows, E, m.ln_f_g, m.ln_f_b, ws.act, awt, kpE, ctx->d_ln_fallbacks, s);
-    MatmulEpilogue st; st.mode = EPI_STORE; st.out = ws.logits; st.ldo = m.n_out_vocab;
-    lane_matmul(m.lm_head[nn - 1], ws.act, kpE, rows, st, s);
-    ctx->last_logits = ws.logits;
+    if (!fine_embed(ctx, in_buffer, nn, row0, rows, __func__)) return false;
+    run_layers(ctx, m, rows, ShardKV{row0});
+    output_head(ctx, m, ctx->ws.x, rows, m.lm_head[nn - 1], ctx->ws.logits);
     m.t_predict_us += now_us() - t0;
     return true;
 }

@@ -269,7 +269,7 @@ BARK_API int  bark_b200_parity_gemm(const void * A, const void * W, void * C, in
  * _q8_1 of weight row o against activation row m after quantize_row_q8_0 / q8_1, for A [M][K] f32 and W [N][K/32] blocks as the model
  * file stores them, wtype (enum ggml_type) 2 q4_0 (18-byte blocks), 3 q4_1 (20), 6 q5_0 (22), 7 q5_1 (24) or 8 q8_0 (34), K % 32 == 0.
  * epilogue as bark_b200_parity_gemm (GELU_ACT: f32 [M][N], the operand a quantised model's next mat-mul quantises; QKV: N % 3 == 0).
- *   path 0: the per-op kernels the library runs for M rows (quantize_q8_kernel + q4_matmul_kernel, or quantize_q8x_kernel + qx_matmul_kernel)
+ *   path 0: the per-op kernels the library runs for M rows (quantize_q8x_kernel + q4_matmul_kernel or qx_matmul_kernel)
  *   path 1 / 2: q4_0, M == 1, K <= 4096 only: the persistent decode step's quantize_act_q8 + row_dot_q4 in one CTA, the weight rows
  *               staged in shared memory (1) or read from global memory (2)
  * q [M][K] int8, d [M][K/32] f32 (the f16 scale, widened), s [M][K/32] f32 (q4_1 / q5_1 only, the f16 q8_1 sum): the quantised

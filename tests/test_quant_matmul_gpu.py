@@ -1,7 +1,7 @@
 """GPU: the quantised mat-muls kernel by kernel (bark_b200_quant_matmul) against the unmodified reference's stored block dots
 (tests/golden/ref_pairs/quant_dots.npz) and against the C oracle's quantiser and per-type dots, bit for bit.
 
-Three device implementations are covered: q4_0 on the per-op path (quantize_q8_kernel + q4_matmul_kernel<1,1> / <8,4>), q4_1 / q5_0 /
+Three device implementations are covered: q4_0 on the per-op path (quantize_q8x_kernel + q4_matmul_kernel<1,1> / <8,4>), q4_1 / q5_0 /
 q5_1 / q8_0 (quantize_q8x_kernel + qx_matmul_kernel), and q4_0 inside the persistent decode step (quantize_act_q8 + row_dot_q4, staged
 in shared memory or read from global memory).  The model tests only reach them with well-conditioned activations at the models' widths;
 these add row counts on both sides of the 8-row tile, output counts around the 4-, 16- and 128-output tiles (the <8,4> kernel clamps
@@ -176,8 +176,9 @@ def test_decode_path_reference_rows(pkg, path):
 @pytest.mark.gpu
 @pytest.mark.parametrize("qtype,ftype", [("q4_0", 2), ("q4_1", 3)])
 def test_a_context_on_the_same_thread_is_unaffected(pkg, orc, weights_file, tmp_path, qtype, ftype):
-    """the hook quantises into its own scratch and puts the thread's scratch pointers back: a context's quantised passes between and
-    after hook calls (and the hook on a thread that never had a context) give the oracle's logits"""
+    """the hook quantises into scratch it allocates and passes to the mat-mul, and a context passes its own scratch to every
+    quantised mat-mul: a context's passes between and after hook calls (and the hook on a thread that never had a context) give
+    the oracle's logits"""
     path = str(tmp_path / f"tiny_{qtype}.bin")
     assert pkg.lib().bark_model_quantize(weights_file("tiny", "f16").encode(), path.encode(), ftype)
     o = orc.Oracle(path, seed=0, n_steps=8)
