@@ -889,7 +889,7 @@ static int bark_b200_encodec_encode_impl(struct bark_context * ctx, const float 
     if (!ctx || !audio) { fprintf(stderr, "%s: null %s\n", fn, ctx ? "audio" : "context"); return -1; }
     BARK_CUDA_CHECK(cudaSetDevice(ctx->device));
     std::vector<int32_t> c; std::vector<float> l;
-    if (!codec_encode(ctx->codec, ctx->codec_scratch, ctx->stream, 1, &audio, &n_samples, 8, &c, &l, nullptr, nullptr, fmt)) return -1;
+    if (!codec_encode(ctx->codec, ctx->codec_scratch, ctx->stream, 1, &audio, &n_samples, 8, {&c, &l}, nullptr, fmt)) return -1;
     if (codes) memcpy(codes, c.data(), sizeof(int32_t) * std::min(c.size(), (size_t) std::max(codes_cap, 0)));
     if (latent) memcpy(latent, l.data(), sizeof(float) * std::min(l.size(), (size_t) std::max(latent_cap, 0)));
     return (int)(c.size() / 8);

@@ -1,0 +1,274 @@
+// The EnCodec pipelines on the host: the device-side replacement of encodec_eval (encodec.cpp/encodec.cpp:819-847) for the decoder and
+// of encodec_compress_audio's encoder (encodec.cpp:878-900), for n clips at once.  Every item is checked first; the items then run in
+// launches of consecutive items, each one pass of the codec kernels over its items into a scratch grown on demand.
+#include "codec_kernels.h"
+#include "context.h"
+
+#include <algorithm>
+#include <climits>
+#include <cmath>
+#include <string>
+#include <vector>
+
+namespace bark {
+
+// codec scratch for one launch of `frames` frames over its items: three activation buffers of 10240 floats per frame (the decoder's largest
+// activation is [64][160T] = [32][320T]; the encoder's, [32][n_samples], is no larger), the LSTM input projections and the [n_q][T] codes
+static bool codec_scratch(CodecScratch & sc, size_t frames, int n_q, const char * caller) {
+    const size_t need = (size_t) 10240 * frames + 1024, codes_need = (size_t) n_q * frames;
+    if (need > sc.cap || codes_need > sc.codes_cap) {
+        // out of memory here is recoverable (a very long clip): report it and return false like the reference's failed encodec_eval
+        auto grow = [&](void ** p, size_t bytes) { if (*p) { cudaFree(*p); *p = nullptr; } return cudaMalloc(p, bytes) == cudaSuccess; };
+        const size_t cap = std::max(need, sc.cap), ccap = std::max(codes_need, sc.codes_cap);
+        sc.cap = sc.codes_cap = 0;
+        bool ok = true;
+        for (int i = 0; i < 3; i++) ok = ok && grow((void **) &sc.buf[i], cap * sizeof(float));
+        ok = ok && grow((void **) &sc.gi, (cap - 1024) / 10240 * 2048 * sizeof(float)) && grow((void **) &sc.codes, ccap * sizeof(int32_t));
+        if (ok && !sc.hbuf) ok = cudaMalloc((void **) &sc.hbuf, (size_t) 2 * kCodecMaxItems * 512 * sizeof(float)) == cudaSuccess &&
+                                 cudaMalloc((void **) &sc.counter, sizeof(unsigned)) == cudaSuccess;
+        if (!ok) { (void) cudaGetLastError(); fprintf(stderr, "%s: out of device memory for %zu frames\n", caller, frames); return false; }
+        sc.cap = cap; sc.codes_cap = ccap;
+    }
+    return true;
+}
+
+void CodecScratch::release() {
+    for (int i = 0; i < 3; i++) if (buf[i]) cudaFree(buf[i]);
+    for (void * p : {(void *) gi, (void *) hbuf, (void *) counter, (void *) codes, (void *) stage}) if (p) cudaFree(p);
+    for (auto & t : tables) if (t.second) cudaFree(t.second);
+    *this = CodecScratch();
+}
+
+// Rate pairs whose taps a scratch keeps; a launch needs at most kCodecMaxItems of them, and the cache is emptied between launches
+// when a new one would pass this
+constexpr size_t kResampleTablesKept = 64;
+
+// the taps of sr -> kCodecSampleRate, built and uploaded on first use
+static ResampleTable scratch_table(CodecScratch & sc, int sr) {
+    for (const auto & t : sc.tables) if (t.first.sr == sr) return t.first;
+    ResampleTable t;
+    const std::vector<unsigned char> bytes = resample_table(sr, kCodecSampleRate, &t);
+    void * d = nullptr;
+    if (!bytes.empty()) {
+        BARK_CUDA_CHECK(cudaMalloc(&d, bytes.size()));
+        sc.tables.emplace_back(t, d);                    // owned from here, so a failed copy does not leak it
+        BARK_CUDA_CHECK(cudaMemcpy(d, bytes.data(), bytes.size(), cudaMemcpyHostToDevice)); g_h2d_bytes += bytes.size();
+        resample_bind(sc.tables.back().first, d);
+        return sc.tables.back().first;
+    }
+    sc.tables.emplace_back(t, nullptr);
+    return t;
+}
+
+bool resample_input_ok(const char * fn, const std::string & item, const float * x, int n_frames, int channels, int sample_rate) {
+    if (channels < 1 || channels > kResampleMaxChannels) { fprintf(stderr, "%s: %s%d channels (1 to %d)\n", fn, item.c_str(), channels, kResampleMaxChannels); return false; }
+    if (sample_rate < kResampleMinRate || sample_rate > kResampleMaxRate) {
+        fprintf(stderr, "%s: %ssample rate %d Hz (%d to %d)\n", fn, item.c_str(), sample_rate, kResampleMinRate, kResampleMaxRate); return false;
+    }
+    if (n_frames < 1 || (long long) n_frames * channels > INT_MAX) {
+        fprintf(stderr, "%s: %s%d frames of %d channels (1 frame to 2^31 - 1 samples)\n", fn, item.c_str(), n_frames, channels); return false;
+    }
+    // |x| <= 2^64: neither the channel sum nor the filter's double sum can overflow
+    for (long long k = 0; k < (long long) n_frames * channels; k++) if (!(std::fabs(x[k]) <= 0x1p64f)) {
+        fprintf(stderr, "%s: %ssample %lld (frame %lld, channel %lld) is not finite or exceeds 2^64 in magnitude (%g)\n", fn, item.c_str(), k, k / channels,
+                k % channels, (double) x[k]);
+        return false;
+    }
+    return true;
+}
+
+// [first, last) item ranges of the launches: consecutive items, at most kCodecMaxItems and kCodecLaunchFrames frames, at least one item
+static std::vector<std::pair<int, int>> codec_launches(const int * T, int n) {
+    std::vector<std::pair<int, int>> groups;
+    for (int i = 0; i < n;) {
+        int j = i + 1;
+        long long frames = T[i];
+        while (j < n && j - i < kCodecMaxItems && frames + T[j] <= kCodecLaunchFrames) frames += T[j++];
+        groups.emplace_back(i, j);
+        i = j;
+    }
+    return groups;
+}
+
+std::string item_tag(const char * batch_fn, int i) { return batch_fn ? "item " + std::to_string(i) + ": " : std::string(); }
+
+// The two LSTM layers on x [C][L_b] per item: the first to y, the second plus x (decoder.h:72, encoder.h:98) to out
+static void lstm2(const CodecLSTM & w, const float * x, int C, const int * l, int n, CodecScratch & sc, float * y, float * out, cudaStream_t s) {
+    lstm_layer(x, C, l, n, w.ih_w[0], w.hh_w[0], w.Kp, w.ih_b[0], w.hh_b[0], nullptr, sc.gi, sc.hbuf, sc.counter, y, s);
+    lstm_layer(y, C, l, n, w.ih_w[1], w.hh_w[1], w.Kp, w.ih_b[1], w.hh_b[1], x, sc.gi, sc.hbuf, sc.counter, out, s);
+}
+
+// The decoder on the codes in sc.codes ([n_q][T_b] per item, item-major) of n items of T[b] frames; returns the waveforms, [kCodecHop T_b] per item.
+static const float * decode_launch(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, const int * T, int n, int n_q) {
+    std::vector<int> L(T, T + n);
+    int * l = L.data();
+    float * a = sc.buf[0], * b = sc.buf[1], * c = sc.buf[2];
+    rvq_decode(cm, sc.codes, n_q, l, n, a, s);                                               // [128][T]
+    conv1d(a, cm.hidden_dim, l, n, cm.init, false, nullptr, b, s);                          // [512][T]
+    int C = cm.init.cout;
+    lstm2(cm.lstm, b, C, l, n, sc, a, c, s);
+    float * cur = c, * t1 = a, * t2 = b;
+    for (int i = 0; i < 4; i++) {
+        convtr1d(cur, C, l, n, cm.blk[i].us, kCodecRatios[i], t1, s);    // ELU fused on the input; -> [C/2][L*r]
+        C /= 2;
+        for (int & x : L) x *= kCodecRatios[i];
+        conv1d(t1, C, l, n, cm.blk[i].sc, false, nullptr, t2, s);        // shortcut on the raw up-sampled signal
+        conv1d(t1, C, l, n, cm.blk[i].c1, true, nullptr, cur, s);        // ELU -> k3 -> [C/2][L]
+        conv1d(cur, C / 2, l, n, cm.blk[i].c2, true, t2, t1, s);         // ELU -> k1, + shortcut
+        std::swap(cur, t1);
+    }
+    conv1d(cur, C, l, n, cm.final_conv, true, nullptr, t1, s);           // ELU -> k7 -> [1][kCodecHop T]
+    return t1;
+}
+
+// The encoder and the RVQ on the samples in sc.buf[2] ([n_b] per item, concatenated) of n items; codes to sc.codes ([n_q][T_b] per
+// item); returns the latents ([128][T_b] per item), null (message) on an unsupported shape.
+static const float * encode_launch(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, const int * n_samples, int n, int n_q, const char * caller) {
+    const CodecModel::Encoder & e = cm.enc;
+    std::vector<int> L(n_samples, n_samples + n);
+    int * l = L.data();
+    float * cur = sc.buf[0], * t1 = sc.buf[1], * t2 = sc.buf[2];
+    conv1d(t2, 1, l, n, e.init, false, nullptr, cur, s);                   // encoder.h:49 -> [32][n]
+    int C = e.init.cout;
+    for (int i = 0; i < 4; i++) {                                        // encoder.h:52-83
+        const int r = kCodecRatios[3 - i];
+        conv1d(cur, C, l, n, e.blk[i].sc, false, nullptr, t1, s);           // shortcut on the block input
+        conv1d(cur, C, l, n, e.blk[i].c1, true, nullptr, t2, s);            // ELU -> k3 -> [C/2][L]
+        conv1d(t2, C / 2, l, n, e.blk[i].c2, true, t1, cur, s);             // ELU -> k1, + shortcut
+        conv1d(cur, C, l, n, e.blk[i].ds, true, nullptr, t1, s, r);         // ELU -> k 2r, stride r -> [2C][ceil(L / r)]
+        for (int & x : L) x = conv1d_out_len(x, e.blk[i].ds.k, r);
+        C *= 2;
+        std::swap(cur, t1);
+    }
+    for (int b = 0; b < n; b++)
+        if (L[(size_t) b] != (n_samples[b] - 1) / kCodecHop + 1) { fprintf(stderr, "%s: internal error: %d latent frames for %d samples\n", caller, L[(size_t) b], n_samples[b]); return nullptr; }
+    lstm2(e.lstm, cur, C, l, n, sc, t1, t2, s);
+    conv1d(t2, C, l, n, e.final_conv, true, nullptr, t1, s);                // ELU -> k7 -> latent [128][T]
+    if (!rvq_encode(cm.embed, cm.embed_norm, n_q, cm.n_bins, cm.hidden_dim, t1, l, n, sc.codes, s)) { fprintf(stderr, "%s: unsupported codebook shape (%d bins of %d)\n", caller, cm.n_bins, cm.hidden_dim); return nullptr; }
+    return t1;
+}
+
+// v = the count values at src, copied back on s
+template <class V> static void fetch(std::vector<V> & v, const V * src, size_t count, cudaStream_t s) {
+    v.resize(count);
+    BARK_CUDA_CHECK(cudaMemcpyAsync(v.data(), src, count * sizeof(V), cudaMemcpyDeviceToHost, s)); g_d2h_bytes += count * sizeof(V);
+}
+
+// The launches of n checked items of T[i] frames.  Per launch: the scratch sized, upload(first, last, &latent) enqueues the items'
+// inputs (for an encode, and the encoder, whose latents it points latent at; false with a message on failure), then the outputs of
+// `out` come back item by item (codes and latent, then the decoder's waveform of the codes in the scratch), and one synchronisation.
+template <class Upload>
+static bool run_launches(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, int n, const int * T, int n_q, const CodecOutputs & out,
+                         const char * fn, const Upload & upload) {
+    const size_t Hd = (size_t) cm.hidden_dim;
+    for (const auto & g : codec_launches(T, n)) {
+        size_t frames = 0;
+        for (int i = g.first; i < g.second; i++) frames += (size_t) T[i];
+        if (!codec_scratch(sc, frames, n_q, fn)) return false;
+        const float * lat = nullptr;
+        if (!upload(g.first, g.second, &lat)) return false;
+        size_t f = 0;
+        for (int i = g.first; i < g.second; f += (size_t) T[i], i++) {
+            if (out.codes) fetch(out.codes[i], sc.codes + (size_t) n_q * f, (size_t) n_q * T[i], s);
+            if (out.latent) fetch(out.latent[i], lat + Hd * f, Hd * T[i], s);
+        }
+        if (out.audio) {                                                 // decodes the codes in the scratch (encodec.cpp:592-602)
+            const float * wav = decode_launch(cm, sc, s, T + g.first, g.second - g.first, n_q);
+            f = 0;
+            for (int i = g.first; i < g.second; f += (size_t) T[i], i++) fetch(out.audio[i], wav + (size_t) kCodecHop * f, (size_t) kCodecHop * T[i], s);
+        }
+        BARK_CUDA_CHECK(cudaStreamSynchronize(s));
+    }
+    return true;
+}
+
+bool codec_decode(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, int n, const int32_t * const * codes, const int * T, int n_q, std::vector<float> * audio,
+                  const char * batch_fn) {
+    const char * fn = batch_fn ? batch_fn : "codec_decode";
+    for (int i = 0; i < n; i++)
+        if (T[i] < kCodecMinFrames) {
+            fprintf(stderr, "%s: %sneed at least %d frames (reflect padding of the k=7 convolutions), got %d\n", fn, item_tag(batch_fn, i).c_str(), kCodecMinFrames, T[i]);
+            return false;
+        }
+    if (n_q < 1 || n_q > cm.n_q) { fprintf(stderr, "%s: %d codebooks requested, %d loaded\n", fn, n_q, cm.n_q); return false; }
+    for (int i = 0; i < n; i++)
+        for (size_t k = 0; k < (size_t) n_q * T[i]; k++) if (codes[i][k] < 0 || codes[i][k] >= cm.n_bins) {
+            fprintf(stderr, "%s: %scode %d (codebook %zu, frame %zu) is outside the codebooks (%d bins)\n", fn, item_tag(batch_fn, i).c_str(), codes[i][k], k / T[i], k % T[i], cm.n_bins);
+            return false;
+        }
+    CodecOutputs out;
+    out.audio = audio;
+    return run_launches(cm, sc, s, n, T, n_q, out, fn, [&](int first, int last, const float **) {
+        size_t f = 0;
+        for (int i = first; i < last; f += (size_t) T[i], i++) {
+            const size_t nb = (size_t) n_q * T[i] * sizeof(int32_t);
+            BARK_CUDA_CHECK(cudaMemcpyAsync(sc.codes + (size_t) n_q * f, codes[i], nb, cudaMemcpyHostToDevice, s)); g_h2d_bytes += nb;
+        }
+        return true;
+    });
+}
+
+bool codec_encode(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, int n, const float * const * audio, const int * n_samples, int n_q,
+                  const CodecOutputs & out, const char * batch_fn, const AudioFormat * fmt) {
+    const char * fn = batch_fn ? batch_fn : "codec_encode";
+    if (!cm.enc.present) { fprintf(stderr, "%s: the model file has no EnCodec encoder tensors (encoder.*)\n", fn); return false; }
+    if (n_q < 1 || n_q > cm.n_q) { fprintf(stderr, "%s: %d codebooks requested, %d loaded\n", fn, n_q, cm.n_q); return false; }
+    // the encoder's input samples per item, and whether the item goes through the resampler (mono 24 kHz does not)
+    std::vector<int> len(n_samples, n_samples + n);
+    std::vector<char> resampled((size_t) n, 0);
+    size_t stage = 0;                                    // floats of the largest resampled item's source
+    for (int i = 0; i < n; i++) {
+        if (fmt) {
+            const std::string item = item_tag(batch_fn, i);
+            if (!resample_input_ok(fn, item, audio[i], n_samples[i], fmt[i].channels, fmt[i].sample_rate)) return false;
+            const long long L = resample_len(n_samples[i], fmt[i].sample_rate, kCodecSampleRate);
+            if (L < kCodecMinSamples || L > INT_MAX) {
+                fprintf(stderr, "%s: %s%d frames at %d Hz resample to %lld samples at %d Hz (%d to 2^31 - 1: at least %d frames)\n", fn, item.c_str(),
+                        n_samples[i], fmt[i].sample_rate, L, kCodecSampleRate, kCodecMinSamples, kCodecMinFrames);
+                return false;
+            }
+            len[(size_t) i] = (int) L;
+            resampled[(size_t) i] = fmt[i].channels != 1 || fmt[i].sample_rate != kCodecSampleRate;
+            if (resampled[(size_t) i]) stage = std::max(stage, (size_t) n_samples[i] * fmt[i].channels);
+            continue;
+        }
+        if (n_samples[i] < kCodecMinSamples) {
+            fprintf(stderr, "%s: %sneed at least %d samples (%d frames), got %d\n", fn, item_tag(batch_fn, i).c_str(), kCodecMinSamples, kCodecMinFrames, n_samples[i]);
+            return false;
+        }
+        for (int k = 0; k < n_samples[i]; k++) if (!std::isfinite(audio[i][k])) {
+            fprintf(stderr, "%s: %ssample %d is not finite (%g)\n", fn, item_tag(batch_fn, i).c_str(), k, (double) audio[i][k]); return false;
+        }
+    }
+    if (stage > sc.stage_cap) {
+        if (sc.stage) { cudaFree(sc.stage); sc.stage = nullptr; }
+        sc.stage_cap = 0;
+        if (cudaMalloc((void **) &sc.stage, stage * sizeof(float)) != cudaSuccess) {
+            (void) cudaGetLastError(); fprintf(stderr, "%s: out of device memory for %zu source samples\n", fn, stage); return false;
+        }
+        sc.stage_cap = stage;
+    }
+    std::vector<int> T((size_t) n);
+    for (int i = 0; i < n; i++) T[(size_t) i] = (len[(size_t) i] - 1) / kCodecHop + 1;
+    return run_launches(cm, sc, s, n, T.data(), n_q, out, fn, [&](int first, int last, const float ** lat) {
+        if (fmt && sc.tables.size() + (size_t)(last - first) > kResampleTablesKept) {
+            for (auto & t : sc.tables) if (t.second) cudaFree(t.second);          // no launch in flight: the last one synchronised
+            sc.tables.clear();
+        }
+        size_t off = 0;
+        for (int i = first; i < last; off += (size_t) len[(size_t) i], i++) {
+            if (resampled[(size_t) i]) {                 // the source through the staging buffer, reused item by item on the stream
+                const size_t nb = (size_t) n_samples[i] * fmt[i].channels * sizeof(float);
+                BARK_CUDA_CHECK(cudaMemcpyAsync(sc.stage, audio[i], nb, cudaMemcpyHostToDevice, s)); g_h2d_bytes += nb;
+                resample(sc.stage, n_samples[i], fmt[i].channels, scratch_table(sc, fmt[i].sample_rate), sc.buf[2] + off, len[(size_t) i], s);
+                continue;
+            }
+            const size_t nb = (size_t) n_samples[i] * sizeof(float);
+            BARK_CUDA_CHECK(cudaMemcpyAsync(sc.buf[2] + off, audio[i], nb, cudaMemcpyHostToDevice, s)); g_h2d_bytes += nb;
+        }
+        *lat = encode_launch(cm, sc, s, len.data() + first, last - first, n_q, fn);
+        return *lat != nullptr;
+    });
+}
+
+}  // namespace bark

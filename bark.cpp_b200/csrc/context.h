@@ -143,32 +143,36 @@ struct ShardKV {
     void store(bark_context * ctx, const GPTModel & m, int il, int rows, MatmulEpilogue & qkv) const;
     void attend(bark_context * ctx, const GPTModel & m, int il, int rows, const ActLayout & a) const;
 };
-// The EnCodec pipelines, shared by bark_context (8 codebooks) and encodec_context (encodec_api.cu).
-// Reads the codec section at f's position into c: every tensor, codebooks 0..max_q-1 (at least 8 must exist); buffers from arena.
+// loader.cu: reads the codec section at f's position into c: every tensor, codebooks 0..max_q-1 (at least 8 must exist); buffers from
+// arena.  Shared by bark_context (8 codebooks) and encodec_context (encodec_api.cu).
 bool load_codec(std::ifstream & f, CodecModel & c, int max_q, DeviceArena & arena, cudaStream_t s, bool verbose);
+// codec_pipeline.cu — the EnCodec pipelines, shared by bark_context and encodec_context.
 // Both take n clips of independent lengths.  Every item is validated before anything is enqueued; batch_fn: the public batch call, whose
 // name the messages carry and which name the item (null: a single call's messages, under the pipeline's own name);
 // the items then run in consecutive launches, each one pass of the codec kernels over all its items with one
 // synchronisation at its end.  Item i's results are bit-identical to the same clip run alone.
 // Frames of one launch (about 320 s of audio): its scratch is 131 KB per frame, 3.1 GB at the budget.  A longer clip runs alone.
 constexpr int kCodecLaunchFrames = 24000;
-// Decode codes[i] ([n_q][T[i]] on the host, checked against the codebooks, T[i] >= 7) to 320 T[i] samples in audio[i].
+// Decode codes[i] ([n_q][T[i]] on the host, checked against the codebooks, T[i] >= kCodecMinFrames) to kCodecHop T[i] samples in audio[i].
 bool codec_decode(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, int n, const int32_t * const * codes, const int * T, int n_q,
                   std::vector<float> * audio, const char * batch_fn = nullptr);
-// Encode (encodec_compress_audio): audio[i], n_samples[i] mono 24 kHz samples -> codes [n_q][T_i], T_i = ceil(n_samples[i] / 320), copied to
-// codes[i], the latent [128][T_i] to latent[i] and the decoder's waveform of those codes (encodec_reconstruct_audio) to decoded[i] where
-// the arrays are set.  false (message on stderr) without encoder tensors, for n_samples < 1921, a non-finite sample or n_q outside the
-// loaded codebooks.
+// What an encode copies back for item i where the array is set: its codes [n_q][T_i] to codes[i], its latent [128][T_i] to latent[i]
+// and the decoder's waveform of those codes (encodec_reconstruct_audio) to audio[i].
+struct CodecOutputs { std::vector<int32_t> * codes = nullptr; std::vector<float> * latent = nullptr, * audio = nullptr; };
+// Encode (encodec_compress_audio): audio[i], n_samples[i] mono 24 kHz samples -> T_i = ceil(n_samples[i] / kCodecHop) frames, the
+// outputs of out.  false (message on stderr) without encoder tensors, for n_samples < kCodecMinSamples, a non-finite sample or n_q
+// outside the loaded codebooks.
 // With fmt, item i is n_samples[i] interleaved frames [n][fmt[i].channels] at fmt[i].sample_rate, down-mixed and resampled to 24 kHz on
 // the device first (DESIGN.md §16); its resampled length L_i then stands for n_samples[i].  Mono 24 kHz items go in unchanged.
 constexpr int kCodecSampleRate = 24000;
 struct AudioFormat { int channels, sample_rate; };
 bool codec_encode(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, int n, const float * const * audio, const int * n_samples, int n_q,
-                  std::vector<int32_t> * codes, std::vector<float> * latent, std::vector<float> * decoded, const char * batch_fn = nullptr,
-                  const AudioFormat * fmt = nullptr);
+                  const CodecOutputs & out, const char * batch_fn = nullptr, const AudioFormat * fmt = nullptr);
 // false (message naming fn, and the item for a batch) for a format or clip outside the resampler's limits: 1 to 8 channels, 4000 to
 // 384000 Hz, fewer than 2^31 samples, every sample finite with |x| <= 2^64
 bool resample_input_ok(const char * fn, const std::string & item, const float * x, int n_frames, int channels, int sample_rate);
+// "item i: " in the messages of a batch call (batch_fn set), whatever its size; nothing for a single call, whose messages stay as they were
+std::string item_tag(const char * batch_fn, int i);
 
 // sampling.cu
 constexpr int kSampleMaxLogits = 16384;          // logits of one row: sample_rows_kernel holds the row in 64 KB of shared memory

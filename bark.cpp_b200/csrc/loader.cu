@@ -247,19 +247,18 @@ bool load_codec(std::ifstream & f, CodecModel & c, int max_q, DeviceArena & aren
     struct CSlot { ConvW * cv = nullptr; bool is_w = false, transposed = false; __half ** hw = nullptr; int * kp = nullptr; float ** fb = nullptr; int ne[3]; };
     std::map<std::string, CSlot> slots;
     const int nf = c.n_filters, ks = c.kernel_size, rk = c.res_kernel;
-    static const int ratios[4] = {8, 5, 4, 2};
     auto conv = [&](const std::string & base, ConvW * cv, int k, int cin, int cout, bool transposed) {
         cv->k = k; cv->cin = cin; cv->cout = cout;
         CSlot w; w.cv = cv; w.is_w = true; w.transposed = transposed; w.ne[0] = k; w.ne[1] = transposed ? cout : cin; w.ne[2] = transposed ? cin : cout; slots[base + ".weight"] = w;
         CSlot b; b.cv = cv; b.is_w = false; b.ne[0] = cout; b.ne[1] = 1; b.ne[2] = 1; slots[base + ".bias"] = b;
     };
-    auto lstm = [&](const std::string & base, __half ** ih_w, __half ** hh_w, float ** ih_b, float ** hh_b, int * kp, int Hn) {
+    auto lstm = [&](const std::string & base, CodecLSTM & w, int Hn) {
         for (int l = 0; l < 2; l++) {
             const std::string sfx = "_l" + std::to_string(l);
-            CSlot a; a.hw = &ih_w[l]; a.kp = kp; a.ne[0] = Hn; a.ne[1] = 4 * Hn; a.ne[2] = 1; slots[base + ".weight_ih" + sfx] = a;
-            CSlot b; b.hw = &hh_w[l]; b.kp = kp; b.ne[0] = Hn; b.ne[1] = 4 * Hn; b.ne[2] = 1; slots[base + ".weight_hh" + sfx] = b;
-            CSlot d; d.fb = &ih_b[l]; d.ne[0] = 4 * Hn; d.ne[1] = 1; d.ne[2] = 1; slots[base + ".bias_ih" + sfx] = d;
-            CSlot e; e.fb = &hh_b[l]; e.ne[0] = 4 * Hn; e.ne[1] = 1; e.ne[2] = 1; slots[base + ".bias_hh" + sfx] = e;
+            CSlot a; a.hw = &w.ih_w[l]; a.kp = &w.Kp; a.ne[0] = Hn; a.ne[1] = 4 * Hn; a.ne[2] = 1; slots[base + ".weight_ih" + sfx] = a;
+            CSlot b; b.hw = &w.hh_w[l]; b.kp = &w.Kp; b.ne[0] = Hn; b.ne[1] = 4 * Hn; b.ne[2] = 1; slots[base + ".weight_hh" + sfx] = b;
+            CSlot d; d.fb = &w.ih_b[l]; d.ne[0] = 4 * Hn; d.ne[1] = 1; d.ne[2] = 1; slots[base + ".bias_ih" + sfx] = d;
+            CSlot e; e.fb = &w.hh_b[l]; e.ne[0] = 4 * Hn; e.ne[1] = 1; e.ne[2] = 1; slots[base + ".bias_hh" + sfx] = e;
         }
     };
     {   // encoder (encodec.cpp:225-330 names): [C][L] -> [2C][L/r] per block, C = 32 .. 256, r = 2, 4, 5, 8
@@ -271,19 +270,19 @@ bool load_codec(std::ifstream & f, CodecModel & c, int max_q, DeviceArena & aren
             conv(rb + ".block.1.conv.conv", &e.blk[i].c1, rk, ch, ch / 2, false);
             conv(rb + ".block.3.conv.conv", &e.blk[i].c2, 1, ch / 2, ch, false);
             conv(rb + ".shortcut.conv.conv", &e.blk[i].sc, 1, ch, ch, false);
-            conv("encoder.model." + std::to_string(3 * (i + 1)) + ".conv.conv", &e.blk[i].ds, 2 * ratios[3 - i], ch, 2 * ch, false);
+            conv("encoder.model." + std::to_string(3 * (i + 1)) + ".conv.conv", &e.blk[i].ds, 2 * kCodecRatios[3 - i], ch, 2 * ch, false);
             ch *= 2;
         }
-        lstm("encoder.model.13.lstm", e.lstm_ih_w, e.lstm_hh_w, e.lstm_ih_b, e.lstm_hh_b, &e.lstm_Kp, ch);
+        lstm("encoder.model.13.lstm", e.lstm, ch);
         conv("encoder.model.15.conv.conv", &e.final_conv, ks, ch, c.hidden_dim, false);
     }
     int mult = 16;
     conv("decoder.model.0.conv.conv", &c.init, ks, c.hidden_dim, mult * nf, false);
-    lstm("decoder.model.1.lstm", c.lstm_ih_w, c.lstm_hh_w, c.lstm_ih_b, c.lstm_hh_b, &c.lstm_Kp, mult * nf);
+    lstm("decoder.model.1.lstm", c.lstm, mult * nf);
     for (int i = 0; i < 4; i++) {
         const int ch = mult * nf;
         const std::string up = "decoder.model." + std::to_string(3 * (i + 1)), rb = "decoder.model." + std::to_string(3 * (i + 1) + 1);
-        conv(up + ".convtr.convtr", &c.blk[i].us, 2 * ratios[i], ch, ch / 2, true);
+        conv(up + ".convtr.convtr", &c.blk[i].us, 2 * kCodecRatios[i], ch, ch / 2, true);
         conv(rb + ".block.1.conv.conv", &c.blk[i].c1, rk, ch / 2, ch / 4, false);
         conv(rb + ".block.3.conv.conv", &c.blk[i].c2, 1, ch / 4, ch / 2, false);
         conv(rb + ".shortcut.conv.conv", &c.blk[i].sc, 1, ch / 2, ch / 2, false);

@@ -49,12 +49,24 @@ struct ConvW { __half * w = nullptr; float * b = nullptr; int k = 0, cin = 0, co
 
 constexpr int kMaxCodebooks = 32;          // codebooks of the 24 kHz EnCodec (24 kbps)
 
+// The 24 kHz EnCodec's time axis: the decoder up-samples by the ratios in this order and the encoder down-samples by them in reverse,
+// so a latent frame is kCodecHop samples.  The final k=7 convolutions reflect-pad 6 frames: a clip needs kCodecMinFrames frames, that
+// is kCodecMinSamples samples (the reference reads out of bounds below that).
+constexpr int kCodecRatios[4] = {8, 5, 4, 2};
+constexpr int kCodecHop = kCodecRatios[0] * kCodecRatios[1] * kCodecRatios[2] * kCodecRatios[3];   // 320
+constexpr int kCodecMinFrames = 7;
+constexpr int kCodecMinSamples = kCodecHop * (kCodecMinFrames - 1) + 1;                               // 1921
+
+struct CodecLSTM {                          // two layers (encodec.cpp/lstm.h); the second's input is added to its output
+    __half * ih_w[2] = {nullptr, nullptr}, * hh_w[2] = {nullptr, nullptr};   // [4H] x H, LI16 rows of Kp
+    int Kp = 0;
+    float  * ih_b[2] = {nullptr, nullptr}, * hh_b[2] = {nullptr, nullptr};
+};
+
 struct CodecModel {
     int hidden_dim = 128, n_filters = 32, kernel_size = 7, res_kernel = 3, n_bins = 1024;
     ConvW init, final_conv;
-    __half * lstm_ih_w[2] = {nullptr, nullptr}, * lstm_hh_w[2] = {nullptr, nullptr};   // [4H] x H, LI16 rows
-    int lstm_Kp = 0;
-    float  * lstm_ih_b[2] = {nullptr, nullptr}, * lstm_hh_b[2] = {nullptr, nullptr};
+    CodecLSTM lstm;
     struct Block { ConvW us, c1, c2, sc; } blk[4];   // us: transposed conv
     int bandwidth = 24, sample_rate = 24000;           // the file's hyper-parameters (kbps, Hz)
     int n_q = 0;                            // codebooks loaded: 0..n_q-1
@@ -64,9 +76,7 @@ struct CodecModel {
         bool present = false;
         ConvW init, final_conv;
         struct Block { ConvW sc, c1, c2, ds; } blk[4];   // ds: down-sampling conv, k = 2r, stride r
-        __half * lstm_ih_w[2] = {nullptr, nullptr}, * lstm_hh_w[2] = {nullptr, nullptr};
-        int lstm_Kp = 0;
-        float  * lstm_ih_b[2] = {nullptr, nullptr}, * lstm_hh_b[2] = {nullptr, nullptr};
+        CodecLSTM lstm;
     } enc;
 };
 
@@ -87,7 +97,7 @@ struct ResampleTable {
     const float * taps = nullptr;
 };
 
-// EnCodec scratch for one launch's items (T frames in all), grown on demand by codec_scratch (gpt_forward.cu), freed by release()
+// EnCodec scratch for one launch's items (T frames in all), grown on demand by codec_scratch (codec_pipeline.cu), freed by release()
 struct CodecScratch {
     float * buf[3] = {nullptr, nullptr, nullptr}; size_t cap = 0;   // ping-pong activations (floats), item-major
     float * gi = nullptr;                                            // LSTM input projections
