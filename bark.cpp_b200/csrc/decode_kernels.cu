@@ -474,8 +474,9 @@ __device__ __forceinline__ void embed_token(const void * wte, const float * wpe,
     }
 }
 
-constexpr int kMaxTasks = 8;        // (h, k) score tasks per warp with their K rows prefetched: H * block_size / (n_score_cta * kWarps) = 12 * 1024 / (100 * 16) < 8 (bark-small);
-                                    // beyond that (bark-large past n_kv = 672) the remaining tasks run without the prefetch
+constexpr int kMaxTasks = 8;        // (h, k) score tasks per warp per batch of the transposed butterfly; a warp's key tail holds up to 2 * kMaxTasks (key_tail).
+                                    // 128 CTAs: bark-small has 80 score CTAs, H * block_size / (80 * kWarps) = 12 * 1024 / 1280 < 10 tasks per warp; bark-large f16
+                                    // has 64 score CTAs whose tails hold 8 tasks, so past n_kv = 513 (16 * n_past > 8 * 1024) the rest run without the prefetch
 
 // Block-wide state of the phases, in static shared memory (a by-reference struct in local memory cost L1/L2 round trips on
 // the critical path: the 72 KB of per-thread stack frames do not fit the L1 left over next to 220 KB of shared memory).

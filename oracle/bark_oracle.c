@@ -1112,9 +1112,14 @@ int orc_generate(orc_ctx * c, const char * text, int32_t * semantic, int * n_sem
                  int * n_frames, float * audio) {
     int32_t prompt[513];
     orc_tokenize(c, text, prompt);
-    int32_t * sem = malloc(1024 * 4), * co = malloc(2 * 1024 * 4), * fi = malloc(8 * 1024 * 4), * codes = malloc(8 * 1024 * 4);
+    /* 1024 semantic ids make at most 1539 coarse frames (orc_coarse) */
+    int32_t * sem = malloc(1024 * 4), * co = malloc(2 * 2048 * 4), * fi = malloc(8 * 1024 * 4), * codes = malloc(8 * 1024 * 4);
     int ns = orc_semantic(c, prompt, sem);
     int T = orc_coarse(c, sem, ns, co);
+    if (T > 1024) {                        /* the reference's fine stage writes out of bounds there (orc_fine) */
+        free(sem); free(co); free(fi); free(codes);
+        return -1;
+    }
     orc_fine(c, co, T, fi);
     for (int cb = 0; cb < 8; cb++) for (int t = 0; t < T; t++) codes[cb * T + t] = fi[t * 8 + cb];   /* bark.cpp:2151-2159 */
     int n = orc_encodec_decode(c, codes, T, audio);

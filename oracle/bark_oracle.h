@@ -42,13 +42,15 @@ int  orc_fine_eval(orc_ctx * c, const int32_t * in_buffer, int nn, float * logit
 int  orc_sample(orc_ctx * c, const float * logits, int n, float temp, float * eos_p);
 int  orc_sample_u(const float * logits, int n, float temp, double u, float * eos_p);   /* the same with the uniform draw given */
 
-/* stage loops; return counts.  Buffers sized by the caller (<=768 semantic, frames<=1024) */
+/* stage loops; return counts.  Buffers sized by the caller: <= 1024 semantic ids, <= 1539 coarse frames (1024 semantic ids),
+ * fine frames <= 1024 (orc_fine asserts it: the reference's fine stage writes out of bounds beyond) */
 int  orc_semantic(orc_ctx * c, const int32_t * prompt513, int32_t * out);
 int  orc_coarse(orc_ctx * c, const int32_t * semantic, int n_semantic, int32_t * out_Tx2);
 int  orc_fine(orc_ctx * c, const int32_t * coarse_Tx2, int n_frames, int32_t * out_Tx8);
 /* EnCodec decode; codes [8][T]; returns samples (320*T) written to out */
 int  orc_encodec_decode(orc_ctx * c, const int32_t * codes_8xT, int T, float * out);
-/* full bark_generate_audio (bark.cpp:2125); audio_out must hold 320*1024 floats.  Token buffers may be NULL. */
+/* full bark_generate_audio (bark.cpp:2125); audio_out must hold 320*1024 floats.  Token buffers may be NULL.  Returns -1 for a clip
+ * of more than 1024 coarse frames (more than 681 semantic ids), which the reference's fine stage cannot hold. */
 int  orc_generate(orc_ctx * c, const char * text, int32_t * semantic, int * n_semantic,
                   int32_t * coarse, int32_t * fine, int * n_frames, float * audio_out);
 

@@ -115,7 +115,26 @@ class Oracle:
         sem = np.zeros(1024, np.int32); co = np.zeros((1024, 2), np.int32); fi = np.zeros((1024, 8), np.int32)
         au = np.zeros(320 * 1024, np.float32); ns = C.c_int(0); T = C.c_int(0)
         n = self.L.orc_generate(self.ctx, text.encode(), _p(sem), C.byref(ns), _p(co), _p(fi), C.byref(T), _p(au))
+        if n < 0:
+            raise RuntimeError("the clip has more than 1024 coarse frames: the reference's fine stage cannot hold it (use the stage calls)")
         return dict(semantic=sem[:ns.value].copy(), coarse=co[:T.value].copy(), fine=fi[:T.value].copy(), audio=au[:n].copy())
+
+    # the stages of generate one at a time, on the context's RNG stream (generate calls them in this order)
+    def semantic(self, prompt):
+        """semantic ids of a tokenized prompt (tokenize)"""
+        p = np.ascontiguousarray(prompt, np.int32); out = np.zeros(1024, np.int32)
+        return out[:self.L.orc_semantic(self.ctx, _p(p), _p(out))].copy()
+
+    def coarse(self, semantic):
+        """coarse ids [T][2] (codebook ids, 0 .. 1023) of semantic ids"""
+        s = np.ascontiguousarray(semantic, np.int32); out = np.zeros((2048, 2), np.int32)
+        return out[:self.L.orc_coarse(self.ctx, _p(s), s.size, _p(out))].copy()
+
+    def fine(self, coarse):
+        """fine ids [T][8] of coarse ids [T][2], T <= 1024"""
+        c = np.ascontiguousarray(coarse, np.int32); out = np.zeros((c.shape[0], 8), np.int32)
+        self.L.orc_fine(self.ctx, _p(c), c.shape[0], _p(out))
+        return out
 
 
 class Ref:

@@ -5,6 +5,7 @@ where the reference sources exist) returns for exactly the inputs of
     tests/test_parity_gpu.py::test_full_size_against_the_reference_itself -> ref_pairs/small_f16_n12.npz (CUDA vs reference)
     tests/test_quantize.py (the reference tool's quantised files, the reference on them) -> ref_pairs/quantized.npz
     tests/test_prefix_rows.py (the reference's from-scratch coarse evaluation)             -> ref_pairs/prefix_rows.npz
+    tests/test_oracle_vs_ref.py::test_long_context_bit_exact (steps up to n_kv 1024)        -> ref_pairs/long_context.npz
 
 so these comparisons run on machines that have no reference build.  Run once where the reference library exists:
 
@@ -162,6 +163,31 @@ def prefix_rows(orc, weights, tmp):
     return d
 
 
+LONG_CONTEXT_SEED = 6               # tests/test_oracle_vs_ref.py test_long_context_bit_exact
+LONG_SEMANTIC_PAST = 1015           # semantic steps at n_past 1015 .. 1023: the last one sees n_kv = 1024
+LONG_COARSE_PROMPT = 887            # 256 semantic ids + 1 + 630 coarse history ids: the longest coarse window prompt
+
+
+def long_context(orc, path):
+    """tiny f16: semantic steps at n_past 1015 .. 1023 after the merged prompt and a 758-id continuation, and coarse steps at n_past
+    887 .. 902 after a whole window prompt, teacher-forced, every step's logits pinned."""
+    r = orc.Ref(path)
+    d = dict(reference_build=r.build_info())
+    rng = np.random.default_rng(LONG_CONTEXT_SEED)
+    lg, n_past = r.gpt_eval(0, r.tokenize("hello world"), 0, True)
+    lg, n_past = r.gpt_eval(0, rng.integers(0, 10000, LONG_SEMANTIC_PAST - n_past).astype(np.int32), n_past, False)
+    for i in range(1024 - LONG_SEMANTIC_PAST):
+        lg, n_past = r.gpt_eval(0, np.array([int(np.argmax(lg[:10000]))], np.int32), n_past, False)
+        pin(d, f"semantic{i}", lg)
+    prompt = np.concatenate([rng.integers(0, 10000, 256), [12050], rng.integers(10000, 12048, LONG_COARSE_PROMPT - 257)]).astype(np.int32)
+    lg, n_past = r.gpt_eval(1, prompt, 0, False)
+    for i in range(16):
+        lg, n_past = r.gpt_eval(1, np.array([10000 + int(np.argmax(lg[10000:12048]))], np.int32), n_past, False)
+        pin(d, f"coarse{i}", lg)
+    r.close()
+    return d
+
+
 def main():
     graft.load_package()
     weights = importlib.import_module("bark_cpp_b200.weights")
@@ -175,6 +201,9 @@ def main():
             weights.write_weights(path, weights.CONFIGS[config](weights.F16), 1234)
             np.savez_compressed(os.path.join(OUT, name), **fn(orc, path))
             print(name, os.path.getsize(os.path.join(OUT, name)), "bytes")
+        path = os.path.join(tmp, "tiny_f16_1234.bin")
+        np.savez_compressed(os.path.join(OUT, "long_context.npz"), **long_context(orc, path))
+        print("long_context.npz", os.path.getsize(os.path.join(OUT, "long_context.npz")), "bytes")
         for fn, name in ((quantized, "quantized.npz"), (prefix_rows, "prefix_rows.npz")):
             np.savez_compressed(os.path.join(OUT, name), **fn(orc, weights, tmp))
             print(name, os.path.getsize(os.path.join(OUT, name)), "bytes")

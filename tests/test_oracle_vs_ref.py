@@ -82,3 +82,22 @@ def test_full_generate(pair):
     for k in ("semantic", "coarse", "fine"):
         assert np.array_equal(a[k], r[f"generate_{k}"]), k
     assert_pinned(a["audio"], r, "generate_audio")
+
+
+def test_long_context_bit_exact(orc, weights_file):
+    """Steps up to n_kv 1024: semantic steps at n_past 1015 .. 1023 after the merged prompt and a 758-id continuation, coarse steps at
+    n_past 887 .. 902 after a whole window prompt (the reference's logits in ref_pairs/long_context.npz)."""
+    r = np.load(os.path.join(GOLDEN_DIR, "ref_pairs", "long_context.npz"))
+    o = orc.Oracle(weights_file("tiny", "f16"))
+    rng = np.random.default_rng(6)
+    lg, n_past = o.gpt_eval(0, o.tokenize("hello world"), 0, True)
+    lg, n_past = o.gpt_eval(0, rng.integers(0, 10000, 1015 - n_past).astype(np.int32), n_past, False)
+    for i in range(9):
+        lg, n_past = o.gpt_eval(0, np.array([int(np.argmax(lg[:10000]))], np.int32), n_past, False)
+        assert_pinned(lg, r, f"semantic{i}", f"semantic step at n_past {n_past - 1}")
+    assert n_past == 1024
+    prompt = np.concatenate([rng.integers(0, 10000, 256), [12050], rng.integers(10000, 12048, 630)]).astype(np.int32)
+    lg, n_past = o.gpt_eval(1, prompt, 0, False)
+    for i in range(16):
+        lg, n_past = o.gpt_eval(1, np.array([10000 + int(np.argmax(lg[10000:12048]))], np.int32), n_past, False)
+        assert_pinned(lg, r, f"coarse{i}", f"coarse step at n_past {n_past - 1}")
