@@ -109,7 +109,7 @@ EXPORTS = [
     "bark_b200_get_stats", "bark_b200_get_hparams", "bark_b200_kernel_launches", "bark_b200_layernorm_fallbacks",
     "bark_b200_profile_enable", "bark_b200_profile_report", "bark_b200_io_counters", "bark_b200_decode_timing",
     "bark_b200_shard_init", "bark_b200_shard_connect", "bark_b200_shard_nvlink_bytes",
-    "bark_b200_fast_mode", "bark_b200_fast_gemm", "bark_b200_fast_attention", "bark_b200_parity_attention", "bark_b200_parity_gemm",
+    "bark_b200_fast_mode", "bark_b200_fast_gemm", "bark_b200_fast_attention", "bark_b200_parity_attention", "bark_b200_batch_attention", "bark_b200_parity_gemm",
     "bark_b200_parity_rows", "bark_b200_sample_given_u", "bark_b200_generate_batch", "bark_b200_batch_audio", "bark_b200_batch_tokens", "bark_b200_gpt_eval_slot", "bark_b200_gpt_step_batch",
     "bark_b200_set_history_prompt", "bark_b200_generate_batch_prompted", "bark_b200_set_sampling", "bark_b200_sample_filtered_given_u",
     "bark_b200_quant_matmul", "bark_b200_fast_convert",
@@ -207,6 +207,8 @@ def lib() -> C.CDLL:
     L.bark_b200_fast_attention.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int]
     L.bark_b200_parity_attention.restype = C.c_int
     L.bark_b200_parity_attention.argtypes = [vp, vp, vp, vp] + [C.c_int] * 7
+    L.bark_b200_batch_attention.restype = C.c_int
+    L.bark_b200_batch_attention.argtypes = [f32p, f32p, f32p, f32p, f32p, i32p] + [C.c_int] * 5 + [vp]
     L.bark_b200_parity_gemm.restype = C.c_int
     L.bark_b200_parity_gemm.argtypes = [vp, vp, vp] + [C.c_int] * 6 + [vp]
     L.bark_b200_quant_matmul.restype = C.c_int
@@ -648,6 +650,33 @@ def parity_attention(q: np.ndarray, k: np.ndarray, v: np.ndarray, n_head: int, n
     return out
 
 
+BATCH_ACTS = {"f32": 0, "f16": 1, "f32_gm": 2}      # the result's operand format: f32 rows, f16 / f32 group-major
+
+
+def batch_attention(q: np.ndarray, k_new: np.ndarray, v_new: np.ndarray, k_cache: np.ndarray, v_cache: np.ndarray, pos, n_head: int,
+                    act: str = "f32"):
+    """The batched decode step's attention (attention_batch) for B <= 8 rows of different sequences; q, k_new, v_new [B][E] float32,
+    k_cache, v_cache [B][cap][E] float32 (cap <= 1024), pos [B] with 0 <= pos[b] < cap.  Row b appends k_new[b] / v_new[b] at row
+    pos[b] of its caches and attends over its pos[b] + 1 keys.  Returns (out [B][E], k_cache, v_cache): out float32, or float16 for
+    act "f16" ("f32" is stored as f32 rows, "f16" / "f32_gm" as the group-major operand; every form comes back row-major), and copies
+    of the caches after the call, NaN from row pos[b] + 1 on.  Raises GuardBandError when a store landed outside the output or a
+    cache, RuntimeError when the hook failed or rejected its arguments."""
+    q, k_new, v_new = (np.ascontiguousarray(a, np.float32) for a in (q, k_new, v_new))
+    kc = np.array(k_cache, np.float32, order="C", copy=True); vc = np.array(v_cache, np.float32, order="C", copy=True)
+    pos = np.ascontiguousarray(pos, np.int32)
+    B, E = q.shape
+    cap = kc.shape[1]
+    assert k_new.shape == v_new.shape == (B, E) and kc.shape == vc.shape == (B, cap, E) and pos.shape == (B,), \
+        (q.shape, k_new.shape, v_new.shape, kc.shape, vc.shape, pos.shape)
+    out = np.zeros((B, E), np.float16 if act == "f16" else np.float32)
+    r = lib().bark_b200_batch_attention(_p(q), _p(k_new), _p(v_new), _p(kc), _p(vc), _p(pos), B, cap, E, n_head, BATCH_ACTS[act], _p(out))
+    if r == -1:
+        raise GuardBandError(f"bark_b200_batch_attention ({B} rows, E {E}, {n_head} heads) wrote outside its output or a cache")
+    if r != 1:
+        raise RuntimeError(f"bark_b200_batch_attention ({B} rows, E {E}, {n_head} heads, cap {cap}) failed")
+    return out, kc, vc
+
+
 PARITY_EPILOGUES = {"store": 0, "resid": 1, "gelu": 2, "qkv": 3}      # EPI_* (csrc/gpt_kernels.h)
 
 
@@ -660,13 +689,19 @@ def _gelu_table(epilogue: str, gelu_tab):
     return tab
 
 
-def parity_gemm(A: np.ndarray, W: np.ndarray, epilogue: str = "store", variant: int = 0, resid: np.ndarray | None = None,
+GEMM_VARIANTS = {"auto": 0, "tile32x16": 1, "tile32x32": 2, "rows": 3}
+
+
+def parity_gemm(A: np.ndarray, W: np.ndarray, epilogue: str = "store", variant: int | str = 0, resid: np.ndarray | None = None,
                 gelu_tab: np.ndarray | None = None, return_variant: bool = False):
-    """Bit-exact A W^T on the parity path's tiled GEMM; A [M][K], W [N][K] both float16 or both float32, K % 32 == 0.
+    """Bit-exact A W^T on the parity path's dense mat-muls; A [M][K], W [N][K] both float16 or both float32, K % 32 == 0.
 
     Returns float32 [M][N] for "store" and for "resid" (resid [M][N] float32 + A W^T), [M][N] in the operands' dtype for "gelu"
     (GELU through gelu_tab, 65536 uint16 f16 bits), and for "qkv" (N % 3 == 0) the triple Q, K, V of float32 [M][N/3].
-    variant = 0 lets the library pick the block tile, 1 (32 x 16) / 2 (32 x 32) force one; with return_variant the result is (outputs, variant)."""
+    variant = 0 ("auto") runs what the library picks for M rows (the few-row kernel below 16 rows, else the tiled GEMM's tile), 1
+    ("tile32x16") / 2 ("tile32x32") force a tiled GEMM block tile, 3 ("rows") the few-row kernel at any M; with return_variant the
+    result is (outputs, the variant that ran)."""
+    variant = GEMM_VARIANTS.get(variant, variant)
     dt = np.float16 if np.asarray(A).dtype == np.float16 else np.float32
     A = np.ascontiguousarray(A, dt); W = np.ascontiguousarray(W, dt)
     M, K = A.shape; N = W.shape[0]

@@ -176,7 +176,8 @@ template <> struct Quad<float> {
     __device__ static void unpack(const uint4 & u, float (&f)[4]) { f[0] = __uint_as_float(u.x); f[1] = __uint_as_float(u.y); f[2] = __uint_as_float(u.z); f[3] = __uint_as_float(u.w); }
 };
 
-// Few-row version (rows < 16: the 1-row lm_head of a prefill, tiny test shapes).  Weights in the row-major LI layout the
+// Few-row version (rows < 16: every mat-mul of a batched decode step, the 1-row lm_head of a prefill, the per-op single-token path;
+// launched by lane_matmul_rows).  Weights in the row-major LI layout the
 // decode kernel streams; activations in the group-major layout every producer writes.
 template <typename T, int MT>
 __global__ void __launch_bounds__(256) lane_matmul_kernel(const T * __restrict__ W, int K, int Kp, int O, const T * __restrict__ act, int act_gs, int M, MatmulEpilogue ep) {
@@ -219,16 +220,8 @@ __global__ void __launch_bounds__(256) lane_matmul_kernel(const T * __restrict__
     }
 }
 
-void lane_matmul(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, const Q8Scratch * q8, cudaStream_t s) {
-    if (W.type == W_Q4_0) { q4_matmul(W, act, act_gs, rows, ep, q8, s); return; }      // act_gs = f32 row stride for this type
-    if (qx_supported(W.type)) { qx_matmul(W, act, act_gs, rows, ep, q8, s); return; }
+void lane_matmul_rows(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, cudaStream_t s) {
     const int gx = (W.n_out + 7) / 8;
-    {   // roofline annotation: algorithmic HBM bytes (weights once + operands) and flops of this mat-mul
-        const double es = W.type == W_F16 ? 2.0 : 4.0;
-        g_next_bytes = (double) W.n_out * W.K * es + (double) rows * (W.K * es + W.n_out * 4.0);
-        g_next_flops = 2.0 * rows * (double) W.n_out * W.K;
-    }
-    if (rows >= 16 && (W.type == W_F16 || W.type == W_F32)) { lane_gemm_tiled(W, act, act_gs, rows, ep, s); return; }
     if (W.type == W_F16) {
         if (rows == 1) BARK_LAUNCH((lane_matmul_kernel<__half, 1>), dim3(gx, 1), 256, 0, s, (const __half *) W.p, W.K, W.Kp, W.n_out, (const __half *) act, act_gs, rows, ep);
         else           BARK_LAUNCH((lane_matmul_kernel<__half, 8>), dim3(gx, (rows + 7) / 8), 256, 0, s, (const __half *) W.p, W.K, W.Kp, W.n_out, (const __half *) act, act_gs, rows, ep);
@@ -238,6 +231,19 @@ void lane_matmul(const DMat & W, const void * act, int act_gs, int rows, const M
     } else {
         fprintf(stderr, "bark_b200: q4_0 mul_mat is not built in this revision\n"); throw std::runtime_error("unsupported configuration (see the message above)");
     }
+}
+
+int lane_matmul(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, const Q8Scratch * q8, cudaStream_t s) {
+    if (W.type == W_Q4_0) { q4_matmul(W, act, act_gs, rows, ep, q8, s); return 0; }      // act_gs = f32 row stride for this type
+    if (qx_supported(W.type)) { qx_matmul(W, act, act_gs, rows, ep, q8, s); return 0; }
+    {   // roofline annotation: algorithmic HBM bytes (weights once + operands) and flops of this mat-mul
+        const double es = W.type == W_F16 ? 2.0 : 4.0;
+        g_next_bytes = (double) W.n_out * W.K * es + (double) rows * (W.K * es + W.n_out * 4.0);
+        g_next_flops = 2.0 * rows * (double) W.n_out * W.K;
+    }
+    if (rows >= 16 && (W.type == W_F16 || W.type == W_F32)) return lane_gemm_tiled(W, act, act_gs, rows, ep, s);
+    lane_matmul_rows(W, act, act_gs, rows, ep, s);
+    return kLaneRowsVariant;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -32,8 +32,14 @@ void layernorm_act(const float * x, int rows, int E, const float * g, const floa
 // [rows][K/32] (sums for q4_1 / q5_1 only)
 struct Q8Scratch { int8_t * q = nullptr; float * d = nullptr, * s = nullptr; };
 
-// q8: the scratch a quantised W needs (null for f32 / f16 weights)
-void lane_matmul(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, const Q8Scratch * q8, cudaStream_t s);
+// q8: the scratch a quantised W needs (null for f32 / f16 weights).  f32 / f16 W: below 16 rows the few-row kernel (lane_matmul_rows,
+// on W's row-major LI copy), else lane_gemm_tiled (on its group-major copy).  Returns the kernel launched: kLaneRowsVariant for the
+// few-row kernel, else lane_gemm_tiled's block-tile variant; 0 for quantised W.
+constexpr int kLaneRowsVariant = 3;
+int  lane_matmul(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, const Q8Scratch * q8, cudaStream_t s);
+// The few-row kernel at any row count: lane_matmul_kernel<T, 1> for one row, <T, 8> over 8-row blocks otherwise; f32 / f16 W in the
+// row-major LI layout (W.p, W.Kp), activations group-major.
+void lane_matmul_rows(const DMat & W, const void * act, int act_gs, int rows, const MatmulEpilogue & ep, cudaStream_t s);
 
 // Multi-row attention (gemm_kernels.cu): N query rows Q[N][E] against n_kv <= 1024 key / value rows Kc, Vc [n_kv][E], H heads of 32, 64,
 // 96 or 128; causal masks key k for query q when k > n_past + q.  Result -> activation operand for c_proj.

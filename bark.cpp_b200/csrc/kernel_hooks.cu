@@ -75,6 +75,31 @@ bool finish(const char * fn) {
     return e == cudaSuccess;
 }
 
+// Every padding element of a permuted mat-mul operand -> NaN (all bits set: NaN in f16 and in f32), so a kernel that folds one into a
+// stored sum returns NaN.  gm: the group-major layout of group stride gs (row capacity * 128), padding = rows >= rows or columns >= K;
+// else the row-major LI layout of rows of gs = Kp elements, padding = columns >= K.
+template <typename U>               // U: the element's bits, uint16_t (f16) or uint32_t (f32)
+__global__ void poison_padding_kernel(U * p, size_t total, size_t gs, int rows, int K, bool gm) {
+    constexpr int G = 16 / sizeof(U);
+    for (size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t) gridDim.x * blockDim.x) {
+        int r = 0, k;
+        if (gm) { const int w = (int)(i % kGmGroup); r = (int)(i % gs / kGmGroup); k = (int)(i / gs) * kGmGroup + (w & 3) * 32 + (w >> 2); }
+        else    { const int j = (int)(i % gs), e = j % G, gv = j / G; k = ((gv / 32) * G + e) * 32 + gv % 32; }     // as permute_to_li_kernel
+        if (r >= rows || k >= K) p[i] = (U) ~0u;
+    }
+}
+
+void poison_padding(void * p, size_t es, size_t total, size_t gs, int rows, int K, bool gm) {
+    if (es == 2) BARK_LAUNCH(poison_padding_kernel<uint16_t>, 1184, 256, 0, 0, (uint16_t *) p, total, gs, rows, K, gm);
+    else         BARK_LAUNCH(poison_padding_kernel<uint32_t>, 1184, 256, 0, 0, (uint32_t *) p, total, gs, rows, K, gm);
+}
+
+// a group-major operand of group stride gs (host) -> row-major [M][N] elements of es bytes
+void gm_to_rows(const unsigned char * gm, void * dst, int M, int N, size_t gs, size_t es) {
+    for (int m = 0; m < M; m++)
+        for (int k = 0; k < N; k++) memcpy((unsigned char *) dst + ((size_t) m * N + k) * es, gm + gm_offset(m, k, gs) * es, es);
+}
+
 int sm_count() {
     int dev = 0, n_sm = 0;
     BARK_CUDA_CHECK(cudaGetDevice(&dev)); BARK_CUDA_CHECK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
@@ -265,6 +290,50 @@ extern "C" int bark_b200_parity_attention(const float * q, const float * k, cons
     });
 }
 
+// the batched decode step's attention, called as SlotKV::attend calls it (max_kv = the largest pos + 1): row b's query, new K and V rows
+// are q / k_new / v_new [b] (ws.q, ws.kbuf, ws.vbuf), its cache [cap][E] at k_cache / v_cache + b * cap * E.  Each cache is its own
+// guarded allocation whose rows from pos[b] on are NaN before the launch, so a key or value read before the append or from a wrong row
+// shows up, and so does a missing append; the scores start as NaN too.  act: the operand format of the result, 0 f32 rows (quantised
+// c_proj), 1 f16 / 2 f32 group-major at row capacity B; it comes back row-major [B][E].
+extern "C" int bark_b200_batch_attention(const float * q, const float * k_new, const float * v_new, float * k_cache, float * v_cache, const int32_t * pos,
+                                         int B, int cap, int E, int H, int act, void * out) {
+    return guarded(0, [&] {
+        const char * fn = "bark_b200_batch_attention";
+        if (!q || !k_new || !v_new || !k_cache || !v_cache || !pos || !out || B < 1 || B > 8 || cap < 1 || cap > 1024 || H < 1 || E % H) return 0;
+        const int D = E / H;
+        if ((D != 32 && D != 64 && D != 96 && D != 128) || act < 0 || act > 2) return 0;
+        int max_kv = 0;
+        for (int b = 0; b < B; b++) {
+            if (pos[b] < 0 || pos[b] >= cap) return 0;
+            max_kv = std::max(max_kv, pos[b] + 1);
+        }
+        DeviceBuffers mem;
+        const size_t row = (size_t) E * 4, slab = (size_t) cap * E;
+        const float * dq = mem.upload(q, B * row), * dk = mem.upload(k_new, B * row), * dv = mem.upload(v_new, B * row);
+        const int32_t * d_pos = mem.upload(pos, (size_t) B * sizeof(int32_t));
+        std::vector<GuardedOutput> kc, vc;
+        BatchKV kv{};
+        for (int b = 0; b < B; b++) {
+            kc.emplace_back(mem, slab * 4, k_cache + b * slab); vc.emplace_back(mem, slab * 4, v_cache + b * slab);
+            kv.k[b] = kc[b].out<float>(); kv.v[b] = vc[b].out<float>();
+            BARK_CUDA_CHECK(cudaMemset(kv.k[b] + (size_t) pos[b] * E, 0xff, (cap - pos[b]) * row));
+            BARK_CUDA_CHECK(cudaMemset(kv.v[b] + (size_t) pos[b] * E, 0xff, (cap - pos[b]) * row));
+        }
+        float * scores = mem.poisoned<float>((size_t) B * H * max_kv * 4);
+        const WType wt = act == 0 ? W_Q4_0 : act == 1 ? W_F16 : W_F32;
+        const size_t es = act == 1 ? 2 : 4, gs = act == 0 ? (size_t) E : (size_t) B * kGmGroup;
+        const GuardedOutput o(mem, act == 0 ? B * row : gm_groups(E) * gs * es, nullptr);
+        attention_batch(dq, dk, dv, kv, d_pos, B, max_kv, E, H, scores, o.out<void>(), wt, (int) gs, 0);
+        if (!finish(fn)) return 0;
+        bool clean = true;
+        for (int b = 0; b < B; b++) clean = kc[b].read(fn, k_cache + b * slab) && vc[b].read(fn, v_cache + b * slab) && clean;
+        std::vector<unsigned char> h(act == 0 ? 0 : o.bytes);
+        clean = o.read(fn, act == 0 ? out : h.data()) && clean;
+        if (act != 0) gm_to_rows(h.data(), out, B, E, gs, es);
+        return clean ? 1 : -1;
+    });
+}
+
 // the parity path's row reductions: op 0 LayerNorm, op 1 soft_max; impl 0 the multi-row kernels (layernorm_act_kernel writing plain
 // f32 rows, softmax_row), impl 1 the decode kernels' block_layernorm / softmax_exp_rcp
 extern "C" int bark_b200_parity_rows(int op, int impl, const float * x, int rows, int n, const float * g, const float * b, float * out, unsigned * replays) {
@@ -303,8 +372,9 @@ extern "C" int bark_b200_sample_filtered_given_u(const float * logits, int n, in
     });
 }
 
-// parity-path tiled GEMM (tools/gemm_bench.py too): A [M][K] and W [N][K] go through permute_to_gm, as the loader and the activation
-// writers lay them out (row capacity and o_pad rounded up to the tallest / widest tile); the result comes back row-major.
+// parity-path dense mat-muls (tools/gemm_bench.py too): A [M][K] and W [N][K] go through permute_to_gm, as the loader and the activation
+// writers lay them out (row capacity and o_pad rounded up to the tallest / widest tile), and for the few-row kernel W also through
+// permute_to_li, as the loader lays out its row-major copy; every padding element of both is NaN.  The result comes back row-major.
 extern "C" int bark_b200_parity_gemm(const void * A, const void * W, void * C, int M, int N, int K, int wtype, int epilogue, int variant,
                                      const uint16_t * gelu_tab) {
     return guarded(0, [&] {
@@ -312,24 +382,32 @@ extern "C" int bark_b200_parity_gemm(const void * A, const void * W, void * C, i
         if (epilogue < EPI_STORE || epilogue > EPI_QKV || (epilogue == EPI_QKV && N % 3) || (epilogue == EPI_GELU_ACT && !gelu_tab)) return 0;
         const size_t es = wtype == W_F16 ? 2 : 4;
         const int rows_cap = (M + 31) / 32 * 32, o_pad = (N + kGemmOPad - 1) / kGemmOPad * kGemmOPad;
+        const size_t gs = (size_t) rows_cap * kGmGroup, w_gs = (size_t) o_pad * kGmGroup;
         DeviceBuffers mem;
-        void * d_a = mem.alloc((size_t) gm_groups(K) * rows_cap * kGmGroup * es), * d_w = mem.alloc((size_t) gm_groups(K) * o_pad * kGmGroup * es);
+        void * d_a = mem.alloc(gm_groups(K) * gs * es), * d_w = mem.alloc(gm_groups(K) * w_gs * es);
+        const void * d_w_rows = mem.upload(W, (size_t) N * K * es);
         permute_to_gm(mem.upload(A, (size_t) M * K * es), d_a, M, rows_cap, K, (WType) wtype, 0);
-        permute_to_gm(mem.upload(W, (size_t) N * K * es), d_w, N, o_pad, K, (WType) wtype, 0);
+        permute_to_gm(d_w_rows, d_w, N, o_pad, K, (WType) wtype, 0);
+        poison_padding(d_a, es, gm_groups(K) * gs, gs, M, K, true);
+        poison_padding(d_w, es, gm_groups(K) * w_gs, w_gs, N, K, true);
+        DMat dm; dm.n_out = N; dm.K = K; dm.type = (WType) wtype; dm.p_gm = d_w; dm.o_pad = o_pad;
+        if (variant == 0 || variant == kLaneRowsVariant) {
+            dm.Kp = li_padded_k(K, (int) es); dm.p = mem.alloc((size_t) N * dm.Kp * es);
+            permute_to_li(d_w_rows, dm.p, N, K, (WType) wtype, 0);
+            poison_padding(dm.p, es, (size_t) N * dm.Kp, dm.Kp, N, K, false);
+        }
         // output: STORE / RESID / QKV f32 [M][N] (QKV: Q, K, V blocks of [M][N/3] each); GELU_ACT: the group-major operand of the next mul_mat
         const bool gm = epilogue == EPI_GELU_ACT;
-        const GuardedOutput c(mem, gm ? (size_t) gm_groups(N) * rows_cap * kGmGroup * es : (size_t) M * N * 4, epilogue == EPI_RESID ? C : nullptr);
-        DMat dm; dm.n_out = N; dm.K = K; dm.type = (WType) wtype; dm.p_gm = d_w; dm.o_pad = o_pad;
-        const MatmulEpilogue ep = matmul_epilogue(mem, epilogue, c.out<float>(), M, N, gelu_tab, wtype, rows_cap * kGmGroup);
-        const int ran = lane_gemm_tiled(dm, d_a, rows_cap * kGmGroup, M, ep, 0, variant);
+        const GuardedOutput c(mem, gm ? gm_groups(N) * gs * es : (size_t) M * N * 4, epilogue == EPI_RESID ? C : nullptr);
+        const MatmulEpilogue ep = matmul_epilogue(mem, epilogue, c.out<float>(), M, N, gelu_tab, wtype, (int) gs);
+        int ran;
+        if (variant == 0)                     ran = lane_matmul(dm, d_a, (int) gs, M, ep, nullptr, 0);
+        else if (variant == kLaneRowsVariant) { lane_matmul_rows(dm, d_a, (int) gs, M, ep, 0); ran = kLaneRowsVariant; }
+        else                                  ran = lane_gemm_tiled(dm, d_a, (int) gs, M, ep, 0, variant);
         if (!finish("bark_b200_parity_gemm") || !ran) return 0;
         std::vector<unsigned char> h(gm ? c.bytes : 0);
         if (!c.read("bark_b200_parity_gemm", gm ? h.data() : C)) return -1;
-        if (gm) {                                                      // group-major -> row-major [M][N]
-            const size_t gs = (size_t) rows_cap * kGmGroup;
-            for (int m = 0; m < M; m++)
-                for (int k = 0; k < N; k++) memcpy((unsigned char *) C + ((size_t) m * N + k) * es, h.data() + gm_offset(m, k, gs) * es, es);
-        }
+        if (gm) gm_to_rows(h.data(), C, M, N, gs, es);
         return ran;
     });
 }

@@ -237,6 +237,17 @@ BARK_API int  bark_b200_fast_attention(const uint16_t * q, const uint16_t * k, c
 BARK_API int  bark_b200_parity_attention(const float * q, const float * k, const float * v, float * out, int N, int n_kv, int n_past, int E, int H, int causal,
                                          int path);
 
+/* The batched decode step's attention on host buffers without a context (tests): B <= 8 rows of different sequences, row b the one new
+ * query q[b] at position pos[b] of its own sequence, attending over its pos[b] + 1 keys.  q, k_new, v_new: [B][E] f32, the step's query
+ * and new K / V rows; k_cache, v_cache: [B][cap][E] f32, row b's caches, cap <= 1024, 0 <= pos[b] < cap, head size E/H in
+ * {32, 64, 96, 128}.  The kernels append k_new[b] / v_new[b] at row pos[b] of row b's caches and attend; on return the caches hold
+ * rows < pos[b] as given, the appended row, and NaN from pos[b] + 1 on (those rows are NaN while the kernels run).  act: the operand
+ * format the result is stored in, 0 f32 rows (quantised models), 1 f16 group-major (f16 models), 2 f32 group-major (f32 models);
+ * out: [B][E] row-major, f32, or f16 bits for act 1.  Returns 1, 0 on invalid arguments or failure, -1 if a store landed in the
+ * guard bands around the output or a cache. */
+BARK_API int  bark_b200_batch_attention(const float * q, const float * k_new, const float * v_new, float * k_cache, float * v_cache, const int32_t * pos,
+                                        int B, int cap, int E, int H, int act, void * out);
+
 /* Parity-path row reductions on host buffers without a context (tests).  op 0: LayerNorm (eps 1e-5, g required, b may be NULL), the f32
  * value before any operand rounding; op 1: soft_max, the probability as its consumers form it.  impl 0: the multi-row kernels
  * (layernorm_act_kernel / softmax_row), impl 1: the decode kernels' device functions (block_layernorm / softmax_exp_rcp) in a
@@ -253,15 +264,17 @@ BARK_API int  bark_b200_parity_rows(int op, int impl, const float * x, int rows,
 BARK_API int  bark_b200_sample_given_u(const float * logits, int n, int rows, float temp, const double * u, int threads, int32_t * tokens,
                                        int32_t * device_tokens, int32_t * flags, float * eos_p);
 
-/* Parity-path tiled GEMM on host buffers without a context (tests, tools/gemm_bench.py): C = A W^T with every output the reference's
- * vec_dot of its two rows, for A [M][K] and W [N][K] of wtype 0 (f32) or 1 (f16 bits), K % 32 == 0, through the multi-row passes'
+/* Parity-path dense mat-muls on host buffers without a context (tests, tools/gemm_bench.py): C = A W^T with every output the reference's
+ * vec_dot of its two rows, for A [M][K] and W [N][K] of wtype 0 (f32) or 1 (f16 bits), K % 32 == 0, through the parity passes'
  * epilogue `epilogue`:
  *   0 STORE     C = f32 [M][N]
  *   1 RESID     C = f32 [M][N], holds the residual on entry and residual + A W^T on return
  *   2 GELU_ACT  C = [M][N] in wtype: GELU of the product through gelu_tab (65536 f16 entries), as the next mat-mul's operand holds it
  *   3 QKV       N % 3 == 0; C = f32 Q [M][N/3], then K [M][N/3], then V [M][N/3]
- * variant: 0 = the block tile the library picks, 1 = 32 x 16 outputs (8 warps, two CTAs per SM), 2 = 32 x 32 (16 warps, one CTA
- * per SM).  Returns the variant that ran, 0 on failure or invalid arguments, -1 if a store landed in the guard bands around the output. */
+ * variant: 0 = the kernel the library picks for M rows (the few-row kernel below 16 rows, else the tiled GEMM's block tile for wtype),
+ * 1 = the tiled GEMM's 32 x 16 outputs (8 warps, two CTAs per SM), 2 = its 32 x 32 (16 warps, one CTA per SM), 3 = the few-row kernel
+ * (one warp per output, 1 or 8 rows per CTA) at any M.  Every padding element of the permuted operands is NaN.  Returns the variant
+ * that ran, 0 on failure or invalid arguments, -1 if a store landed in the guard bands around the output. */
 BARK_API int  bark_b200_parity_gemm(const void * A, const void * W, void * C, int M, int N, int K, int wtype, int epilogue, int variant,
                                     const uint16_t * gelu_tab);
 

@@ -4,7 +4,8 @@ orc_gelu_table) — bit for bit.
 
 The model tests reach the kernel only at the models' own widths.  These cover row counts on both sides of the 32-row block tile,
 output counts on both sides of the 16- and 32-wide ones, K with a partial last 128-column group, bark-large's widths, every epilogue,
-both operand types and every block-tile variant forced.  Every variant must give the same bits on every output; the oracle is asked
+both operand types and every block-tile variant forced, and the few-row kernel (lane_matmul_kernel, variant 3) forced at the same
+shapes.  Every variant must give the same bits on every output; the oracle is asked
 for all outputs of the small shapes and for a sample (whole rows, whole columns and random elements) of the big ones.  Each call also
 checks the guard bands around its output (GuardBandError)."""
 import ctypes as C
@@ -14,7 +15,7 @@ import pytest
 
 from conftest import bits
 
-VARIANTS = {np.float16: (0, 1, 2), np.float32: (0, 1)}
+VARIANTS = {np.float16: (0, 1, 2, 3), np.float32: (0, 1, 3)}     # 3: the few-row kernel, forced at every row count
 MAX_REF = 6000              # oracle dots per case beyond which a sample is taken
 
 
@@ -141,6 +142,8 @@ def test_invalid_arguments_fail_without_aborting(pkg):
         pkg.parity_gemm(A, W, variant=2)                       # f32 has only the 32 x 16 tile
     with pytest.raises(RuntimeError):
         pkg.parity_gemm(A, W, variant=-1)
+    with pytest.raises(RuntimeError):
+        pkg.parity_gemm(A, W, variant=4)
     with pytest.raises(RuntimeError):
         pkg.parity_gemm(A[:, :48], W[:, :48])                  # K % 32 != 0
     with pytest.raises(RuntimeError):
