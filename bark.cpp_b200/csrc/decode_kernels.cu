@@ -5,9 +5,10 @@
 //
 // One CTA per SM, 512 threads.
 //  * Weights are a pure stream: each CTA owns a contiguous row range of every matrix (lane-interleaved rows), each warp a
-//    contiguous slice of that range.  As soon as a warp finishes a phase, its lane 0 issues ONE TMA bulk copy
-//    (cp.async.bulk + a per-warp mbarrier) of its rows of the phase after next into a private shared-memory staging area, so
-//    HBM latency hides behind two phases and no block-wide barrier surrounds the weight stream (a CTA-wide TMA ring fed by one
+//    contiguous slice of that range.  Once a warp has finished a phase and the exchange after it is through, its lane 0 issues
+//    ONE TMA bulk copy (cp.async.bulk + a per-warp mbarrier) of its rows of the phase after next into a private shared-memory
+//    staging area, so HBM latency hides behind the phases in between, the copies stay out of the exchanges' way in the L2,
+//    and no block-wide barrier surrounds the weight stream (a CTA-wide TMA ring fed by one
 //    elected thread puts that thread on the critical path of every phase).  The copies carry an L2 evict-first policy: the
 //    weights streamed per token (188 MB for bark-small, ≈ 625 MB for bark-large) would otherwise flush the KV cache, the exchange words, local memory and
 //    the kernel's own code out of the 50 MB L2 on every token, and every other CTA waits for the one that missed.
@@ -555,7 +556,7 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
 // This warp's rows of `phase`: lane-order dot against the shared activation operand; outputs are published with epoch
-// `otag` (or stored, for the logits).  Then the rows of the phase after next start streaming in.  No block-wide synchronisation.
+// `otag` (or stored, for the logits).  No block-wide synchronisation.  The half it read is refilled by the caller (stage_rows).
 template <typename WT, bool TM>
 __device__ __noinline__ void run_phase(int phase, int ep, int layer, uint32_t otag, int sb) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -611,8 +612,6 @@ __device__ __noinline__ void run_phase(int phase, int ep, int layer, uint32_t ot
         }
         __syncwarp();
         tstamp<TM>(sb + 1);
-        stage_rows(phase + 2);
-        tstamp<TM>(sb + 2);
         return;
     } else {
     int j = 0;
@@ -648,8 +647,6 @@ __device__ __noinline__ void run_phase(int phase, int ep, int layer, uint32_t ot
     }
     __syncwarp();                                             // all lanes are done reading this half
     tstamp<TM>(sb + 1);
-    stage_rows(phase + 2);
-    tstamp<TM>(sb + 2);
     }
 }
 
@@ -1017,6 +1014,11 @@ __global__ void __launch_bounds__(kThreads, 1) gpt_decode_step_kernel(DecodeArgs
         }
         if (pv_cta) p3_attention<DSTEPS, TM>(il, n_kv, t_qkv, t_sc, t_att, A.ln_fallbacks);
         tstamp<TM>(16);
+        // The weight rows of each phase after next are issued where they cannot slow an exchange: a bulk copy in flight fills the L2
+        // queues that the exchange's loads wait in (q and x1 take 1.9 us per exchange with the rows issued right behind the row
+        // phases, 1 us issued here; DESIGN.md 4.1).  The fc rows go out here: CTAs without a soft_max tile wait for the attention output anyway, the
+        // soft_max CTAs have just published it; the other three behind the consume of the exchange that follows their half's phase.
+        stage_rows(4 * il + 2);
 
         // ---- P4: c_proj + residual ----
         consume_to_smem<2>(s_bc.gatt, E, t_att, act, kSinkAct, XT_ATT);    // (CTAs without a soft_max tile would otherwise poll for the whole of P3)
@@ -1026,6 +1028,7 @@ __global__ void __launch_bounds__(kThreads, 1) gpt_decode_step_kernel(DecodeArgs
 
         // ---- P5: LN2 -> c_fc -> GELU ----
         consume_to_smem<2>(s_bc.gx, E, t_x1, xs, SINK_PLAIN, XT_X1);
+        stage_rows(4 * il + 3);
         tstamp<TM>(21);
         block_layernorm<kRound, TM, kQ4>(xs, E, inv_E, lv.ln_2_g, lv.ln_2_b, act, red, A.ln_fallbacks, 22);
         if constexpr (kQ4) quantize_act_q8(act, E, act_q, act_d);
@@ -1036,11 +1039,14 @@ __global__ void __launch_bounds__(kThreads, 1) gpt_decode_step_kernel(DecodeArgs
 
         // ---- P6: mlp/c_proj + residual ----
         consume_to_smem<8>(s_bc.gff, 4 * E, t_ff, act, kSinkAct, XT_FF);
+        stage_rows(4 * il + 4);
         if constexpr (kQ4) quantize_act_q8(act, 4 * E, act_q, act_d);
         tstamp<TM>(28);
         run_phase<WT, TM>(4 * il + 3, EP_RESID, il, t_x2, 29);
 
         consume_to_smem<2>(s_bc.gx, E, t_x2, xs, SINK_PLAIN, XT_X2);
+        stage_rows(4 * il + 5);
+        tstamp<TM>(14);
     }
     if (tid == A.timing_tid) s_tim_layer = L;                 // row L: start of the final norm
     // ---- final norm + lm_head window ----

@@ -22,13 +22,33 @@ os.environ.setdefault("BARK_B200_QUIET", "1")
 import bench  # noqa: E402
 import __graft_entry__ as graft  # noqa: E402
 
-NAMES = {0: "layer start", 1: "LN1 mean", 2: "LN1 done", 3: "QKV rows ready (mbarrier)", 4: "QKV rows done", 5: "QKV next rows issued", 6: "K prefetched",
-         7: "q arrived", 8: "scores done", 9: "V prefetched + v_new", 10: "scores arrived", 11: "max", 12: "exp", 13: "sum", 14: "probabilities", 15: "PV partials",
-         16: "P3 done", 17: "att arrived", 18: "c_proj rows ready", 19: "c_proj rows done", 20: "c_proj next issued", 21: "x arrived", 22: "LN2 mean", 23: "LN2 done",
-         24: "fc rows ready", 25: "fc rows done", 26: "fc next issued", 27: "fc block sync", 28: "ff arrived", 29: "proj rows ready", 30: "proj rows done", 31: "proj next issued"}
+NAMES = {0: "layer start", 1: "LN1 mean", 2: "LN1 done", 3: "QKV rows ready (mbarrier)", 4: "QKV rows done", 6: "K prefetched",
+         7: "q arrived", 8: "scores done", 9: "V prefetched + v_new", 10: "scores arrived", 11: "max", 12: "exp", 13: "sum", 14: "x2 arrived", 15: "PV partials",
+         16: "P3 done", 17: "att arrived", 18: "c_proj rows ready", 19: "c_proj rows done", 21: "x arrived", 22: "LN2 mean", 23: "LN2 done",
+         24: "fc rows ready", 25: "fc rows done", 27: "fc block sync", 28: "ff arrived", 29: "proj rows ready", 30: "proj rows done"}
 
 
 SUMMARY = []
+
+
+# exchange -> (stamp after which the stamping warp has published its outputs, stamp at which the consumer holds the whole vector)
+EXCHANGES = (("q", 4, 7), ("scores", 8, 10), ("att", 16, 17), ("x1", 19, 21), ("ff", 25, 28), ("x2", 30, 14))
+
+
+def exchange_table(cta, base, n_kv):
+    """Layer 5, over the CTAs that stamp both ends: when the last producer published, when the consumers held the vector, and the gap
+    between the last publish and the last consumer (the cost of the exchange itself); the producers' spread is what precedes it.
+    The stamping warp must produce in every phase (BARK_B200_DECODE_TIMING_TID=480: warp 15 owns rows of all four row phases)."""
+    print(f"   exchange table, layer 5, n_kv {n_kv} (us from the first CTA's layer start)")
+    print("   exchange  first publish  last publish  consumer median  consumer last   gap (last publish -> last consumer)")
+    for name, prod, cons in EXCHANGES:
+        pv, cv = cta[:, prod], cta[:, cons]
+        pv, cv = (pv[pv != 0] - base) / 1e3, (cv[cv != 0] - base) / 1e3
+        if not len(pv) or not len(cv):
+            continue
+        print(f"   {name:<8s}  {pv.min():13.2f}  {pv.max():12.2f}  {np.median(cv):15.2f}  {cv.max():13.2f}   {cv.max() - pv.max():6.2f}")
+        SUMMARY.append(dict(exchange=name, n_kv=n_kv, first_publish=round(float(pv.min()), 3), last_publish=round(float(pv.max()), 3),
+                            consumer_median=round(float(np.median(cv)), 3), consumer_last=round(float(cv.max()), 3), gap=round(float(cv.max() - pv.max()), 3)))
 
 
 def measure(pkg, path, pasts, tid, poll):
@@ -50,7 +70,7 @@ def measure(pkg, path, pasts, tid, poll):
             lay = t[:L + 1]
             SUMMARY.append(dict(tid=tid, poll_ns=poll, n_kv=int(p), us_per_layer=float((lay[L, 0] - lay[0, 0]) / 1e3 / L)))
             print(f"== [{tag}] n_kv {p}: {(lay[L, 0] - lay[0, 0]) / 1e3:.1f} us for {L} layers on CTA 0 ({(lay[L, 0] - lay[0, 0]) / 1e3 / L:.2f} us per layer)")
-            used = [i for i in range(32) if lay[1, i] != 0]
+            used = sorted((i for i in range(32) if lay[1, i] != 0), key=lambda i: (i == 14, i))     # stamp 14 closes the layer
             for a, c in zip(used[:-1], used[1:]):
                 d = (lay[:L, c] - lay[:L, a]) / 1e3
                 print(f"   -> {c:2d} {NAMES[c]:<28s} median {np.median(d):6.2f} us   min {d.min():6.2f}   max {d.max():6.2f}")
@@ -64,12 +84,13 @@ def measure(pkg, path, pasts, tid, poll):
                     idx = [i for i in sorted(names) if sub[1, g0 + i] != 0]
                     if not idx: continue
                     print(f"   [{gname}] stamps relative to entry (median over layers, us): " + "  ".join(f"{names[i]}={np.median((sub[1:L, g0 + i] - sub[1:L, g0 + idx[0]]) / 1e3):.2f}" for i in idx))
-            cta = t[64:64 + 132]
-            base = cta[:, 0].min()
+            cta = t[64:64 + 132]                             # rows of CTAs beyond the grid stay zero
+            base = cta[:, 0][cta[:, 0] != 0].min()
             for c in used:
                 col = cta[:, c]; col = col[col != 0]
                 v = (col - base) / 1e3
                 print(f"   layer5 stamp {c:2d} over {len(v):3d} CTAs: min {v.min():7.2f}  median {np.median(v):7.2f}  max {v.max():7.2f} us   {NAMES[c]}")
+            exchange_table(cta, base, int(p))
 
 
 def main():
