@@ -117,6 +117,7 @@ EXPORTS = [
     "bark_b200_encodec_batch_codes", "bark_b200_encodec_batch_audio",
     "bark_b200_encodec_compress_resampled", "bark_b200_encodec_reconstruct_resampled", "bark_b200_encodec_compress_batch_resampled",
     "bark_b200_encodec_reconstruct_batch_resampled", "bark_b200_encodec_encode_resampled", "bark_b200_resample",
+    "bark_b200_set_tokenizer", "bark_b200_text_ids", "bark_b200_bert_tokenize",
     "ggml_time_init", "ggml_time_us", "ggml_time_ms", "ggml_init", "ggml_free",
 ]
 
@@ -252,6 +253,12 @@ def lib() -> C.CDLL:
     L.bark_b200_encodec_encode_resampled.argtypes = [vp, f32p, C.c_int, C.c_int, C.c_int, i32p, C.c_int, f32p, C.c_int]
     L.bark_b200_resample.restype = C.c_int
     L.bark_b200_resample.argtypes = [f32p, C.c_int, C.c_int, C.c_int, C.c_int, f32p, C.c_int]
+    L.bark_b200_set_tokenizer.restype = C.c_int
+    L.bark_b200_set_tokenizer.argtypes = [vp, C.c_int]
+    L.bark_b200_text_ids.restype = C.c_int
+    L.bark_b200_text_ids.argtypes = [vp, C.c_int, C.c_char_p, i32p, C.c_int]
+    L.bark_b200_bert_tokenize.restype = C.c_int
+    L.bark_b200_bert_tokenize.argtypes = [C.POINTER(C.c_char_p), C.c_int, C.c_char_p, i32p, C.c_int]
     L.ggml_time_us.restype = C.c_int64
     L.encodec_load_model.restype = vp
     L.encodec_load_model.argtypes = [C.c_char_p, C.c_int, C.c_int]
@@ -313,11 +320,49 @@ def resample(audio, sr: int, new_sr: int) -> np.ndarray:
     return out[:r]
 
 
+TOKENIZERS = {"reference": 0, "bert": 1}      # BARK_B200_TOKENIZER_REFERENCE / _BERT (include/bark_b200.h, DESIGN.md §17)
+
+
+def _tokenizer_kind(name: str) -> int:
+    if name not in TOKENIZERS:
+        raise ValueError(f"tokenizer {name!r}: 'reference' (bark.cpp's, the default) or 'bert' (upstream Bark's)")
+    return TOKENIZERS[name]
+
+
+def _text_bytes(text) -> bytes:
+    """text (str, or UTF-8 bytes) as the C string the library reads, which ends at a NUL: a text holding one is refused here."""
+    b = text if isinstance(text, bytes) else text.encode()
+    if b"\0" in b:
+        raise ValueError("text holds a NUL byte, where the library's C string would end")
+    return b
+
+
+def _ids(run, what: str) -> np.ndarray:
+    """The ids a (out, cap) -> count call returns, asked for twice: once for the count, once for the ids."""
+    n = run(None, 0)
+    if n < 0:
+        raise ValueError(f"{what} refused the text (see stderr)")
+    a = np.zeros(max(n, 1), np.int32)
+    run(_p(a), n)
+    return a[:n]
+
+
+def bert_tokenize(vocab, text) -> np.ndarray:
+    """Upstream Bark's text ids (bark_b200_bert_tokenize, DESIGN.md §17) of text (str, or UTF-8 bytes) over vocab, a list of WordPiece
+    entries whose ids are their indices (a later duplicate wins); no context or device needed.  Raises ValueError for invalid UTF-8."""
+    entries = [_text_bytes(v) for v in vocab]
+    arr = (C.c_char_p * max(len(entries), 1))(*entries)
+    t = _text_bytes(text)
+    return _ids(lambda out, cap: lib().bark_b200_bert_tokenize(arr, len(entries), t, out, cap), "bark_b200_bert_tokenize")
+
+
 class Bark:
     """One bark_context on one GPU.  Mirrors how examples/main/main.cpp uses bark.h."""
 
     def __init__(self, model_path: str, seed: int = 0, n_steps_text_encoder: int | None = None, temp=None, fine_temp=None,
-                 min_eos_p=None, device: int | None = None, progress=None):
+                 min_eos_p=None, device: int | None = None, progress=None, tokenizer: str | None = None):
+        """tokenizer: "reference" (bark.cpp's) or "bert" (upstream Bark's, for text in any of its languages); None keeps what
+        BARK_B200_TOKENIZER chose at load (the reference's when it is unset)."""
         L = lib()
         p = L.bark_context_default_params()
         if n_steps_text_encoder is not None:
@@ -337,6 +382,9 @@ class Bark:
         if not self.ctx:
             raise RuntimeError(f"bark_load_model failed for {model_path} (see stderr); no CPU fallback exists")
         self.ctx = C.c_void_p(self.ctx)
+        self.tokenizer = os.environ.get("BARK_B200_TOKENIZER") or "reference"     # what bark_load_model read (it refuses anything else)
+        if tokenizer is not None:
+            self.set_tokenizer(tokenizer)
 
     def close(self):
         if getattr(self, "ctx", None):
@@ -419,6 +467,19 @@ class Bark:
         a = np.zeros(513, np.int32)
         lib().bark_b200_tokenize(self.ctx, text.encode(), _p(a))
         return a
+
+    def set_tokenizer(self, kind: str):
+        """The text tokenizer of the later generations and batches on this context (bark_b200_set_tokenizer): "reference" or "bert"."""
+        if not lib().bark_b200_set_tokenizer(self.ctx, _tokenizer_kind(kind)):
+            raise ValueError(f"bark_b200_set_tokenizer rejected {kind!r} (see stderr)")
+        self.tokenizer = kind
+
+    def text_ids(self, text, tokenizer: str | None = None) -> np.ndarray:
+        """The raw WordPiece ids of text (str, or UTF-8 bytes) under tokenizer (None: this context's), before truncation, offset and
+        padding (bark_b200_text_ids).  Raises ValueError for a text the tokenizer refuses."""
+        k = _tokenizer_kind(tokenizer or self.tokenizer)
+        t = _text_bytes(text)
+        return _ids(lambda out, cap: lib().bark_b200_text_ids(self.ctx, k, t, out, cap), "bark_b200_text_ids")
 
     def gpt_eval(self, which: int, tokens, n_past: int, merge_ctx: bool):
         t = np.ascontiguousarray(tokens, np.int32)

@@ -56,6 +56,7 @@ struct bark_context {
     bark::GPTModel semantic, coarse, fine;
     bark::CodecModel codec;
     std::map<std::string, int32_t> token_to_id;      // WordPiece vocabulary (bark.cpp:664-690)
+    int tokenizer = BARK_B200_TOKENIZER_REFERENCE;   // bark_b200_set_tokenizer / BARK_B200_TOKENIZER; every batch item follows it
 
     __half * d_gelu_tab = nullptr;                   // 65536-entry table, ggml.c:3795-3810
     unsigned * d_ln_fallbacks = nullptr;             // [0] LayerNorm rows, [1] soft_max rows replayed sequentially
@@ -206,6 +207,10 @@ inline bool sample_flagged(const bark_context * ctx, int r, bool filtered) { ret
 int sample_and_replay(bark_context * ctx, const float * d_logits, int ld, int lo, int n, int rows, float temp, bool want_eos, const bark_b200_sampling * f = nullptr);
 // sample_and_replay with `rows` uniforms drawn from rng; tokens to out_tok, eos probabilities to out_eos when it is set
 bool sample_device(bark_context * ctx, GPTModel & m, std::mt19937 & rng, const float * d_logits, int ld, int n, int rows, float temp, int32_t * out_tok, float * out_eos);
+
+// bert_tokenizer.cu — upstream Bark's text ids (DESIGN.md §17) over vocab, untruncated, to out; false with a message naming fn for
+// invalid UTF-8 or a vocabulary without [UNK]
+bool bert_tokenize(const std::map<std::string, int32_t> & vocab, const std::string & text, std::vector<int32_t> & out, const char * fn);
 
 int64_t now_us();
 // bark_api.cu: the device of the calling thread's next context (bark_b200_set_device, else BARK_B200_DEVICE, else 0), made current;
