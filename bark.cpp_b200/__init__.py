@@ -13,6 +13,7 @@ from __future__ import annotations
 import ctypes as C
 import math
 import os
+import re
 
 import numpy as np
 
@@ -98,6 +99,15 @@ def _history_struct(p):
     return HistoryPromptStruct(_p(s), s.size, _p(c), c.shape[1], _p(f) if f.size else None, f.shape[1]), p
 
 
+class LongFormStruct(C.Structure):
+    """struct bark_b200_long_form (include/bark_b200.h)"""
+    _fields_ = [("voice", C.c_int32), ("max_chunk_ids", C.c_int32), ("gap_samples", C.c_int32)]
+
+
+VOICES = {"chain": 0, "fixed": 1}             # BARK_B200_VOICE_CHAIN / _FIXED
+LONG_FORM_DEFAULTS = dict(max_chunk_ids=48, gap_samples=6000)
+
+
 # every symbol the two public headers declare (tests check the library exports exactly these)
 EXPORTS = [
     "bark_context_default_params", "bark_load_model", "bark_generate_audio", "bark_get_audio_data", "bark_get_audio_data_size",
@@ -118,6 +128,7 @@ EXPORTS = [
     "bark_b200_encodec_compress_resampled", "bark_b200_encodec_reconstruct_resampled", "bark_b200_encodec_compress_batch_resampled",
     "bark_b200_encodec_reconstruct_batch_resampled", "bark_b200_encodec_encode_resampled", "bark_b200_resample",
     "bark_b200_set_tokenizer", "bark_b200_text_ids", "bark_b200_bert_tokenize",
+    "bark_b200_set_long_form", "bark_b200_long_chunks", "bark_b200_long_chunk_text", "bark_b200_long_chunk_tokens", "bark_b200_split_text",
     "ggml_time_init", "ggml_time_us", "ggml_time_ms", "ggml_init", "ggml_free",
 ]
 
@@ -259,6 +270,16 @@ def lib() -> C.CDLL:
     L.bark_b200_text_ids.argtypes = [vp, C.c_int, C.c_char_p, i32p, C.c_int]
     L.bark_b200_bert_tokenize.restype = C.c_int
     L.bark_b200_bert_tokenize.argtypes = [C.POINTER(C.c_char_p), C.c_int, C.c_char_p, i32p, C.c_int]
+    L.bark_b200_set_long_form.restype = C.c_int
+    L.bark_b200_set_long_form.argtypes = [vp, C.POINTER(LongFormStruct)]
+    L.bark_b200_long_chunks.restype = C.c_int
+    L.bark_b200_long_chunks.argtypes = [vp]
+    L.bark_b200_long_chunk_text.restype = C.c_int
+    L.bark_b200_long_chunk_text.argtypes = [vp, C.c_int, C.c_char_p, C.c_int]
+    L.bark_b200_long_chunk_tokens.restype = C.c_int
+    L.bark_b200_long_chunk_tokens.argtypes = [vp, C.c_int, C.c_int, i32p, C.c_int]
+    L.bark_b200_split_text.restype = C.c_int
+    L.bark_b200_split_text.argtypes = [C.POINTER(C.c_char_p), C.c_int, C.c_int, C.c_char_p, C.c_int, i32p, C.c_int]
     L.ggml_time_us.restype = C.c_int64
     L.encodec_load_model.restype = vp
     L.encodec_load_model.argtypes = [C.c_char_p, C.c_int, C.c_int]
@@ -356,6 +377,28 @@ def bert_tokenize(vocab, text) -> np.ndarray:
     return _ids(lambda out, cap: lib().bark_b200_bert_tokenize(arr, len(entries), t, out, cap), "bark_b200_bert_tokenize")
 
 
+def _normalize_whitespace(text: str) -> str:
+    """Upstream Bark's _normalize_whitespace: every run of \\s one space, both ends stripped (long-form rule 1)."""
+    return re.sub(r"\s+", " ", text).strip()
+
+
+def split_text(vocab, text, tokenizer: str = "reference", max_chunk_ids: int = 48) -> list:
+    """The chunks long-form generation makes of text (str, or UTF-8 bytes) under tokenizer over vocab, a list of WordPiece entries
+    whose ids are their indices (bark_b200_split_text, DESIGN.md §18); no context or device needed.  Returns the chunk texts, pieces of
+    the whitespace-normalised text.  Raises ValueError for a text or budget the library refuses."""
+    entries = [_text_bytes(v) for v in vocab]
+    arr = (C.c_char_p * max(len(entries), 1))(*entries)
+    t = _text_bytes(text)
+    run = lambda out, cap: lib().bark_b200_split_text(arr, len(entries), _tokenizer_kind(tokenizer), t, int(max_chunk_ids), out, cap)
+    n = run(None, 0)
+    if n < 0:
+        raise ValueError("bark_b200_split_text refused the text (see stderr)")
+    b = np.zeros((n, 2), np.int32)
+    run(_p(b), n)
+    norm = _normalize_whitespace(t.decode()).encode()
+    return [norm[s:e].decode() for s, e in b]
+
+
 class Bark:
     """One bark_context on one GPU.  Mirrors how examples/main/main.cpp uses bark.h."""
 
@@ -383,6 +426,8 @@ class Bark:
             raise RuntimeError(f"bark_load_model failed for {model_path} (see stderr); no CPU fallback exists")
         self.ctx = C.c_void_p(self.ctx)
         self.tokenizer = os.environ.get("BARK_B200_TOKENIZER") or "reference"     # what bark_load_model read (it refuses anything else)
+        voice = os.environ.get("BARK_B200_LONG_FORM") or "off"                      # likewise
+        self.long_form = None if voice == "off" else dict(voice=voice, **LONG_FORM_DEFAULTS)
         if tokenizer is not None:
             self.set_tokenizer(tokenizer)
 
@@ -421,6 +466,41 @@ class Bark:
         st, _keep = _history_struct(prompt)
         if not lib().bark_b200_set_history_prompt(self.ctx, C.byref(st)):
             raise ValueError("bark_b200_set_history_prompt rejected the prompt (see stderr)")
+
+    def set_long_form(self, voice: str | None = "chain", max_chunk_ids: int = 48, gap_samples: int = 6000):
+        """Long-form generation for the later generate calls on this context (bark_b200_set_long_form, DESIGN.md §18): the text split
+        into sentences, each generated on a prompt that keeps one voice ("chain": the previous chunk's ids; "fixed": the context's
+        history prompt, or none), joined with gap_samples zeros.  voice None turns it off.  Raises ValueError for settings the library
+        rejects; the previous ones then stay."""
+        if voice is None:
+            lib().bark_b200_set_long_form(self.ctx, None)
+            self.long_form = None
+            return
+        if voice not in VOICES:
+            raise ValueError(f"voice {voice!r}: 'chain', 'fixed' or None")
+        st = LongFormStruct(VOICES[voice], int(max_chunk_ids), int(gap_samples))
+        if not lib().bark_b200_set_long_form(self.ctx, C.byref(st)):
+            raise ValueError(f"bark_b200_set_long_form rejected max_chunk_ids={max_chunk_ids!r}, gap_samples={gap_samples!r} (see stderr)")
+        self.long_form = dict(voice=voice, max_chunk_ids=int(max_chunk_ids), gap_samples=int(gap_samples))
+
+    def long_chunks(self) -> list:
+        """The chunks of the last long-form generation ([] after a generation without it): per chunk a dict of its text, its ids as
+        tokens() shapes them (prompt: the 513 prompt ids, semantic, coarse [T][2], fine [T][8]), and start / n_samples, its span in the
+        joined waveform (with the gap of the current long-form settings)."""
+        L = lib()
+        gap = self.long_form["gap_samples"] if self.long_form else 0
+        out, start = [], 0
+        for k in range(L.bark_b200_long_chunks(self.ctx)):
+            t = C.create_string_buffer(max(L.bark_b200_long_chunk_text(self.ctx, k, None, 0), 1))
+            n_text = L.bark_b200_long_chunk_text(self.ctx, k, t, len(t))
+            ids = {}
+            for stage, name in ((3, "prompt"), (0, "semantic"), (1, "coarse"), (2, "fine")):
+                a = _ids(lambda o, cap: L.bark_b200_long_chunk_tokens(self.ctx, k, stage, o, cap), "bark_b200_long_chunk_tokens")
+                ids[name] = a.reshape(-1, 2) if stage == 1 else a.reshape(-1, 8) if stage == 2 else a
+            n = 320 * ids["fine"].shape[0]
+            out.append(dict(text=t.raw[:n_text].decode(), **ids, start=start, n_samples=n))
+            start += n + gap
+        return out
 
     def set_sampling(self, stage: str, top_k=None, top_p=None):
         """Top-k / top-p filter of the "semantic" or "coarse" stage for the later generations and batches on this context

@@ -25,8 +25,13 @@ Class char_class(uint32_t cp) {
     return (Class) r[-1].cls;
 }
 
+}  // namespace
+
+// shared with the long-form splitter (long_form.cu)
+namespace bark {
+
 bool py_space(uint32_t cp) {
-    for (const Range & r : kPySpace) if (cp >= r.lo && cp <= r.hi) return true;
+    for (const bert_chars::Range & r : bert_chars::kPySpace) if (cp >= r.lo && cp <= r.hi) return true;
     return false;
 }
 
@@ -60,6 +65,12 @@ void append_utf8(std::string & s, uint32_t cp) {
     else if (cp < 0x10000) { s.push_back((char)(0xE0 | cp >> 12)); s.push_back((char)(0x80 | (cp >> 6 & 0x3F))); s.push_back((char)(0x80 | (cp & 0x3F))); }
     else { s.push_back((char)(0xF0 | cp >> 18)); s.push_back((char)(0x80 | (cp >> 12 & 0x3F))); s.push_back((char)(0x80 | (cp >> 6 & 0x3F))); s.push_back((char)(0x80 | (cp & 0x3F))); }
 }
+
+}  // namespace bark
+
+namespace {
+
+using bark::append_utf8;
 
 // WordPiece of one word (tokenizers' WordPiece::tokenize): at each position the longest vocabulary entry, "##" after the first piece,
 // shortened one code point at a time

@@ -5,6 +5,7 @@
 #include "gpt_kernels.h"
 
 #include <fstream>
+#include <functional>
 #include <map>
 #include <random>
 #include <string>
@@ -47,6 +48,20 @@ struct BatchSlots {
     float * d_logits = nullptr;                      // [8][max n_out of the causal models]
     int32_t * d_step = nullptr, * h_step = nullptr;  // [0, 8): input ids, [8, 16): positions (n_past) of the step's rows
     std::vector<Generation> results;                 // the last batch's items (bark_b200_batch_audio / bark_b200_batch_tokens)
+};
+
+// One chunk of the last long-form generation (long_form.cu): its text and its ids, as the Generation fields of the same names hold them
+struct LongFormChunk {
+    std::string text;
+    std::vector<int32_t> tokens, semantic_tokens, coarse_tokens, fine_tokens;
+};
+
+// Long-form generation (bark_b200_set_long_form, DESIGN.md §18): the settings of the context's later bark_generate_audio calls, and the
+// chunks of the last successful long-form call (bark_b200_long_chunk_*)
+struct LongForm {
+    bool on = false;
+    bark_b200_long_form settings{BARK_B200_VOICE_CHAIN, 48, 6000};
+    std::vector<LongFormChunk> chunks;
 };
 
 struct bark_context {
@@ -95,6 +110,7 @@ struct bark_context {
 
     Generation gen;                                  // the bark.h calls' generation state
     BatchSlots batch;
+    LongForm long_form;
 
     bark_context_params params;
     bark_statistics stats{};
@@ -211,6 +227,31 @@ bool sample_device(bark_context * ctx, GPTModel & m, std::mt19937 & rng, const f
 // bert_tokenizer.cu — upstream Bark's text ids (DESIGN.md §17) over vocab, untruncated, to out; false with a message naming fn for
 // invalid UTF-8 or a vocabulary without [UNK]
 bool bert_tokenize(const std::map<std::string, int32_t> & vocab, const std::string & text, std::vector<int32_t> & out, const char * fn);
+// Python's \s (str.isspace)
+bool py_space(uint32_t cp);
+// Strict UTF-8 (RFC 3629) to code points; false with the offending byte's offset in *bad
+bool decode_utf8(const std::string & s, std::vector<uint32_t> & out, size_t * bad);
+void append_utf8(std::string & s, uint32_t cp);
+
+// bark_api.cu: the ids of text under tokenizer kind (BARK_B200_TOKENIZER_*) over vocab, counted as bark_b200_text_ids counts them
+// (uncapped); -1 with a message naming fn for a text or vocabulary the tokenizer refuses
+int count_text_ids(const std::map<std::string, int32_t> & vocab, int kind, const std::string & text, const char * fn);
+// bark_api.cu: one bark_generate_audio on the context's generation state (text tokenized, three stages, codec, statistics); false with a
+// message, and nothing changed when the tokenizer refuses the text
+bool generate_one(bark_context * ctx, const std::string & text);
+// bark_api.cu: upstream Bark's checks of a history prompt; true and h set, or false with a message (h untouched)
+bool make_history_prompt(const bark_context_params & P, const bark_b200_history_prompt & p, HistoryPrompt & h);
+
+// long_form.cu (DESIGN.md §18).  The chunks of text under long-form rules 1-4: text validated and its whitespace normalised into norm,
+// split into sentences and over-long sentences into pieces of at most max_ids ids by count (count_text_ids on the chunk text); chunks
+// without ids dropped.  [begin, end) byte offsets into norm go to bounds.  Returns their number, or -1 with a message naming fn (invalid
+// UTF-8, max_ids outside [1, 255], a count that fails, no chunk left or more than kLongFormMaxChunks).
+constexpr int kLongFormMaxChunks = 1024;
+int split_text(const std::string & text, int max_ids, const std::function<int(const std::string &)> & count, std::string & norm,
+               std::vector<std::pair<size_t, size_t>> & bounds, const char * fn);
+// bark_generate_audio with long form on: every chunk one generate_one on the context's generation, prompted as the voice setting says,
+// the waveforms joined with gap_samples zeros; the context's prompt restored at the end.  A refused text changes nothing.
+bool generate_long(bark_context * ctx, const std::string & text);
 
 int64_t now_us();
 // bark_api.cu: the device of the calling thread's next context (bark_b200_set_device, else BARK_B200_DEVICE, else 0), made current;

@@ -176,6 +176,55 @@ BARK_API int bark_b200_text_ids(struct bark_context * ctx, int kind, const char 
  * bark_b200_text_ids; -1 with a message for invalid UTF-8, NULL arguments or a vocabulary without [UNK]. */
 BARK_API int bark_b200_bert_tokenize(const char * const * vocab, int n_vocab, const char * text, int32_t * out, int cap);
 
+/* LONG-FORM GENERATION (DESIGN.md §18): upstream Bark's long-form recipe inside bark_generate_audio.  One call generates at most
+ * about 14 s (255 text ids, n_steps_text_encoder semantic ids); with long form on, the text is split into sentences, each generated as
+ * its own bark_generate_audio on a speaker prompt that keeps one voice, and the waveforms are joined with silence between them.
+ *   1. normalise  the text must be valid UTF-8 (under either tokenizer); every run of Python's \s becomes one space, both ends stripped
+ *   2. sentences  a sentence ends after a run of . ! ? … 。 ！ ？ ｡ । ॥ and the closing marks " ' ) ] } » ” ’ 」 』 ） directly after
+ *                 it, when the run holds one of 。！？｡।॥ or a space or the end of the text follows; the space after it is dropped.  So
+ *                 "3.5" and "e.g.x" do not split and "Mr. Smith" does: no abbreviation list is kept.  Empty sentences are dropped
+ *   3. pieces     a sentence with more than max_chunk_ids ids under the context's tokenizer (as bark_b200_text_ids counts them) is
+ *                 split greedily: words (split at spaces) while the piece stays within max_chunk_ids, a first word that is over
+ *                 alone split the same way code point by code point (at least one); repeated on the rest.  Short sentences are not
+ *                 merged.  A chunk is a sentence or a piece of one
+ *   4. drop, cap  a chunk without ids is dropped; a text that leaves no chunk or more than 1024 is refused
+ *   5. voice      BARK_B200_VOICE_CHAIN: chunk 0 uses the context's history prompt (or none), chunk k > 0 chunk k-1's own ids
+ *                 (semantic, coarse, fine) when they are a valid prompt, else chunk k-1's prompt.  BARK_B200_VOICE_FIXED: every chunk
+ *                 uses the context's prompt (or none)
+ *   6. calls      the whole call equals, bit for bit, setting chunk k's prompt and calling bark_generate_audio on chunk k's text, in
+ *                 order on this context: same RNG stream, progress callbacks and stage functions.  Afterwards the history prompt is what
+ *                 it was before the call
+ *   7. results    bark_get_audio_data: the chunks' waveforms in order with gap_samples zeros between consecutive ones; chunk k starts at
+ *                 the sum over j < k of (320 fine frames of j + gap_samples).  bark_b200_get_tokens: the last chunk's ids.  The
+ *                 statistics count the whole call: each stage's samples and time summed over the chunks, t_eval_us its wall time
+ * A refused text (invalid UTF-8, no chunk, more than 1024 chunks) fails bark_generate_audio before anything runs: ids, waveform,
+ * statistics, prompt, RNG and the chunk results stay as they were.  A context whose fine stage is sharded refuses long-form generation. */
+#define BARK_B200_VOICE_CHAIN 0   /* each chunk prompted by the previous chunk's ids (default) */
+#define BARK_B200_VOICE_FIXED 1   /* every chunk prompted by the context's history prompt, or none */
+struct bark_b200_long_form {
+    int32_t voice;           /* BARK_B200_VOICE_CHAIN or BARK_B200_VOICE_FIXED */
+    int32_t max_chunk_ids;   /* 1 to 255 text ids per chunk (default 48) */
+    int32_t gap_samples;     /* 0 to 240000 zeros between chunks (default 6000: 0.25 s at 24 kHz) */
+};
+/* Validates and copies; NULL turns long form off.  Returns 1, or 0 with a message (the previous settings stay).  Applies to later
+ * bark_generate_audio calls only: bark_b200_tokenize, bark_b200_forward_* and bark_b200_generate_batch[_prompted] ignore it.
+ * BARK_B200_LONG_FORM=chain or fixed in the environment at bark_load_model turns it on with that voice and the defaults; empty or off
+ * leaves it off; another value fails the load. */
+BARK_API int bark_b200_set_long_form(struct bark_context * ctx, const struct bark_b200_long_form * lf);
+/* Chunks of the last successful long-form bark_generate_audio; 0 after a later generation without long form (-1 for a NULL context). */
+BARK_API int bark_b200_long_chunks(struct bark_context * ctx);
+/* Chunk k's text (UTF-8, a piece of the normalised text, no NUL appended): copies min(bytes, cap) to out (may be NULL) and returns its
+ * bytes, or -1 for no such chunk. */
+BARK_API int bark_b200_long_chunk_text(struct bark_context * ctx, int k, char * out, int cap);
+/* Chunk k's ids of stage 0-3, as bark_b200_get_tokens returns them for a single call; -1 for no such chunk or stage. */
+BARK_API int bark_b200_long_chunk_tokens(struct bark_context * ctx, int k, int stage, int32_t * out, int cap);
+/* Test hook, no context, no device: rules 1-4 on text over vocab[0..n_vocab) (id = index, later duplicates win) under tokenizer kind.
+ * Writes chunk i's [begin, end) byte offsets into the normalised text to bounds[2 i], bounds[2 i + 1] for i < cap (bounds may be NULL)
+ * and returns the chunk count, or -1 with a message (invalid UTF-8, NULL arguments, unknown kind, max_chunk_ids outside [1, 255], no
+ * chunk left, more than 1024 chunks). */
+BARK_API int bark_b200_split_text(const char * const * vocab, int n_vocab, int kind, const char * text, int max_chunk_ids, int32_t * bounds,
+                                  int cap);
+
 /* BATCHED ENCODEC on an encodec_context (include/encodec.h): n clips of independent lengths in one call, for tokenising a dataset.
  * Item i's codes and waveform are bit-identical to encodec_compress_audio / _decompress_audio / _reconstruct_audio of that clip alone on
  * the same context: they do not depend on n, on i's place in the batch or on the other items.  The context's current bandwidth and
