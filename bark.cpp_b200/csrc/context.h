@@ -4,6 +4,7 @@
 #include "../../include/bark_b200.h"
 #include "gpt_kernels.h"
 
+#include <algorithm>
 #include <fstream>
 #include <functional>
 #include <map>
@@ -32,7 +33,7 @@ struct HistoryPrompt {
 // (bark.h's single-prompt calls); every item of a batch (bark_b200_generate_batch) holds its own, so a batch leaves the context's untouched.
 struct Generation {
     std::mt19937 rng;                                // seeded once at load (bark.cpp:1179), or per batch item
-    HistoryPrompt prompt;                            // conditions the three stages (bark_api.cu); empty: every generation starts from nothing
+    HistoryPrompt prompt;                            // conditions the three stages (generation.cu); empty: every generation starts from nothing
     std::vector<int32_t> tokens;                     // 513 prompt ids
     std::vector<int32_t> semantic_tokens;
     std::vector<int32_t> coarse_tokens;              // [T][2] flattened
@@ -40,7 +41,7 @@ struct Generation {
     std::vector<float> audio;
 };
 
-// Batched generation (bark_api.cu): one f32 KV cache [L][block_size][E] per item and causal model, allocated on the first batch and
+// Batched generation (generation.cu): one f32 KV cache [L][block_size][E] per item and causal model, allocated on the first batch and
 // grown when a later one has more items; the [8][n_out] logits of the batched step; the step's ids and positions (device + pinned).
 struct BatchSlots {
     int cap = 0;
@@ -77,7 +78,7 @@ struct bark_context {
     unsigned * d_ln_fallbacks = nullptr;             // [0] LayerNorm rows, [1] soft_max rows replayed sequentially
     unsigned tag_base = 0;                           // epoch counter of the decode kernel's tagged exchanges (advances 6*L per token)
     int n_sm = 0, n_sm_total = 0; bool use_decode_kernel = true;   // n_sm: CTAs of the persistent decode kernel (knob); n_sm_total: SMs of the device
-    bool kv_reuse = true; unsigned long long n_kv_reused = 0;   // coarse windows start from the cached prefix (bark_api.cu run_coarse)
+    bool kv_reuse = true; unsigned long long n_kv_reused = 0;   // coarse windows start from the cached prefix (generation.cu run_coarse)
     // decode-kernel knobs (BARK_B200_DECODE_TIMING_TID / BARK_B200_POLL_NS / BARK_B200_HEADSTART); defaults:
     // 40 ns back-off between polls, 500 ns head start for the two residual exchanges
     unsigned headstart[6] = {0, 2000, 500, 400, 500, 0};   // BARK_B200_HEADSTART=q:att:x1:ff:x2:scores (ns): sleep before the first poll of each exchange
@@ -224,8 +225,16 @@ int sample_and_replay(bark_context * ctx, const float * d_logits, int ld, int lo
 // sample_and_replay with `rows` uniforms drawn from rng; tokens to out_tok, eos probabilities to out_eos when it is set
 bool sample_device(bark_context * ctx, GPTModel & m, std::mt19937 & rng, const float * d_logits, int ld, int n, int rows, float temp, int32_t * out_tok, float * out_eos);
 
-// bert_tokenizer.cu — upstream Bark's text ids (DESIGN.md §17) over vocab, untruncated, to out; false with a message naming fn for
-// invalid UTF-8 or a vocabulary without [UNK]
+// tokenizer.cu — the reference's tokenizer and upstream Bark's (DESIGN.md §17), by kind (BARK_B200_TOKENIZER_*).  tokenizer_known: false
+// (message naming fn) for an unknown kind; tokenizer_from_env: BARK_B200_TOKENIZER's kind, -1 (message) for a value it does not name.
+bool tokenizer_known(int kind, const char * fn);
+int tokenizer_from_env(const char * fn);
+// The ids of text under kind, cut to a prompt of cap ids as each tokenizer cuts it (the reference's stops at cap - 1 pieces, upstream's
+// keeps the first cap); false with a message naming fn for an unknown kind or a refused text or vocabulary.  warn: the reference's
+// message for a character it skips.  count_text_ids: their uncapped number, without that message; -1 where text_ids fails.
+bool text_ids(const std::map<std::string, int32_t> & vocab, int kind, const std::string & text, int cap, std::vector<int32_t> & ids, const char * fn, bool warn);
+int count_text_ids(const std::map<std::string, int32_t> & vocab, int kind, const std::string & text, const char * fn);
+// upstream Bark's ids, untruncated; false with a message naming fn for invalid UTF-8 or a vocabulary without [UNK]
 bool bert_tokenize(const std::map<std::string, int32_t> & vocab, const std::string & text, std::vector<int32_t> & out, const char * fn);
 // Python's \s (str.isspace)
 bool py_space(uint32_t cp);
@@ -233,14 +242,16 @@ bool py_space(uint32_t cp);
 bool decode_utf8(const std::string & s, std::vector<uint32_t> & out, size_t * bad);
 void append_utf8(std::string & s, uint32_t cp);
 
-// bark_api.cu: the ids of text under tokenizer kind (BARK_B200_TOKENIZER_*) over vocab, counted as bark_b200_text_ids counts them
-// (uncapped); -1 with a message naming fn for a text or vocabulary the tokenizer refuses
-int count_text_ids(const std::map<std::string, int32_t> & vocab, int kind, const std::string & text, const char * fn);
-// bark_api.cu: one bark_generate_audio on the context's generation state (text tokenized, three stages, codec, statistics); false with a
-// message, and nothing changed when the tokenizer refuses the text
+// generation.cu — the prompt, the three stages and the codec of one generation, and batches of up to kMaxBatch of them
+constexpr int kMaxBatch = 8;
+bool tokenize_input(bark_context * ctx, Generation & g, const std::string & text, const char * fn);
+bool run_semantic(bark_context * ctx, Generation & g);
+bool run_coarse(bark_context * ctx, Generation & g);
+bool run_fine(bark_context * ctx, Generation & g, bool progress = true);
 bool generate_one(bark_context * ctx, const std::string & text);
-// bark_api.cu: upstream Bark's checks of a history prompt; true and h set, or false with a message (h untouched)
 bool make_history_prompt(const bark_context_params & P, const bark_b200_history_prompt & p, HistoryPrompt & h);
+bool generate_batch(bark_context * ctx, const char * const * texts, const uint32_t * seeds, const bark_b200_history_prompt * const * prompts, int n);
+bool ensure_batch_slots(bark_context * ctx, int n);
 
 // long_form.cu (DESIGN.md §18).  The chunks of text under long-form rules 1-4: text validated and its whitespace normalised into norm,
 // split into sentences and over-long sentences into pieces of at most max_ids ids by count (count_text_ids on the chunk text); chunks
@@ -257,5 +268,19 @@ int64_t now_us();
 // bark_api.cu: the device of the calling thread's next context (bark_b200_set_device, else BARK_B200_DEVICE, else 0), made current;
 // -1 with a message from `caller` when it is missing or not an sm_90 device
 int select_device(const char * caller, cudaDeviceProp * prop);
+
+// The call path of every bark_context entry point: a null context is "fn: invalid bark context" and fail; otherwise f() runs with the
+// context's device current (a host thread may drive contexts on several devices), and a CUDA failure or exception is fail.
+template <typename R, typename F> R with_context(bark_context * ctx, const char * fn, R fail, F && f) {
+    if (!ctx) { fprintf(stderr, "%s: invalid bark context\n", fn); return fail; }
+    return guarded(fail, [&]() -> R { BARK_CUDA_CHECK(cudaSetDevice(ctx->device)); return f(); });
+}
+
+// The copy-out of the entry points that fill a caller's array: the first min(size, cap) elements of v to out when it is set (none for
+// cap < 0); returns v's size
+template <class V> int copy_out(const V & v, typename V::value_type * out, int cap) {
+    if (out) std::copy_n(v.data(), std::min(v.size(), (size_t) std::max(cap, 0)), out);
+    return (int) v.size();
+}
 
 }  // namespace bark

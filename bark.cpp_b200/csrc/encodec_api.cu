@@ -70,13 +70,6 @@ bool resampled_batch_formats(const char * fn, const float * const * audio, const
     return true;
 }
 
-template <typename V> int batch_item(const std::vector<std::vector<V>> & items, int i, V * out, int cap) {
-    if (i < 0 || i >= (int) items.size()) return -1;
-    const std::vector<V> & v = items[(size_t) i];
-    if (out) memcpy(out, v.data(), sizeof(V) * std::min(v.size(), (size_t) std::max(cap, 0)));
-    return (int) v.size();
-}
-
 // The clips of an encoder call: n arrays of lens[i] mono 24 kHz samples, or for a resampled call lens[i] frames of channels[i] channels
 // at rates[i] Hz (one of each for a single call)
 struct Clips {
@@ -200,12 +193,12 @@ extern "C" bool bark_b200_encodec_reconstruct_batch_resampled(struct encodec_con
 
 extern "C" int bark_b200_encodec_batch_codes(struct encodec_context * e, int i, int32_t * out, int cap) {
     if (!e) { fprintf(stderr, "%s: null context\n", __func__); return -1; }
-    return batch_item(e->batch_codes, i, out, cap);
+    return i < 0 || i >= (int) e->batch_codes.size() ? -1 : copy_out(e->batch_codes[(size_t) i], out, cap);
 }
 
 extern "C" int bark_b200_encodec_batch_audio(struct encodec_context * e, int i, float * out, int cap) {
     if (!e) { fprintf(stderr, "%s: null context\n", __func__); return -1; }
-    return batch_item(e->batch_audio, i, out, cap);
+    return i < 0 || i >= (int) e->batch_audio.size() ? -1 : copy_out(e->batch_audio[(size_t) i], out, cap);
 }
 
 extern "C" float * encodec_get_audio(struct encodec_context * e) {

@@ -2,7 +2,7 @@
 // over-long sentences into pieces the prompt can hold, and each chunk is one ordinary generation on the context, prompted so that the
 // voice stays the same; the waveforms are joined with silence.  Host code only: every chunk runs the existing device stages.
 //
-//   1. normalise  strict UTF-8 (bert_tokenizer.cu decode_utf8); every run of Python's \s one space, both ends stripped (upstream's
+//   1. normalise  strict UTF-8 (tokenizer.cu decode_utf8); every run of Python's \s one space, both ends stripped (upstream's
 //                 _normalize_whitespace)
 //   2. sentences  a run of end marks, with the closing marks directly after it, ends a sentence when the run holds a mark that needs no
 //                 space (。！？｡।॥) or a space or the end of the text follows; that space is dropped.  No abbreviation list.

@@ -133,46 +133,47 @@ bool sample_shard(bark_context * ctx, std::mt19937 & rng, int n, float temp, int
 using namespace bark;
 
 // rank / world of this context in a row-sharded fine stage; writes this rank's 64-byte CUDA IPC handle to handle_out
-static int bark_b200_shard_init_impl(struct bark_context * ctx, int rank, int world, void * handle_out) {
-    if (!ctx || !handle_out || world < 1 || world > 8 || rank < 0 || rank >= world || 1024 % world) return 0;
-    BARK_CUDA_CHECK(cudaSetDevice(ctx->device));
-    ShardState & S = ctx->shard;
-    if (S.local) return 0;
-    S.rank = rank; S.world = world;
-    const size_t bytes = shard_bytes(ctx->fine);
-    if (cudaMalloc((void **) &S.local, bytes) != cudaSuccess) { (void) cudaGetLastError(); return 0; }
-    BARK_CUDA_CHECK(cudaMemset(S.local, 0, bytes));
-    S.d_err = (unsigned *) ctx_alloc(ctx, 16); BARK_CUDA_CHECK(cudaMemset(S.d_err, 0, 16));
-    cudaIpcMemHandle_t h;
-    if (cudaIpcGetMemHandle(&h, S.local) != cudaSuccess) { fprintf(stderr, "%s: cudaIpcGetMemHandle failed: %s\n", __func__, cudaGetErrorString(cudaGetLastError())); return 0; }
-    static_assert(sizeof(h) == 64, "CUDA IPC handles are 64 bytes");
-    memcpy(handle_out, &h, 64);
-    S.peer[rank] = S.local;
-    return 1;
+extern "C" int bark_b200_shard_init(struct bark_context * ctx, int rank, int world, void * handle_out) {
+    return with_context(ctx, __func__, 0, [&] {
+        if (!handle_out || world < 1 || world > 8 || rank < 0 || rank >= world || 1024 % world) return 0;
+        ShardState & S = ctx->shard;
+        if (S.local) return 0;
+        S.rank = rank; S.world = world;
+        const size_t bytes = shard_bytes(ctx->fine);
+        if (cudaMalloc((void **) &S.local, bytes) != cudaSuccess) { (void) cudaGetLastError(); return 0; }
+        BARK_CUDA_CHECK(cudaMemset(S.local, 0, bytes));
+        S.d_err = (unsigned *) ctx_alloc(ctx, 16); BARK_CUDA_CHECK(cudaMemset(S.d_err, 0, 16));
+        cudaIpcMemHandle_t h;
+        if (cudaIpcGetMemHandle(&h, S.local) != cudaSuccess) { fprintf(stderr, "bark_b200_shard_init: cudaIpcGetMemHandle failed: %s\n", cudaGetErrorString(cudaGetLastError())); return 0; }
+        static_assert(sizeof(h) == 64, "CUDA IPC handles are 64 bytes");
+        memcpy(handle_out, &h, 64);
+        S.peer[rank] = S.local;
+        return 1;
+    });
 }
-extern "C" int bark_b200_shard_init(struct bark_context * ctx, int rank, int world, void * handle_out) { return guarded((int) 0, [&] { return bark_b200_shard_init_impl(ctx, rank, world, handle_out); }); }
 
 // all_handles: world x 64 bytes, rank order (what every rank's bark_b200_shard_init returned, all-gathered by the caller)
-static int bark_b200_shard_connect_impl(struct bark_context * ctx, const void * all_handles) {
-    if (!ctx || !all_handles || !ctx->shard.local) return 0;
-    BARK_CUDA_CHECK(cudaSetDevice(ctx->device));
-    ShardState & S = ctx->shard;
-    for (int p = 0; p < S.world; p++) {
-        if (p == S.rank) continue;
-        cudaIpcMemHandle_t h; memcpy(&h, (const unsigned char *) all_handles + (size_t) p * 64, 64);
-        void * ptr = nullptr;
-        const cudaError_t e = cudaIpcOpenMemHandle(&ptr, h, cudaIpcMemLazyEnablePeerAccess);
-        if (e != cudaSuccess) { fprintf(stderr, "%s: cudaIpcOpenMemHandle for rank %d failed: %s\n", __func__, p, cudaGetErrorString(e)); (void) cudaGetLastError(); return 0; }
-        S.peer[p] = (unsigned char *) ptr;
-    }
-    S.on = true;
-    return 1;
+extern "C" int bark_b200_shard_connect(struct bark_context * ctx, const void * all_handles) {
+    return with_context(ctx, __func__, 0, [&] {
+        if (!all_handles || !ctx->shard.local) return 0;
+        ShardState & S = ctx->shard;
+        for (int p = 0; p < S.world; p++) {
+            if (p == S.rank) continue;
+            cudaIpcMemHandle_t h; memcpy(&h, (const unsigned char *) all_handles + (size_t) p * 64, 64);
+            void * ptr = nullptr;
+            const cudaError_t e = cudaIpcOpenMemHandle(&ptr, h, cudaIpcMemLazyEnablePeerAccess);
+            if (e != cudaSuccess) { fprintf(stderr, "bark_b200_shard_connect: cudaIpcOpenMemHandle for rank %d failed: %s\n", p, cudaGetErrorString(e)); (void) cudaGetLastError(); return 0; }
+            S.peer[p] = (unsigned char *) ptr;
+        }
+        S.on = true;
+        return 1;
+    });
 }
-extern "C" int bark_b200_shard_connect(struct bark_context * ctx, const void * all_handles) { return guarded((int) 0, [&] { return bark_b200_shard_connect_impl(ctx, all_handles); }); }
 
 extern "C" unsigned long long bark_b200_shard_nvlink_bytes(struct bark_context * ctx, int reset) {
-    if (!ctx) return 0;
-    const unsigned long long v = ctx->shard.nvlink_bytes;
-    if (reset) ctx->shard.nvlink_bytes = 0;
-    return v;
+    return with_context(ctx, __func__, 0ull, [&] {
+        const unsigned long long v = ctx->shard.nvlink_bytes;
+        if (reset) ctx->shard.nvlink_bytes = 0;
+        return v;
+    });
 }

@@ -197,7 +197,7 @@ def test_resampled_refusals(pkg, codec, capfd):
     del keep
 
 
-def test_bark_hook_refusals(pkg, bark, capfd):
+def test_bark_context_hook_refusals(pkg, bark, capfd):
     L, b = pkg.lib(), bark.ctx
     x, short, inf = noise(4000, 5), np.zeros(1920, np.float32), np.where(np.arange(4000) == 7, np.inf, 0.1).astype(np.float32)
     stereo_nan = with_nan(5000, 77)
@@ -209,14 +209,14 @@ def test_bark_hook_refusals(pkg, bark, capfd):
     o = (out.ctypes.data, out.size, lat.ctypes.data, lat.size)
     fn = "bark_b200_encodec_encode"
     cases = [
-        (fn, (None, x.ctypes.data, x.size) + o, -1, f"{fn}: null context"),
+        (fn, (None, x.ctypes.data, x.size) + o, -1, f"{fn}: invalid bark context"),
         (fn, (b, None, x.size) + o, -1, f"{fn}: null audio"),
         (fn, (b, short.ctypes.data, short.size) + o, -1, f"codec_encode: {SHORT}"),
         (fn, (b, inf.ctypes.data, inf.size) + o, -1, "codec_encode: sample 7 is not finite (inf)"),
     ]
     fn = "bark_b200_encodec_encode_resampled"
     cases += [
-        (fn, (None, x.ctypes.data, 2000, 2, 44100) + o, -1, f"{fn}: null context"),
+        (fn, (None, x.ctypes.data, 2000, 2, 44100) + o, -1, f"{fn}: invalid bark context"),
         (fn, (b, None, 2000, 2, 44100) + o, -1, f"{fn}: null audio"),
         (fn, (b, x.ctypes.data, 3840, 1, 48000) + o, -1, f"codec_encode: {RESAMPLED_SHORT}"),
         (fn, (b, x.ctypes.data, 400, 9, 24000) + o, -1, "codec_encode: 9 channels (1 to 8)"),
@@ -226,7 +226,7 @@ def test_bark_hook_refusals(pkg, bark, capfd):
     fn = "bark_b200_encodec_decode"
     wav = np.zeros(320 * 9, np.float32)
     cases += [
-        (fn, (None, codes.ctypes.data, 9, wav.ctypes.data, wav.size), -1, None),
+        (fn, (None, codes.ctypes.data, 9, wav.ctypes.data, wav.size), -1, f"{fn}: invalid bark context"),
         (fn, (b, None, 9, wav.ctypes.data, wav.size), -1, None),
         (fn, (b, few.ctypes.data, 6, wav.ctypes.data, wav.size), -1, f"codec_decode: {FEW_FRAMES}"),
         (fn, (b, outside.ctypes.data, 9, wav.ctypes.data, wav.size), -1, f"codec_decode: {OUTSIDE}"),

@@ -46,7 +46,7 @@ def test_teacher_forced_logits_bit_exact(pkg, orc, weights_file, config, ftype):
             assert np.array_equal(bits(lg), bits(lo)), f"coarse step {step} (n_past {po}): {int((lg != lo).sum())} logits differ, max {np.abs(lg - lo).max():.3e}"
             toks = np.array([10000 + int(np.argmax(lo[10000:12048]))], np.int32)
         # a multi-row evaluation on top of a filled cache (a coarse window start with prefix reuse): rows below n_kv & ~31 of
-        # an evaluation do not depend on its n_kv (bark_api.cu run_coarse), so evaluating the tail on top of them must equal
+        # an evaluation do not depend on its n_kv (generation.cu run_coarse), so evaluating the tail on top of them must equal
         # the oracle's from-scratch evaluation of the whole sequence
         full = np.concatenate([rng.integers(0, 10000, 256), [12050], rng.integers(10000, 12048, 75)]).astype(np.int32)
         for cut in (256, 288, 320):

@@ -1,4 +1,4 @@
-"""Canonical rows (bark_api.cu run_coarse, "Prefix reuse"): row p of a causal evaluation does not depend on the call's n_kv as
+"""Canonical rows (generation.cu run_coarse, "Prefix reuse"): row p of a causal evaluation does not depend on the call's n_kv as
 long as p < n_kv & ~31, so a coarse window may start from the cached rows of the previous window.  Checked here on the CPU
 on the C restatement, whose from-scratch logits must equal the unmodified reference's (stored in
 tests/golden/ref_pairs/prefix_rows.npz by tests/golden/make_golden_ref_pairs.py): evaluating the tail of a sequence on
