@@ -123,6 +123,7 @@ EXPORTS = [
     "bark_b200_parity_rows", "bark_b200_sample_given_u", "bark_b200_generate_batch", "bark_b200_batch_audio", "bark_b200_batch_tokens", "bark_b200_gpt_eval_slot", "bark_b200_gpt_step_batch",
     "bark_b200_set_history_prompt", "bark_b200_generate_batch_prompted", "bark_b200_set_sampling", "bark_b200_sample_filtered_given_u",
     "bark_b200_quant_matmul", "bark_b200_fast_convert",
+    "bark_b200_codec_conv1d", "bark_b200_codec_convtr1d", "bark_b200_codec_lstm", "bark_b200_codec_rvq_decode", "bark_b200_device_math",
     "bark_b200_encodec_compress_batch", "bark_b200_encodec_decompress_batch", "bark_b200_encodec_reconstruct_batch",
     "bark_b200_encodec_batch_codes", "bark_b200_encodec_batch_audio",
     "bark_b200_encodec_compress_resampled", "bark_b200_encodec_reconstruct_resampled", "bark_b200_encodec_compress_batch_resampled",
@@ -225,6 +226,16 @@ def lib() -> C.CDLL:
     L.bark_b200_parity_gemm.argtypes = [vp, vp, vp] + [C.c_int] * 6 + [vp]
     L.bark_b200_quant_matmul.restype = C.c_int
     L.bark_b200_quant_matmul.argtypes = [C.c_int, vp, vp, vp] + [C.c_int] * 5 + [vp, vp, vp, vp]
+    L.bark_b200_codec_conv1d.restype = C.c_int
+    L.bark_b200_codec_conv1d.argtypes = [f32p, C.c_int, vp, C.c_int, vp, f32p] + [C.c_int] * 4 + [f32p, f32p]
+    L.bark_b200_codec_convtr1d.restype = C.c_int
+    L.bark_b200_codec_convtr1d.argtypes = [f32p, C.c_int, vp, C.c_int, vp, f32p, C.c_int, C.c_int, f32p]
+    L.bark_b200_codec_lstm.restype = C.c_int
+    L.bark_b200_codec_lstm.argtypes = [f32p, C.c_int, vp, C.c_int, vp, vp, f32p, f32p, f32p, f32p]
+    L.bark_b200_codec_rvq_decode.restype = C.c_int
+    L.bark_b200_codec_rvq_decode.argtypes = [i32p, C.c_int, vp, C.c_int, f32p, C.c_int, C.c_int, f32p]
+    L.bark_b200_device_math.restype = C.c_int
+    L.bark_b200_device_math.argtypes = [C.c_int, C.c_uint32, C.c_uint32, C.c_uint32, f32p]
     L.bark_b200_parity_rows.restype = C.c_int
     L.bark_b200_parity_rows.argtypes = [C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, vp, vp, C.POINTER(C.c_uint)]
     L.bark_b200_sample_given_u.restype = C.c_int
@@ -880,6 +891,104 @@ def quant_matmul(qtype: str, W: np.ndarray, A: np.ndarray, epilogue: str = "stor
     if not return_q8:
         return out
     return out, q, d.astype(np.float16), None if s is None else s.astype(np.float16)
+
+
+def _codec_call(what: str, r: int):
+    """The value a codec hook returned; GuardBandError when it stored outside its output, RuntimeError when it refused or failed."""
+    if r == -1:
+        raise GuardBandError(f"{what} wrote outside its output")
+    if r <= 0:
+        raise RuntimeError(f"{what} failed or refused the shape (see stderr)")
+    return r
+
+
+def _items(xs, C: int, dtype=np.float32):
+    """Items [C][L_b] -> (their concatenation, int32 lengths)."""
+    xs = [np.asarray(x, dtype).reshape(C, -1) for x in xs]
+    return np.ascontiguousarray(np.concatenate([x.ravel() for x in xs])), np.array([x.shape[1] for x in xs], np.int32)
+
+
+def _split(flat: np.ndarray, C: int, lengths):
+    out, o = [], 0
+    for L in lengths:
+        out.append(flat[o:o + C * L].reshape(C, L))
+        o += C * L
+    return out
+
+
+def codec_conv1d(xs, w: np.ndarray, bias: np.ndarray, stride: int = 1, elu_in: bool = False, resid=None, return_kernel: bool = False):
+    """The EnCodec convolution launcher (bark_b200_codec_conv1d) on the items xs, each float32 [Cin][L_b]; w float16 [Cout][Cin][k] as the
+    file stores it, bias float32 [Cout], resid (stride 1) a list of [Cout][L_b] or None.  Returns the items' outputs [Cout][T_b], and with
+    return_kernel the id of the kernel that ran (include/bark_b200.h)."""
+    w = np.ascontiguousarray(w, np.float16); Cout, Cin, k = w.shape
+    x, L = _items(xs, Cin)
+    T = [conv1d_out_len(int(l), k, stride) for l in L]
+    y = np.zeros(Cout * sum(T), np.float32)
+    r_flat = None if resid is None else _items(resid, Cout)[0]
+    r = _codec_call(f"bark_b200_codec_conv1d (Cin {Cin}, Cout {Cout}, k {k}, stride {stride}, L {L.tolist()})",
+                    lib().bark_b200_codec_conv1d(_p(x), Cin, _p(L), L.size, _p(w), _p(np.ascontiguousarray(bias, np.float32)), Cout, k, stride,
+                                                 int(elu_in), None if r_flat is None else _p(r_flat), _p(y)))
+    out = _split(y, Cout, T)
+    return (out, r) if return_kernel else out
+
+
+def conv1d_out_len(L: int, k: int, stride: int) -> int:
+    """strided_conv_1d's output length: get_extra_padding_for_conv_1d evaluated in float32, as the reference does."""
+    f32 = np.float32
+    n_frames = (f32(L) - f32(k) + f32(k - stride)) / f32(stride) + f32(1)
+    ideal = int((np.ceil(n_frames) - f32(1)) * f32(stride) + (f32(k) - f32(k - stride)))
+    extra = int(f32(ideal) - f32(L))
+    return (L + (k - stride) + extra - k) // stride + 1
+
+
+def codec_convtr1d(xs, w: np.ndarray, bias: np.ndarray, stride: int, return_kernel: bool = False):
+    """ELU and the transposed convolution (bark_b200_codec_convtr1d) on items [Cin][T_b]; w float16 [Cin][Cout][2 stride] as stored.
+    Returns the items' outputs [Cout][T_b stride] (and the NG of the kernel that ran)."""
+    w = np.ascontiguousarray(w, np.float16); Cin, Cout, k = w.shape
+    assert k == 2 * stride, (w.shape, stride)
+    x, T = _items(xs, Cin)
+    y = np.zeros(Cout * int(T.sum()) * stride, np.float32)
+    r = _codec_call(f"bark_b200_codec_convtr1d (Cin {Cin}, Cout {Cout}, stride {stride}, T {T.tolist()})",
+                    lib().bark_b200_codec_convtr1d(_p(x), Cin, _p(T), T.size, _p(w), _p(np.ascontiguousarray(bias, np.float32)), Cout, stride, _p(y)))
+    out = _split(y, Cout, [int(t) * stride for t in T])
+    return (out, r) if return_kernel else out
+
+
+def codec_lstm(xs, wih: np.ndarray, whh: np.ndarray, bih: np.ndarray, bhh: np.ndarray, skip=None, return_kernel: bool = False):
+    """One LSTM layer (bark_b200_codec_lstm) on items [C][T_b]; wih, whh float16 [4C][C], bih, bhh float32 [4C], skip a list of [C][T_b]
+    added to the output, or None.  Returns the items' outputs (and 1 / 2: the one-item / batched recurrence ran)."""
+    wih = np.ascontiguousarray(wih, np.float16); whh = np.ascontiguousarray(whh, np.float16)
+    C = wih.shape[1]
+    x, T = _items(xs, C)
+    s_flat = None if skip is None else _items(skip, C)[0]
+    out = np.zeros(x.size, np.float32)
+    r = _codec_call(f"bark_b200_codec_lstm (C {C}, T {T.tolist()})",
+                    lib().bark_b200_codec_lstm(_p(x), C, _p(T), T.size, _p(wih), _p(whh), _p(np.ascontiguousarray(bih, np.float32)),
+                                               _p(np.ascontiguousarray(bhh, np.float32)), None if s_flat is None else _p(s_flat), _p(out)))
+    res = _split(out, C, T)
+    return (res, r) if return_kernel else res
+
+
+def codec_rvq_decode(codes, codebooks: np.ndarray):
+    """The quantizer decode (bark_b200_codec_rvq_decode) on items of codes int32 [n_q][T_b] through codebooks float32 [n_q][n_bins][hidden].
+    Returns the items' latents [hidden][T_b]."""
+    cb = np.ascontiguousarray(codebooks, np.float32); n_q, n_bins, hidden = cb.shape
+    c, T = _items(codes, n_q, np.int32)
+    x = np.zeros(hidden * int(T.sum()), np.float32)
+    _codec_call(f"bark_b200_codec_rvq_decode (n_q {n_q}, T {T.tolist()})",
+                lib().bark_b200_codec_rvq_decode(_p(c), n_q, _p(T), T.size, _p(cb), hidden, n_bins, _p(x)))
+    return _split(x, hidden, T)
+
+
+DEVICE_MATH = {"expm1f": 0, "tanhf": 1, "expf": 2, "v_expf": 3, "elu": 4, "sigmoid": 5, "round_f16": 6}
+
+
+def device_math(fn: str, lo_bits: int, count: int, stride: int = 1) -> np.ndarray:
+    """A device function of the codec and soft_max (bark_b200_device_math) on the floats of bit patterns lo_bits + i stride (mod 2^32),
+    i < count <= 2^24: float32 [count]."""
+    out = np.zeros(count, np.float32)
+    _codec_call(f"bark_b200_device_math ({fn})", lib().bark_b200_device_math(DEVICE_MATH[fn], lo_bits & 0xFFFFFFFF, stride, count, _p(out)))
+    return out
 
 
 def fast_convert(wtype: str, W: np.ndarray):

@@ -444,12 +444,13 @@ static void strided_conv_lengths(int L, int k, int stride, int * Lp, int * Tout)
 int conv1d_out_len(int L, int k, int stride) { int Lp, Tout; strided_conv_lengths(L, k, stride, &Lp, &Tout); return Tout; }
 
 // shapes the stream kernel is instantiated for: the encoder's down-sampling convs (k = 2r, stride r) and its final conv
-static void conv1d_stream(const float * x, int Cin, const int * L, int n, const ConvW & cv, int stride, bool elu_in, float * y, cudaStream_t s) {
+static int conv1d_stream(const float * x, int Cin, const int * L, int n, const ConvW & cv, int stride, bool elu_in, float * y, cudaStream_t s) {
     const int K = Cin * cv.k;
     std::vector<int> Lp((size_t) n), Tout((size_t) n);
     for (int b = 0; b < n; b++) {
         strided_conv_lengths(L[b], cv.k, stride, &Lp[b], &Tout[b]);
-        if (K % 32 != 0 || Lp[b] - L[b] - (cv.k - stride) > L[b] - 1) {
+        // both reflections must stay inside the input: the left one reads up to k - stride past position 0, the right one `extra`
+        if (K % 32 != 0 || cv.k - stride > L[b] - 1 || Lp[b] - L[b] - (cv.k - stride) > L[b] - 1) {
             fprintf(stderr, "bark_b200: unsupported conv shape Cin=%d k=%d stride=%d L=%d\n", Cin, cv.k, stride, L[b]); throw std::runtime_error("unsupported configuration (see the message above)");
         }
     }
@@ -467,14 +468,14 @@ static void conv1d_stream(const float * x, int Cin, const int * L, int n, const 
     if (cv.k == KW && stride == ST) {                                                                                        \
         BARK_CUDA_CHECK(cudaFuncSetAttribute(conv1d_stream_kernel<KW, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem)); \
         BARK_LAUNCH((conv1d_stream_kernel<KW, ST>), grid, 256, smem, s, x, Cin, cv.w, cv.Kp, cv.b, cv.cout, o_per_block, elu_in ? 1 : 0, y, it); \
-        return;                                                                                                              \
+        return kConvStream + KW * 100 + ST;                                                                                  \
     }
     STREAM_CASE(4, 2) STREAM_CASE(8, 4) STREAM_CASE(10, 5) STREAM_CASE(16, 8) STREAM_CASE(7, 1)
 #undef STREAM_CASE
     fprintf(stderr, "bark_b200: unsupported conv kernel size %d with stride %d\n", cv.k, stride); throw std::runtime_error("unsupported configuration (see the message above)");
 }
 
-void conv1d(const float * x, int Cin, const int * L, int n, const ConvW & cv, bool elu_in, const float * resid, float * y, cudaStream_t s, int stride) {
+int conv1d(const float * x, int Cin, const int * L, int n, const ConvW & cv, bool elu_in, const float * resid, float * y, cudaStream_t s, int stride) {
     const int K = Cin * cv.k, nsteps = K / 32, ngroups = (nsteps + 7) / 8;
     if (K < 32 && stride == 1) {
         const int TT = 128;
@@ -487,13 +488,12 @@ void conv1d(const float * x, int Cin, const int * L, int n, const ConvW & cv, bo
         g_next_flops = 2.0 * (double) it.base_in[n] * cv.cout * K;
         BARK_LAUNCH(conv1d_short_kernel, dim3(tiles, (cv.cout + o_per_block - 1) / o_per_block), TT, smem, s, x, Cin, cv.k, cv.w, cv.Kp, cv.b,
                     cv.cout, o_per_block, elu_in ? 1 : 0, resid, y, it);
-        return;
+        return kConvShort;
     }
     const bool lane_fits = stride == 1 && ((cv.k == 1 && ngroups <= 2) || (cv.k == 3 && ngroups <= 3) || (cv.k == 7 && ngroups <= 4));
     if (!lane_fits) {
         if (resid) { fprintf(stderr, "bark_b200: unsupported conv shape Cin=%d k=%d stride=%d with a residual\n", Cin, cv.k, stride); throw std::runtime_error("unsupported configuration (see the message above)"); }
-        conv1d_stream(x, Cin, L, n, cv, stride, elu_in, y, s);
-        return;
+        return conv1d_stream(x, Cin, L, n, cv, stride, elu_in, y, s);
     }
     const int TT = 32;
     const int S = (TT + cv.k - 1) | 1;
@@ -508,7 +508,8 @@ void conv1d(const float * x, int Cin, const int * L, int n, const ConvW & cv, bo
     g_next_flops = 2.0 * (double) it.base_in[n] * cv.cout * K;
 #define CONV_CASE(KW, NG)                                                                                                   \
     { BARK_CUDA_CHECK(cudaFuncSetAttribute(conv1d_lane_kernel<KW, NG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024)); \
-      BARK_LAUNCH((conv1d_lane_kernel<KW, NG>), grid, 256, smem, s, x, Cin, cv.w, cv.Kp, cv.b, cv.cout, o_per_block, elu_in ? 1 : 0, resid, y, it); }
+      BARK_LAUNCH((conv1d_lane_kernel<KW, NG>), grid, 256, smem, s, x, Cin, cv.w, cv.Kp, cv.b, cv.cout, o_per_block, elu_in ? 1 : 0, resid, y, it); \
+      return kConvLane + KW * 10 + NG; }
     if (cv.k == 1)      { if (ngroups <= 1) CONV_CASE(1, 1) else CONV_CASE(1, 2) }
     else if (cv.k == 3) { if (ngroups <= 1) CONV_CASE(3, 1) else if (ngroups <= 2) CONV_CASE(3, 2) else CONV_CASE(3, 3) }
     else if (cv.k == 7) { if (ngroups <= 1) CONV_CASE(7, 1) else CONV_CASE(7, 4) }
@@ -569,7 +570,7 @@ __global__ void __launch_bounds__(256) convtr1d_lane_kernel(const float * __rest
     }
 }
 
-void convtr1d(const float * x, int Cin, const int * T, int n, const ConvW & cv, int stride, float * y, cudaStream_t s) {
+int convtr1d(const float * x, int Cin, const int * T, int n, const ConvW & cv, int stride, float * y, cudaStream_t s) {
     const int nsteps = Cin / 32, ngroups = (nsteps + 7) / 8;
     if (Cin % 32 != 0 || ngroups > 2 || cv.k != 2 * stride) { fprintf(stderr, "bark_b200: unsupported transposed conv Cin=%d k=%d s=%d\n", Cin, cv.k, stride); throw std::runtime_error("unsupported configuration (see the message above)"); }
     const int TF = 16, S = TF + 1 + ((TF + 1) % 2 == 0);
@@ -584,6 +585,7 @@ void convtr1d(const float * x, int Cin, const int * T, int n, const ConvW & cv, 
     g_next_flops = 2.0 * 2.0 * (double) it.base_out[n] * cv.cout * Cin;
     if (ngroups <= 1) BARK_LAUNCH(convtr1d_lane_kernel<1>, dim3(tiles, gy), 256, smem, s, x, Cin, cv.w, cv.Kp, cv.b, cv.cout, stride, y, it);
     else              BARK_LAUNCH(convtr1d_lane_kernel<2>, dim3(tiles, gy), 256, smem, s, x, Cin, cv.w, cv.Kp, cv.b, cv.cout, stride, y, it);
+    return ngroups <= 1 ? 1 : 2;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -735,8 +737,8 @@ __global__ void __launch_bounds__(UPB * 4 * 32) lstm_recur_kernel(const float * 
     }
 }
 
-void lstm_layer(const float * x, int C, const int * T, int n, const __half * wih_li, const __half * whh_li, int Kp, const float * bih, const float * bhh,
-                const float * skip, float * gi_scratch, float * hbuf, unsigned * counter, float * out, cudaStream_t s) {
+int lstm_layer(const float * x, int C, const int * T, int n, const __half * wih_li, const __half * whh_li, int Kp, const float * bih, const float * bhh,
+               const float * skip, float * gi_scratch, float * hbuf, unsigned * counter, float * out, cudaStream_t s) {
     const int Hn = C, G4 = 4 * Hn;
     if (Hn % 32 != 0 || Hn > 512 || Hn % 4 != 0) { fprintf(stderr, "bark_b200: unsupported LSTM width %d\n", Hn); throw std::runtime_error("unsupported configuration (see the message above)"); }
     const CodecItems it = codec_items(n, T, T, T, 8);
@@ -768,6 +770,7 @@ void lstm_layer(const float * x, int C, const int * T, int n, const __half * wih
     }
     if (g_prof_on) prof_end(s);
     ++g_kernel_launches;
+    return n == 1 ? kLstmOne : kLstmBatched;
 }
 
 // [Cin][Cout][k] (torch ConvTranspose1d layout as stored, ggml [k, Cout, Cin]) -> rows [o][tap][Cin]

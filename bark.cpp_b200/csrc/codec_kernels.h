@@ -19,14 +19,19 @@ void rvq_norms(const float * embed, int n_bins, int Hd, float * out, cudaStream_
 // n_q <= 32, n_bins <= 1024, Hd % 32 == 0 and Hd <= 128
 bool rvq_encode(const float * const * embed, const float * const * norms, int n_q, int n_bins, int Hd, const float * latent, const int * T, int n,
                 int32_t * codes, cudaStream_t s);
+// The kernel a convolution launcher ran: conv1d_short_kernel, conv1d_lane_kernel<KW, NG> as kConvLane + 10 KW + NG, conv1d_stream_kernel<KW,
+// STRIDE> as kConvStream + 100 KW + STRIDE; the LSTM recurrence of one item or of several.  The pipeline ignores them; the tests count them.
+constexpr int kConvShort = 1, kConvLane = 1000, kConvStream = 10000, kLstmOne = 1, kLstmBatched = 2;
 // strided_conv_1d (ops.cpp:59-75) on x [Cin][L_b]: ELU on the input when elu_in, resid added to the output (stride 1 only).
 // y is [Cout][conv1d_out_len(L_b, k, stride)]; the launcher picks the kernel from the contraction length and the stride.
-void conv1d(const float * x, int Cin, const int * L, int n, const ConvW & cv, bool elu_in, const float * resid, float * y, cudaStream_t s, int stride = 1);
+int conv1d(const float * x, int Cin, const int * L, int n, const ConvW & cv, bool elu_in, const float * resid, float * y, cudaStream_t s, int stride = 1);
 int conv1d_out_len(int T, int k, int stride);
-void convtr1d(const float * x, int Cin, const int * L, int n, const ConvW & cv, int stride, float * y /*[Cout][L_b*stride]*/, cudaStream_t s);
-void lstm_layer(const float * x, int C, const int * T, int n, const __half * wih_li, const __half * whh_li, int Kp, const float * bih, const float * bhh,
-                const float * skip, float * gi_scratch /*[T_b][4C]*/, float * hbuf /*[2][kCodecMaxItems][C]*/, unsigned * counter, float * out,
-                cudaStream_t s);
+// returns the NG of the convtr1d_lane_kernel<NG> it ran
+int convtr1d(const float * x, int Cin, const int * L, int n, const ConvW & cv, int stride, float * y /*[Cout][L_b*stride]*/, cudaStream_t s);
+// returns kLstmOne or kLstmBatched
+int lstm_layer(const float * x, int C, const int * T, int n, const __half * wih_li, const __half * whh_li, int Kp, const float * bih, const float * bhh,
+               const float * skip, float * gi_scratch /*[T_b][4C]*/, float * hbuf /*[2][kCodecMaxItems][C]*/, unsigned * counter, float * out,
+               cudaStream_t s);
 // load-time re-layout of a transposed-conv weight: [Cin][Cout][k] -> rows [Cout][k][Cin]
 void convtr_rows(const __half * src, __half * dst, int Cin, int Cout, int k, cudaStream_t s);
 

@@ -200,7 +200,9 @@ __device__ __forceinline__ float glibc_expf_dev(float x) {
     double kd = __dadd_rn(z, 0x1.8p+52);
     const uint64_t ki = (uint64_t) __double_as_longlong(kd);
     kd = __dsub_rn(kd, 0x1.8p+52);
-    const double r = __dsub_rn(z, kd);
+    // glibc's x86-64 build selects its FMA variant of expf, where gcc contracts z - kd into one fused operation; rounding z first
+    // differs from it at x = 0x1.04845ep+5 and -0x1.f8cbb2p+5 (tests/test_codec_kernels_gpu.py::test_device_libm)
+    const double r = __fma_rn(0x1.71547652b82fep+0 * 32.0, xd, -kd);
     uint64_t t = c_exp2f_tab[ki & 31];
     t += ki << 47;
     const double s = __longlong_as_double((long long) t);

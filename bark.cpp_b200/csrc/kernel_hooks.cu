@@ -94,6 +94,45 @@ void poison_padding(void * p, size_t es, size_t total, size_t gs, int rows, int 
     else         BARK_LAUNCH(poison_padding_kernel<uint32_t>, 1184, 256, 0, 0, (uint32_t *) p, total, gs, rows, K, gm);
 }
 
+// One device function of common.cuh on the floats of bit patterns lo + i * stride (mod 2^32), i < count, generated here: the device
+// libm against the host's (tests/test_codec_kernels_gpu.py).  fn: the DeviceMathFn order of bark_b200_device_math.
+__global__ void device_math_kernel(int fn, uint32_t lo, uint32_t stride, uint32_t count, float * out) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < count; i += gridDim.x * blockDim.x) {
+        const float x = __uint_as_float(lo + i * stride);
+        float r;
+        switch (fn) {
+        case 0:  r = glibc_expm1f_dev(x); break;
+        case 1:  r = glibc_tanhf_dev(x); break;
+        case 2:  r = glibc_expf_dev(x); break;
+        case 3:  r = ggml_v_expf_dev(x); break;
+        case 4:  r = elu_exact(x); break;
+        case 5:  r = sigmoid_exact(x); break;
+        default: r = round_f16(x); break;
+        }
+        out[i] = r;
+    }
+}
+
+// the loader's re-layout of an f16 weight of `rows` rows of K (loader.cu): LI rows of li_padded_k(K, 2), every padding element NaN
+__half * li_weight(DeviceBuffers & mem, const __half * d_rows, int rows, int K, int * Kp) {
+    *Kp = li_padded_k(K, 2);
+    __half * li = mem.alloc<__half>((size_t) rows * *Kp * 2);
+    permute_to_li(d_rows, li, rows, K, W_F16, 0);
+    poison_padding(li, 2, (size_t) rows * *Kp, *Kp, rows, K, false);
+    return li;
+}
+
+// n item lengths of a codec hook: 1 to kCodecMaxItems items, each at least `min_len`; their sum through `total`
+bool codec_lengths(const char * fn, const int * L, int n, int min_len, size_t * total) {
+    if (!L || n < 1 || n > kCodecMaxItems) { fprintf(stderr, "%s: %d items (1 to %d)\n", fn, n, kCodecMaxItems); return false; }
+    *total = 0;
+    for (int b = 0; b < n; b++) {
+        if (L[b] < min_len) { fprintf(stderr, "%s: item %d has length %d (at least %d)\n", fn, b, L[b], min_len); return false; }
+        *total += (size_t) L[b];
+    }
+    return true;
+}
+
 // a group-major operand of group stride gs (host) -> row-major [M][N] elements of es bytes
 void gm_to_rows(const unsigned char * gm, void * dst, int M, int N, size_t gs, size_t es) {
     for (int m = 0; m < M; m++)
@@ -446,5 +485,111 @@ extern "C" int bark_b200_quant_matmul(int wtype, const void * W, const float * A
         if (d_out) download(d_out, q8.d, (size_t) M * nb * 4);
         if (s_out) download(s_out, q8.s, (size_t) M * nb * 4);
         return 1;
+    });
+}
+
+// the EnCodec convolution launcher conv1d on n items of x [Cin][L_b], its weight laid out as loader.cu lays it out
+extern "C" int bark_b200_codec_conv1d(const float * x, int Cin, const int * L, int n, const uint16_t * w, const float * bias, int Cout, int k, int stride,
+                                      int elu_in, const float * resid, float * y) {
+    return guarded(0, [&] {
+        const char * fn = "bark_b200_codec_conv1d";
+        size_t total = 0;
+        if (!x || !w || !bias || !y || Cin < 1 || Cout < 1 || k < 1 || stride < 1 || stride > k) { fprintf(stderr, "%s: invalid arguments\n", fn); return 0; }
+        // stride 1: the k - 1 reflected on the left must lie inside the item (ggml_pad_reflect_1d; the short and lane kernels would read
+        // zeros there).  Strided: conv1d's own check refuses an item too short for either reflection.
+        if (!codec_lengths(fn, L, n, stride == 1 ? k : 1, &total)) return 0;
+        size_t out_total = 0;
+        for (int b = 0; b < n; b++) out_total += (size_t) conv1d_out_len(L[b], k, stride);
+        DeviceBuffers mem;
+        ConvW cv; cv.k = k; cv.cin = Cin; cv.cout = Cout;
+        cv.w = li_weight(mem, mem.upload((const __half *) w, (size_t) Cout * Cin * k * 2), Cout, Cin * k, &cv.Kp);
+        cv.b = mem.upload(bias, (size_t) Cout * 4);
+        const float * dx = mem.upload(x, total * Cin * 4), * dr = resid ? mem.upload(resid, out_total * Cout * 4) : nullptr;
+        const GuardedOutput o(mem, out_total * Cout * 4, nullptr);
+        const int ran = conv1d(dx, Cin, L, n, cv, elu_in != 0, dr, o.out<float>(), 0, stride);
+        if (!finish(fn)) return 0;
+        return o.read(fn, y) ? ran : -1;
+    });
+}
+
+// convtr1d (ELU on the input, k = 2 stride, right trim, bias) on n items of x [Cin][T_b]; w [Cin][Cout][k] as stored, through the
+// loader's convtr_rows and permute_to_li
+extern "C" int bark_b200_codec_convtr1d(const float * x, int Cin, const int * T, int n, const uint16_t * w, const float * bias, int Cout, int stride,
+                                        float * y) {
+    return guarded(0, [&] {
+        const char * fn = "bark_b200_codec_convtr1d";
+        size_t total = 0;
+        if (!x || !w || !bias || !y || Cin < 1 || Cout < 1 || stride < 1) { fprintf(stderr, "%s: invalid arguments\n", fn); return 0; }
+        if (!codec_lengths(fn, T, n, 1, &total)) return 0;
+        const int k = 2 * stride;
+        DeviceBuffers mem;
+        ConvW cv; cv.k = k; cv.cin = Cin; cv.cout = Cout;
+        __half * rows = mem.alloc<__half>((size_t) Cin * Cout * k * 2);
+        convtr_rows(mem.upload((const __half *) w, (size_t) Cin * Cout * k * 2), rows, Cin, Cout, k, 0);
+        cv.w = li_weight(mem, rows, Cout * k, Cin, &cv.Kp);
+        cv.b = mem.upload(bias, (size_t) Cout * 4);
+        const float * dx = mem.upload(x, total * Cin * 4);
+        const GuardedOutput o(mem, total * stride * Cout * 4, nullptr);
+        const int ran = convtr1d(dx, Cin, T, n, cv, stride, o.out<float>(), 0);
+        if (!finish(fn)) return 0;
+        return o.read(fn, y) ? ran : -1;
+    });
+}
+
+// lstm_layer on n items of x [C][T_b] (wih, whh [4C][C] f16 as stored; bih, bhh [4C]); skip (may be null) added to the output
+extern "C" int bark_b200_codec_lstm(const float * x, int C, const int * T, int n, const uint16_t * wih, const uint16_t * whh, const float * bih,
+                                    const float * bhh, const float * skip, float * out) {
+    return guarded(0, [&] {
+        const char * fn = "bark_b200_codec_lstm";
+        size_t total = 0;
+        if (!x || !wih || !whh || !bih || !bhh || !out || C < 1) { fprintf(stderr, "%s: invalid arguments\n", fn); return 0; }
+        if (!codec_lengths(fn, T, n, 1, &total)) return 0;
+        const size_t G4 = (size_t) 4 * C;
+        DeviceBuffers mem;
+        int Kp = 0;
+        const __half * dih = li_weight(mem, mem.upload((const __half *) wih, G4 * C * 2), (int) G4, C, &Kp);
+        const __half * dhh = li_weight(mem, mem.upload((const __half *) whh, G4 * C * 2), (int) G4, C, &Kp);
+        const float * dbi = mem.upload(bih, G4 * 4), * dbh = mem.upload(bhh, G4 * 4);
+        const float * dx = mem.upload(x, total * C * 4), * ds = skip ? mem.upload(skip, total * C * 4) : nullptr;
+        float * gi = mem.poisoned<float>(total * G4 * 4), * hbuf = mem.poisoned<float>((size_t) 2 * kCodecMaxItems * C * 4);
+        unsigned * counter = mem.alloc<unsigned>(sizeof(unsigned));
+        const GuardedOutput o(mem, total * C * 4, nullptr);
+        const int ran = lstm_layer(dx, C, T, n, dih, dhh, Kp, dbi, dbh, ds, gi, hbuf, counter, o.out<float>(), 0);
+        if (!finish(fn)) return 0;
+        return o.read(fn, out) ? ran : -1;
+    });
+}
+
+// rvq_decode on n items of codes [n_q][T_b] through codebooks [n_q][n_bins][hidden] -> x [hidden][T_b]
+extern "C" int bark_b200_codec_rvq_decode(const int32_t * codes, int n_q, const int * T, int n, const float * codebooks, int hidden, int n_bins, float * x) {
+    return guarded(0, [&] {
+        const char * fn = "bark_b200_codec_rvq_decode";
+        size_t total = 0;
+        if (!codes || !codebooks || !x || n_q < 1 || n_q > kMaxCodebooks || hidden < 1 || n_bins < 1) { fprintf(stderr, "%s: invalid arguments\n", fn); return 0; }
+        if (!codec_lengths(fn, T, n, 1, &total)) return 0;
+        for (size_t i = 0; i < total * n_q; i++)
+            if (codes[i] < 0 || codes[i] >= n_bins) { fprintf(stderr, "%s: code %d outside [0, %d)\n", fn, codes[i], n_bins); return 0; }
+        DeviceBuffers mem;
+        CodecModel cm;
+        cm.hidden_dim = hidden;
+        const float * dcb = mem.upload(codebooks, (size_t) n_q * n_bins * hidden * 4);
+        for (int q = 0; q < n_q; q++) cm.embed[q] = (float *) dcb + (size_t) q * n_bins * hidden;
+        const int32_t * dc = mem.upload(codes, total * n_q * 4);
+        const GuardedOutput o(mem, total * hidden * 4, nullptr);
+        rvq_decode(cm, dc, n_q, T, n, o.out<float>(), 0);
+        if (!finish(fn)) return 0;
+        return o.read(fn, x) ? 1 : -1;
+    });
+}
+
+// device_math_kernel: count <= 2^24 results, one 64 MB output at most
+extern "C" int bark_b200_device_math(int fn, uint32_t lo_bits, uint32_t stride, uint32_t count, float * out) {
+    return guarded(0, [&] {
+        if (!out || fn < 0 || fn > 6 || stride < 1 || count < 1 || count > (1u << 24)) { fprintf(stderr, "bark_b200_device_math: invalid arguments\n"); return 0; }
+        DeviceBuffers mem;
+        const GuardedOutput o(mem, (size_t) count * 4, nullptr);
+        BARK_LAUNCH(device_math_kernel, std::min<uint32_t>((count + 255) / 256, 4096), 256, 0, 0, fn, lo_bits, stride, count, o.out<float>());
+        if (!finish("bark_b200_device_math")) return 0;
+        return o.read("bark_b200_device_math", out) ? 1 : -1;
     });
 }

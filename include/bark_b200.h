@@ -363,6 +363,31 @@ BARK_API int  bark_b200_parity_gemm(const void * A, const void * W, void * C, in
 BARK_API int  bark_b200_quant_matmul(int wtype, const void * W, const float * A, float * C, int M, int N, int K, int epilogue, int path,
                                      const uint16_t * gelu_tab, int8_t * q, float * d, float * s);
 
+/* EnCodec kernels on host buffers without a context (tests), each on n items (1 to 32 clips) of their own lengths, concatenated item by
+ * item: item b of an activation [C][L_b] follows items 0..b-1.  f16 weights arrive as the model file stores them and are laid out by
+ * the loader's own routines, with every padding element NaN.  Each returns a positive value on success, 0 on invalid arguments, on a
+ * shape the launcher refuses (with a message) or on failure, -1 if a store landed in the guard bands around the output.
+ *   bark_b200_codec_conv1d ....... strided_conv_1d: x [Cin][L_b] (ELU'd first when elu_in) -> y [Cout][T_b], T_b the reference's output
+ *                                  length (L_b at stride 1), w [Cout][Cin][k] f16, bias [Cout], resid (stride 1 only, may be NULL)
+ *                                  [Cout][T_b] added to the result; L_b > k - stride (refused by the launcher above stride 1).  Returns the kernel that ran: 1 conv1d_short_kernel,
+ *                                  1000 + 10 KW + NG conv1d_lane_kernel<KW, NG>, 10000 + 100 KW + STRIDE conv1d_stream_kernel<KW, STRIDE>.
+ *   bark_b200_codec_convtr1d ..... ELU, then strided_conv_transpose_1d with k = 2 stride, right-trimmed: x [Cin][T_b] -> y [Cout][T_b stride],
+ *                                  w [Cin][Cout][k] f16, bias [Cout].  Returns the NG of convtr1d_lane_kernel<NG>.
+ *   bark_b200_codec_lstm ......... one LSTM layer: x [C][T_b] -> out [C][T_b] (plus skip [C][T_b] when not NULL), wih / whh [4C][C] f16,
+ *                                  bih / bhh [4C].  Returns 1 for the one-item recurrence, 2 for the batched one.
+ *   bark_b200_codec_rvq_decode ... codes [n_q][T_b] (each in [0, n_bins)) through codebooks [n_q][n_bins][hidden] f32 -> x [hidden][T_b].
+ * bark_b200_device_math evaluates one device function of the codec and soft_max, fn 0 glibc expm1f, 1 tanhf, 2 expf (restated), 3 ggml's
+ * AVX2 ggml_v_expf, 4 ELU, 5 the sigmoid, 6 the round trip through f16, on the floats of bit patterns lo_bits + i * stride (mod 2^32),
+ * i < count <= 2^24, into out [count].  Returns 1, 0 on invalid arguments or failure, -1 on a guard band store. */
+BARK_API int  bark_b200_codec_conv1d(const float * x, int Cin, const int * L, int n, const uint16_t * w, const float * bias, int Cout, int k, int stride,
+                                     int elu_in, const float * resid, float * y);
+BARK_API int  bark_b200_codec_convtr1d(const float * x, int Cin, const int * T, int n, const uint16_t * w, const float * bias, int Cout, int stride,
+                                       float * y);
+BARK_API int  bark_b200_codec_lstm(const float * x, int C, const int * T, int n, const uint16_t * wih, const uint16_t * whh, const float * bih,
+                                   const float * bhh, const float * skip, float * out);
+BARK_API int  bark_b200_codec_rvq_decode(const int32_t * codes, int n_q, const int * T, int n, const float * codebooks, int hidden, int n_bins, float * x);
+BARK_API int  bark_b200_device_math(int fn, uint32_t lo_bits, uint32_t stride, uint32_t count, float * out);
+
 #ifdef __cplusplus
 }
 #endif

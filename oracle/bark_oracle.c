@@ -1073,16 +1073,21 @@ static float * lstm_layer(const float * x, int C, int T, const tensor_t * wih, c
     return hs;
 }
 
+/* quantizer decode (quantizer.h:78-111): zero-initialised accumulator, q = 0..n_q-1 in order; cb[q] [n_bins][Hd], codes [n_q][T] */
+static void quantizer_decode(const int32_t * codes, int n_q, int T, const float * const * cb, int Hd, float * x) {
+    memset(x, 0, (size_t) Hd * T * 4);
+    for (int q = 0; q < n_q; q++)
+        for (int t = 0; t < T; t++) for (int d = 0; d < Hd; d++) x[(size_t) d * T + t] = x[(size_t) d * T + t] + cb[q][(size_t) codes[q * T + t] * Hd + d];
+}
+
 int orc_encodec_decode(orc_ctx * c, const int32_t * codes, int T, float * out) {
     codec_t * cd = &c->codec;
     const int Hd = cd->hidden_dim;
     static const int ratios[4] = {8, 5, 4, 2};
-    /* quantizer decode (quantizer.h:78-111): zero-initialised accumulator, q = 0..7 in order */
-    float * x = calloc((size_t) Hd * T, 4);
-    for (int q = 0; q < 8; q++) {
-        const float * emb = cd->embed[q].data;
-        for (int t = 0; t < T; t++) for (int d = 0; d < Hd; d++) x[(size_t) d * T + t] = x[(size_t) d * T + t] + emb[(size_t) codes[q * T + t] * Hd + d];
-    }
+    const float * cb[8];
+    for (int q = 0; q < 8; q++) cb[q] = cd->embed[q].data;
+    float * x = malloc((size_t) Hd * T * 4);
+    quantizer_decode(codes, 8, T, cb, Hd, x);
     float * y = conv1d(x, Hd, T, &cd->init); free(x);
     int C = cd->init.w.ne[2];
     float * h1 = lstm_layer(y, C, T, &cd->lstm_ih_w[0], &cd->lstm_hh_w[0], &cd->lstm_ih_b[0], &cd->lstm_hh_b[0]);

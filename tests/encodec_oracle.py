@@ -26,8 +26,9 @@ def n_q_for(bandwidth: int, sample_rate: int = 24000, n_bins: int = 1024) -> int
     return int(max(f32(1), np.floor(f32(bandwidth) * f32(1000) / bw_per_q)))
 
 
-def codebooks(path: str, offset: int) -> np.ndarray:
-    """Every quantizer.vq.layers.<q>._codebook.embed of the codec section at byte `offset`: [n_q][n_bins][hidden] float32."""
+def codec_tensors(path: str, offset: int) -> dict:
+    """Every tensor of the codec section at byte `offset`, by name: float32 or float16 arrays in the file's shape, outermost dimension
+    first (ggml's ne reversed)."""
     out = {}
     with open(path, "rb") as f:
         f.seek(offset + 4 + 9 * 4)                               # magic, 9 hyper-parameters (encodec.cpp:156-165)
@@ -38,11 +39,17 @@ def codebooks(path: str, offset: int) -> np.ndarray:
             n_dims, name_len, ttype = struct.unpack("<iii", head)
             ne = struct.unpack("<%di" % n_dims, f.read(4 * n_dims))
             name = f.read(name_len).decode()
-            n = int(np.prod(ne)) * (4 if ttype == 0 else 2)
-            data = f.read(n)
-            if name.startswith("quantizer.vq.layers."):
-                out[int(name.split(".")[3])] = np.frombuffer(data, np.float32).reshape(ne[1], ne[0])
-    return np.stack([out[q] for q in range(len(out))])
+            dt = np.float32 if ttype == 0 else np.float16
+            n = int(np.prod(ne))
+            out[name] = np.frombuffer(f.read(n * np.dtype(dt).itemsize), dt).reshape(ne[::-1])
+    return out
+
+
+def codebooks(path: str, offset: int) -> np.ndarray:
+    """Every quantizer.vq.layers.<q>._codebook.embed of the codec section at byte `offset`: [n_q][n_bins][hidden] float32."""
+    t = codec_tensors(path, offset)
+    cb = {int(k.split(".")[3]): v for k, v in t.items() if k.startswith("quantizer.vq.layers.")}
+    return np.stack([cb[q] for q in range(len(cb))])
 
 
 class CodecOracle:

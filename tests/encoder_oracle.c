@@ -198,3 +198,77 @@ int orc_encodec_encode(oenc_t * m, const float * audio, int n, int32_t * codes, 
     free(lat);
     return T;
 }
+
+/* ------------------------------------------------------------------------------------------ */
+/* The EnCodec ops one at a time on raw arrays, for the kernel-by-kernel GPU tests: thin wrappers around the static cores above, */
+/* one item each.  tests/test_codec_oracle_ops.py chains them into orc_encodec_decode and this file's encoder latent.          */
+/* ------------------------------------------------------------------------------------------ */
+static float * elu_copy(const float * x, size_t n, int elu_in) {
+    float * y = malloc(n * 4);
+    memcpy(y, x, n * 4);
+    if (elu_in) elu_inplace(y, n);
+    return y;
+}
+
+/* strided_conv_1d on x [Cin][L], w [Cout][Cin][k] f16: ELU on the input when elu_in, stride 1 through the decoder's conv1d, else
+ * conv_strided; resid [Cout][T] (may be NULL) added to the result.  Returns T, y [Cout][T]. */
+int orc_codec_conv1d(const float * x, int Cin, int L, const uint16_t * w, const float * bias, int Cout, int k, int stride, int elu_in,
+                     const float * resid, float * y) {
+    conv_t cv = {{1, {k, Cin, Cout}, 3, (void *) w}, {0, {Cout, 1, 1}, 1, (void *) bias}};
+    float * xin = elu_copy(x, (size_t) Cin * L, elu_in), * out;
+    int T = L;
+    if (stride == 1) out = conv1d(xin, Cin, L, &cv);
+    else             out = conv_strided(xin, Cin, L, &cv, stride, &T);
+    if (resid) for (size_t i = 0; i < (size_t) Cout * T; i++) out[i] = out[i] + resid[i];
+    memcpy(y, out, (size_t) Cout * T * 4);
+    free(xin); free(out);
+    return T;
+}
+
+/* ELU, then strided_conv_transpose_1d with k = 2 stride (right trim, bias): x [Cin][T], w [Cin][Cout][k] f16 -> y [Cout][T stride] */
+int orc_codec_convtr1d(const float * x, int Cin, int T, const uint16_t * w, const float * bias, int Cout, int stride, float * y) {
+    conv_t cv = {{1, {2 * stride, Cout, Cin}, 3, (void *) w}, {0, {Cout, 1, 1}, 1, (void *) bias}};
+    float * xin = elu_copy(x, (size_t) Cin * T, 1);
+    int L;
+    float * out = convtr1d(xin, Cin, T, &cv, stride, &L);
+    memcpy(y, out, (size_t) Cout * L * 4);
+    free(xin); free(out);
+    return L;
+}
+
+/* one LSTM layer: x [C][T], wih / whh [4C][C] f16, bih / bhh [4C] -> out [C][T], plus skip [C][T] (decoder.h:72) when not NULL */
+void orc_codec_lstm(const float * x, int C, int T, const uint16_t * wih, const uint16_t * whh, const float * bih, const float * bhh, const float * skip,
+                    float * out) {
+    const tensor_t ih = {1, {C, 4 * C, 1}, 2, (void *) wih}, hh = {1, {C, 4 * C, 1}, 2, (void *) whh};
+    const tensor_t bi = {0, {4 * C, 1, 1}, 1, (void *) bih}, bh = {0, {4 * C, 1, 1}, 1, (void *) bhh};
+    float * h = lstm_layer(x, C, T, &ih, &hh, &bi, &bh);
+    for (size_t i = 0; i < (size_t) C * T; i++) out[i] = skip ? skip[i] + h[i] : h[i];
+    free(h);
+}
+
+/* the quantizer decode over codebooks [n_q][n_bins][hidden]: codes [n_q][T] -> x [hidden][T] */
+void orc_codec_rvq_decode(const int32_t * codes, int n_q, int T, const float * codebooks, int hidden, int n_bins, float * x) {
+    const float * cb[32];
+    for (int q = 0; q < n_q && q < 32; q++) cb[q] = codebooks + (size_t) q * n_bins * hidden;
+    quantizer_decode(codes, n_q, T, cb, hidden, x);
+}
+
+/* The host libm under the codec and soft_max, as the oracle calls it, on the floats of bit patterns x[0..n): fn 0 expm1f, 1 tanhf,
+ * 2 expf, 3 ggml_v_expf, 4 ELU, 5 the LSTM's sigmoid, 6 the f16 round trip (bark_b200_device_math's order). */
+void orc_libm(int fn, const uint32_t * x, long long n, float * out) {
+    #pragma omp parallel for schedule(static)
+    for (long long i = 0; i < n; i++) {
+        const float v = u2f(x[i]);
+        float r;
+        switch (fn) {
+        case 0:  r = expm1f(v); break;
+        case 1:  r = tanhf(v); break;
+        case 2:  r = expf(v); break;
+        case 3:  r = orc_v_expf(v); break;
+        case 4:  r = (v > 0.f) ? v : expm1f(v); break;
+        case 5:  r = 1.f / (1.f + expf(-v)); break;
+        default: r = orc_f16_to_f32(orc_f32_to_f16(v)); break;
+        }
+        out[i] = r;
+    }
+}

@@ -44,6 +44,13 @@ def lib() -> C.CDLL:
         L.orc_encodec_encode.restype = C.c_int
         L.orc_encodec_encode.argtypes = [vp, vp, C.c_int, vp, vp]
         L.orc_rvq_encode.argtypes = [vp, C.c_int, vp, C.c_int, C.c_int, C.c_int, vp]
+        L.orc_codec_conv1d.restype = C.c_int
+        L.orc_codec_conv1d.argtypes = [vp, C.c_int, C.c_int, vp, vp] + [C.c_int] * 4 + [vp, vp]
+        L.orc_codec_convtr1d.restype = C.c_int
+        L.orc_codec_convtr1d.argtypes = [vp, C.c_int, C.c_int, vp, vp, C.c_int, C.c_int, vp]
+        L.orc_codec_lstm.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]
+        L.orc_codec_rvq_decode.argtypes = [vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp]
+        L.orc_libm.argtypes = [C.c_int, vp, C.c_longlong, vp]
         _lib = L
     return _lib
 
@@ -74,6 +81,86 @@ def rvq_encode(latent, codebooks) -> np.ndarray:
     codes = np.zeros((n_q, T), np.int32)
     lib().orc_rvq_encode(_p(lat), T, _p(cb), hidden, n_bins, n_q, _p(codes))
     return codes
+
+
+def _opt(a):
+    return None if a is None else _p(a)
+
+
+def conv1d(x, w, bias, stride: int = 1, elu_in: bool = False, resid=None) -> np.ndarray:
+    """orc_codec_conv1d on one item: x [Cin][L] float32, w [Cout][Cin][k] float16, bias [Cout] -> [Cout][T]."""
+    x = np.ascontiguousarray(x, np.float32); w = np.ascontiguousarray(w, np.float16); b = np.ascontiguousarray(bias, np.float32)
+    Cout, Cin, k = w.shape
+    assert x.shape[0] == Cin and x.shape[1] > k - stride, (x.shape, w.shape, stride)
+    r = None if resid is None else np.ascontiguousarray(resid, np.float32)
+    y = np.zeros(Cout * x.shape[1], np.float32)           # T <= L for every stride >= 1
+    T = lib().orc_codec_conv1d(_p(x), Cin, x.shape[1], _p(w), _p(b), Cout, k, stride, int(elu_in), _opt(r), _p(y))
+    return y[:Cout * T].reshape(Cout, T)
+
+
+def convtr1d(x, w, bias, stride: int) -> np.ndarray:
+    """orc_codec_convtr1d on one item: ELU, then the transposed conv; x [Cin][T], w [Cin][Cout][2 stride] float16 -> [Cout][T stride]."""
+    x = np.ascontiguousarray(x, np.float32); w = np.ascontiguousarray(w, np.float16)
+    Cin, Cout, k = w.shape
+    y = np.zeros((Cout, x.shape[1] * stride), np.float32)
+    L = lib().orc_codec_convtr1d(_p(x), Cin, x.shape[1], _p(w), _p(np.ascontiguousarray(bias, np.float32)), Cout, stride, _p(y))
+    assert L == y.shape[1], (L, y.shape)
+    return y
+
+
+def lstm(x, wih, whh, bih, bhh, skip=None) -> np.ndarray:
+    """orc_codec_lstm on one item: x [C][T], wih / whh [4C][C] float16, bih / bhh [4C]; skip [C][T] added when given."""
+    x = np.ascontiguousarray(x, np.float32)
+    C, T = x.shape
+    out = np.zeros((C, T), np.float32)
+    lib().orc_codec_lstm(_p(x), C, T, _p(np.ascontiguousarray(wih, np.float16)), _p(np.ascontiguousarray(whh, np.float16)),
+                         _p(np.ascontiguousarray(bih, np.float32)), _p(np.ascontiguousarray(bhh, np.float32)),
+                         _opt(None if skip is None else np.ascontiguousarray(skip, np.float32)), _p(out))
+    return out
+
+
+def rvq_decode(codes, codebooks) -> np.ndarray:
+    """orc_codec_rvq_decode on one item: codes [n_q][T] int32, codebooks [n_q][n_bins][hidden] float32 -> [hidden][T]."""
+    c = np.ascontiguousarray(codes, np.int32); cb = np.ascontiguousarray(codebooks, np.float32)
+    n_q, n_bins, hidden = cb.shape
+    x = np.zeros((hidden, c.shape[1]), np.float32)
+    lib().orc_codec_rvq_decode(_p(c), n_q, c.shape[1], _p(cb), hidden, n_bins, _p(x))
+    return x
+
+
+LIBM = {"expm1f": 0, "tanhf": 1, "expf": 2, "v_expf": 3, "elu": 4, "sigmoid": 5, "round_f16": 6}   # bark_b200_device_math's fn
+
+
+def libm(fn: str, x_bits) -> np.ndarray:
+    """orc_libm: the host's function on the floats of bit patterns x_bits (uint32)."""
+    x = np.ascontiguousarray(x_bits, np.uint32)
+    out = np.zeros(x.size, np.float32)
+    lib().orc_libm(LIBM[fn], _p(x), x.size, _p(out))
+    return out
+
+
+LIBM_FIXTURE = os.path.join(HERE, "golden", "libm", "glibc_2_39.npz")
+
+
+def libm_fixture_mismatch() -> str | None:
+    """None when this host's expm1f, tanhf and expf and the oracle's ggml_v_expf give, bit for bit and NaN for NaN, the values stored
+    in tests/golden/libm/glibc_2_39.npz (tests/golden/make_golden_libm.py); else what differs."""
+    g = np.load(LIBM_FIXTURE)
+    x = g["x"]
+    for fn in ("expm1f", "tanhf", "expf", "v_expf"):
+        got, want = libm(fn, x), g[fn].view(np.float32)
+        bad = np.flatnonzero((got.view(np.uint32) != want.view(np.uint32)) & ~(np.isnan(got) & np.isnan(want)))
+        if bad.size:
+            i = bad[0]
+            return (f"the host libm is not the reference's (glibc {g['glibc']} on x86-64 with FMA): {fn} differs on {bad.size} of {x.size} "
+                    f"stored inputs, first at bits {int(x[i]):#010x}: host {got[i]!r}, stored {want[i]!r}.  The oracle's waveforms would "
+                    f"then not be the reference's either, and the device libm cannot be checked against this host.")
+    return None
+
+
+def pattern_bits(lo_bits: int, count: int, stride: int = 1) -> np.ndarray:
+    """The bit patterns lo_bits + i stride (mod 2^32), i < count, as bark_b200_device_math walks them."""
+    return (np.uint32(lo_bits & 0xFFFFFFFF) + np.arange(count, dtype=np.uint32) * np.uint32(stride)).astype(np.uint32)
 
 
 # test signals, regenerated from seeds (tests/golden/make_golden_encoder.py stores only the reference's outputs)
