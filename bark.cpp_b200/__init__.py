@@ -130,6 +130,9 @@ EXPORTS = [
     "bark_b200_encodec_reconstruct_batch_resampled", "bark_b200_encodec_encode_resampled", "bark_b200_resample",
     "bark_b200_set_tokenizer", "bark_b200_text_ids", "bark_b200_bert_tokenize",
     "bark_b200_set_long_form", "bark_b200_long_chunks", "bark_b200_long_chunk_text", "bark_b200_long_chunk_tokens", "bark_b200_split_text",
+    "bark_b200_encodec_stream_open", "bark_b200_encodec_stream_push", "bark_b200_encodec_stream_push_batch", "bark_b200_encodec_stream_read",
+    "bark_b200_encodec_stream_finish", "bark_b200_encodec_stream_ready", "bark_b200_encodec_stream_codebooks", "bark_b200_encodec_stream_close",
+    "bark_b200_codec_conv1d_window", "bark_b200_codec_convtr1d_window", "bark_b200_codec_lstm_state",
     "ggml_time_init", "ggml_time_us", "ggml_time_ms", "ggml_init", "ggml_free",
 ]
 
@@ -232,6 +235,26 @@ def lib() -> C.CDLL:
     L.bark_b200_codec_convtr1d.argtypes = [f32p, C.c_int, vp, C.c_int, vp, f32p, C.c_int, C.c_int, f32p]
     L.bark_b200_codec_lstm.restype = C.c_int
     L.bark_b200_codec_lstm.argtypes = [f32p, C.c_int, vp, C.c_int, vp, vp, f32p, f32p, f32p, f32p]
+    L.bark_b200_codec_conv1d_window.restype = C.c_int
+    L.bark_b200_codec_conv1d_window.argtypes = [f32p, C.c_int, vp, C.c_int, vp, vp, vp, vp, f32p] + [C.c_int] * 4 + [f32p, f32p]
+    L.bark_b200_codec_convtr1d_window.restype = C.c_int
+    L.bark_b200_codec_convtr1d_window.argtypes = [f32p, C.c_int, vp, C.c_int, vp, vp, vp, vp, f32p, C.c_int, C.c_int, f32p]
+    L.bark_b200_codec_lstm_state.restype = C.c_int
+    L.bark_b200_codec_lstm_state.argtypes = [f32p, C.c_int, vp, C.c_int, vp, vp, f32p, f32p, f32p, f32p, f32p]
+    L.bark_b200_encodec_stream_open.restype = vp
+    L.bark_b200_encodec_stream_open.argtypes = [vp, C.c_int]
+    for n in ("bark_b200_encodec_stream_push", "bark_b200_encodec_stream_read"):
+        getattr(L, n).restype = C.c_int
+        getattr(L, n).argtypes = [vp, vp, C.c_int]
+    L.bark_b200_encodec_stream_push_batch.restype = C.c_int
+    L.bark_b200_encodec_stream_push_batch.argtypes = [vp, vp, vp, C.c_int]
+    for n in ("bark_b200_encodec_stream_finish", "bark_b200_encodec_stream_codebooks"):
+        getattr(L, n).restype = C.c_int
+        getattr(L, n).argtypes = [vp]
+    L.bark_b200_encodec_stream_ready.restype = C.c_longlong
+    L.bark_b200_encodec_stream_ready.argtypes = [C.c_int, C.c_longlong]
+    L.bark_b200_encodec_stream_close.restype = None
+    L.bark_b200_encodec_stream_close.argtypes = [vp]
     L.bark_b200_codec_rvq_decode.restype = C.c_int
     L.bark_b200_codec_rvq_decode.argtypes = [i32p, C.c_int, vp, C.c_int, f32p, C.c_int, C.c_int, f32p]
     L.bark_b200_device_math.restype = C.c_int
@@ -969,6 +992,53 @@ def codec_lstm(xs, wih: np.ndarray, whh: np.ndarray, bih: np.ndarray, bhh: np.nd
     return (res, r) if return_kernel else res
 
 
+def _window(org, first, n_out):
+    return tuple(np.ascontiguousarray(a, t) for a, t in ((org, np.int64), (first, np.int64), (n_out, np.int32)))
+
+
+def codec_conv1d_window(xs, org, first, n_out, w: np.ndarray, bias: np.ndarray, stride: int = 1, elu_in: bool = False, resid=None, return_kernel: bool = False):
+    """codec_conv1d over windows (bark_b200_codec_conv1d_window): item b's columns xs[b] [Cin][L_b] are global positions org[b].. of its
+    signal, and its outputs first[b] .. first[b] + n_out[b] - 1 come back, [Cout][n_out[b]]; resid (stride 1) a list of [Cout][n_out[b]]."""
+    w = np.ascontiguousarray(w, np.float16); Cout, Cin, k = w.shape
+    x, L = _items(xs, Cin)
+    o, f, no = _window(org, first, n_out)
+    y = np.zeros(Cout * int(no.sum()), np.float32)
+    r_flat = None if resid is None else _items(resid, Cout)[0]
+    r = _codec_call(f"bark_b200_codec_conv1d_window (Cin {Cin}, Cout {Cout}, k {k}, stride {stride}, L {L.tolist()}, org {o.tolist()}, first {f.tolist()})",
+                    lib().bark_b200_codec_conv1d_window(_p(x), Cin, _p(L), L.size, _p(o), _p(f), _p(no), _p(w), _p(np.ascontiguousarray(bias, np.float32)),
+                                                        Cout, k, stride, int(elu_in), None if r_flat is None else _p(r_flat), _p(y)))
+    out = _split(y, Cout, no.tolist())
+    return (out, r) if return_kernel else out
+
+
+def codec_convtr1d_window(xs, org, first, n_out, w: np.ndarray, bias: np.ndarray, stride: int):
+    """codec_convtr1d over windows (bark_b200_codec_convtr1d_window): item b's frames xs[b] [Cin][L_b] are global frames org[b].., and the
+    output blocks of frames first[b] .. first[b] + n_out[b] - 1 come back, [Cout][n_out[b] stride]."""
+    w = np.ascontiguousarray(w, np.float16); Cin, Cout, k = w.shape
+    x, L = _items(xs, Cin)
+    o, f, no = _window(org, first, n_out)
+    y = np.zeros(Cout * int(no.sum()) * stride, np.float32)
+    _codec_call(f"bark_b200_codec_convtr1d_window (Cin {Cin}, Cout {Cout}, stride {stride}, L {L.tolist()}, org {o.tolist()}, first {f.tolist()})",
+                lib().bark_b200_codec_convtr1d_window(_p(x), Cin, _p(L), L.size, _p(o), _p(f), _p(no), _p(w), _p(np.ascontiguousarray(bias, np.float32)),
+                                                      Cout, stride, _p(y)))
+    return _split(y, Cout, [int(t) * stride for t in no])
+
+
+def codec_lstm_state(xs, wih: np.ndarray, whh: np.ndarray, bih: np.ndarray, bhh: np.ndarray, state=None, skip=None):
+    """codec_lstm from the state (h, c) float32 [n][2][C] (None: zeros) (bark_b200_codec_lstm_state).  Returns (the items' outputs,
+    the state after each item's last step)."""
+    wih = np.ascontiguousarray(wih, np.float16); whh = np.ascontiguousarray(whh, np.float16)
+    C = wih.shape[1]
+    x, T = _items(xs, C)
+    st = np.zeros((T.size, 2, C), np.float32) if state is None else np.array(state, np.float32).reshape(T.size, 2, C)
+    s_flat = None if skip is None else _items(skip, C)[0]
+    out = np.zeros(x.size, np.float32)
+    _codec_call(f"bark_b200_codec_lstm_state (C {C}, T {T.tolist()})",
+                lib().bark_b200_codec_lstm_state(_p(x), C, _p(T), T.size, _p(wih), _p(whh), _p(np.ascontiguousarray(bih, np.float32)),
+                                                 _p(np.ascontiguousarray(bhh, np.float32)), None if s_flat is None else _p(s_flat), _p(st), _p(out)))
+    return _split(out, C, T), st
+
+
 def codec_rvq_decode(codes, codebooks: np.ndarray):
     """The quantizer decode (bark_b200_codec_rvq_decode) on items of codes int32 [n_q][T_b] through codebooks float32 [n_q][n_bins][hidden].
     Returns the items' latents [hidden][T_b]."""
@@ -1091,9 +1161,12 @@ class Encodec:
             raise RuntimeError(f"encodec_load_model failed for {model_path} at offset {offset} (see stderr); no CPU fallback exists")
         self.ctx = C.c_void_p(self.ctx)
         self._bandwidth, self._sample_rate = None, None
+        self._streams = []
 
     def close(self):
         if getattr(self, "ctx", None):
+            for s in self._streams:                      # a stream must not outlive its context
+                s.close()
             lib().encodec_free(self.ctx)
             self.ctx = None
 
@@ -1231,12 +1304,103 @@ class Encodec:
         getattr(lib(), fn)(self.ctx, i, _p(out), n)
         return out
 
+    # ---- streams (bark_b200_encodec_stream_*): their outputs joined equal the whole-clip call on their input joined --------------
+    def stream(self, direction: str) -> "EncodecStream":
+        """A stream on this context: "encode" (mono 24 kHz samples in, codes out) or "decode" (codes in, samples out), at the n_q of the
+        current bandwidth."""
+        s = EncodecStream(self, direction)
+        self._streams.append(s)
+        return s
+
     def stats(self) -> dict:
         s = lib().encodec_get_statistics(self.ctx).contents
         return {"t_load_us": s.t_load_us, "t_compute_us": s.t_compute_us}
 
     def reset_stats(self):
         lib().encodec_reset_statistics(self.ctx)
+
+
+STREAM_DIRECTIONS = {"encode": 0, "decode": 1}
+
+
+class EncodecStream:
+    """A streaming EnCodec coder (bark_b200_encodec_stream_*) on an Encodec context, made by Encodec.stream.  push(x) returns the outputs
+    that became final: codes [n_q][k] int32 for an encode of float32 samples, float32 samples for a decode of codes [n_q][k]; finish()
+    returns the rest.  Everything returned, joined, equals compress / decompress of everything pushed."""
+
+    def __init__(self, codec: "Encodec", direction: str):
+        self.direction = direction
+        self.handle = lib().bark_b200_encodec_stream_open(codec.ctx, STREAM_DIRECTIONS[direction])
+        if not self.handle:
+            raise RuntimeError(f"bark_b200_encodec_stream_open ({direction}) failed (see stderr)")
+        self.handle = C.c_void_p(self.handle)
+        self.n_q = lib().bark_b200_encodec_stream_codebooks(self.handle)
+
+    def close(self):
+        if getattr(self, "handle", None):
+            lib().bark_b200_encodec_stream_close(self.handle)
+            self.handle = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    def _chunk(self, x):
+        """x as the C call takes it: (array, count) of samples or of frames"""
+        if self.direction == "encode":
+            a = np.ascontiguousarray(x, np.float32).ravel()
+            n = a.size
+        else:
+            a = np.ascontiguousarray(x, np.int32)
+            if a.ndim != 2 or a.shape[0] != self.n_q:
+                raise ValueError(f"decode stream: codes must be [{self.n_q}][k], got shape {a.shape}")
+            n = a.shape[1]
+        return (a if n else np.zeros(1, a.dtype)), n          # an empty chunk still passes a valid pointer
+
+    def read(self) -> np.ndarray:
+        """Every final output not yet returned."""
+        k = lib().bark_b200_encodec_stream_read(self.handle, None, 0)
+        if self.direction == "decode":
+            out = np.zeros(k, np.float32)
+        else:
+            out = np.zeros((self.n_q, k), np.int32)
+        got = lib().bark_b200_encodec_stream_read(self.handle, _p(out), k)
+        assert got == k, (got, k)
+        return out
+
+    def push(self, x) -> np.ndarray:
+        a, n = self._chunk(x)
+        if lib().bark_b200_encodec_stream_push(self.handle, _p(a), n) < 0:
+            raise RuntimeError("bark_b200_encodec_stream_push refused (see stderr)")
+        return self.read()
+
+    def finish(self) -> np.ndarray:
+        if lib().bark_b200_encodec_stream_finish(self.handle) < 0:
+            raise RuntimeError("bark_b200_encodec_stream_finish refused (see stderr)")
+        return self.read()
+
+
+def encodec_stream_push_batch(streams, chunks) -> list:
+    """Pushes chunks[i] to streams[i] (at most 32 streams of one context and direction) in one pass of the kernels
+    (bark_b200_encodec_stream_push_batch); returns each stream's new final outputs, as its own push would."""
+    if len(streams) != len(chunks):
+        raise ValueError(f"{len(streams)} streams but {len(chunks)} chunks")
+    arrs = [s._chunk(x) for s, x in zip(streams, chunks)]
+    n = len(streams)
+    hs = (C.c_void_p * max(n, 1))(*[s.handle.value for s in streams])
+    ptrs = (C.c_void_p * max(n, 1))(*[a.ctypes.data for a, _ in arrs])
+    cnt = (C.c_int * max(n, 1))(*[k for _, k in arrs])
+    if lib().bark_b200_encodec_stream_push_batch(hs, ptrs, cnt, n) < 0:
+        raise RuntimeError("bark_b200_encodec_stream_push_batch refused (see stderr)")
+    return [s.read() for s in streams]
+
+
+def encodec_stream_ready(direction: str, n: int) -> int:
+    """The outputs a stream has made final after n inputs, before finish (bark_b200_encodec_stream_ready): frames after n samples for
+    "encode", samples after n frames for "decode"."""
+    return int(lib().bark_b200_encodec_stream_ready(STREAM_DIRECTIONS[direction], int(n)))
 
 
 def rvq_encode(latent: np.ndarray, codebooks: np.ndarray) -> np.ndarray:

@@ -30,12 +30,16 @@ namespace bark {
 // Items of one launch, passed by value (__grid_constant__: indexed in the parameter space, never copied).  Item b reads [C][L_in[b]] at
 // C * base_in[b] and writes [C'][L_out[b]] at C' * base_out[b]; base_* are prefix sums of the lengths, base_*[n] their total.  Grids are
 // one flattened run of tiles: item b owns tiles [tile0[b], tile0[b+1]) of the kernel's tile size, so a launch costs the sum of the
-// items' tiles, not n times the longest.  Lp: the stream kernel's padded input length.
+// items' tiles, not n times the longest.  Lp: the stream kernel's padded input length.  A window of an item (CodecWindow,
+// codec_kernels.h): shift = first * stride - org, the column of its first output's input position 0, and whether its first output is
+// global output 0 (first0, for the transposed conv); 0 and 1 for whole signals.  A position left of column 0 is read only by a window
+// that starts at the signal's position 0, so the column is then the global position and the left reflection stays in 32 bits.
 // ------------------------------------------------------------------------------------------------
 struct CodecItems {
     int n;
     int L_in[kCodecMaxItems], L_out[kCodecMaxItems], Lp[kCodecMaxItems];
     int base_in[kCodecMaxItems + 1], base_out[kCodecMaxItems + 1], tile0[kCodecMaxItems + 1];
+    int shift[kCodecMaxItems], first0[kCodecMaxItems];
 };
 
 // tiled[b]: the positions item b's tiles of TT cover (its input or output length, as the kernel walks them)
@@ -44,9 +48,29 @@ static CodecItems codec_items(int n, const int * L_in, const int * L_out, const 
     CodecItems it{};
     it.n = n;
     for (int b = 0; b < n; b++) {
-        it.L_in[b] = L_in[b]; it.L_out[b] = L_out[b];
+        it.L_in[b] = L_in[b]; it.L_out[b] = L_out[b]; it.first0[b] = 1;
         it.base_in[b + 1] = it.base_in[b] + L_in[b]; it.base_out[b + 1] = it.base_out[b] + L_out[b];
         it.tile0[b + 1] = it.tile0[b] + (tiled[b] + TT - 1) / TT;
+    }
+    return it;
+}
+
+// The items of a convolution over windows: item b's L_in[b] columns hold global positions win.org[b].., and its outputs are the
+// win.n_out[b] from win.first[b] on; tiles of TT over the outputs.  Output t reads positions t stride - (k - stride) + j, j < k.  A window
+// whose outputs read a column it does not hold (the left reflection included where `reflect`; the right one only where the kernel
+// reflects, up to `right` columns past the end) is refused.
+static CodecItems window_items(int n, const int * L_in, const CodecWindow & win, int k, int stride, bool reflect, int right, int TT, const char * what) {
+    std::vector<int> L_out(win.n_out, win.n_out + n);
+    CodecItems it = codec_items(n, L_in, L_out.data(), L_out.data(), TT);
+    for (int b = 0; b < n; b++) {
+        const long long org = win.org[b], lo = win.first[b] * stride - (k - stride), hi = (win.first[b] + win.n_out[b] - 1) * stride - (k - stride) + k - 1;
+        const long long need_lo = lo < 0 ? 0 : lo, need_hi = reflect ? std::max(hi, -lo) : hi;
+        if (org < 0 || win.first[b] < 0 || L_in[b] < 1 || win.n_out[b] < 1 || need_lo < org || need_hi - org > (long long) L_in[b] - 1 + right || (right && hi - org > 2LL * (L_in[b] - 1))) {
+            fprintf(stderr, "bark_b200: %s window of item %d (columns %lld + %d, outputs %lld + %d) reads outside its columns\n", what, b, org, L_in[b],
+                    win.first[b], win.n_out[b]);
+            throw std::runtime_error("unsupported configuration (see the message above)");
+        }
+        it.shift[b] = (int)(win.first[b] * stride - org); it.first0[b] = win.first[b] == 0;
     }
     return it;
 }
@@ -263,15 +287,15 @@ __global__ void __launch_bounds__(256) conv1d_lane_kernel(const float * __restri
     constexpr int TT = 32;
     constexpr int S = ((TT + KW - 1) | 1);               // odd row stride: conflict-free lane -> (c, j) gathers
     extern __shared__ float xs[];                        // [Cin][S]
-    const int b = item_at(it.tile0, it.n, blockIdx.x), T = it.L_in[b], t0 = (blockIdx.x - it.tile0[b]) * TT;
-    x += (size_t) Cin * it.base_in[b]; y += (size_t) Cout * it.base_in[b];
-    if (resid) resid += (size_t) Cout * it.base_in[b];
+    const int b = item_at(it.tile0, it.n, blockIdx.x), L = it.L_in[b], T = it.L_out[b], t0 = (blockIdx.x - it.tile0[b]) * TT;
+    x += (size_t) Cin * it.base_in[b]; y += (size_t) Cout * it.base_out[b];
+    if (resid) resid += (size_t) Cout * it.base_out[b];
     for (int i = threadIdx.x; i < Cin * (TT + KW - 1); i += blockDim.x) {
         const int c = i / (TT + KW - 1), j = i % (TT + KW - 1);
-        int t = t0 + j - (KW - 1);
+        int t = it.shift[b] + t0 + j - (KW - 1);
         if (t < 0) t = -t;
         float v = 0.f;
-        if (t < T) { v = x[(size_t) c * T + t]; if (elu_in) v = elu_exact(v); v = round_f16(v); }
+        if (t < L) { v = x[(size_t) c * L + t]; if (elu_in) v = elu_exact(v); v = round_f16(v); }
         xs[c * S + j] = v;
     }
     __syncthreads();
@@ -326,16 +350,16 @@ __global__ void __launch_bounds__(128) conv1d_short_kernel(const float * __restr
                                                            const float * __restrict__ resid, float * __restrict__ y, const __grid_constant__ CodecItems it) {
     constexpr int TT = 128;
     extern __shared__ float xs[];                        // [Cin][TT + k - 1]
-    const int b = item_at(it.tile0, it.n, blockIdx.x), T = it.L_in[b];
+    const int b = item_at(it.tile0, it.n, blockIdx.x), L = it.L_in[b], T = it.L_out[b];
     const int W = TT + k - 1, t0 = (blockIdx.x - it.tile0[b]) * TT;
-    x += (size_t) Cin * it.base_in[b]; y += (size_t) Cout * it.base_in[b];
-    if (resid) resid += (size_t) Cout * it.base_in[b];
+    x += (size_t) Cin * it.base_in[b]; y += (size_t) Cout * it.base_out[b];
+    if (resid) resid += (size_t) Cout * it.base_out[b];
     for (int i = threadIdx.x; i < Cin * W; i += blockDim.x) {
         const int c = i / W, j = i % W;
-        int t = t0 + j - (k - 1);
+        int t = it.shift[b] + t0 + j - (k - 1);
         if (t < 0) t = -t;
         float v = 0.f;
-        if (t < T) { v = x[(size_t) c * T + t]; if (elu_in) v = elu_exact(v); v = round_f16(v); }
+        if (t < L) { v = x[(size_t) c * L + t]; if (elu_in) v = elu_exact(v); v = round_f16(v); }
         xs[i] = v;
     }
     __syncthreads();
@@ -375,7 +399,7 @@ __global__ void __launch_bounds__(256) conv1d_stream_kernel(const float * __rest
         const int c = i / SPAN, u = i % SPAN, p = t0 * STRIDE + u;
         float v = 0.f;
         if (p < Lp) {
-            int t = p - PADL;
+            int t = it.shift[b] + p - PADL;
             if (t < 0) t = -t;                           // reflect left (ggml.c:15587)
             if (t >= L) t = 2 * (L - 1) - t;             // reflect right (ggml.c:15588)
             v = x[(size_t) c * L + t];
@@ -444,19 +468,27 @@ static void strided_conv_lengths(int L, int k, int stride, int * Lp, int * Tout)
 int conv1d_out_len(int L, int k, int stride) { int Lp, Tout; strided_conv_lengths(L, k, stride, &Lp, &Tout); return Tout; }
 
 // shapes the stream kernel is instantiated for: the encoder's down-sampling convs (k = 2r, stride r) and its final conv
-static int conv1d_stream(const float * x, int Cin, const int * L, int n, const ConvW & cv, int stride, bool elu_in, float * y, cudaStream_t s) {
+static int conv1d_stream(const float * x, int Cin, const int * L, int n, const ConvW & cv, int stride, bool elu_in, float * y, cudaStream_t s,
+                         const CodecWindow * win) {
     const int K = Cin * cv.k;
-    std::vector<int> Lp((size_t) n), Tout((size_t) n);
-    for (int b = 0; b < n; b++) {
-        strided_conv_lengths(L[b], cv.k, stride, &Lp[b], &Tout[b]);
-        // both reflections must stay inside the input: the left one reads up to k - stride past position 0, the right one `extra`
-        if (K % 32 != 0 || cv.k - stride > L[b] - 1 || Lp[b] - L[b] - (cv.k - stride) > L[b] - 1) {
-            fprintf(stderr, "bark_b200: unsupported conv shape Cin=%d k=%d stride=%d L=%d\n", Cin, cv.k, stride, L[b]); throw std::runtime_error("unsupported configuration (see the message above)");
-        }
-    }
     const int TT = stride >= 8 ? 8 : 16, SR = ((TT - 1) * stride + cv.k) | 1;
-    CodecItems it = codec_items(n, L, Tout.data(), Tout.data(), TT);
-    for (int b = 0; b < n; b++) it.Lp[b] = Lp[b];
+    if (K % 32 != 0) { fprintf(stderr, "bark_b200: unsupported conv shape Cin=%d k=%d stride=%d\n", Cin, cv.k, stride); throw std::runtime_error("unsupported configuration (see the message above)"); }
+    CodecItems it;
+    if (win) {                                           // the padded positions the window's outputs read, from first * stride on
+        it = window_items(n, L, *win, cv.k, stride, true, stride - 1, TT, "strided conv");
+        for (int b = 0; b < n; b++) it.Lp[b] = (win->n_out[b] - 1) * stride + cv.k;
+    } else {
+        std::vector<int> Lp((size_t) n), Tout((size_t) n);
+        for (int b = 0; b < n; b++) {
+            strided_conv_lengths(L[b], cv.k, stride, &Lp[b], &Tout[b]);
+            // both reflections must stay inside the input: the left one reads up to k - stride past position 0, the right one `extra`
+            if (cv.k - stride > L[b] - 1 || Lp[b] - L[b] - (cv.k - stride) > L[b] - 1) {
+                fprintf(stderr, "bark_b200: unsupported conv shape Cin=%d k=%d stride=%d L=%d\n", Cin, cv.k, stride, L[b]); throw std::runtime_error("unsupported configuration (see the message above)");
+            }
+        }
+        it = codec_items(n, L, Tout.data(), Tout.data(), TT);
+        for (int b = 0; b < n; b++) it.Lp[b] = Lp[b];
+    }
     const size_t smem = (size_t) Cin * SR * sizeof(float);
     const int tiles = it.tile0[n];
     int o_per_block = cv.cout;
@@ -475,17 +507,20 @@ static int conv1d_stream(const float * x, int Cin, const int * L, int n, const C
     fprintf(stderr, "bark_b200: unsupported conv kernel size %d with stride %d\n", cv.k, stride); throw std::runtime_error("unsupported configuration (see the message above)");
 }
 
-int conv1d(const float * x, int Cin, const int * L, int n, const ConvW & cv, bool elu_in, const float * resid, float * y, cudaStream_t s, int stride) {
+int conv1d(const float * x, int Cin, const int * L, int n, const ConvW & cv, bool elu_in, const float * resid, float * y, cudaStream_t s, int stride,
+           const CodecWindow * win) {
     const int K = Cin * cv.k, nsteps = K / 32, ngroups = (nsteps + 7) / 8;
+    // the stride-1 kernels over whole signals, or over windows (whose outputs never reach the right end: stride 1 pads nothing there)
+    auto items = [&](int TT) { return win ? window_items(n, L, *win, cv.k, 1, true, 0, TT, "conv") : codec_items(n, L, L, L, TT); };
     if (K < 32 && stride == 1) {
         const int TT = 128;
-        const CodecItems it = codec_items(n, L, L, L, TT);
+        const CodecItems it = items(TT);
         const int tiles = it.tile0[n];
         int o_per_block = cv.cout;
         const int n_sm = device_sms();
         while (o_per_block > 1 && tiles * ((cv.cout + o_per_block - 1) / o_per_block) < 4 * n_sm) o_per_block = (o_per_block + 1) / 2;
         const size_t smem = (size_t) Cin * (TT + cv.k - 1) * sizeof(float);
-        g_next_flops = 2.0 * (double) it.base_in[n] * cv.cout * K;
+        g_next_flops = 2.0 * (double) it.base_out[n] * cv.cout * K;
         BARK_LAUNCH(conv1d_short_kernel, dim3(tiles, (cv.cout + o_per_block - 1) / o_per_block), TT, smem, s, x, Cin, cv.k, cv.w, cv.Kp, cv.b,
                     cv.cout, o_per_block, elu_in ? 1 : 0, resid, y, it);
         return kConvShort;
@@ -493,19 +528,19 @@ int conv1d(const float * x, int Cin, const int * L, int n, const ConvW & cv, boo
     const bool lane_fits = stride == 1 && ((cv.k == 1 && ngroups <= 2) || (cv.k == 3 && ngroups <= 3) || (cv.k == 7 && ngroups <= 4));
     if (!lane_fits) {
         if (resid) { fprintf(stderr, "bark_b200: unsupported conv shape Cin=%d k=%d stride=%d with a residual\n", Cin, cv.k, stride); throw std::runtime_error("unsupported configuration (see the message above)"); }
-        return conv1d_stream(x, Cin, L, n, cv, stride, elu_in, y, s);
+        return conv1d_stream(x, Cin, L, n, cv, stride, elu_in, y, s, win);
     }
     const int TT = 32;
     const int S = (TT + cv.k - 1) | 1;
     const size_t smem = (size_t) Cin * S * sizeof(float);
-    const CodecItems it = codec_items(n, L, L, L, TT);
+    const CodecItems it = items(TT);
     const int tiles = it.tile0[n];
     // enough blocks to fill the machine: split the output channels when there are few time tiles
     int o_per_block = cv.cout;
     const int n_sm = device_sms();
     while (o_per_block > 8 && tiles * ((cv.cout + o_per_block - 1) / o_per_block) < 4 * n_sm) o_per_block = (o_per_block + 1) / 2;
     const dim3 grid(tiles, (cv.cout + o_per_block - 1) / o_per_block);
-    g_next_flops = 2.0 * (double) it.base_in[n] * cv.cout * K;
+    g_next_flops = 2.0 * (double) it.base_out[n] * cv.cout * K;
 #define CONV_CASE(KW, NG)                                                                                                   \
     { BARK_CUDA_CHECK(cudaFuncSetAttribute(conv1d_lane_kernel<KW, NG>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024)); \
       BARK_LAUNCH((conv1d_lane_kernel<KW, NG>), grid, 256, smem, s, x, Cin, cv.w, cv.Kp, cv.b, cv.cout, o_per_block, elu_in ? 1 : 0, resid, y, it); \
@@ -531,12 +566,13 @@ __global__ void __launch_bounds__(256) convtr1d_lane_kernel(const float * __rest
     constexpr int TF = 16;                               // input frames per block
     constexpr int S = TF + 1 + ((TF + 1) % 2 == 0);      // odd stride
     extern __shared__ float xs[];                        // [Cin][S]: frames t0-1 .. t0+TF-1, ELU'd, f16-rounded
-    const int b = item_at(its.tile0, its.n, blockIdx.x), T = its.L_in[b], t0 = (blockIdx.x - its.tile0[b]) * TF;
-    x += (size_t) Cin * its.base_in[b]; y += (size_t) Cout * its.base_out[b];
+    const int b = item_at(its.tile0, its.n, blockIdx.x), Lin = its.L_in[b], T = its.L_out[b], t0 = (blockIdx.x - its.tile0[b]) * TF;
+    const bool first0 = its.first0[b];                   // output block 0 is the signal's frame 0: it has no frame before it
+    x += (size_t) Cin * its.base_in[b]; y += (size_t) Cout * its.base_out[b] * stride;
     for (int i = threadIdx.x; i < Cin * (TF + 1); i += blockDim.x) {
         const int c = i / (TF + 1), j = i % (TF + 1);
-        const int t = t0 + j - 1;
-        xs[c * S + j] = (t >= 0 && t < T) ? round_f16(elu_exact(x[(size_t) c * T + t])) : 0.f;
+        const int t = its.shift[b] + t0 + j - 1;
+        xs[c * S + j] = (t >= 0 && t < Lin) ? round_f16(elu_exact(x[(size_t) c * Lin + t])) : 0.f;
     }
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -562,7 +598,7 @@ __global__ void __launch_bounds__(256) convtr1d_lane_kernel(const float * __rest
             const float r1 = lane_tree_reduce(a1), r0 = lane_tree_reduce(a0);
             if (lane == 0) {
                 float acc = 0.0f;
-                if (t > 0) acc = __fadd_rn(acc, r1);
+                if (t > 0 || !first0) acc = __fadd_rn(acc, r1);
                 acc = __fadd_rn(acc, r0);
                 y[(size_t) o * L + (size_t) t * stride + j] = __fadd_rn(bo, acc);
             }
@@ -570,19 +606,19 @@ __global__ void __launch_bounds__(256) convtr1d_lane_kernel(const float * __rest
     }
 }
 
-int convtr1d(const float * x, int Cin, const int * T, int n, const ConvW & cv, int stride, float * y, cudaStream_t s) {
+int convtr1d(const float * x, int Cin, const int * T, int n, const ConvW & cv, int stride, float * y, cudaStream_t s, const CodecWindow * win) {
     const int nsteps = Cin / 32, ngroups = (nsteps + 7) / 8;
     if (Cin % 32 != 0 || ngroups > 2 || cv.k != 2 * stride) { fprintf(stderr, "bark_b200: unsupported transposed conv Cin=%d k=%d s=%d\n", Cin, cv.k, stride); throw std::runtime_error("unsupported configuration (see the message above)"); }
     const int TF = 16, S = TF + 1 + ((TF + 1) % 2 == 0);
     const size_t smem = (size_t) Cin * S * sizeof(float);
-    std::vector<int> L((size_t) n);
-    for (int b = 0; b < n; b++) L[(size_t) b] = T[b] * stride;
-    const CodecItems it = codec_items(n, T, L.data(), T, TF);
+    // items in input frames: output block t reads frames t - 1 (none for t = 0) and t, like a k = 2 conv without reflection; base_out
+    // counts frames, stride samples each
+    const CodecItems it = win ? window_items(n, T, *win, 2, 1, false, 0, TF, "transposed conv") : codec_items(n, T, T, T, TF);
     const int tiles = it.tile0[n];
     int gy = (cv.cout * stride + 7) / 8;
     const int n_sm = device_sms();
     while (gy > 1 && tiles * gy > 8 * n_sm) gy = (gy + 1) / 2;
-    g_next_flops = 2.0 * 2.0 * (double) it.base_out[n] * cv.cout * Cin;
+    g_next_flops = 2.0 * 2.0 * (double) it.base_out[n] * stride * cv.cout * Cin;
     if (ngroups <= 1) BARK_LAUNCH(convtr1d_lane_kernel<1>, dim3(tiles, gy), 256, smem, s, x, Cin, cv.w, cv.Kp, cv.b, cv.cout, stride, y, it);
     else              BARK_LAUNCH(convtr1d_lane_kernel<2>, dim3(tiles, gy), 256, smem, s, x, Cin, cv.w, cv.Kp, cv.b, cv.cout, stride, y, it);
     return ngroups <= 1 ? 1 : 2;
@@ -638,10 +674,13 @@ __device__ __forceinline__ void grid_barrier(unsigned * counter, unsigned target
 // One sequence (every single-clip call): CTA b owns UPB hidden units; every step it reads h_{t-1}, computes its 4*UPB gates, updates its
 // units and publishes h_t.  Kept beside the batched kernel below because that one, run with one item, is measurably slower per step
 // (DESIGN.md §15); lstm_layer picks between them by the number of items.
+// state (may be null: zeros): (h, c) [2][Hn] before step 0, read by every CTA before the first grid barrier, and after step T - 1, each
+// CTA writing its own units after the last one.
 template <int UPB>
 __global__ void __launch_bounds__(UPB * 4 * 32) lstm_recur_one_kernel(const float * __restrict__ gi, int T, int Hn, const __half * __restrict__ whh_li, int Kp,
                                                                       const float * __restrict__ bhh, const float * __restrict__ skip,
-                                                                      float * __restrict__ hbuf /*[2][Hn]*/, unsigned * __restrict__ counter, float * __restrict__ out) {
+                                                                      float * __restrict__ hbuf /*[2][Hn]*/, unsigned * __restrict__ counter, float * __restrict__ out,
+                                                                      float * state) {
     extern __shared__ float hs[];                        // [Hn] f16-rounded h_{t-1}; then [4*UPB] gate pre-activations
     float * gates = hs + Hn;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;       // warp = local gate row: unit u = warp % UPB, gate q = warp / UPB
@@ -652,10 +691,11 @@ __global__ void __launch_bounds__(UPB * 4 * 32) lstm_recur_one_kernel(const floa
     float wch[16];
     load_chain<2>(whh_li + (size_t) row * Kp, lane, (nsteps + 7) >> 3, wch);
     const float bg = bhh[row];
-    float c_state = 0.f;                                 // kept by threads 0..UPB-1, one per unit
+    float c_state = 0.f, h = 0.f;                        // kept by threads 0..UPB-1, one per unit
+    if (state && (int) threadIdx.x < UPB) c_state = state[Hn + blockIdx.x * UPB + threadIdx.x];
     for (int t = 0; t < T; t++) {
         const float * hprev = hbuf + (size_t)((t + 1) & 1) * Hn;
-        for (int j = threadIdx.x; j < Hn; j += blockDim.x) hs[j] = (t == 0) ? 0.f : round_f16(__ldcg(hprev + j));
+        for (int j = threadIdx.x; j < Hn; j += blockDim.x) hs[j] = (t == 0) ? (state ? round_f16(state[j]) : 0.f) : round_f16(__ldcg(hprev + j));
         __syncthreads();
         float acc = 0.f;
 #pragma unroll
@@ -670,23 +710,25 @@ __global__ void __launch_bounds__(UPB * 4 * 32) lstm_recur_one_kernel(const floa
             const float gt = glibc_tanhf_dev(gates[2 * UPB + uu]);
             const float ot = sigmoid_exact(gates[3 * UPB + uu]);
             c_state = __fadd_rn(__fmul_rn(ft, c_state), __fmul_rn(it, gt));
-            const float h = __fmul_rn(ot, glibc_tanhf_dev(c_state));
+            h = __fmul_rn(ot, glibc_tanhf_dev(c_state));
             __stcg(hbuf + (size_t)(t & 1) * Hn + un, h);
             out[(size_t) un * T + t] = skip ? __fadd_rn(skip[(size_t) un * T + t], h) : h;               // decoder.h:72 inpL + out
         }
         grid_barrier(counter, (unsigned)(t + 1) * gridDim.x);
     }
+    if (state && (int) threadIdx.x < UPB) { const int un = blockIdx.x * UPB + threadIdx.x; state[un] = h; state[Hn + un] = c_state; }
 }
 
 // Several items: every step carries all B items of the launch; a warp computes its gate row's dot for each item still inside its own
 // sequence (t < T_b), in that item's order and arithmetic (lstm_recur_one_kernel's), so an item's values do not depend on the others.
 // The loop runs max T_b steps with one grid barrier per step; an item past its T_b neither updates nor stores.  Thread (u, b) =
-// (tid % UPB, tid / UPB) keeps unit u's cell state of item b, so B <= blockDim / UPB.
+// (tid % UPB, tid / UPB) keeps unit u's cell state of item b, so B <= blockDim / UPB.  st.p[b]: item b's state, as the one-item kernel's.
+struct LstmState { float * p[kCodecMaxItems]; };
 template <int UPB>
 __global__ void __launch_bounds__(UPB * 4 * 32) lstm_recur_kernel(const float * __restrict__ gi, int T_max, int Hn, const __half * __restrict__ whh_li, int Kp,
                                                                   const float * __restrict__ bhh, const float * __restrict__ skip,
                                                                   float * __restrict__ hbuf /*[2][B][Hn]*/, unsigned * __restrict__ counter, float * __restrict__ out,
-                                                                  const __grid_constant__ CodecItems its) {
+                                                                  const __grid_constant__ CodecItems its, const __grid_constant__ LstmState st) {
     extern __shared__ float hs[];                        // [B][Hn] f16-rounded h_{t-1} of every item; then [B][4*UPB] gate pre-activations
     __shared__ int s_T[kCodecMaxItems], s_base[kCodecMaxItems];   // the items' lengths and offsets, read every step
     const int B = its.n;
@@ -701,14 +743,18 @@ __global__ void __launch_bounds__(UPB * 4 * 32) lstm_recur_kernel(const float * 
     float wch[16];
     load_chain<2>(whh_li + (size_t) row * Kp, lane, (nsteps + 7) >> 3, wch);
     const float bg = bhh[row];
-    float c_state = 0.f;                                 // kept by thread (u, b) for unit u of item b
+    float c_state = 0.f, h = 0.f;                        // kept by thread (u, b) for unit u of item b
     const bool owner = (int) threadIdx.x < UPB * B;
     const int my_T = owner ? s_T[threadIdx.x / UPB] : 0, my_base = owner ? s_base[threadIdx.x / UPB] : 0;
+    float * const my_state = owner ? st.p[threadIdx.x / UPB] : nullptr;
+    const int my_unit = blockIdx.x * UPB + threadIdx.x % UPB;
+    if (my_state) c_state = my_state[Hn + my_unit];
     for (int t = 0; t < T_max; t++) {
         const float * hprev = hbuf + (size_t)((t + 1) & 1) * B * Hn;
         for (int b = 0; b < B; b++)
             if (t < s_T[b])
-                for (int j = threadIdx.x; j < Hn; j += blockDim.x) hs[b * Hn + j] = (t == 0) ? 0.f : round_f16(__ldcg(hprev + (size_t) b * Hn + j));
+                for (int j = threadIdx.x; j < Hn; j += blockDim.x)
+                    hs[b * Hn + j] = (t == 0) ? (st.p[b] ? round_f16(st.p[b][j]) : 0.f) : round_f16(__ldcg(hprev + (size_t) b * Hn + j));
         __syncthreads();
         for (int b = 0; b < B; b++) {
             if (t >= s_T[b]) continue;
@@ -728,17 +774,18 @@ __global__ void __launch_bounds__(UPB * 4 * 32) lstm_recur_kernel(const float * 
             const float gt = glibc_tanhf_dev(g[2 * UPB + uu]);
             const float ot = sigmoid_exact(g[3 * UPB + uu]);
             c_state = __fadd_rn(__fmul_rn(ft, c_state), __fmul_rn(it, gt));
-            const float h = __fmul_rn(ot, glibc_tanhf_dev(c_state));
+            h = __fmul_rn(ot, glibc_tanhf_dev(c_state));
             __stcg(hbuf + (size_t)(t & 1) * B * Hn + (size_t) b * Hn + un, h);
             const size_t o = (size_t) Hn * my_base + (size_t) un * my_T + t;
             out[o] = skip ? __fadd_rn(skip[o], h) : h;                                                     // decoder.h:72 inpL + out
         }
         grid_barrier(counter, (unsigned)(t + 1) * gridDim.x);
     }
+    if (my_state && my_T > 0) { my_state[my_unit] = h; my_state[Hn + my_unit] = c_state; }
 }
 
 int lstm_layer(const float * x, int C, const int * T, int n, const __half * wih_li, const __half * whh_li, int Kp, const float * bih, const float * bhh,
-               const float * skip, float * gi_scratch, float * hbuf, unsigned * counter, float * out, cudaStream_t s) {
+               const float * skip, float * gi_scratch, float * hbuf, unsigned * counter, float * out, cudaStream_t s, float * const * state) {
     const int Hn = C, G4 = 4 * Hn;
     if (Hn % 32 != 0 || Hn > 512 || Hn % 4 != 0) { fprintf(stderr, "bark_b200: unsupported LSTM width %d\n", Hn); throw std::runtime_error("unsupported configuration (see the message above)"); }
     const CodecItems it = codec_items(n, T, T, T, 8);
@@ -754,8 +801,9 @@ int lstm_layer(const float * x, int C, const int * T, int n, const __half * wih_
     const size_t smem = (size_t) n * (Hn + 4 * UPB) * sizeof(float);
     if (g_prof_on) prof_begin("lstm_recur_kernel", s, 0.0, 2.0 * (double) frames * G4 * Hn);
     if (n == 1) {
+        float * st = state ? state[0] : nullptr;
         void * args[] = {(void *) &gi_scratch, (void *) &T_max, (void *) &Hn, (void *) &whh_li, (void *) &Kp, (void *) &bhh, (void *) &skip, (void *) &hbuf,
-                         (void *) &counter, (void *) &out};
+                         (void *) &counter, (void *) &out, (void *) &st};
         BARK_CUDA_CHECK(cudaLaunchCooperativeKernel((const void *) lstm_recur_one_kernel<UPB>, dim3(blocks), dim3(UPB * 4 * 32), args, smem, s));
     } else {
         // The attribute belongs to the function on the device, shared by every context and thread: set once, to the largest launch
@@ -764,8 +812,10 @@ int lstm_layer(const float * x, int C, const int * T, int n, const __half * wih_
         if (first_use_on_this_device(configured))
             BARK_CUDA_CHECK(cudaFuncSetAttribute(lstm_recur_kernel<UPB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                  (int)((size_t) kCodecMaxItems * (512 + 4 * UPB) * sizeof(float))));
+        LstmState st{};
+        for (int b = 0; b < n && state; b++) st.p[b] = state[b];
         void * args[] = {(void *) &gi_scratch, (void *) &T_max, (void *) &Hn, (void *) &whh_li, (void *) &Kp, (void *) &bhh, (void *) &skip, (void *) &hbuf,
-                         (void *) &counter, (void *) &out, (void *) &it};
+                         (void *) &counter, (void *) &out, (void *) &it, (void *) &st};
         BARK_CUDA_CHECK(cudaLaunchCooperativeKernel((const void *) lstm_recur_kernel<UPB>, dim3(blocks), dim3(UPB * 4 * 32), args, smem, s));
     }
     if (g_prof_on) prof_end(s);
@@ -783,6 +833,23 @@ __global__ void convtr_rows_kernel(const __half * __restrict__ src, __half * __r
 }
 void convtr_rows(const __half * src, __half * dst, int Cin, int Cout, int k, cudaStream_t s) {
     BARK_LAUNCH(convtr_rows_kernel, 592, 256, 0, s, src, dst, Cin, Cout, k);
+}
+
+// job blockIdx.y of a ColumnCopies, its rows x cols elements spread over the blocks of x
+__global__ void copy_columns_kernel(const __grid_constant__ ColumnCopies c, int rows) {
+    const int j = blockIdx.y, cols = c.cols[j];
+    const long long total = (long long) rows * cols;
+    for (long long i = (long long) blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long) gridDim.x * blockDim.x) {
+        const long long r = i / cols, k = i % cols;
+        c.dst[j][r * c.dst_ld[j] + k] = c.src[j][r * c.src_ld[j] + k];
+    }
+}
+
+void copy_columns(const ColumnCopies & c, int rows, cudaStream_t s) {
+    if (c.n == 0) return;
+    long long most = 0;
+    for (int j = 0; j < c.n; j++) most = std::max(most, (long long) rows * c.cols[j]);
+    BARK_LAUNCH(copy_columns_kernel, dim3((unsigned) std::min<long long>(std::max<long long>((most + 255) / 256, 1), 256), c.n), 256, 0, s, c, rows);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -22,16 +22,31 @@ bool rvq_encode(const float * const * embed, const float * const * norms, int n_
 // The kernel a convolution launcher ran: conv1d_short_kernel, conv1d_lane_kernel<KW, NG> as kConvLane + 10 KW + NG, conv1d_stream_kernel<KW,
 // STRIDE> as kConvStream + 100 KW + STRIDE; the LSTM recurrence of one item or of several.  The pipeline ignores them; the tests count them.
 constexpr int kConvShort = 1, kConvLane = 1000, kConvStream = 10000, kLstmOne = 1, kLstmBatched = 2;
+// A window of each item's signal (the streams of codec_stream.cu): item b's input columns [C][L_b] are the global positions org[b] ..
+// org[b] + L_b - 1 of its signal, and the launch computes the n_out[b] outputs from global output first[b] on, [Cout][n_out[b]] per item.
+// The reflections apply where the global position is outside the signal: below 0 on the left, past the window's last column on the
+// right (a window ends where its signal ends, or its outputs read no further).  A launcher without a window runs whole signals:
+// org = first = 0 and every output.  Outputs that read outside a window are refused.
+struct CodecWindow { long long org[kCodecMaxItems] = {}, first[kCodecMaxItems] = {}; int n_out[kCodecMaxItems] = {}; };
 // strided_conv_1d (ops.cpp:59-75) on x [Cin][L_b]: ELU on the input when elu_in, resid added to the output (stride 1 only).
 // y is [Cout][conv1d_out_len(L_b, k, stride)]; the launcher picks the kernel from the contraction length and the stride.
-int conv1d(const float * x, int Cin, const int * L, int n, const ConvW & cv, bool elu_in, const float * resid, float * y, cudaStream_t s, int stride = 1);
+int conv1d(const float * x, int Cin, const int * L, int n, const ConvW & cv, bool elu_in, const float * resid, float * y, cudaStream_t s, int stride = 1,
+           const CodecWindow * win = nullptr);
 int conv1d_out_len(int T, int k, int stride);
-// returns the NG of the convtr1d_lane_kernel<NG> it ran
-int convtr1d(const float * x, int Cin, const int * L, int n, const ConvW & cv, int stride, float * y /*[Cout][L_b*stride]*/, cudaStream_t s);
-// returns kLstmOne or kLstmBatched
+// returns the NG of the convtr1d_lane_kernel<NG> it ran.  With a window, output block t reads input frames t - 1 and t: a window from
+// first[b] > 0 on starts with frame first[b] - 1.
+int convtr1d(const float * x, int Cin, const int * L, int n, const ConvW & cv, int stride, float * y /*[Cout][L_b*stride]*/, cudaStream_t s,
+             const CodecWindow * win = nullptr);
+// returns kLstmOne or kLstmBatched.  state (may be null, as may its entries): item b's (h, c) [2][C] before its first step, zeros where
+// null, and after its last step (not touched for T_b = 0)
 int lstm_layer(const float * x, int C, const int * T, int n, const __half * wih_li, const __half * whh_li, int Kp, const float * bih, const float * bhh,
                const float * skip, float * gi_scratch /*[T_b][4C]*/, float * hbuf /*[2][kCodecMaxItems][C]*/, unsigned * counter, float * out,
-               cudaStream_t s);
+               cudaStream_t s, float * const * state = nullptr);
+// Copies of column blocks between device matrices of `rows` rows, all in one launch: job j copies [rows][cols[j]] from src[j] (row
+// stride src_ld[j]) to dst[j] (row stride dst_ld[j]).  The streams' windows and histories move through it.
+constexpr int kColumnCopyJobs = 2 * kCodecMaxItems;
+struct ColumnCopies { int n = 0; const float * src[kColumnCopyJobs]; float * dst[kColumnCopyJobs]; int src_ld[kColumnCopyJobs], dst_ld[kColumnCopyJobs], cols[kColumnCopyJobs]; };
+void copy_columns(const ColumnCopies & c, int rows, cudaStream_t s);
 // load-time re-layout of a transposed-conv weight: [Cin][Cout][k] -> rows [Cout][k][Cin]
 void convtr_rows(const __half * src, __half * dst, int Cin, int Cout, int k, cudaStream_t s);
 

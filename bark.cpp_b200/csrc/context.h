@@ -191,6 +191,34 @@ bool codec_encode(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, int 
 bool resample_input_ok(const char * fn, const std::string & item, const float * x, int n_frames, int channels, int sample_rate);
 // "item i: " in the messages of a batch call (batch_fn set), whatever its size; nothing for a single call, whose messages stay as they were
 std::string item_tag(const char * batch_fn, int i);
+// sizes sc for one launch of `frames` frames of n_q codebooks: false (message naming caller) when the device is out of memory
+bool codec_scratch(CodecScratch & sc, size_t frames, int n_q, const char * caller);
+
+// codec_stream.cu — streaming EnCodec (DESIGN.md §19).  A stream goes one way: mono 24 kHz samples to codes, or codes to samples, at the
+// n_q it opened with.  Its state lives on the device: per windowed layer the input columns later outputs still read, per LSTM layer
+// (h, c).  Pending outputs wait on the host until read: codes frame-major [k][n_q], or samples.
+constexpr int kStreamEncode = 0, kStreamDecode = 1;
+// the outputs final after n inputs, before finish: frames after n samples (encode), samples after n frames (decode)
+long long codec_stream_ready(int direction, long long n);
+struct CodecStream {
+    int direction = kStreamEncode, n_q = 0;
+    bool finished = false, failed = false;               // failed: a pass did not complete (a CUDA failure); the state is lost
+    long long n_in = 0, n_out = 0;                       // inputs pushed, outputs final
+    struct Window { int C = 0, cap = 0, h = 0; long long in = 0, out = 0; float * hist = nullptr; };   // hist [C][cap], h columns held
+    std::vector<Window> win;                             // in layer-list order
+    float * lstm[4] = {nullptr, nullptr, nullptr, nullptr};   // (h, c) [2][512] of the four LSTM layers (two for the direction's model)
+    float * mem = nullptr;                               // the device allocation behind win and lstm
+    std::vector<int32_t> codes;
+    std::vector<float> audio;
+    void release();
+};
+// allocates st's device state for direction at n_q codebooks (a CUDA failure throws)
+bool codec_stream_init(const CodecModel & cm, CodecStream & st, int direction, int n_q);
+// pushes n[i] inputs at in[i] (samples, or codes [n_q][n[i]]) to the count <= kCodecMaxItems checked streams st[i] of one model and
+// direction in one pass of the kernels (or several for a long push), or with finish none, closing them.  Returns the outputs that
+// became final, -1 (message naming fn) on a failure.
+int codec_stream_run(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, CodecStream * const * st, const void * const * in, const int * n, int count,
+                     bool finish, const char * fn);
 
 // sampling.cu
 constexpr int kSampleMaxLogits = 16384;          // logits of one row: sample_rows_kernel holds the row in 64 KB of shared memory

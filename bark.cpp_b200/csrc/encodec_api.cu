@@ -2,10 +2,12 @@
 // stream, the codec weights with all the file's codebooks and their norms, the codec scratch and the output vectors, and no GPT.
 // Semantics follow encodec.cpp/encodec.cpp:933-1050; the inputs the reference asserts on or cannot run are refused with a message.
 #include "../../include/encodec.h"
+#include "../../include/bark_b200.h"
 #include "context.h"
 #include "codec_kernels.h"
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstring>
 
@@ -234,4 +236,133 @@ extern "C" void encodec_free(struct encodec_context * e) {
     e->scratch.release();
     if (e->stream) cudaStreamDestroy(e->stream);
     delete e;
+}
+
+// ---- streaming (include/bark_b200.h, STREAMING ENCODEC; DESIGN.md §19) ----------------------------------------------------------
+static_assert(BARK_B200_STREAM_MAX_BATCH == kCodecMaxItems, "a batch of streams is one pass of the codec kernels");
+struct bark_b200_encodec_stream {
+    encodec_context * e;
+    CodecStream st;
+};
+
+namespace {
+
+// The checks of a push or finish on `count` streams (after which nothing can refuse it): false (message naming fn) for a null or
+// repeated stream, streams of several contexts or directions, a finished stream, or a count outside [1, kCodecMaxItems]; with in and n,
+// a null chunk, a negative count, a non-finite sample or a code outside the codebooks
+bool stream_args(const char * fn, bark_b200_encodec_stream * const * s, const void * const * in, const int * n, int count) {
+    if (!s || count < 1 || count > kCodecMaxItems) { fprintf(stderr, "%s: %d streams (1 to %d per call)\n", fn, s ? count : 0, kCodecMaxItems); return false; }
+    for (int i = 0; i < count; i++) {
+        const std::string tag = count > 1 ? "stream " + std::to_string(i) + ": " : std::string();
+        if (!s[i]) { fprintf(stderr, "%s: %snull stream\n", fn, tag.c_str()); return false; }
+        for (int j = 0; j < i; j++) if (s[j] == s[i]) { fprintf(stderr, "%s: stream %d is stream %d again\n", fn, i, j); return false; }
+        if (s[i]->e != s[0]->e || s[i]->st.direction != s[0]->st.direction) { fprintf(stderr, "%s: %sanother context or direction than stream 0\n", fn, tag.c_str()); return false; }
+        if (s[i]->st.finished) { fprintf(stderr, "%s: %sthe stream is finished\n", fn, tag.c_str()); return false; }
+        if (s[i]->st.failed) { fprintf(stderr, "%s: %sthe stream failed earlier and has lost its state\n", fn, tag.c_str()); return false; }
+        if (!in) continue;
+        if (!in[i] || n[i] < 0) { fprintf(stderr, "%s: %s%s\n", fn, tag.c_str(), in[i] ? "negative count" : "null input"); return false; }
+        const CodecStream & t = s[i]->st;
+        if (t.direction == kStreamEncode) {
+            const float * x = (const float *) in[i];
+            for (int k = 0; k < n[i]; k++) if (!std::isfinite(x[k])) { fprintf(stderr, "%s: %ssample %d is not finite (%g)\n", fn, tag.c_str(), k, (double) x[k]); return false; }
+        } else {
+            const int32_t * c = (const int32_t *) in[i];
+            const int bins = s[i]->e->model.n_bins;
+            for (size_t k = 0; k < (size_t) t.n_q * n[i]; k++) if (c[k] < 0 || c[k] >= bins) {
+                fprintf(stderr, "%s: %scode %d (codebook %zu, frame %zu) is outside the codebooks (%d bins)\n", fn, tag.c_str(), c[k], k / n[i], k % n[i], bins);
+                return false;
+            }
+        }
+    }
+    return true;
+}
+
+// the stream calls: the context's device current, a CUDA failure or exception is `fail`; the context's statistics are left alone
+template <typename R, typename F> R stream_call(bark_b200_encodec_stream * s, R fail, F && f) {
+    return guarded(fail, [&]() -> R { BARK_CUDA_CHECK(cudaSetDevice(s->e->device)); return f(); });
+}
+
+int push(const char * fn, bark_b200_encodec_stream * const * s, const void * const * in, const int * n, int count) {
+    if (!in || !n) { fprintf(stderr, "%s: null %s\n", fn, in ? "count array" : "input array"); return -1; }
+    if (!stream_args(fn, s, in, n, count)) return -1;
+    std::vector<CodecStream *> st((size_t) count);
+    for (int i = 0; i < count; i++) st[(size_t) i] = &s[i]->st;
+    return stream_call(s[0], -1, [&] { return codec_stream_run(s[0]->e->model, s[0]->e->scratch, s[0]->e->stream, st.data(), in, n, count, false, fn); });
+}
+
+}  // namespace
+
+extern "C" struct bark_b200_encodec_stream * bark_b200_encodec_stream_open(struct encodec_context * e, int direction) {
+    const char * fn = __func__;
+    if (!e) { fprintf(stderr, "%s: null context\n", fn); return nullptr; }
+    if (direction != BARK_B200_STREAM_ENCODE && direction != BARK_B200_STREAM_DECODE) { fprintf(stderr, "%s: unknown direction %d\n", fn, direction); return nullptr; }
+    if (direction == BARK_B200_STREAM_ENCODE && !e->model.enc.present) { fprintf(stderr, "%s: the model file has no EnCodec encoder tensors (encoder.*)\n", fn); return nullptr; }
+    int n_q;
+    if (!codebooks_for(e, fn, &n_q)) return nullptr;
+    auto * s = new bark_b200_encodec_stream{e, CodecStream()};
+    if (!guarded(false, [&] { BARK_CUDA_CHECK(cudaSetDevice(e->device)); return codec_stream_init(e->model, s->st, direction, n_q); })) {
+        fprintf(stderr, "%s: could not allocate the stream's state\n", fn);
+        bark_b200_encodec_stream_close(s);
+        return nullptr;
+    }
+    return s;
+}
+
+extern "C" int bark_b200_encodec_stream_push(struct bark_b200_encodec_stream * s, const void * in, int n) {
+    return push(__func__, &s, &in, &n, 1);
+}
+
+extern "C" int bark_b200_encodec_stream_push_batch(struct bark_b200_encodec_stream * const * s, const void * const * in, const int * n, int count) {
+    return push(__func__, s, in, n, count);
+}
+
+extern "C" int bark_b200_encodec_stream_read(struct bark_b200_encodec_stream * s, void * out, int cap) {
+    if (!s) { fprintf(stderr, "%s: null stream\n", __func__); return -1; }
+    CodecStream & t = s->st;
+    const size_t per = t.direction == kStreamEncode ? (size_t) t.n_q : 1, ready = (t.direction == kStreamEncode ? t.codes.size() : t.audio.size()) / per;
+    const size_t k = std::min(ready, (size_t) std::max(cap, 0));
+    if (!out) return (int) std::min(ready, (size_t) INT_MAX);
+    if (t.direction == kStreamDecode) {
+        std::copy_n(t.audio.begin(), k, (float *) out);
+        t.audio.erase(t.audio.begin(), t.audio.begin() + (ptrdiff_t) k);
+    } else {                                             // frame-major pending -> [n_q][k]
+        int32_t * o = (int32_t *) out;
+        for (size_t f = 0; f < k; f++)
+            for (size_t q = 0; q < per; q++) o[q * k + f] = t.codes[f * per + q];
+        t.codes.erase(t.codes.begin(), t.codes.begin() + (ptrdiff_t)(k * per));
+    }
+    return (int) k;
+}
+
+extern "C" int bark_b200_encodec_stream_finish(struct bark_b200_encodec_stream * s) {
+    const char * fn = __func__;
+    if (!stream_args(fn, &s, nullptr, nullptr, 1)) return -1;
+    const CodecStream & t = s->st;
+    if (t.direction == kStreamEncode ? t.n_in < kCodecMinSamples : t.n_in < kCodecMinFrames) {
+        fprintf(stderr, "%s: need at least %d %s (reflect padding of the k=7 convolutions), got %lld\n", fn, t.direction == kStreamEncode ? kCodecMinSamples : kCodecMinFrames,
+                t.direction == kStreamEncode ? "samples" : "frames", t.n_in);
+        return -1;
+    }
+    CodecStream * st = &s->st;
+    const int zero = 0;
+    const void * none = nullptr;
+    return stream_call(s, -1, [&] { return codec_stream_run(s->e->model, s->e->scratch, s->e->stream, &st, &none, &zero, 1, true, fn); });
+}
+
+extern "C" long long bark_b200_encodec_stream_ready(int direction, long long n) {
+    if ((direction != BARK_B200_STREAM_ENCODE && direction != BARK_B200_STREAM_DECODE) || n < 0) return -1;
+    return codec_stream_ready(direction, n);
+}
+
+extern "C" int bark_b200_encodec_stream_codebooks(struct bark_b200_encodec_stream * s) {
+    if (!s) { fprintf(stderr, "%s: null stream\n", __func__); return -1; }
+    return s->st.n_q;
+}
+
+extern "C" void bark_b200_encodec_stream_close(struct bark_b200_encodec_stream * s) {
+    if (!s) return;
+    cudaSetDevice(s->e->device);
+    if (s->e->stream) cudaStreamSynchronize(s->e->stream);
+    s->st.release();
+    delete s;
 }

@@ -560,6 +560,92 @@ extern "C" int bark_b200_codec_lstm(const float * x, int C, const int * T, int n
     });
 }
 
+// A CodecWindow from the hook's arrays; false (message naming fn) for a null array or an item without outputs
+static bool hook_window(const char * fn, int n, const long long * org, const long long * first, const int * n_out, CodecWindow * w, size_t * out_total) {
+    if (!org || !first || !n_out) { fprintf(stderr, "%s: null window array\n", fn); return false; }
+    *out_total = 0;
+    for (int b = 0; b < n; b++) {
+        if (n_out[b] < 1) { fprintf(stderr, "%s: item %d has %d outputs (at least 1)\n", fn, b, n_out[b]); return false; }
+        w->org[b] = org[b]; w->first[b] = first[b]; w->n_out[b] = n_out[b]; *out_total += (size_t) n_out[b];
+    }
+    return true;
+}
+
+// conv1d over windows (the launcher refuses a window whose outputs read outside it)
+extern "C" int bark_b200_codec_conv1d_window(const float * x, int Cin, const int * L, int n, const long long * org, const long long * first, const int * n_out,
+                                             const uint16_t * w, const float * bias, int Cout, int k, int stride, int elu_in, const float * resid, float * y) {
+    return guarded(0, [&] {
+        const char * fn = "bark_b200_codec_conv1d_window";
+        size_t total = 0, out_total = 0;
+        if (!x || !w || !bias || !y || Cin < 1 || Cout < 1 || k < 1 || stride < 1 || stride > k || (resid && stride > 1)) { fprintf(stderr, "%s: invalid arguments\n", fn); return 0; }
+        CodecWindow win;
+        if (!codec_lengths(fn, L, n, 1, &total) || !hook_window(fn, n, org, first, n_out, &win, &out_total)) return 0;
+        DeviceBuffers mem;
+        ConvW cv; cv.k = k; cv.cin = Cin; cv.cout = Cout;
+        cv.w = li_weight(mem, mem.upload((const __half *) w, (size_t) Cout * Cin * k * 2), Cout, Cin * k, &cv.Kp);
+        cv.b = mem.upload(bias, (size_t) Cout * 4);
+        const float * dx = mem.upload(x, total * Cin * 4), * dr = resid ? mem.upload(resid, out_total * Cout * 4) : nullptr;
+        const GuardedOutput o(mem, out_total * Cout * 4, nullptr);
+        const int ran = conv1d(dx, Cin, L, n, cv, elu_in != 0, dr, o.out<float>(), 0, stride, &win);
+        if (!finish(fn)) return 0;
+        return o.read(fn, y) ? ran : -1;
+    });
+}
+
+// convtr1d over windows
+extern "C" int bark_b200_codec_convtr1d_window(const float * x, int Cin, const int * L, int n, const long long * org, const long long * first, const int * n_out,
+                                               const uint16_t * w, const float * bias, int Cout, int stride, float * y) {
+    return guarded(0, [&] {
+        const char * fn = "bark_b200_codec_convtr1d_window";
+        size_t total = 0, out_total = 0;
+        if (!x || !w || !bias || !y || Cin < 1 || Cout < 1 || stride < 1) { fprintf(stderr, "%s: invalid arguments\n", fn); return 0; }
+        CodecWindow win;
+        if (!codec_lengths(fn, L, n, 1, &total) || !hook_window(fn, n, org, first, n_out, &win, &out_total)) return 0;
+        const int k = 2 * stride;
+        DeviceBuffers mem;
+        ConvW cv; cv.k = k; cv.cin = Cin; cv.cout = Cout;
+        __half * rows = mem.alloc<__half>((size_t) Cin * Cout * k * 2);
+        convtr_rows(mem.upload((const __half *) w, (size_t) Cin * Cout * k * 2), rows, Cin, Cout, k, 0);
+        cv.w = li_weight(mem, rows, Cout * k, Cin, &cv.Kp);
+        cv.b = mem.upload(bias, (size_t) Cout * 4);
+        const float * dx = mem.upload(x, total * Cin * 4);
+        const GuardedOutput o(mem, out_total * stride * Cout * 4, nullptr);
+        const int ran = convtr1d(dx, Cin, L, n, cv, stride, o.out<float>(), 0, &win);
+        if (!finish(fn)) return 0;
+        return o.read(fn, y) ? ran : -1;
+    });
+}
+
+// lstm_layer from a state [n][2][C] (null: zeros), written back
+extern "C" int bark_b200_codec_lstm_state(const float * x, int C, const int * T, int n, const uint16_t * wih, const uint16_t * whh, const float * bih,
+                                          const float * bhh, const float * skip, float * state, float * out) {
+    return guarded(0, [&] {
+        const char * fn = "bark_b200_codec_lstm_state";
+        size_t total = 0;
+        if (!x || !wih || !whh || !bih || !bhh || !out || C < 1) { fprintf(stderr, "%s: invalid arguments\n", fn); return 0; }
+        if (!codec_lengths(fn, T, n, 1, &total)) return 0;
+        const size_t G4 = (size_t) 4 * C, sb = (size_t) n * 2 * C * 4;
+        DeviceBuffers mem;
+        int Kp = 0;
+        const __half * dih = li_weight(mem, mem.upload((const __half *) wih, G4 * C * 2), (int) G4, C, &Kp);
+        const __half * dhh = li_weight(mem, mem.upload((const __half *) whh, G4 * C * 2), (int) G4, C, &Kp);
+        const float * dbi = mem.upload(bih, G4 * 4), * dbh = mem.upload(bhh, G4 * 4);
+        const float * dx = mem.upload(x, total * C * 4), * ds = skip ? mem.upload(skip, total * C * 4) : nullptr;
+        float * gi = mem.poisoned<float>(total * G4 * 4), * hbuf = mem.poisoned<float>((size_t) 2 * kCodecMaxItems * C * 4);
+        unsigned * counter = mem.alloc<unsigned>(sizeof(unsigned));
+        std::vector<float> zeros;
+        if (!state) zeros.assign((size_t) n * 2 * C, 0.f);
+        float * dst = mem.upload(state ? state : zeros.data(), sb);
+        std::vector<float *> per((size_t) n);
+        for (int b = 0; b < n; b++) per[(size_t) b] = dst + (size_t) b * 2 * C;
+        const GuardedOutput o(mem, total * C * 4, nullptr);
+        const int ran = lstm_layer(dx, C, T, n, dih, dhh, Kp, dbi, dbh, ds, gi, hbuf, counter, o.out<float>(), 0, per.data());
+        if (!finish(fn)) return 0;
+        if (state) download(state, dst, sb);
+        return o.read(fn, out) ? ran : -1;
+    });
+}
+
 // rvq_decode on n items of codes [n_q][T_b] through codebooks [n_q][n_bins][hidden] -> x [hidden][T_b]
 extern "C" int bark_b200_codec_rvq_decode(const int32_t * codes, int n_q, const int * T, int n, const float * codebooks, int hidden, int n_bins, float * x) {
     return guarded(0, [&] {

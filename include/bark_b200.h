@@ -277,6 +277,45 @@ BARK_API int  bark_b200_encodec_encode_resampled(struct bark_context * ctx, cons
                                                  int codes_cap, float * latent, int latent_cap);
 BARK_API int  bark_b200_resample(const float * in, int n_frames, int channels, int in_rate, int out_rate, float * out, int cap);
 
+/* STREAMING ENCODEC on an encodec_context (DESIGN.md §19): code live audio chunk by chunk, or play codes as they arrive.  A stream goes one
+ * way, BARK_B200_STREAM_ENCODE (mono 24 kHz samples in, codes out) or BARK_B200_STREAM_DECODE (codes in, samples out), at the n_q of the
+ * context's bandwidth when it opens; a later encodec_set_target_bandwidth does not touch it.  Pushes take chunks of any size, 0 included,
+ * and a stream hands back each output as soon as no later input can change it.  Everything a stream returns, up to and including
+ * finish, is bit-identical to the single call on all its input: encodec_compress_audio's codes [n_q][ceil(n / 320)] for an encode,
+ * encodec_decompress_audio's 320 T samples for a decode, whatever the chunk sizes and whatever else runs on the context in between.
+ *   encode: after n samples, frames 0 .. n / 320 - 1 are final once n >= 2240 (7 frames), none before; finish adds the last
+ *           ceil(n / 320) - floor(n / 320) frames, padded on the right as the whole clip is, and refuses n < 1921.
+ *   decode: after T >= 7 frames all 320 T samples are final, none before; finish adds nothing and refuses T < 7.
+ * bark_b200_encodec_stream_ready(direction, n) is that rule: the outputs final after n inputs before finish (-1 for an unknown direction
+ * or n < 0).  A stream's state is a few columns per layer on the device and its counters are 64-bit: it may run for hours.  Streams
+ * leave the context's codes, audio and statistics alone, and the context's other calls leave streams alone.
+ *   bark_b200_encodec_stream_open ........ NULL with a message for a null context, an unknown direction, an encode without encoder tensors
+ *                                          or a bandwidth the file cannot give
+ *   bark_b200_encodec_stream_push ........ encode: in = n float samples; decode: in = n frames of codes [n_q][n], codebook-major.  Returns
+ *                                          the outputs that became final (frames, or samples), waiting for read; -1 refused
+ *   bark_b200_encodec_stream_push_batch .. count <= 32 streams of one context and one direction in one pass of the kernels, stream i
+ *                                          pushed in[i], n[i]; each gets exactly what its own push would have.  Returns the sum
+ *   bark_b200_encodec_stream_read ........ takes k = min(ready, cap) final outputs to out: codes [n_q][k] for k frames, or k samples;
+ *                                          returns k (out NULL: only returns the count ready, taking nothing), -1 for a null stream
+ *   bark_b200_encodec_stream_finish ...... ends the stream: returns the outputs it added, -1 refused (the stream is unchanged)
+ *   bark_b200_encodec_stream_codebooks ... the stream's n_q
+ *   bark_b200_encodec_stream_close ....... frees the stream; close every stream before encodec_free of its context
+ * A push or finish is refused with a message, leaving every stream of the call exactly as it was, for a null argument, a negative count,
+ * a non-finite sample, a code outside [0, n_bins), a finished stream, or a batch that mixes contexts or directions, repeats a stream or
+ * holds more than 32.  The refused call followed by the corrected one gives the same bits as the corrected one alone. */
+#define BARK_B200_STREAM_ENCODE 0
+#define BARK_B200_STREAM_DECODE 1
+#define BARK_B200_STREAM_MAX_BATCH 32
+struct bark_b200_encodec_stream;
+BARK_API struct bark_b200_encodec_stream * bark_b200_encodec_stream_open(struct encodec_context * e, int direction);
+BARK_API int  bark_b200_encodec_stream_push(struct bark_b200_encodec_stream * s, const void * in, int n);
+BARK_API int  bark_b200_encodec_stream_push_batch(struct bark_b200_encodec_stream * const * s, const void * const * in, const int * n, int count);
+BARK_API int  bark_b200_encodec_stream_read(struct bark_b200_encodec_stream * s, void * out, int cap);
+BARK_API int  bark_b200_encodec_stream_finish(struct bark_b200_encodec_stream * s);
+BARK_API long long bark_b200_encodec_stream_ready(int direction, long long n);
+BARK_API int  bark_b200_encodec_stream_codebooks(struct bark_b200_encodec_stream * s);
+BARK_API void bark_b200_encodec_stream_close(struct bark_b200_encodec_stream * s);
+
 /* FAST MODE (BARK_B200_MODE=fast in the environment at load; opt-in, NOT bit-identical to the reference): the fine model's
  * 1024-row passes (bark.cpp:1416-1584) run as wgmma tensor-core GEMMs + flash-style attention (csrc/fast_kernels.cu).
  * Every weight type the loader reads runs it: an f16 file's fine matrices are used as stored; those of an f32, q4_0, q4_1, q5_0, q5_1
@@ -387,6 +426,21 @@ BARK_API int  bark_b200_codec_lstm(const float * x, int C, const int * T, int n,
                                    const float * bhh, const float * skip, float * out);
 BARK_API int  bark_b200_codec_rvq_decode(const int32_t * codes, int n_q, const int * T, int n, const float * codebooks, int hidden, int n_bins, float * x);
 BARK_API int  bark_b200_device_math(int fn, uint32_t lo_bits, uint32_t stride, uint32_t count, float * out);
+/* The same launchers over a window of each item's signal, as the streams run them (DESIGN.md §19): item b's columns [C][L_b] are the
+ * global positions org[b] .. org[b] + L_b - 1 of its signal, and outputs first[b] .. first[b] + n_out[b] - 1 are computed, concatenated as
+ * [Cout][n_out[b]] (the transposed conv: [Cout][n_out[b] stride], output frames of input frames).  Reflections apply where the global
+ * position is outside the signal: below 0, and (strided convs) past the window's last column.  A window whose outputs read a column it
+ * does not hold is refused.  Each equals the matching slice of the whole-signal hook's result.
+ *   bark_b200_codec_conv1d_window .... bark_b200_codec_conv1d over windows; resid [Cout][n_out[b]] (stride 1, may be NULL)
+ *   bark_b200_codec_convtr1d_window .. bark_b200_codec_convtr1d over windows; output frame t reads frames t - 1 (none for t = 0) and t
+ *   bark_b200_codec_lstm_state ....... bark_b200_codec_lstm from the state (h, c) [n][2][C] (NULL: zeros), which on return holds each
+ *                                      item's state after its last step */
+BARK_API int  bark_b200_codec_conv1d_window(const float * x, int Cin, const int * L, int n, const long long * org, const long long * first, const int * n_out,
+                                            const uint16_t * w, const float * bias, int Cout, int k, int stride, int elu_in, const float * resid, float * y);
+BARK_API int  bark_b200_codec_convtr1d_window(const float * x, int Cin, const int * L, int n, const long long * org, const long long * first, const int * n_out,
+                                              const uint16_t * w, const float * bias, int Cout, int stride, float * y);
+BARK_API int  bark_b200_codec_lstm_state(const float * x, int C, const int * T, int n, const uint16_t * wih, const uint16_t * whh, const float * bih,
+                                         const float * bhh, const float * skip, float * state, float * out);
 
 #ifdef __cplusplus
 }
