@@ -133,6 +133,7 @@ EXPORTS = [
     "bark_b200_encodec_stream_open", "bark_b200_encodec_stream_push", "bark_b200_encodec_stream_push_batch", "bark_b200_encodec_stream_read",
     "bark_b200_encodec_stream_finish", "bark_b200_encodec_stream_ready", "bark_b200_encodec_stream_codebooks", "bark_b200_encodec_stream_close",
     "bark_b200_codec_conv1d_window", "bark_b200_codec_convtr1d_window", "bark_b200_codec_lstm_state",
+    "bark_b200_encodec_stream_open_resampled", "bark_b200_encodec_stream_ready_resampled", "bark_b200_resample_window",
     "ggml_time_init", "ggml_time_us", "ggml_time_ms", "ggml_init", "ggml_free",
 ]
 
@@ -253,6 +254,12 @@ def lib() -> C.CDLL:
         getattr(L, n).argtypes = [vp]
     L.bark_b200_encodec_stream_ready.restype = C.c_longlong
     L.bark_b200_encodec_stream_ready.argtypes = [C.c_int, C.c_longlong]
+    L.bark_b200_encodec_stream_open_resampled.restype = vp
+    L.bark_b200_encodec_stream_open_resampled.argtypes = [vp, C.c_int, C.c_int, C.c_int]
+    L.bark_b200_encodec_stream_ready_resampled.restype = C.c_longlong
+    L.bark_b200_encodec_stream_ready_resampled.argtypes = [C.c_int, C.c_int, C.c_longlong]
+    L.bark_b200_resample_window.restype = C.c_int
+    L.bark_b200_resample_window.argtypes = [f32p, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int, f32p]
     L.bark_b200_encodec_stream_close.restype = None
     L.bark_b200_encodec_stream_close.argtypes = [vp]
     L.bark_b200_codec_rvq_decode.restype = C.c_int
@@ -992,6 +999,26 @@ def codec_lstm(xs, wih: np.ndarray, whh: np.ndarray, bih: np.ndarray, bhh: np.nd
     return (res, r) if return_kernel else res
 
 
+def resample_window(items) -> list:
+    """resample_kernel over windows (bark_b200_resample_window), all items in one launch.  items: dicts with frames (mono [n] or
+    interleaved [n][channels] float32, the global frames org ..), sr, new_sr, org, first, n_out and optionally end (the signal's
+    length; frames at or past it read as zeros).  Returns each item's outputs first .. first + n_out - 1, float32."""
+    fr = [np.ascontiguousarray(it["frames"], np.float32) for it in items]
+    n = len(items)
+    flat = np.ascontiguousarray(np.concatenate([f.ravel() for f in fr] + [np.zeros(1, np.float32)]))
+    ints = lambda v: np.ascontiguousarray(v, np.int32)          # noqa: E731
+    longs = lambda v: np.ascontiguousarray(v, np.int64)         # noqa: E731
+    nf = ints([f.shape[0] for f in fr])
+    ch = ints([1 if f.ndim == 1 else f.shape[1] for f in fr])
+    sr, nsr = ints([it["sr"] for it in items]), ints([it["new_sr"] for it in items])
+    o, f, no = _window([it["org"] for it in items], [it["first"] for it in items], [it["n_out"] for it in items])
+    end = longs([it.get("end", -1) for it in items])
+    y = np.zeros(max(int(no.sum()), 1), np.float32)
+    _codec_call(f"bark_b200_resample_window ({n} items)",
+                lib().bark_b200_resample_window(_p(flat), _p(nf), _p(ch), _p(sr), _p(nsr), _p(o), _p(f), _p(no), _p(end), n, _p(y)))
+    return np.split(y[:int(no.sum())], np.cumsum(no)[:-1])
+
+
 def _window(org, first, n_out):
     return tuple(np.ascontiguousarray(a, t) for a, t in ((org, np.int64), (first, np.int64), (n_out, np.int32)))
 
@@ -1305,10 +1332,11 @@ class Encodec:
         return out
 
     # ---- streams (bark_b200_encodec_stream_*): their outputs joined equal the whole-clip call on their input joined --------------
-    def stream(self, direction: str) -> "EncodecStream":
+    def stream(self, direction: str, sample_rate: int | None = None, channels: int | None = None) -> "EncodecStream":
         """A stream on this context: "encode" (mono 24 kHz samples in, codes out) or "decode" (codes in, samples out), at the n_q of the
-        current bandwidth."""
-        s = EncodecStream(self, direction)
+        current bandwidth.  With sample_rate or channels (bark_b200_encodec_stream_open_resampled, DESIGN.md §20), an encode takes
+        interleaved frames [n][channels] (or mono [n]) at sample_rate, and a decode (mono only) gives samples at sample_rate."""
+        s = EncodecStream(self, direction, sample_rate, channels)
         self._streams.append(s)
         return s
 
@@ -1328,11 +1356,16 @@ class EncodecStream:
     that became final: codes [n_q][k] int32 for an encode of float32 samples, float32 samples for a decode of codes [n_q][k]; finish()
     returns the rest.  Everything returned, joined, equals compress / decompress of everything pushed."""
 
-    def __init__(self, codec: "Encodec", direction: str):
+    def __init__(self, codec: "Encodec", direction: str, sample_rate: int | None = None, channels: int | None = None):
         self.direction = direction
-        self.handle = lib().bark_b200_encodec_stream_open(codec.ctx, STREAM_DIRECTIONS[direction])
+        self.sample_rate = CODEC_RATE if sample_rate is None else int(sample_rate)
+        self.channels = 1 if channels is None else int(channels)
+        if sample_rate is None and channels is None:
+            self.handle = lib().bark_b200_encodec_stream_open(codec.ctx, STREAM_DIRECTIONS[direction])
+        else:
+            self.handle = lib().bark_b200_encodec_stream_open_resampled(codec.ctx, STREAM_DIRECTIONS[direction], self.channels, self.sample_rate)
         if not self.handle:
-            raise RuntimeError(f"bark_b200_encodec_stream_open ({direction}) failed (see stderr)")
+            raise RuntimeError(f"bark_b200_encodec_stream_open ({direction}, {self.channels} channels at {self.sample_rate} Hz) failed (see stderr)")
         self.handle = C.c_void_p(self.handle)
         self.n_q = lib().bark_b200_encodec_stream_codebooks(self.handle)
 
@@ -1348,8 +1381,13 @@ class EncodecStream:
         self.close()
 
     def _chunk(self, x):
-        """x as the C call takes it: (array, count) of samples or of frames"""
-        if self.direction == "encode":
+        """x as the C call takes it: (array, count) of samples, of interleaved frames [n][channels], or of code frames"""
+        if self.direction == "encode" and self.channels > 1:
+            a = np.ascontiguousarray(x, np.float32)
+            if a.ndim != 2 or a.shape[1] != self.channels:
+                raise ValueError(f"encode stream of {self.channels} channels: frames must be [n][{self.channels}], got shape {a.shape}")
+            n = a.shape[0]
+        elif self.direction == "encode":
             a = np.ascontiguousarray(x, np.float32).ravel()
             n = a.size
         else:
@@ -1397,10 +1435,13 @@ def encodec_stream_push_batch(streams, chunks) -> list:
     return [s.read() for s in streams]
 
 
-def encodec_stream_ready(direction: str, n: int) -> int:
+def encodec_stream_ready(direction: str, n: int, sample_rate: int | None = None) -> int:
     """The outputs a stream has made final after n inputs, before finish (bark_b200_encodec_stream_ready): frames after n samples for
-    "encode", samples after n frames for "decode"."""
-    return int(lib().bark_b200_encodec_stream_ready(STREAM_DIRECTIONS[direction], int(n)))
+    "encode", samples after n frames for "decode".  With sample_rate, the rule of a stream at that rate
+    (bark_b200_encodec_stream_ready_resampled): frames after n frames at sample_rate, or samples at sample_rate after n frames."""
+    if sample_rate is None:
+        return int(lib().bark_b200_encodec_stream_ready(STREAM_DIRECTIONS[direction], int(n)))
+    return int(lib().bark_b200_encodec_stream_ready_resampled(STREAM_DIRECTIONS[direction], int(sample_rate), int(n)))
 
 
 def rvq_encode(latent: np.ndarray, codebooks: np.ndarray) -> np.ndarray:

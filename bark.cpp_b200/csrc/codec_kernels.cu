@@ -861,9 +861,23 @@ void copy_columns(const ColumnCopies & c, int rows, cudaStream_t s) {
 // ------------------------------------------------------------------------------------------------
 constexpr int kResampleW = 6, kResampleTile = 256, kResampleSmemFloats = 12224;     // outputs per CTA at most; input window within 48 KB
 
+void resample_rates(int sr, int new_sr, int * o, int * q, int * w) {
+    const int g = std::gcd(sr, new_sr);
+    *o = sr / g; *q = new_sr / g;
+    *w = sr == new_sr ? 0 : (int) std::ceil((double)(kResampleW * *o) / (std::min(*o, *q) * 0.99));
+}
+
 long long resample_len(long long n, int sr, int new_sr) {
     const long long g = std::gcd(sr, new_sr), o = sr / g, q = new_sr / g;
     return (q * n + o - 1) / o;
+}
+
+long long resample_ready(long long n, int sr, int new_sr) {
+    int o, q, w;
+    resample_rates(sr, new_sr, &o, &q, &w);
+    if (n < (long long) w + o) return sr == new_sr ? n : 0;
+    const __int128 r = (__int128) q * ((n - w) / o);                    // 96 n at most: saturates only past 2^56 frames
+    return r > LLONG_MAX ? LLONG_MAX : (long long) r;
 }
 
 std::vector<unsigned char> resample_table(int sr, int new_sr, ResampleTable * t) {
@@ -871,9 +885,9 @@ std::vector<unsigned char> resample_table(int sr, int new_sr, ResampleTable * t)
     r.sr = sr; r.new_sr = new_sr;
     std::vector<unsigned char> bytes;
     if (sr == new_sr) { r.tile = r.smem = kResampleTile; *t = r; return bytes; }
-    const int g = std::gcd(sr, new_sr), o = sr / g, q = new_sr / g;
+    int o, q, w;
+    resample_rates(sr, new_sr, &o, &q, &w);
     const double pi = 3.141592653589793, base = std::min(o, q) * 0.99, reach = (double)(kResampleW * o) / base, scale = base / o;
-    const int w = (int) std::ceil(reach);
     r.o = o; r.q = q; r.w = w;
     // h[j][m] in torchaudio's expression order (_get_sinc_resample_kernel) with the C library's sin and cos
     auto tap = [&](int j, int m) {
@@ -914,15 +928,19 @@ void resample_bind(ResampleTable & t, const void * dev) {
     t.taps = (const float *)((const int4 *) dev + t.q);
 }
 
-// One CTA per `tile` consecutive outputs.  The CTA finds the span of input its outputs read (the first input and tap count of each
-// output's phase), loads it once, down-mixed, into shared memory, and each thread then sums one output over its phase's taps, which
-// are read from global memory (the table stays in L2).  phase null: the identity, y = u.
-__global__ void __launch_bounds__(kResampleTile) resample_kernel(const float * __restrict__ x, long long n, int C, const int4 * __restrict__ phase,
-                                                                 const float * __restrict__ taps, int o, int q, int w, int tile, int L, float * __restrict__ y) {
-    extern __shared__ float su[];
-    __shared__ int window[2];
-    const long long i0 = (long long) blockIdx.x * tile, i = i0 + threadIdx.x, k0 = i0 / q;
-    const bool active = (int) threadIdx.x < tile && i < L;
+// The items of one launch (__grid_constant__, indexed in the parameter space): item b owns CTAs [tile0[b], tile0[b+1]), each of its
+// own tile of outputs.
+struct ResampleItems { int n; int tile0[kCodecMaxItems + 1]; ResampleWindow w[kCodecMaxItems]; };
+
+// One CTA per `tile` consecutive outputs of an item.  The CTA finds the span of input its outputs read (the first input and tap count
+// of each output's phase), loads it once, down-mixed, into shared memory, and each thread then sums one output over its phase's taps,
+// which are read from global memory (the table stays in L2).  Global input positions below 0 or at or past the end read as zeros,
+// the others come from the window's columns.  phase null: the identity, y = u.  cta: the CTA's index among the item's.
+__device__ __forceinline__ void resample_tile(const ResampleWindow & v, int cta, float * su, int * window) {
+    const int4 * __restrict__ phase = v.t.phase;
+    const int o = v.t.o, q = v.t.q, tile = v.t.tile, C = v.C;
+    const long long i0 = v.first + (long long) cta * tile, i = i0 + threadIdx.x, k0 = i0 / q;
+    const bool active = (int) threadIdx.x < tile && i < v.first + v.n_out;
     if (threadIdx.x == 0) { window[0] = INT_MAX; window[1] = INT_MIN; }
     __syncthreads();
     int4 p = make_int4(0, 1, 0, 0);
@@ -930,7 +948,7 @@ __global__ void __launch_bounds__(kResampleTile) resample_kernel(const float * _
     if (active && phase) {
         const long long k = i / q;
         p = phase[i - k * q];
-        r = (int)((k - k0) * o) + p.x - w;
+        r = (int)((k - k0) * o) + p.x - v.t.w;
     }
     if (active && p.y > 0) { atomicMin(&window[0], r); atomicMax(&window[1], r + p.y); }
     __syncthreads();
@@ -938,28 +956,60 @@ __global__ void __launch_bounds__(kResampleTile) resample_kernel(const float * _
     const long long g0 = k0 * o + lo;
     for (int s = threadIdx.x; s < span; s += blockDim.x) {
         const long long g = g0 + s;
-        float v = 0.0f;
-        if (g >= 0 && g < n) {
-            const float * f = x + g * C;
-            v = f[0];
-            for (int c = 1; c < C; c++) v = __fadd_rn(v, f[c]);
-            if (C > 1) v = __fdiv_rn(v, (float) C);
+        float u = 0.0f;
+        if (g >= 0 && g < v.end) {
+            const float * f = v.x + (g - v.org) * C;
+            u = f[0];
+            for (int c = 1; c < C; c++) u = __fadd_rn(u, f[c]);
+            if (C > 1) u = __fdiv_rn(u, (float) C);
         }
-        su[s] = v;
+        su[s] = u;
     }
     __syncthreads();
     if (!active) return;
-    if (!phase) { y[i] = su[r - lo]; return; }
-    const float * u = su + (r - lo), * h = taps + p.z;
+    float * y = v.y + (i - v.first);
+    if (!phase) { *y = su[r - lo]; return; }
+    const float * u = su + (r - lo), * h = v.t.taps + p.z;
     double acc = 0.0;
     for (int c = 0; c < p.y; c++) acc = __fma_rn((double) u[c], (double) h[c], acc);
-    y[i] = __double2float_rn(acc);
+    *y = __double2float_rn(acc);
+}
+
+// One item (every whole-clip call) reads its window at fixed offsets of the parameter space; several find theirs by the CTA index.
+__global__ void __launch_bounds__(kResampleTile) resample_kernel(const __grid_constant__ ResampleItems it) {
+    extern __shared__ float su[];
+    __shared__ int window[2];
+    if (it.n == 1) { resample_tile(it.w[0], blockIdx.x, su, window); return; }
+    const int b = item_at(it.tile0, it.n, blockIdx.x);
+    resample_tile(it.w[b], blockIdx.x - it.tile0[b], su, window);
+}
+
+void resample_windows(const ResampleWindow * w, int n, cudaStream_t s) {
+    if (n < 1 || n > kCodecMaxItems) { fprintf(stderr, "bark_b200: %d resample items in one launch (1 to %d)\n", n, kCodecMaxItems); throw std::runtime_error("unsupported configuration (see the message above)"); }
+    ResampleItems it{};
+    it.n = n;
+    int smem = 0;
+    for (int b = 0; b < n; b++) {
+        const ResampleWindow & v = w[b];
+        // the inputs the outputs read over the filter's full support: block k reads k o - w .. k o + o + w - 1
+        const long long lo = v.first / v.t.q * v.t.o - v.t.w, hi = (v.first + v.n_out - 1) / v.t.q * v.t.o + v.t.o + v.t.w - 1;
+        const long long need_lo = std::max(lo, 0LL), need_hi = std::min(hi, v.end - 1);
+        if (v.first < 0 || v.n_out < 1 || v.org < 0 || v.len < 0 || v.C < 1 || (need_lo <= need_hi && (need_lo < v.org || need_hi > v.org + v.len - 1))) {
+            fprintf(stderr, "bark_b200: resample window of item %d (frames %lld + %d, outputs %lld + %d) reads outside its frames\n", b, v.org, v.len, v.first, v.n_out);
+            throw std::runtime_error("unsupported configuration (see the message above)");
+        }
+        it.w[b] = v;
+        it.tile0[b + 1] = it.tile0[b] + (v.n_out + v.t.tile - 1) / v.t.tile;
+        smem = std::max(smem, v.t.smem);
+    }
+    BARK_LAUNCH(resample_kernel, (unsigned) it.tile0[n], kResampleTile, (size_t) smem * sizeof(float), s, it);
 }
 
 void resample(const float * x, long long n, int C, const ResampleTable & t, float * y, int L, cudaStream_t s) {
     if (L < 1) return;
-    const long long grid = ((long long) L + t.tile - 1) / t.tile;
-    BARK_LAUNCH(resample_kernel, (unsigned) grid, kResampleTile, (size_t) t.smem * sizeof(float), s, x, n, C, t.phase, t.taps, t.o, t.q, t.w, t.tile, L, y);
+    ResampleWindow w;
+    w.t = t; w.x = x; w.y = y; w.C = C; w.len = (int) n; w.end = n; w.n_out = L;
+    resample_windows(&w, 1, s);
 }
 
 }  // namespace bark

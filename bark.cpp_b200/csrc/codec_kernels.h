@@ -5,6 +5,8 @@
 #pragma once
 #include "model.h"
 
+#include <climits>
+
 namespace bark {
 
 // Items of one launch: bounded by the LSTM recurrence, whose CTAs hold h_{t-1} of every item in shared memory ([B][512] floats, 64 KB
@@ -53,8 +55,12 @@ void convtr_rows(const __half * src, __half * dst, int Cin, int Cout, int k, cud
 // Resampling (DESIGN.md §16): torchaudio.functional.resample's default sinc_interp_hann filter with an exact summation order, after
 // upstream EnCodec's channel down-mix.  Both rates lie in [kResampleMinRate, kResampleMaxRate].
 constexpr int kResampleMinRate = 4000, kResampleMaxRate = 384000, kResampleMaxChannels = 8;
+// o = sr / g, q = new_sr / g (g = gcd) and the filter's half width w in input frames (0 for equal rates)
+void resample_rates(int sr, int new_sr, int * o, int * q, int * w);
 // L = ceil(q n / o): samples of n frames at sr resampled to new_sr
 long long resample_len(long long n, int sr, int new_sr);
+// R(n) = q max(0, floor((n - w) / o)), n for equal rates: the outputs that no frame after the first n can change (DESIGN.md §20)
+long long resample_ready(long long n, int sr, int new_sr);
 // The taps of sr -> new_sr in double by the rule, rounded to f32, each phase trimmed to its nonzero span; fills t's sizes and returns
 // the bytes to upload (phases, then taps; empty for the identity)
 std::vector<unsigned char> resample_table(int sr, int new_sr, ResampleTable * t);
@@ -62,5 +68,17 @@ std::vector<unsigned char> resample_table(int sr, int new_sr, ResampleTable * t)
 void resample_bind(ResampleTable & t, const void * dev);
 // x: n interleaved frames [n][C] (device) -> y [L] (device), L = resample_len(n, t.sr, t.new_sr)
 void resample(const float * x, long long n, int C, const ResampleTable & t, float * y, int L, cudaStream_t s);
+// A window of one signal (the streams of codec_stream.cu): x holds len interleaved frames [len][C], the global frames org .. org + len
+// - 1, and y gets the n_out global outputs from first on.  Global frames below 0, and at or past end (LLONG_MAX while the end is not
+// known), read as zeros.  A window whose outputs read, over the filter's full support, a frame it neither holds nor treats as outside
+// the signal is refused.
+struct ResampleWindow {
+    ResampleTable t;
+    const float * x = nullptr; float * y = nullptr;
+    long long org = 0, first = 0, end = LLONG_MAX;
+    int len = 0, n_out = 0, C = 1;
+};
+// n <= kCodecMaxItems windows of their own tables and formats in one launch (shared memory: the largest item's)
+void resample_windows(const ResampleWindow * w, int n, cudaStream_t s);
 
 }  // namespace bark

@@ -33,6 +33,17 @@ bool codec_scratch(CodecScratch & sc, size_t frames, int n_q, const char * calle
     return true;
 }
 
+bool stage_scratch(CodecScratch & sc, size_t floats, const char * caller) {
+    if (floats <= sc.stage_cap) return true;
+    if (sc.stage) { cudaFree(sc.stage); sc.stage = nullptr; }
+    sc.stage_cap = 0;
+    if (cudaMalloc((void **) &sc.stage, floats * sizeof(float)) != cudaSuccess) {
+        (void) cudaGetLastError(); fprintf(stderr, "%s: out of device memory for %zu source samples\n", caller, floats); return false;
+    }
+    sc.stage_cap = floats;
+    return true;
+}
+
 void CodecScratch::release() {
     for (int i = 0; i < 3; i++) if (buf[i]) cudaFree(buf[i]);
     for (void * p : {(void *) gi, (void *) hbuf, (void *) counter, (void *) codes, (void *) stage}) if (p) cudaFree(p);
@@ -230,14 +241,7 @@ bool codec_encode(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, int 
             fprintf(stderr, "%s: %ssample %d is not finite (%g)\n", fn, item_tag(batch_fn, i).c_str(), k, (double) audio[i][k]); return false;
         }
     }
-    if (stage > sc.stage_cap) {
-        if (sc.stage) { cudaFree(sc.stage); sc.stage = nullptr; }
-        sc.stage_cap = 0;
-        if (cudaMalloc((void **) &sc.stage, stage * sizeof(float)) != cudaSuccess) {
-            (void) cudaGetLastError(); fprintf(stderr, "%s: out of device memory for %zu source samples\n", fn, stage); return false;
-        }
-        sc.stage_cap = stage;
-    }
+    if (!stage_scratch(sc, stage, fn)) return false;
     std::vector<int> T((size_t) n);
     for (int i = 0; i < n; i++) T[(size_t) i] = (len[(size_t) i] - 1) / kCodecHop + 1;
     return run_launches(cm, sc, s, n, T.data(), n_q, out, fn, [&](int first, int last, const float ** lat) {

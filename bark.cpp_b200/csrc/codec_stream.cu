@@ -23,7 +23,63 @@ long long codec_stream_ready(int direction, long long n) {
     return n >= kCodecMinFrames ? n * kCodecHop : 0;
 }
 
+long long codec_stream_ready_resampled(int direction, int sample_rate, long long n) {
+    // encode: the resampler's final outputs feed the encoder; decode: the decoder's final samples feed the resampler (DESIGN.md §20)
+    if (direction == kStreamEncode) return codec_stream_ready(kStreamEncode, resample_ready(n, sample_rate, kCodecSampleRate));
+    const long long samples = n < kCodecMinFrames ? 0 : n > LLONG_MAX / kCodecHop ? LLONG_MAX : n * kCodecHop;
+    return resample_ready(samples, kCodecSampleRate, sample_rate);
+}
+
 namespace {
+
+// the outputs of a stream's resampler final once `in` frames have arrived; at finish every output, the signal ending there
+long long resampler_target(const StreamResampler & rs, long long in, bool finish) {
+    return finish ? resample_len(in, rs.t.sr, rs.t.new_sr) : resample_ready(in, rs.t.sr, rs.t.new_sr);
+}
+
+// The resampler step of a pass over the resampled streams among st (DESIGN.md §20).  Stream i's n[i] new frames come from the host at
+// host[i] (an encode's interleaved source) or from the device at dev[i] (a decode's 24 kHz samples); one copy launch gathers them after
+// its history into `gather`, one launch of resample_kernel computes the out[i] outputs that became final into y[i], and a second copy
+// launch keeps the frames from the next block's first read on.  Every output released before finish has an index below the clip's
+// L = ceil(q n / o): block k is released once n >= (k + 1) o + w, and then its last output k q + q - 1 < q n / o.  It reads no frame
+// past n, so the frames that arrive later, and the zeros past the end at finish, cannot change it.
+void resample_step(cudaStream_t s, CodecStream * const * st, int count, const int * n, const void * const * host, const float * const * dev,
+                   float * gather, float * const * y, const int * out, bool finish) {
+    ColumnCopies g, back;
+    auto job = [](ColumnCopies & c, const float * src, float * dst, long long floats) {
+        if (floats <= 0) return;
+        c.src[c.n] = src; c.dst[c.n] = dst; c.src_ld[c.n] = c.dst_ld[c.n] = c.cols[c.n] = (int) floats; c.n++;
+    };
+    ResampleWindow w[kCodecMaxItems];
+    int m = 0;
+    size_t off = 0;
+    for (int i = 0; i < count; i++) {
+        if (!st[i]->resampled) continue;
+        StreamResampler & rs = st[i]->rs;
+        const int C = rs.channels, len = rs.h + n[i];
+        const long long in = rs.in + n[i], org = rs.in - rs.h, target = resampler_target(rs, in, finish);
+        if (target - rs.out != out[i]) throw std::runtime_error("stream resampler: outputs differ from the plan");
+        float * x = gather + off;
+        job(g, rs.hist, x, (long long) rs.h * C);
+        if (n[i] && host) {
+            BARK_CUDA_CHECK(cudaMemcpyAsync(x + (size_t) rs.h * C, host[i], (size_t) n[i] * C * sizeof(float), cudaMemcpyHostToDevice, s));
+            g_h2d_bytes += (size_t) n[i] * C * sizeof(float);
+        } else if (n[i]) job(g, dev[i], x + rs.h, n[i]);
+        if (out[i]) {
+            ResampleWindow & v = w[m++];
+            v.t = rs.t; v.x = x; v.y = y[i]; v.org = org; v.len = len; v.C = C; v.first = rs.out; v.n_out = out[i]; v.end = finish ? in : LLONG_MAX;
+        }
+        const long long keep = finish ? in : std::max(org, target / rs.t.q * rs.t.o - rs.t.w);
+        const int h = (int)(in - keep);
+        if (h > rs.cap) throw std::runtime_error("stream resampler history overflow");
+        job(back, x + (size_t)(keep - org) * C, rs.hist, (long long) h * C);
+        rs.in = in; rs.out = target; rs.h = h;
+        off += (size_t) len * C;
+    }
+    copy_columns(g, 1, s);
+    if (m) resample_windows(w, m, s);
+    copy_columns(back, 1, s);
+}
 
 // A layer over windows.  Output t reads input positions t stride - pad .. t stride - pad + k - 1, pad = k - stride.  A convolution
 // reflects those below 0, so its output 0 waits for its largest reflected read; the transposed convolution (k = 2, stride 1: frames
@@ -161,17 +217,33 @@ int present(const std::vector<int> & N, int * T, int * item) {
 bool stream_pass(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, CodecStream * const * st, const void * const * in, const int * n, int count,
                  bool finish, const char * fn) {
     const int dir = st[0]->direction, n_q = st[0]->n_q;
-    // frames of scratch per stream: its new frames, one more held by the strided convs, and the kCodecMinFrames the first k = 7 conv of a
-    // direction releases at once when a stream reaches them
-    size_t frames = 0;
-    for (int i = 0; i < count; i++) frames += (size_t)(dir == kStreamEncode ? (n[i] + kCodecHop - 1) / kCodecHop : n[i]) + kCodecMinFrames + 1;
-    if (!codec_scratch(sc, frames, n_q, fn)) return false;
-    StreamRunner r{sc, s, count, st, finish, dir == kStreamEncode ? 1 : cm.hidden_dim, std::vector<int>(n, n + count), sc.buf[0], sc.buf[1], sc.buf[2]};
+    // per stream: the codec's new inputs N (a resampled encode's are its resampler's new outputs) and the resampler's new outputs.
+    // Frames of scratch per stream: its new frames, one more held by the strided convs, and the kCodecMinFrames the first k = 7 conv of
+    // a direction releases at once when a stream reaches them; a resampled decode's resampler gathers and writes its samples there too.
+    std::vector<int> N(n, n + count), out((size_t) count, 0);
+    size_t frames = 0, stage = 0;
+    for (int i = 0; i < count; i++) {
+        const CodecStream & t = *st[i];
+        if (t.resampled) {
+            const long long rin = dir == kStreamEncode ? t.rs.in + n[i] : codec_stream_ready(kStreamDecode, t.n_in + n[i]);
+            out[(size_t) i] = (int)(resampler_target(t.rs, rin, finish) - t.rs.out);
+            if (dir == kStreamEncode) { N[(size_t) i] = out[(size_t) i]; stage += (size_t)(t.rs.h + n[i]) * t.rs.channels; }
+            else frames += (size_t)(t.rs.h + (rin - t.rs.in) + out[(size_t) i]) / 10240 + 2;
+        }
+        frames += (size_t)(dir == kStreamEncode ? (N[(size_t) i] + kCodecHop - 1) / kCodecHop : N[(size_t) i]) + kCodecMinFrames + 1;
+    }
+    if (!codec_scratch(sc, frames, n_q, fn) || !stage_scratch(sc, stage, fn)) return false;
+    StreamRunner r{sc, s, count, st, finish, dir == kStreamEncode ? 1 : cm.hidden_dim, N, sc.buf[0], sc.buf[1], sc.buf[2]};
+    std::vector<float *> y((size_t) count, nullptr);
     int T[kCodecMaxItems], item[kCodecMaxItems];
     if (dir == kStreamEncode) {
+        // the source frames through the resamplers, straight into the encoder's input; mono 24 kHz samples copied there
         size_t off = 0;
-        for (int i = 0; i < count; off += (size_t) n[i], i++)
-            if (n[i]) { BARK_CUDA_CHECK(cudaMemcpyAsync(r.cur + off, in[i], (size_t) n[i] * sizeof(float), cudaMemcpyHostToDevice, s)); g_h2d_bytes += (size_t) n[i] * sizeof(float); }
+        for (int i = 0; i < count; off += (size_t) N[(size_t) i], i++) y[(size_t) i] = r.cur + off;
+        resample_step(s, st, count, n, in, nullptr, sc.stage, y.data(), out.data(), finish);
+        off = 0;
+        for (int i = 0; i < count; off += (size_t) N[(size_t) i], i++)
+            if (n[i] && !st[i]->resampled) { BARK_CUDA_CHECK(cudaMemcpyAsync(r.cur + off, in[i], (size_t) n[i] * sizeof(float), cudaMemcpyHostToDevice, s)); g_h2d_bytes += (size_t) n[i] * sizeof(float); }
         encoder_layers(cm.enc, r);
         const int m = present(r.N, T, item);
         if (m && !rvq_encode(cm.embed, cm.embed_norm, n_q, cm.n_bins, cm.hidden_dim, r.cur, T, m, sc.codes, s)) {
@@ -184,32 +256,52 @@ bool stream_pass(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, Codec
         const int m = present(r.N, T, item);
         if (m) rvq_decode(cm, sc.codes, n_q, T, m, r.cur, s);
         decoder_layers(cm, r);
+        // the decoder's new samples through the resamplers, after its last layer: gathered in r.a, resampled into r.b
+        std::vector<const float *> dev((size_t) count, nullptr);
+        size_t yoff = 0;
+        off = 0;
+        for (int i = 0; i < count; off += (size_t) r.N[(size_t) i], i++) {
+            dev[(size_t) i] = r.cur + off;
+            if (st[i]->resampled) { y[(size_t) i] = r.b + yoff; yoff += (size_t) out[(size_t) i]; }
+        }
+        resample_step(s, st, count, r.N.data(), nullptr, dev.data(), r.a, y.data(), out.data(), finish);
     }
-    // the outputs back, one synchronisation
-    const int m = present(r.N, T, item);
-    std::vector<std::vector<int32_t>> codes((size_t) m);
-    std::vector<std::vector<float>> audio((size_t) m);
+    // the outputs back, one synchronisation: codes, or samples (a resampled decode's from its resampler)
+    std::vector<std::vector<int32_t>> codes((size_t) count);
+    std::vector<std::vector<float>> audio((size_t) count);
     size_t off = 0;
-    for (int j = 0; j < m; j++) {
-        const size_t k = (size_t) T[j] * (dir == kStreamEncode ? n_q : 1);
-        if (dir == kStreamEncode) { codes[(size_t) j].resize(k); BARK_CUDA_CHECK(cudaMemcpyAsync(codes[(size_t) j].data(), sc.codes + off, k * sizeof(int32_t), cudaMemcpyDeviceToHost, s)); g_d2h_bytes += k * sizeof(int32_t); }
-        else { audio[(size_t) j].resize(k); BARK_CUDA_CHECK(cudaMemcpyAsync(audio[(size_t) j].data(), r.cur + off, k * sizeof(float), cudaMemcpyDeviceToHost, s)); g_d2h_bytes += k * sizeof(float); }
+    for (int i = 0; i < count; i++) {
+        const size_t k = (size_t) r.N[(size_t) i];
+        if (dir == kStreamEncode) {
+            if (!k) continue;
+            codes[(size_t) i].resize(k * n_q);
+            BARK_CUDA_CHECK(cudaMemcpyAsync(codes[(size_t) i].data(), sc.codes + off, k * n_q * sizeof(int32_t), cudaMemcpyDeviceToHost, s)); g_d2h_bytes += k * n_q * sizeof(int32_t);
+            off += k * n_q;
+            continue;
+        }
+        const float * src = st[i]->resampled ? y[(size_t) i] : r.cur + off;
+        const size_t ks = st[i]->resampled ? (size_t) out[(size_t) i] : k;
         off += k;
+        if (!ks) continue;
+        audio[(size_t) i].resize(ks);
+        BARK_CUDA_CHECK(cudaMemcpyAsync(audio[(size_t) i].data(), src, ks * sizeof(float), cudaMemcpyDeviceToHost, s)); g_d2h_bytes += ks * sizeof(float);
     }
     BARK_CUDA_CHECK(cudaStreamSynchronize(s));
-    for (int j = 0; j < m; j++) {
-        CodecStream & t = *st[item[j]];
-        t.n_out += T[j];
-        if (dir == kStreamDecode) { t.audio.insert(t.audio.end(), audio[(size_t) j].begin(), audio[(size_t) j].end()); continue; }
-        for (int f = 0; f < T[j]; f++)                   // pending codes are frame-major
-            for (int q = 0; q < n_q; q++) t.codes.push_back(codes[(size_t) j][(size_t) q * T[j] + f]);
+    for (int i = 0; i < count; i++) {
+        CodecStream & t = *st[i];
+        const int k = r.N[(size_t) i];
+        t.n_in += dir == kStreamEncode ? N[(size_t) i] : n[i];
+        t.n_out += k;
+        if (dir == kStreamDecode) { t.audio.insert(t.audio.end(), audio[(size_t) i].begin(), audio[(size_t) i].end()); continue; }
+        for (int f = 0; f < k; f++)                      // pending codes are frame-major
+            for (int q = 0; q < n_q; q++) t.codes.push_back(codes[(size_t) i][(size_t) q * k + f]);
     }
     return true;
 }
 
 }  // namespace
 
-bool codec_stream_init(const CodecModel & cm, CodecStream & st, int direction, int n_q) {
+bool codec_stream_init(const CodecModel & cm, CodecStream & st, int direction, int n_q, int channels, int sample_rate) {
     LayoutRunner l{direction == kStreamEncode ? 1 : cm.hidden_dim, {}};
     if (direction == kStreamEncode) encoder_layers(cm.enc, l); else decoder_layers(cm, l);
     size_t floats = (size_t) 4 * 2 * l.lstm_C;
@@ -225,28 +317,51 @@ bool codec_stream_init(const CodecModel & cm, CodecStream & st, int direction, i
         st.win.push_back(x);
         p += (size_t) w.first * w.second;
     }
+    if (channels == 1 && sample_rate == kCodecSampleRate) return true;
+    // the resampler: its own copy of the rate pair's taps, and room for 2w + o - 1 frames, the most it keeps
+    StreamResampler & rs = st.rs;
+    st.resampled = true; rs.channels = channels; rs.rate = sample_rate;
+    const std::vector<unsigned char> bytes = direction == kStreamEncode ? resample_table(sample_rate, kCodecSampleRate, &rs.t)
+                                                                        : resample_table(kCodecSampleRate, sample_rate, &rs.t);
+    if (!bytes.empty()) {
+        BARK_CUDA_CHECK(cudaMalloc(&rs.taps, bytes.size()));
+        BARK_CUDA_CHECK(cudaMemcpy(rs.taps, bytes.data(), bytes.size(), cudaMemcpyHostToDevice)); g_h2d_bytes += bytes.size();
+        resample_bind(rs.t, rs.taps);
+    }
+    rs.cap = 2 * rs.t.w + rs.t.o - 1;
+    if (rs.cap > 0) BARK_CUDA_CHECK(cudaMalloc((void **) &rs.hist, (size_t) rs.cap * channels * sizeof(float)));
     return true;
 }
 
 void CodecStream::release() {
-    if (mem) cudaFree(mem);
-    mem = nullptr;
+    for (void * p : {(void *) mem, rs.taps, (void *) rs.hist}) if (p) cudaFree(p);
+    mem = nullptr; rs.taps = nullptr; rs.hist = nullptr;
 }
+
+// the outputs a stream hands back: frames, or samples (at its own rate on a resampled decode)
+static long long outputs(const CodecStream & t) { return t.resampled && t.direction == kStreamDecode ? t.rs.out : t.n_out; }
 
 int codec_stream_run(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, CodecStream * const * st, const void * const * in, const int * n, int count,
                      bool finish, const char * fn) {
     const int dir = st[0]->direction;
     std::vector<long long> before((size_t) count);
-    for (int i = 0; i < count; i++) before[(size_t) i] = st[i]->n_out;
-    // a long push runs in passes of a bounded size per stream (the outputs do not depend on the chunks), a finish in one pass of none
+    for (int i = 0; i < count; i++) before[(size_t) i] = outputs(*st[i]);
+    // a long push runs in passes of a bounded size per stream (the outputs do not depend on the chunks), a finish in one pass of none.
+    // A resampled encode's pass takes the frames of about as many 24 kHz samples, and at most as many floats.
     const int per_frames = std::max(1, kCodecLaunchFrames / count - 2), per = dir == kStreamEncode ? per_frames * kCodecHop : per_frames;
-    std::vector<int> done((size_t) count, 0), take((size_t) count);
+    std::vector<int> done((size_t) count, 0), take((size_t) count), step((size_t) count, per), width((size_t) count, 1);
+    for (int i = 0; i < count; i++)
+        if (dir == kStreamEncode && st[i]->resampled) {
+            const StreamResampler & rs = st[i]->rs;
+            width[(size_t) i] = rs.channels;
+            step[(size_t) i] = (int) std::max<long long>(1, std::min<long long>((long long) per * rs.t.o / rs.t.q, per / rs.channels));
+        }
     std::vector<const void *> ptr((size_t) count);
     for (bool more = true; more;) {
         more = false;
         for (int i = 0; i < count; i++) {
-            take[(size_t) i] = finish ? 0 : std::min(n[i] - done[(size_t) i], per);
-            ptr[(size_t) i] = dir == kStreamEncode ? (const void *)((const float *) in[i] + done[(size_t) i])
+            take[(size_t) i] = finish ? 0 : std::min(n[i] - done[(size_t) i], step[(size_t) i]);
+            ptr[(size_t) i] = dir == kStreamEncode ? (const void *)((const float *) in[i] + (size_t) width[(size_t) i] * done[(size_t) i])
                                                    : (const void *)((const int32_t *) in[i] + (size_t) st[i]->n_q * done[(size_t) i]);
             more |= take[(size_t) i] > 0;
         }
@@ -263,7 +378,7 @@ int codec_stream_run(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, C
                 ptr[(size_t) i] = part.back().data();
             }
         if (!stream_pass(cm, sc, s, st, ptr.data(), take.data(), count, finish, fn)) return -1;
-        for (int i = 0; i < count; i++) { st[i]->failed = false; st[i]->n_in += take[(size_t) i]; done[(size_t) i] += take[(size_t) i]; }
+        for (int i = 0; i < count; i++) { st[i]->failed = false; done[(size_t) i] += take[(size_t) i]; }
         if (finish) break;
     }
     long long added = 0;
@@ -271,12 +386,17 @@ int codec_stream_run(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, C
         CodecStream & t = *st[i];
         if (finish) t.finished = true;
         const long long want = finish ? (dir == kStreamEncode ? (t.n_in - 1) / kCodecHop + 1 : t.n_in * kCodecHop) : codec_stream_ready(dir, t.n_in);
-        if (t.n_out != want) {
-            fprintf(stderr, "%s: internal error: %lld outputs after %lld inputs, the rule says %lld\n", fn, t.n_out, t.n_in, want);
+        // a resampler's outputs by its own rule, and the codec's inputs or outputs are its outputs or inputs
+        const StreamResampler & rs = t.rs;
+        const bool rs_ok = !t.resampled || (rs.out == resampler_target(rs, rs.in, finish) && (dir == kStreamEncode ? t.n_in == rs.out : rs.in == t.n_out));
+        if (t.n_out != want || !rs_ok) {
+            fprintf(stderr, "%s: internal error: %lld outputs after %lld inputs, the rule says %lld", fn, t.n_out, t.n_in, want);
+            if (t.resampled) fprintf(stderr, "; resampler: %lld outputs after %lld frames, the rule says %lld", rs.out, rs.in, resampler_target(rs, rs.in, finish));
+            fprintf(stderr, "\n");
             t.failed = true;
             return -1;
         }
-        added += t.n_out - before[(size_t) i];
+        added += outputs(t) - before[(size_t) i];
     }
     return (int) std::min<long long>(added, INT_MAX);
 }

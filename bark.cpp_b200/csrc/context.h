@@ -193,6 +193,8 @@ bool resample_input_ok(const char * fn, const std::string & item, const float * 
 std::string item_tag(const char * batch_fn, int i);
 // sizes sc for one launch of `frames` frames of n_q codebooks: false (message naming caller) when the device is out of memory
 bool codec_scratch(CodecScratch & sc, size_t frames, int n_q, const char * caller);
+// sizes sc.stage (source frames before the resampler) to `floats`, the same way
+bool stage_scratch(CodecScratch & sc, size_t floats, const char * caller);
 
 // codec_stream.cu — streaming EnCodec (DESIGN.md §19).  A stream goes one way: mono 24 kHz samples to codes, or codes to samples, at the
 // n_q it opened with.  Its state lives on the device: per windowed layer the input columns later outputs still read, per LSTM layer
@@ -200,10 +202,23 @@ bool codec_scratch(CodecScratch & sc, size_t frames, int n_q, const char * calle
 constexpr int kStreamEncode = 0, kStreamDecode = 1;
 // the outputs final after n inputs, before finish: frames after n samples (encode), samples after n frames (decode)
 long long codec_stream_ready(int direction, long long n);
+// The same for a stream at another format (DESIGN.md §20): frames after n interleaved frames at sample_rate (encode), samples at
+// sample_rate after n frames (decode)
+long long codec_stream_ready_resampled(int direction, int sample_rate, long long n);
+// A stream's resampler (DESIGN.md §20): an encode's interleaved source frames at `rate` to the encoder's 24 kHz samples, or a decode's
+// 24 kHz samples to `rate`.  It keeps its input from the next block's first read on, raw, and its own device copy of the taps.
+struct StreamResampler {
+    int channels = 1, rate = 0;
+    ResampleTable t;                                     // bound to taps (null for equal rates)
+    void * taps = nullptr;
+    float * hist = nullptr; int cap = 0, h = 0;          // hist [cap][channels], h frames held: the global frames in - h .. in - 1
+    long long in = 0, out = 0;                           // frames in, outputs final
+};
 struct CodecStream {
     int direction = kStreamEncode, n_q = 0;
     bool finished = false, failed = false;               // failed: a pass did not complete (a CUDA failure); the state is lost
-    long long n_in = 0, n_out = 0;                       // inputs pushed, outputs final
+    long long n_in = 0, n_out = 0;                       // the codec's inputs pushed, outputs final (24 kHz samples on a resampled stream)
+    bool resampled = false; StreamResampler rs;          // any format other than mono 24 kHz
     struct Window { int C = 0, cap = 0, h = 0; long long in = 0, out = 0; float * hist = nullptr; };   // hist [C][cap], h columns held
     std::vector<Window> win;                             // in layer-list order
     float * lstm[4] = {nullptr, nullptr, nullptr, nullptr};   // (h, c) [2][512] of the four LSTM layers (two for the direction's model)
@@ -212,9 +227,10 @@ struct CodecStream {
     std::vector<float> audio;
     void release();
 };
-// allocates st's device state for direction at n_q codebooks (a CUDA failure throws)
-bool codec_stream_init(const CodecModel & cm, CodecStream & st, int direction, int n_q);
-// pushes n[i] inputs at in[i] (samples, or codes [n_q][n[i]]) to the count <= kCodecMaxItems checked streams st[i] of one model and
+// allocates st's device state for direction at n_q codebooks, and for any format but mono 24 kHz (channels 1 for a decode) its
+// resampler (a CUDA failure throws)
+bool codec_stream_init(const CodecModel & cm, CodecStream & st, int direction, int n_q, int channels = 1, int sample_rate = kCodecSampleRate);
+// pushes n[i] inputs at in[i] (samples, interleaved frames [n[i]][channels] on a resampled encode, or codes [n_q][n[i]]) to the count <= kCodecMaxItems checked streams st[i] of one model and
 // direction in one pass of the kernels (or several for a long push), or with finish none, closing them.  Returns the outputs that
 // became final, -1 (message naming fn) on a failure.
 int codec_stream_run(const CodecModel & cm, CodecScratch & sc, cudaStream_t s, CodecStream * const * st, const void * const * in, const int * n, int count,

@@ -249,7 +249,8 @@ namespace {
 
 // The checks of a push or finish on `count` streams (after which nothing can refuse it): false (message naming fn) for a null or
 // repeated stream, streams of several contexts or directions, a finished stream, or a count outside [1, kCodecMaxItems]; with in and n,
-// a null chunk, a negative count, a non-finite sample or a code outside the codebooks
+// a null chunk, a negative count, a non-finite sample (on a resampled encode: n * channels >= 2^31, or |x| > 2^64, the limits of
+// resample_input_ok) or a code outside the codebooks
 bool stream_args(const char * fn, bark_b200_encodec_stream * const * s, const void * const * in, const int * n, int count) {
     if (!s || count < 1 || count > kCodecMaxItems) { fprintf(stderr, "%s: %d streams (1 to %d per call)\n", fn, s ? count : 0, kCodecMaxItems); return false; }
     for (int i = 0; i < count; i++) {
@@ -262,7 +263,15 @@ bool stream_args(const char * fn, bark_b200_encodec_stream * const * s, const vo
         if (!in) continue;
         if (!in[i] || n[i] < 0) { fprintf(stderr, "%s: %s%s\n", fn, tag.c_str(), in[i] ? "negative count" : "null input"); return false; }
         const CodecStream & t = s[i]->st;
-        if (t.direction == kStreamEncode) {
+        if (t.direction == kStreamEncode && t.resampled) {
+            const float * x = (const float *) in[i];
+            const long long C = t.rs.channels, floats = n[i] * C;
+            if (floats > INT_MAX) { fprintf(stderr, "%s: %s%d frames of %lld channels (at most 2^31 - 1 samples per push)\n", fn, tag.c_str(), n[i], C); return false; }
+            for (long long k = 0; k < floats; k++) if (!(std::fabs(x[k]) <= 0x1p64f)) {
+                fprintf(stderr, "%s: %ssample %lld (frame %lld, channel %lld) is not finite or exceeds 2^64 in magnitude (%g)\n", fn, tag.c_str(), k, k / C, k % C, (double) x[k]);
+                return false;
+            }
+        } else if (t.direction == kStreamEncode) {
             const float * x = (const float *) in[i];
             for (int k = 0; k < n[i]; k++) if (!std::isfinite(x[k])) { fprintf(stderr, "%s: %ssample %d is not finite (%g)\n", fn, tag.c_str(), k, (double) x[k]); return false; }
         } else {
@@ -290,22 +299,35 @@ int push(const char * fn, bark_b200_encodec_stream * const * s, const void * con
     return stream_call(s[0], -1, [&] { return codec_stream_run(s[0]->e->model, s[0]->e->scratch, s[0]->e->stream, st.data(), in, n, count, false, fn); });
 }
 
-}  // namespace
-
-extern "C" struct bark_b200_encodec_stream * bark_b200_encodec_stream_open(struct encodec_context * e, int direction) {
-    const char * fn = __func__;
+// a stream of e in direction at a format (mono 24 kHz: the plain stream), named fn
+bark_b200_encodec_stream * open_stream(const char * fn, encodec_context * e, int direction, int channels, int sample_rate) {
     if (!e) { fprintf(stderr, "%s: null context\n", fn); return nullptr; }
     if (direction != BARK_B200_STREAM_ENCODE && direction != BARK_B200_STREAM_DECODE) { fprintf(stderr, "%s: unknown direction %d\n", fn, direction); return nullptr; }
+    if (channels < 1 || channels > kResampleMaxChannels) { fprintf(stderr, "%s: %d channels (1 to %d)\n", fn, channels, kResampleMaxChannels); return nullptr; }
+    if (sample_rate < kResampleMinRate || sample_rate > kResampleMaxRate) {
+        fprintf(stderr, "%s: sample rate %d Hz (%d to %d)\n", fn, sample_rate, kResampleMinRate, kResampleMaxRate); return nullptr;
+    }
+    if (direction == BARK_B200_STREAM_DECODE && channels != 1) { fprintf(stderr, "%s: a decode stream gives mono samples (channels 1, got %d)\n", fn, channels); return nullptr; }
     if (direction == BARK_B200_STREAM_ENCODE && !e->model.enc.present) { fprintf(stderr, "%s: the model file has no EnCodec encoder tensors (encoder.*)\n", fn); return nullptr; }
     int n_q;
     if (!codebooks_for(e, fn, &n_q)) return nullptr;
     auto * s = new bark_b200_encodec_stream{e, CodecStream()};
-    if (!guarded(false, [&] { BARK_CUDA_CHECK(cudaSetDevice(e->device)); return codec_stream_init(e->model, s->st, direction, n_q); })) {
+    if (!guarded(false, [&] { BARK_CUDA_CHECK(cudaSetDevice(e->device)); return codec_stream_init(e->model, s->st, direction, n_q, channels, sample_rate); })) {
         fprintf(stderr, "%s: could not allocate the stream's state\n", fn);
         bark_b200_encodec_stream_close(s);
         return nullptr;
     }
     return s;
+}
+
+}  // namespace
+
+extern "C" struct bark_b200_encodec_stream * bark_b200_encodec_stream_open(struct encodec_context * e, int direction) {
+    return open_stream(__func__, e, direction, 1, kCodecSampleRate);
+}
+
+extern "C" struct bark_b200_encodec_stream * bark_b200_encodec_stream_open_resampled(struct encodec_context * e, int direction, int channels, int sample_rate) {
+    return open_stream(__func__, e, direction, channels, sample_rate);
 }
 
 extern "C" int bark_b200_encodec_stream_push(struct bark_b200_encodec_stream * s, const void * in, int n) {
@@ -338,7 +360,14 @@ extern "C" int bark_b200_encodec_stream_finish(struct bark_b200_encodec_stream *
     const char * fn = __func__;
     if (!stream_args(fn, &s, nullptr, nullptr, 1)) return -1;
     const CodecStream & t = s->st;
-    if (t.direction == kStreamEncode ? t.n_in < kCodecMinSamples : t.n_in < kCodecMinFrames) {
+    if (t.resampled && t.direction == kStreamEncode) {              // the encoder finishes on the resampled clip's L samples
+        const long long L = resample_len(t.rs.in, t.rs.rate, kCodecSampleRate);
+        if (L < kCodecMinSamples) {
+            fprintf(stderr, "%s: %lld frames at %d Hz resample to %lld samples at %d Hz (at least %d: %d frames)\n", fn, t.rs.in, t.rs.rate, L, kCodecSampleRate,
+                    kCodecMinSamples, kCodecMinFrames);
+            return -1;
+        }
+    } else if (t.direction == kStreamEncode ? t.n_in < kCodecMinSamples : t.n_in < kCodecMinFrames) {
         fprintf(stderr, "%s: need at least %d %s (reflect padding of the k=7 convolutions), got %lld\n", fn, t.direction == kStreamEncode ? kCodecMinSamples : kCodecMinFrames,
                 t.direction == kStreamEncode ? "samples" : "frames", t.n_in);
         return -1;
@@ -352,6 +381,12 @@ extern "C" int bark_b200_encodec_stream_finish(struct bark_b200_encodec_stream *
 extern "C" long long bark_b200_encodec_stream_ready(int direction, long long n) {
     if ((direction != BARK_B200_STREAM_ENCODE && direction != BARK_B200_STREAM_DECODE) || n < 0) return -1;
     return codec_stream_ready(direction, n);
+}
+
+extern "C" long long bark_b200_encodec_stream_ready_resampled(int direction, int sample_rate, long long n) {
+    if ((direction != BARK_B200_STREAM_ENCODE && direction != BARK_B200_STREAM_DECODE) || n < 0) return -1;
+    if (sample_rate < kResampleMinRate || sample_rate > kResampleMaxRate) return -1;
+    return codec_stream_ready_resampled(direction, sample_rate, n);
 }
 
 extern "C" int bark_b200_encodec_stream_codebooks(struct bark_b200_encodec_stream * s) {

@@ -10,6 +10,7 @@
 #include <cmath>
 #include <cstring>
 #include <optional>
+#include <string>
 #include <vector>
 
 using namespace bark;
@@ -677,5 +678,43 @@ extern "C" int bark_b200_device_math(int fn, uint32_t lo_bits, uint32_t stride, 
         BARK_LAUNCH(device_math_kernel, std::min<uint32_t>((count + 255) / 256, 4096), 256, 0, 0, fn, lo_bits, stride, count, o.out<float>());
         if (!finish("bark_b200_device_math")) return 0;
         return o.read("bark_b200_device_math", out) ? 1 : -1;
+    });
+}
+
+// resample_kernel over windows of n items, each with its own table (built as a stream builds it) and format, in one launch
+extern "C" int bark_b200_resample_window(const float * in, const int * n_frames, const int * channels, const int * in_rates, const int * out_rates,
+                                         const long long * org, const long long * first, const int * n_out, const long long * end, int n, float * out) {
+    return guarded(0, [&] {
+        const char * fn = "bark_b200_resample_window";
+        if (!in || !n_frames || !channels || !in_rates || !out_rates || !out) { fprintf(stderr, "%s: null argument\n", fn); return 0; }
+        if (n < 1 || n > kCodecMaxItems) { fprintf(stderr, "%s: %d items (1 to %d)\n", fn, n, kCodecMaxItems); return 0; }
+        CodecWindow cw;
+        size_t out_total = 0, in_total = 0;
+        if (!hook_window(fn, n, org, first, n_out, &cw, &out_total)) return 0;
+        std::vector<ResampleWindow> w((size_t) n);
+        std::vector<std::vector<unsigned char>> bytes((size_t) n);
+        for (int b = 0; b < n; b++) {
+            const std::string item = "item " + std::to_string(b) + ": ";
+            if (n_frames[b] < 0) { fprintf(stderr, "%s: %s%d frames\n", fn, item.c_str(), n_frames[b]); return 0; }
+            if (n_frames[b] > 0 && !resample_input_ok(fn, item, in + in_total, n_frames[b], channels[b], in_rates[b])) return 0;
+            if (channels[b] < 1 || channels[b] > kResampleMaxChannels || std::min(in_rates[b], out_rates[b]) < kResampleMinRate ||
+                std::max(in_rates[b], out_rates[b]) > kResampleMaxRate) { fprintf(stderr, "%s: %sformat outside the resampler's limits\n", fn, item.c_str()); return 0; }
+            bytes[(size_t) b] = resample_table(in_rates[b], out_rates[b], &w[(size_t) b].t);
+            w[(size_t) b].org = org[b]; w[(size_t) b].first = first[b]; w[(size_t) b].n_out = n_out[b]; w[(size_t) b].len = n_frames[b];
+            w[(size_t) b].C = channels[b]; w[(size_t) b].end = end && end[b] >= 0 ? end[b] : LLONG_MAX;
+            in_total += (size_t) n_frames[b] * channels[b];
+        }
+        DeviceBuffers mem;
+        const float * d_in = mem.upload(in, std::max(in_total, (size_t) 1) * sizeof(float));
+        const GuardedOutput y(mem, out_total * sizeof(float), nullptr);
+        size_t xo = 0, yo = 0;
+        for (int b = 0; b < n; b++) {
+            if (!bytes[(size_t) b].empty()) resample_bind(w[(size_t) b].t, mem.upload(bytes[(size_t) b].data(), bytes[(size_t) b].size()));
+            w[(size_t) b].x = d_in + xo; w[(size_t) b].y = y.out<float>() + yo;
+            xo += (size_t) n_frames[b] * channels[b]; yo += (size_t) n_out[b];
+        }
+        resample_windows(w.data(), n, 0);
+        if (!finish(fn)) return 0;
+        return y.read(fn, out) ? 1 : -1;
     });
 }

@@ -316,6 +316,41 @@ BARK_API long long bark_b200_encodec_stream_ready(int direction, long long n);
 BARK_API int  bark_b200_encodec_stream_codebooks(struct bark_b200_encodec_stream * s);
 BARK_API void bark_b200_encodec_stream_close(struct bark_b200_encodec_stream * s);
 
+/* RESAMPLED STREAMS (DESIGN.md §20): a stream at any sample rate and channel count, as the RESAMPLED ENCODEC calls take whole clips.
+ * encode: in = n interleaved frames [n][channels] at sample_rate (1 <= channels <= 8, 4000 <= sample_rate <= 384000), down-mixed and
+ *         resampled to 24 kHz on the GPU, then encoded; the n of a push counts frames.  Everything returned, joined, equals
+ *         bark_b200_encodec_compress_resampled(e, all frames, n, channels, sample_rate) bit for bit.
+ * decode: channels must be 1; the samples read back are at sample_rate, and everything returned, joined, equals
+ *         bark_b200_resample(encodec_decompress_audio's 320 T samples, 320 T, 1, 24000, sample_rate) bit for bit.
+ * Mono 24 kHz is the plain stream, bit for bit and in readiness.  push, push_batch, read, finish, codebooks and close take these streams
+ * unchanged; a push_batch may mix formats and plain streams (one context, one direction), each stream getting what its own push would.
+ * Readiness, an integer closed form of the rates: with o = sr / g, q = new_sr / g (g = gcd) and w = ceil(6 o / (0.99 min(o, q))) the
+ * filter's half width (§16), output k q + j reads the frames k o - w .. k o + o + w - 1, so after n input frames
+ *   R(n) = q * max(0, floor((n - w) / o)) resampled samples are final (R(n) = n for equal rates).
+ *   encode: after n frames, bark_b200_encodec_stream_ready(ENCODE, R(n)) code frames are final (48 kHz: w = 13, o = 2, so the first
+ *           frame needs 4493 frames; 44.1 kHz: w = 12, o = 147);
+ *   decode: after n code frames, R'(bark_b200_encodec_stream_ready(DECODE, n)) samples are final, R' for 24000 -> sample_rate.
+ * finish: an encode resamples its tail up to L = ceil(q n / o) with zeros past the last frame, as the whole clip does, and finishes the
+ * encoder on L samples; it refuses L < 1921 (at 48 kHz 3840 frames are refused, 3841 accepted).  A decode refuses T < 7 as before and
+ * adds the resampler's tail up to ceil(q' 320 T / o').  On top of the plain streams' refusals: open refuses channels outside 1..8, a
+ * rate outside 4000..384000 and a decode with channels != 1 (NULL with a message); a push refuses n * channels >= 2^31 and a sample
+ * with |x| > 2^64, leaving every stream of the call unchanged.  The state stays O(1) in the stream's length: the resampler keeps at most
+ * 2w + o - 1 frames and its own copy of the rate pair's taps (18 MB at 383999 Hz).
+ *   bark_b200_encodec_stream_open_resampled ... a stream at that format
+ *   bark_b200_encodec_stream_ready_resampled .. the rule above: the outputs final after n inputs (frames, or code frames) before
+ *                                               finish; -1 for an unknown direction, a rate outside the limits or n < 0
+ *   bark_b200_resample_window .................. no context, host buffers, for the tests: n <= 32 items of their own channels[b] and
+ *                                               rates in_rates[b] -> out_rates[b] in one launch.  Item b's n_frames[b] interleaved
+ *                                               frames (in, item after item) are the global frames org[b] ..; out (item after item)
+ *                                               gets its n_out[b] global outputs from first[b] on.  Frames below 0, and at or past
+ *                                               end[b] where end is not NULL and end[b] >= 0, read as zeros.  Returns 1, 0 on invalid
+ *                                               arguments or a window whose outputs read a frame it does not hold, -1 if a store
+ *                                               landed in the guard bands around the output. */
+BARK_API struct bark_b200_encodec_stream * bark_b200_encodec_stream_open_resampled(struct encodec_context * e, int direction, int channels, int sample_rate);
+BARK_API long long bark_b200_encodec_stream_ready_resampled(int direction, int sample_rate, long long n);
+BARK_API int  bark_b200_resample_window(const float * in, const int * n_frames, const int * channels, const int * in_rates, const int * out_rates,
+                                        const long long * org, const long long * first, const int * n_out, const long long * end, int n, float * out);
+
 /* FAST MODE (BARK_B200_MODE=fast in the environment at load; opt-in, NOT bit-identical to the reference): the fine model's
  * 1024-row passes (bark.cpp:1416-1584) run as wgmma tensor-core GEMMs + flash-style attention (csrc/fast_kernels.cu).
  * Every weight type the loader reads runs it: an f16 file's fine matrices are used as stored; those of an f32, q4_0, q4_1, q5_0, q5_1
